@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the registrators/ hot path on B200.
+"""bench.py — headline benchmark of the registrators/ hot path on H100.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 One *alignment* is BASELINE.json configs[1]: a synthetic 64-beam 120 000-point scan against a
 500 000-point submap (106 784 target points with normals after the caller-side CalculateNormals),
@@ -16,7 +16,8 @@ sm_align_pairs by --host-threads (2) host threads over --pipelines (16) matcher 
 * `e2e`    : the same through host buffers (pinned host memory -> H2D inside the timed region,
              result records read back, all-gather included).
 * roofline : dominant kernel (transform + k-NN), algorithmic bytes of SURVEY.md section 8d over the
-             CUDA-event time of its launches, measured here with one alignment in flight; the
+             CUDA-event time of its launches, measured here with one alignment in flight, against the
+             H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s) unless MEASURED_PEAKS.json gives one; the
              16-in-flight regime of `value` is reported beside it (kernels of different alignments
              overlap, so the serial sum of one alignment's launches exceeds ms_per_step / batch).
 * cpu_baseline / --impl reference : the CPU oracle (a restatement of the reference's libnabo +
@@ -25,6 +26,9 @@ sm_align_pairs by --host-threads (2) host threads over --pipelines (16) matcher 
              and again with 6 threads (the reference's hard-coded NDT thread count, ndt.cc:32).
 * extra    : BASELINE.json configs[2] (Ndt) and configs[4] (NdtWithGicp loop-closure pairs, sharded
              over the ranks, pose all-gather) measured the same way, CPU oracle beside them at N=1.
+* --dump-outputs DIR : what the last step of the device-resident windows (`value`) returned to its callers
+             (poses, fitness scores, return codes of the batch, in pair order) as DIR/<name>.npy in float64.
+             The inputs are seeded, so two builds can be compared output for output.
 
 One process per GPU (torchrun for N > 1); every rank aligns its own pairs (weak scaling, no
 data-path collective) and the resulting poses are all-gathered over NCCL.
@@ -36,6 +40,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -51,10 +56,7 @@ N_SUBMAP = 500_000
 ITERATIONS = 30
 BYTES_PER_POINT_ITER = 64           # SURVEY.md 8d: whole iteration
 BYTES_KNN_PER_POINT = 40            # of which the k-NN kernel: 16 src + 16 matched + 8 write
-# dram__bytes_read + dram__bytes_write of ONE launch of icp_knn_kernel from the committed
-# `ncu --set full` capture (profiles/r02_ncu_full_icp_knn_final.txt; ncu flushes the caches
-# before the launch, so this is the cold figure; the steady state of an alignment is lower)
-NCU_TRAFFIC_BYTES = 6_438_400
+H100_HBM_GBS = 3350.0               # H100 SXM data sheet (HBM3); not a measured figure
 KNN_KERNEL = "icp_knn_kernel"
 METRIC = "scan-pair alignments/sec (120k->500k pts, 30 ICP iters)"
 UNIT = "alignments/s"
@@ -67,7 +69,7 @@ def log(*a):
 
 def make_workload(pair: int):
     """(source (Ns,3) f64, submap (500k,3) f64, perturbation) for pair index `pair`."""
-    cache = f"/tmp/sm_b200_bench_pair{pair}.npz"
+    cache = os.path.join(tempfile.gettempdir(), f"sm_b200_bench_pair{pair}.npz")
     if os.path.exists(cache):
         try:
             z = np.load(cache)
@@ -211,8 +213,19 @@ def run_reference(args, rank, world):
 
 
 # ------------------------------------------------------------------------------ clocks
+def gpu_identity(index: int, fallback_name: str):
+    """The card a number was measured on: name and power limit (nvidia-smi), read in the same run."""
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=60).stdout
+        name, limit = [x.strip() for x in out.strip().splitlines()[0].split(",")]
+        return {"name": name, "power_limit_w": float(limit)}
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        return {"name": fallback_name, "power_limit_w": None}
+
+
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -297,6 +310,8 @@ def main():
     ap.add_argument("--windows", type=int, default=3, help="timed windows of --steps steps; the median is reported")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the Ndt / NdtWithGicp records")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (poses, scores, return codes) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -371,7 +386,8 @@ def main():
         """`steps` batches of B alignments through sm_align_pairs: host thread j drives the pipelines
         j, j+T, ... with the pairs j, j+T, ... of the batch.  Device time of the whole region: an
         event before (every pipeline stream waits on it) and one after (it waits on every pipeline),
-        plus the all-gather of the last batch's poses."""
+        plus the all-gather of the last batch's poses.  Also returns what the last step gave its callers,
+        in pair order: (return codes (B,), poses (B, 4, 4), fitness scores (B,))."""
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         errors, last = [], [None] * T
         gate = threading.Barrier(T + 1)
@@ -383,8 +399,7 @@ def main():
             try:
                 gate.wait()
                 for _ in range(steps):
-                    rcs, res, sc = smb.AlignPairs(ms, mine)
-                    last[j] = (res, sc)
+                    last[j] = smb.AlignPairs(ms, mine)
             except Exception as e:  # noqa: BLE001
                 errors.append(e)
 
@@ -404,10 +419,10 @@ def main():
             ev = torch.cuda.Event(); ev.record(s); tstream.wait_event(ev)
         e1.record(tstream)
         e1.synchronize()
-        res = np.concatenate([x[0] for x in last if x is not None])
-        sc = np.concatenate([x[1] for x in last if x is not None])
+        inv = np.argsort(np.concatenate([np.arange(B)[j::T] for j in range(T)]))   # thread j ran pairs j, j+T, ...
+        rcs, res, sc = (np.concatenate([x[k] for x in last])[inv] for k in range(3))
         gather_poses(res, sc)                 # once per window, inside the reported time
-        return e0.elapsed_time(e1) + (gather_ms[-1] if world > 1 else 0.0), res
+        return e0.elapsed_time(e1) + (gather_ms[-1] if world > 1 else 0.0), (rcs, res, sc)
 
     # ---- warm-up (graphs captured, allocations done, all-gather warmed) -------------------------
     run_steps(args.warmup, False)
@@ -424,9 +439,13 @@ def main():
     win_dev = []
     for _ in range(args.windows):
         barrier()
-        ms, _ = run_steps(args.steps, False)
+        ms, last_step = run_steps(args.steps, False)
         barrier()
         win_dev.append(max_over_ranks(ms))
+    if args.dump_outputs and rank == 0:          # the headline path's last step
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in zip(("return_codes", "poses", "fitness_scores"), last_step):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr.astype(np.float64))
     # ---- timed: host buffers through the public API (H2D inside) ---------------------------
     win_e2e = []
     for _ in range(args.windows):
@@ -503,13 +522,13 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     achieved = BYTES_KNN_PER_POINT * N_SOURCE / (knn_ms * 1e-3) / 1e9
     iter_ms = (prof["knn"] + prof["accum"] + prof["finish"]) / prof["n"]
     per_gpu_rate = value / world
     roofline = {"bound": "hbm", "kernel": KNN_KERNEL, "achieved": achieved, "peak": peak,
-                "unit": "GB/s", "frac": achieved / peak, "traffic": NCU_TRAFFIC_BYTES,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                "unit": "GB/s", "frac": achieved / peak,
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet",
                 "avg_launch_ms": knn_ms, "bytes_per_launch": BYTES_KNN_PER_POINT * N_SOURCE,
                 "regime": "ONE alignment in flight: CUDA events around every launch of 3 extra profiled "
                           "alignments run right after the timed windows, same stream and inputs. The working set "
@@ -529,7 +548,7 @@ def main():
     cfg = workload_config(d0.nt, B)
     cfg.update({"pipelines_per_gpu": P, "host_threads": T, "windows": args.windows,
                 "entry_point": "sm_align_pairs (one call per host thread and step)",
-                "l2": f"{P} distinct pairs in flight per GPU (combined working set ~{25 * P} MB vs 126 MB L2), every "
+                "l2": f"{P} distinct pairs in flight per GPU (combined working set ~{25 * P} MB vs 50 MB L2), every "
                       "alignment re-uploads / re-reads its clouds and rebuilds its tree; the latency figures flush "
                       "L2 (256 MiB memset) before every alignment",
                 "timed_window_ms": {"device_resident": win_dev, "host_buffers": win_e2e}})
@@ -542,7 +561,8 @@ def main():
                 "d2h_bytes_per_step": (128 + 400) * B, "ms_per_step": ms_e2e_total / args.steps},
         "latency": {"ms_per_alignment_device": ms_lat_dev, "ms_per_alignment_host_buffers": ms_lat_host,
                     "in_flight": 1, "icp_iterations_per_s": ITERATIONS / (iter_ms * 1e-3)},
-        "gpu_launches": gpu_launches, "clocks": clocks, "roofline": roofline,
+        "gpu_launches": gpu_launches, "gpu": gpu_identity(local_rank, torch.cuda.get_device_name(dev)),
+        "clocks": clocks, "roofline": roofline,
         "allgather_ms": allgather_ms,
         "allgather_incl_rank_skew_ms": allgather_incl_wait_ms,   # as it happened inside the timed windows (waits for the slowest rank)
     }

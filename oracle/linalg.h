@@ -1,7 +1,7 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY. Never linked or imported by the product path.
 //
 // Small dense linear algebra (double) restating the Eigen routines the reference's
-// registrators/ hot path calls.  Eigen is NOT vendored in /root/reference and is not
+// registrators/ hot path calls.  Eigen is NOT vendored in the reference and is not
 // installed in this image, so these are restatements of Eigen 3.3's published
 // algorithms; the call sites that pin which routine is used are cited per function.
 // All matrices here are row-major C arrays m[r*n+c] unless stated otherwise.

@@ -1,6 +1,6 @@
 // Dependent-issue latencies on the box (cycles per operation in a serial chain, one warp):
 // DADD, DMUL, DFMA, double division, sqrt, rsqrt, SHFL, shared load, L1-hit global load.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o latency latency.cu ; run: ./latency
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o latency latency.cu ; run: ./latency
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """N single IcpFast alignments of the benchmark pair (one in flight, default options, host buffers):
-the workload the ncu captures under profiles/ are taken from.  argv[2] = knn_queries_per_cta (0: one query
+the launch sequence of bench.py's roofline measurement.  argv[2] = knn_queries_per_cta (0: one query
 per thread = icp_knn_kernel; 1024: the launch shape bench.py uses with many alignments in flight =
 icp_knn_batch_kernel)."""
 import os, sys

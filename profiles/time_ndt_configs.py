@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Timing of the NDT (config 3) and NdtWithGicp (config 5 per-pair) alignments at BASELINE sizes:
 120k-point scan -> 500k-point submap, one pair, device time via the engine's own events plus
-wall clock; the CPU oracle is timed beside it.  Prints one JSON object (kept in profiles/)."""
+wall clock; the CPU oracle is timed beside it.  Prints one JSON object."""
 import json
 import os
 import sys

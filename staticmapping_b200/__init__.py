@@ -1,5 +1,5 @@
-"""staticmapping_b200 — B200-native scan matching behind StaticMapping's
-registrator::Interface.  The compute lives in libsm_b200.so (hand-written sm_100a CUDA,
+"""staticmapping_b200 — H100-native scan matching behind StaticMapping's
+registrator::Interface.  The compute lives in libsm_b200.so (hand-written sm_90a CUDA,
 C ABI in include/sm_b200.h); this package is the thin host-side mirror used by the tests
 and the bench.  There is no CPU fallback."""
 from .registrators import (AlignBatch, AlignPairs, CalculateNormals, CheckFailure, CreateMatcher, EigenCloud, IcpFast, IcpUsingPointMatcher, InnerCloud,  # noqa: F401

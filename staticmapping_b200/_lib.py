@@ -98,7 +98,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a).  staticmapping_b200 has no CPU fallback.")
+                "g.build()'` (nvcc, sm_90a).  staticmapping_b200 has no CPU fallback.")
         _lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(_lib, name)

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libsm_b200 (sm_100a only).
+// Shared device/host helpers for libsm_b200 (sm_90a only).
 #ifndef SM_B200_COMMON_CUH_
 #define SM_B200_COMMON_CUH_
 
@@ -21,7 +21,7 @@ namespace smb {
 void set_cuda_error(cudaError_t e, const char* expr, const char* file, int line);
 const char* last_cuda_error();
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs; grids are sized in multiples
+constexpr int kNumSMs = 132;  // H100 SXM; grids are sized in multiples
 
 inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 

@@ -3,7 +3,7 @@
 // call site registrators/icp_fast.cc:466-467) and, with bucket 7, for the leaf
 // partition of EigenPointCloud::CalculateNormals (builder/data/cloud_types.cc:105-144).
 //
-// B200-first formulation instead of the reference's recursive std::nth_element:
+// GPU formulation instead of the reference's recursive std::nth_element:
 //   * the tree SHAPE depends only on (N, bucket): every node's [first, first+count) is
 //     pure integer arithmetic, so nodes live in an implicit heap layout (children of h
 //     are 2h+1 / 2h+2) and nothing about the shape is stored or communicated;

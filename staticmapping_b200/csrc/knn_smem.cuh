@@ -2,15 +2,14 @@
 // call site registrators/icp_fast.cc:177-178) over the compact tree layout (KdCompact), with
 // the node arrays resident in SHARED MEMORY.
 //
-// B200 formulation
+// H100 formulation
 //   * nodes are {cut f64}[h] + {dim u8}[h] in heap order.  Every CTA stages the TOP levels
 //     (kKnnSmemLevels = 11: 2047 nodes, 18 KB — the part of the tree every query walks) into
 //     shared memory with bulk async copies (cp.async.bulk.shared::cluster.global + mbarrier
 //     complete_tx; SASS UBLKCP / SYNCS) while its threads fetch and transform their queries;
 //     the deeper levels are read through the read-only path (L1).  Staging all 14 inner levels
-//     of a ~107 k-point target (144 KB, one 1024-thread CTA per SM) was measured too: the same
-//     57-60 us per launch, but 850 instead of ~1000 alignments/s with 16 alignments in flight,
-//     because one CTA per SM leaves no room for the kernels of other alignments;
+//     of a ~107 k-point target (144 KB) would fit the 227 KB a block may use, but leaves one
+//     CTA per SM and no room for the kernels of other alignments in flight;
 //   * leaves carry no payload: a leaf's bucket is (in-level index << (levels - level)) in the
 //     padded bucket array, one bucket = x[8] y[8] z[8] = 12 aligned 16-byte loads;
 //   * the heap index of a reached leaf encodes its whole path, so the far-side tests of a frame
@@ -33,9 +32,6 @@ namespace dev {
 #endif
 #ifndef SMB_KNN_SMEM_LEVELS
 #define SMB_KNN_SMEM_LEVELS 11
-#endif
-#ifndef SMB_KNN_LDG256
-#define SMB_KNN_LDG256 1
 #endif
 #ifndef SMB_KNN_HALF_SCAN
 #define SMB_KNN_HALF_SCAN 1
@@ -154,14 +150,14 @@ __device__ __forceinline__ void ldg_node(const double2* __restrict__ g_node, int
   dim = (int)__double_as_longlong(v.y);
 }
 
+// 32 bytes as two 16-byte loads (sm_90 has no 256-bit load), issued back to back
 struct Double4 { double a, b, c, d; };
-__device__ __forceinline__ Double4 ldg_nc_f64x4(const void* p) {      // LDG.E.256 (sm_100), 32-byte aligned
-  Double4 v;
-  asm volatile("ld.global.nc.v4.f64 {%0, %1, %2, %3}, [%4];" : "=d"(v.a), "=d"(v.b), "=d"(v.c), "=d"(v.d) : "l"(p));
-  return v;
+__device__ __forceinline__ Double4 ldg_nc_f64x4(const void* p) {
+  const double2 lo = ldg_nc_f64x2(p), hi = ldg_nc_f64x2(reinterpret_cast<const char*>(p) + 16);
+  return {lo.x, lo.y, hi.x, hi.y};
 }
 
-// One padded bucket: 6 32-byte loads, 8 squared distances in the reference's operation order, then
+// One padded bucket: 12 16-byte loads, 8 squared distances in the reference's operation order, then
 // a tournament on the bit patterns in which the lower index wins ties (libnabo walks the bucket in
 // order and replaces the head on a strict '<').  Padding entries are +inf: their distance is +inf
 // or NaN, never below the head.  SMB_KNN_HALF_SCAN: four points at a time (half the registers).
@@ -191,27 +187,14 @@ __device__ __forceinline__ void scan_bucket(const double* __restrict__ pb, int b
   }
 #else
   unsigned long long key[8];
-#if SMB_KNN_LDG256
-  Double4 v[6];
-#pragma unroll
-  for (int k = 0; k < 6; ++k) v[k] = ldg_nc_f64x4(base + 32 * k);
-#else
   double2 v[12];
 #pragma unroll
   for (int k = 0; k < 12; ++k) v[k] = ldg_nc_f64x2(base + 16 * k);
-#endif
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-#if SMB_KNN_LDG256
-    const Double4 &vx = v[k >> 2], &vy = v[2 + (k >> 2)], &vz = v[4 + (k >> 2)];
-    const double x = (k & 3) == 0 ? vx.a : (k & 3) == 1 ? vx.b : (k & 3) == 2 ? vx.c : vx.d;
-    const double y = (k & 3) == 0 ? vy.a : (k & 3) == 1 ? vy.b : (k & 3) == 2 ? vy.c : vy.d;
-    const double z = (k & 3) == 0 ? vz.a : (k & 3) == 1 ? vz.b : (k & 3) == 2 ? vz.c : vz.d;
-#else
     const double x = (k & 1) ? v[k >> 1].y : v[k >> 1].x;
     const double y = (k & 1) ? v[4 + (k >> 1)].y : v[4 + (k >> 1)].x;
     const double z = (k & 1) ? v[8 + (k >> 1)].y : v[8 + (k >> 1)].x;
-#endif
     key[k] = dist_key(qx, qy, qz, x, y, z);
   }
   int arg[8];

@@ -11,7 +11,7 @@
 //                              step) in double
 //   setInputCloud (:129-153)   A (64 x 512 counts), first singular vectors -> [u1; v1]
 //
-// B200 formulation: the work is N x 64 (point, view) bin updates — integer scatter, no
+// H100 formulation: the work is N x 64 (point, view) bin updates — integer scatter, no
 // contraction.  One CTA owns a chunk of points and a GROUP of 8 views whose 8 x 512 histogram
 // lives in shared memory (16 KB): the point is loaded and projected once per CTA-thread, the
 // eight views hit shared-memory atomics only (the reference's |.| folds everything into the first

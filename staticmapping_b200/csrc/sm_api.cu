@@ -943,7 +943,7 @@ int sm_device_count(void) {
   return n;
 }
 
-const char* sm_version(void) { return "sm_b200 0.1 (sm_100a)"; }
+const char* sm_version(void) { return "sm_b200 0.1 (sm_90a)"; }
 
 int sm_create(int type, int device, sm_handle** out) {
   if (!out) return SM_ERR_BAD_ARGUMENT;

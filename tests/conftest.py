@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     # a fresh checkout has no built artefacts (*.so is git-ignored): build the product library and
     # the oracle once, exactly like __graft_entry__.build() (nvcc cross-compiles without a GPU)
     lib = os.path.join(ROOT, "staticmapping_b200", "libsm_b200.so")
