@@ -17,6 +17,12 @@ namespace smb {
       return -100;                                                               \
     }                                                                            \
   } while (0)
+// propagate the negative return code of an internal call (SMB_CUDA_OK's -100 == SM_ERR_CUDA)
+#define SMB_RC(expr)                                                             \
+  do {                                                                           \
+    const int _rc = (expr);                                                      \
+    if (_rc < 0) return _rc;                                                     \
+  } while (0)
 
 void set_cuda_error(cudaError_t e, const char* expr, const char* file, int line);
 const char* last_cuda_error();

@@ -5,9 +5,31 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <utility>
+
 #include "common.cuh"
 
 namespace smb {
+
+// One device allocation, freed with its owner.  reserve() only grows, with 1/8 + 4 KB slack so
+// that clouds of slightly varying size keep their buffers: the IcpFast graph keys hash buffer
+// pointers, and a reallocation means a new capture.
+struct DevBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }   // move-only
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~DevBuf() { if (p) cudaFree(p); }
+  int reserve(size_t bytes) {
+    if (bytes <= cap) return 0;
+    if (p) { SMB_CUDA_OK(cudaFree(p)); p = nullptr; cap = 0; }
+    const size_t want = bytes + bytes / 8 + 4096;
+    SMB_CUDA_OK(cudaMalloc(&p, want));
+    cap = want;
+    return 0;
+  }
+};
 
 // ---- radix_sort.cu ---------------------------------------------------------------------
 size_t radix_sort_scratch_bytes(int n, int batch);

@@ -27,6 +27,7 @@
 
 #include "../../include/sm_b200.h"
 #include "common.cuh"
+#include "kernels.h"
 
 namespace smb {
 namespace {
@@ -201,11 +202,11 @@ extern "C" int sm_m2dp(int device, const float* points, int64_t n, int64_t strid
   SMB_CUDA_OK(cudaSetDevice(device));
   const int rows = p * q, l = (int)ceil(sqrt(max_distance / r)), cols = l * t;
   const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
-  char* base = nullptr;
   const size_t bytes = in_bytes + 256 + 16 * sizeof(double) + (size_t)rows * sizeof(M2dpView) + 256 +
                        (size_t)rows * cols * sizeof(int) + 256 + (size_t)rows * rows * sizeof(double) + 256;
-  SMB_CUDA_OK(cudaMalloc(&base, bytes));
-  char* cur = base;
+  DevBuf buf;
+  SMB_RC(buf.reserve(bytes));
+  char* cur = (char*)buf.p;
   auto take = [&](size_t b) { char* ptr = cur; cur += (b + 255) & ~(size_t)255; return ptr; };
   char* d_in = take(in_bytes);
   double* d_sums = (double*)take(16 * sizeof(double));
@@ -213,21 +214,19 @@ extern "C" int sm_m2dp(int device, const float* points, int64_t n, int64_t strid
   int* d_A = (int*)take((size_t)rows * cols * sizeof(int));
   double* d_G = (double*)take((size_t)rows * rows * sizeof(double));
   cudaStream_t s = nullptr;
-  auto fail = [&](int code) { cudaFree(base); return code; };
-#define M_CUDA(expr) do { if ((expr) != cudaSuccess) return fail(SM_ERR_CUDA); } while (0)
-  M_CUDA(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s));
-  M_CUDA(cudaMemsetAsync(d_sums, 0, 16 * sizeof(double), s));
-  M_CUDA(cudaMemsetAsync(d_A, 0, (size_t)rows * cols * sizeof(int), s));
+  SMB_CUDA_OK(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s));
+  SMB_CUDA_OK(cudaMemsetAsync(d_sums, 0, 16 * sizeof(double), s));
+  SMB_CUDA_OK(cudaMemsetAsync(d_A, 0, (size_t)rows * cols * sizeof(int), s));
   const int red_blocks = (int)std::min<int64_t>(4 * kNumSMs, (n + 255) / 256);
   m2dp_mean_kernel<<<red_blocks, 256, 0, s>>>(d_in, stride_bytes, n, d_sums);
   double h[16];
-  M_CUDA(cudaMemcpyAsync(h, d_sums, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  M_CUDA(cudaStreamSynchronize(s));
+  SMB_CUDA_OK(cudaMemcpyAsync(h, d_sums, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
   M2dpParams P;
   for (int d = 0; d < 3; ++d) P.mean[d] = (float)(h[d] / (double)n);
   m2dp_cov_kernel<<<red_blocks, 256, 0, s>>>(d_in, stride_bytes, n, P.mean[0], P.mean[1], P.mean[2], d_sums + 8);
-  M_CUDA(cudaMemcpyAsync(h, d_sums + 8, 6 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  M_CUDA(cudaStreamSynchronize(s));
+  SMB_CUDA_OK(cudaMemcpyAsync(h, d_sums + 8, 6 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
   {   // axes of the float covariance matrix, descending eigenvalue (pcl::PCA::initCompute)
     const double denom = (double)(float)(n - 1);
     const float c0 = (float)(h[0] / denom), c1 = (float)(h[1] / denom), c2 = (float)(h[2] / denom),
@@ -264,20 +263,18 @@ extern "C" int sm_m2dp(int device, const float* points, int64_t n, int64_t strid
         v.xa[0] = 1.f - sgl * mx; v.xa[1] = 0.f - sgl * my; v.xa[2] = 0.f - sgl * mz;
         v.ya[0] = my * v.xa[2] - mz * v.xa[1]; v.ya[1] = mz * v.xa[0] - mx * v.xa[2]; v.ya[2] = mx * v.xa[1] - my * v.xa[0];
       }
-    M_CUDA(cudaMemcpyAsync(d_views, hv.data(), (size_t)rows * sizeof(M2dpView), cudaMemcpyHostToDevice, s));
-    M_CUDA(cudaStreamSynchronize(s));          // hv goes out of scope
+    SMB_CUDA_OK(cudaMemcpyAsync(d_views, hv.data(), (size_t)rows * sizeof(M2dpView), cudaMemcpyHostToDevice, s));
+    SMB_CUDA_OK(cudaStreamSynchronize(s));          // hv goes out of scope
   }
   const dim3 grid((unsigned)((n + kPointsPerCta - 1) / kPointsPerCta), (unsigned)((rows + kViewsPerCta - 1) / kViewsPerCta));
   m2dp_hist_kernel<<<grid, kHistThreads, (size_t)kViewsPerCta * cols * sizeof(int), s>>>(d_in, stride_bytes, n, P, d_views, d_A);
   m2dp_gram_kernel<<<dim3((unsigned)rows, (unsigned)rows), 256, 0, s>>>(d_A, rows, cols, d_G);
-  M_CUDA(cudaGetLastError());
+  SMB_CUDA_OK(cudaGetLastError());
   std::vector<int> A((size_t)rows * cols);
   std::vector<double> G((size_t)rows * rows);
-  M_CUDA(cudaMemcpyAsync(A.data(), d_A, A.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  M_CUDA(cudaMemcpyAsync(G.data(), d_G, G.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-  M_CUDA(cudaStreamSynchronize(s));
-#undef M_CUDA
-  cudaFree(base);
+  SMB_CUDA_OK(cudaMemcpyAsync(A.data(), d_A, A.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(G.data(), d_G, G.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
   if (A_out) memcpy(A_out, A.data(), A.size() * sizeof(int));
   // first singular pair: u1 = dominant eigenvector of A A^T, sigma1^2 its eigenvalue, v1 = A^T u1 / sigma1
   std::vector<double> u;

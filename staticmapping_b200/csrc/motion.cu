@@ -16,6 +16,7 @@
 
 #include "../../include/sm_b200.h"
 #include "common.cuh"
+#include "kernels.h"
 
 namespace smb {
 namespace {
@@ -139,14 +140,12 @@ int sm_motion_compensation_device(int device, const float* dev_points, int64_t n
   SMB_CUDA_OK(cudaSetDevice(device));
   if (n == 0) return SM_OK;
   cudaStream_t s = (cudaStream_t)cuda_stream;
-  int* bad = nullptr;
-  SMB_CUDA_OK(cudaMalloc(&bad, sizeof(int)));
-  int rc = run((const char*)dev_points, (char*)dev_out, n, stride_bytes, delta_4x4, bad, s);
+  DevBuf bad;
+  SMB_RC(bad.reserve(sizeof(int)));
+  SMB_RC(run((const char*)dev_points, (char*)dev_out, n, stride_bytes, delta_4x4, (int*)bad.p, s));
   int host_bad = 0;
-  if (rc == 0 && cudaMemcpyAsync(&host_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess) rc = SM_ERR_CUDA;
-  if (rc == 0 && cudaStreamSynchronize(s) != cudaSuccess) rc = SM_ERR_CUDA;
-  cudaFree(bad);
-  if (rc) return rc;
+  SMB_CUDA_OK(cudaMemcpyAsync(&host_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
   return host_bad ? SM_ERR_BAD_ARGUMENT : SM_OK;
 }
 
@@ -173,16 +172,15 @@ int sm_motion_compensation(int device, const float* points, int64_t n, int64_t s
   SMB_CUDA_OK(cudaSetDevice(device));
   if (n == 0) return SM_OK;
   const size_t bytes = (size_t)n * (size_t)stride_bytes;
-  char *din = nullptr, *dout = nullptr;
-  if (cudaMalloc(&din, bytes) != cudaSuccess) return SM_ERR_CUDA;
-  if (cudaMalloc(&dout, bytes) != cudaSuccess) { cudaFree(din); return SM_ERR_CUDA; }
-  int rc = SM_OK;
-  if (cudaMemcpy(din, points, bytes, cudaMemcpyHostToDevice) != cudaSuccess) rc = SM_ERR_CUDA;
+  DevBuf din, dout;
+  SMB_RC(din.reserve(bytes));
+  SMB_RC(dout.reserve(bytes));
+  SMB_CUDA_OK(cudaMemcpy(din.p, points, bytes, cudaMemcpyHostToDevice));
   // bytes between the points (stride > 20) travel unchanged
-  if (rc == SM_OK && stride_bytes > 20 && cudaMemcpy(dout, din, bytes, cudaMemcpyDeviceToDevice) != cudaSuccess) rc = SM_ERR_CUDA;
-  if (rc == SM_OK) rc = sm_motion_compensation_device(device, (const float*)din, n, stride_bytes, delta_4x4, (float*)dout, nullptr);
-  if ((rc == SM_OK || rc == SM_ERR_BAD_ARGUMENT) && cudaMemcpy(out, dout, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) rc = SM_ERR_CUDA;
-  cudaFree(din); cudaFree(dout);
+  if (stride_bytes > 20) SMB_CUDA_OK(cudaMemcpy(dout.p, din.p, bytes, cudaMemcpyDeviceToDevice));
+  const int rc = sm_motion_compensation_device(device, (const float*)din.p, n, stride_bytes, delta_4x4, (float*)dout.p, nullptr);
+  if (rc != SM_OK && rc != SM_ERR_BAD_ARGUMENT) return rc;
+  SMB_CUDA_OK(cudaMemcpy(out, dout.p, bytes, cudaMemcpyDeviceToHost));   // also for a bad time factor
   return rc;
 }
 

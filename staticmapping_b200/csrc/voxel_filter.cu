@@ -180,9 +180,9 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   bytes += radix_sort_scratch_bytes(ni, 1) + 256;
   bytes += ((size_t)nblk + 8) * sizeof(uint32_t) + ((size_t)n + 8) * sizeof(uint32_t);   // block sums, voxel_start
   bytes += (size_t)n * sizeof(float4) + (size_t)n * 5 * sizeof(float) + 1024;
-  char* base = nullptr;
-  if (cudaMalloc(&base, bytes) != cudaSuccess) return SM_ERR_CUDA;
-  char* cur = base;
+  DevBuf buf;
+  SMB_RC(buf.reserve(bytes));
+  char* cur = (char*)buf.p;
   auto take = [&](size_t b) { char* p = cur; cur += (b + 255) & ~(size_t)255; return p; };
   char* d_in = take(in_bytes);
   uint64_t* keys0 = (uint64_t*)take(st * sizeof(uint64_t));
@@ -196,16 +196,12 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   float* d_out = (float*)take((size_t)n * 5 * sizeof(float));
   long long* meta = (long long*)take(256);
   cudaStream_t s = nullptr;
-  int rc = SM_OK;
-  auto fail = [&](int code) { cudaFree(base); return code; };
   const long long meta_init[8] = {LLONG_MAX, LLONG_MAX, LLONG_MAX, 0, 0, 0, 0, 0};
-  if (cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-      cudaMemcpyAsync(meta, meta_init, sizeof(meta_init), cudaMemcpyHostToDevice, s) != cudaSuccess)
-    return fail(SM_ERR_CUDA);
+  SMB_CUDA_OK(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(meta, meta_init, sizeof(meta_init), cudaMemcpyHostToDevice, s));
   vf_min_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ni, voxel_size, meta);
   vf_key_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ni, voxel_size, keys0, ord0, meta);
-  rc = radix_sort_pairs_u64(keys0, ord0, keys1, ord1, ni, 1, st, scratch, s, 8);   // 8 passes: result back in [0]
-  if (rc) return fail(rc == -100 ? SM_ERR_CUDA : rc);
+  SMB_RC(radix_sort_pairs_u64(keys0, ord0, keys1, ord1, ni, 1, st, scratch, s, 8));   // 8 passes: result back in [0]
   vf_heads_count_kernel<<<nblk, kT, 0, s>>>(keys0, ni, block_sum);
   cudaMemsetAsync(block_sum + nblk, 0, sizeof(uint32_t), s);
   radix_scan_kernel_launch(block_sum, nblk + 1, 1, s);                                // block_sum[nblk] = number of voxels
@@ -214,15 +210,12 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sorted, voxel_start, block_sum + nblk, d_out);
   uint32_t m = 0;
   long long host_meta[8] = {0};
-  if (cudaGetLastError() != cudaSuccess ||
-      cudaMemcpyAsync(&m, block_sum + nblk, sizeof(uint32_t), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-      cudaMemcpyAsync(host_meta, meta, sizeof(host_meta), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-      cudaStreamSynchronize(s) != cudaSuccess)
-    return fail(SM_ERR_CUDA);
-  if (host_meta[4]) return fail(SM_ERR_BAD_ARGUMENT);   // the finite points span 2^21 voxels or more along an axis
-  if (m > 0 && cudaMemcpy(out, d_out, (size_t)m * 5 * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)
-    return fail(SM_ERR_CUDA);
+  SMB_CUDA_OK(cudaGetLastError());
+  SMB_CUDA_OK(cudaMemcpyAsync(&m, block_sum + nblk, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(host_meta, meta, sizeof(host_meta), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  if (host_meta[4]) return SM_ERR_BAD_ARGUMENT;   // the finite points span 2^21 voxels or more along an axis
+  if (m > 0) SMB_CUDA_OK(cudaMemcpy(out, d_out, (size_t)m * 5 * sizeof(float), cudaMemcpyDeviceToHost));
   *m_out = (int64_t)m;
-  cudaFree(base);
   return SM_OK;
 }
