@@ -68,23 +68,6 @@ center_kernel(const double* __restrict__ raw, double* __restrict__ out, int64_t 
   }
 }
 
-__global__ void fill_buckets_kernel(const double* __restrict__ coord, int64_t cstride,
-                                    const double* __restrict__ nrm, int64_t nstride,
-                                    const uint32_t* __restrict__ leaf_order, int n,
-                                    BucketPoint* __restrict__ bpts, BucketNormal* __restrict__ bnrm) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= n) return;
-  const uint32_t id = leaf_order[s];
-  BucketPoint p;
-  p.x = coord[id]; p.y = coord[cstride + id]; p.z = coord[2 * cstride + id]; p.id = id;
-  bpts[s] = p;
-  if (nrm != nullptr) {
-    BucketNormal q;
-    q.x = nrm[id]; q.y = nrm[nstride + id]; q.z = nrm[2 * nstride + id]; q.pad = 0.0;
-    bnrm[s] = q;
-  }
-}
-
 // one block: G0 = T_mean^-1 * guess, state reset, histogram clear (icp_fast.cc:460-480)
 __global__ void icp_init_kernel(IcpState* __restrict__ st, const double* __restrict__ guess,
                                 uint32_t* __restrict__ hist) {
@@ -342,16 +325,6 @@ knn_query_batch_kernel(KdCompact kc, const double* __restrict__ query, int64_t q
 
 int icp_accum_blocks(int n_source) { return ceil_div(n_source, kAccTile); }
 
-
-int kd_fill_buckets(const double* coord, int64_t cstride, const double* nrm, int64_t nstride,
-                    const uint32_t* leaf_order, int n, BucketPoint* bpts, BucketNormal* bnrm,
-                    cudaStream_t stream) {
-  fill_buckets_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(coord, cstride, nrm, nstride,
-                                                            leaf_order, n, bpts, bnrm);
-  SMB_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
 // Launch geometry of the search kernels: `per_cta` consecutive queries per 256-thread CTA.
 // queries_per_cta == 0: one query per thread (120 000 queries = 469 CTAs, ~3 per SM, all
 // resident at once); a larger value makes a CTA loop over its range, which amortises the staging
@@ -385,27 +358,23 @@ int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq,
 
 // icp_fast.cc:456-480: centre the target, rebuild the tree, G0, initial source transform.
 int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_dev,
-                 KdWorkspace& ws, cudaStream_t stream) {
+                 KdWorkspace& ws, const KdCompactTree& tree, cudaStream_t stream) {
   const int nt = p.n_target, ns = p.n_source;
   const int nparts = ceil_div(nt, 1024);
   mean_partial_kernel<<<nparts, 256, 0, stream>>>(b.tgt_raw, b.tstride, nt, b.mean_partials);
   center_kernel<<<ceil_div(nt, 256), 256, 0, stream>>>(b.tgt_raw, b.tgt, b.tstride, nt,
                                                       b.mean_partials, nparts, b.state);
   nvtxRangePushA("BuildKdTree");                 // icp_fast.cc:465
-  int rc = kd_build(b.tgt, b.tstride, nt, 8, ws, b.nodes, b.leaf_order, stream, b.ccut, b.cdim, false, b.cnode);
-  if (rc) { nvtxRangePop(); return rc; }
-  rc = kd_compact_buckets(b.tgt, b.tstride, b.nrm, b.tstride, b.leaf_order, nt, 8, p.tree_levels, b.cpb, b.cpn,
-                          nullptr, stream);
+  int rc = tree.build(b.tgt, b.nrm, b.tstride, nt, 8, ws, stream);
   nvtxRangePop();
   if (rc) return rc;
+  const RadixPairs& sp = b.src_sort;
   icp_init_kernel<<<1, 256, 0, stream>>>(b.state, guess_dev, b.hist);
   apply_g0_kernel<<<ceil_div(ns, 256), 256, 0, stream>>>(b.src_raw, b.src_g0, b.sstride, ns, b.state,
-                                                        b.src_keys[0], b.src_vals[0]);
-  rc = radix_sort_pairs_u64(b.src_keys[0], b.src_vals[0], b.src_keys[1], b.src_vals[1], ns, 1,
-                            b.sstride, b.src_scratch, stream, 4);
+                                                        sp.keys[0], sp.vals[0]);
+  rc = radix_sort_pairs_u64(sp.keys[0], sp.vals[0], sp.keys[1], sp.vals[1], ns, 1, b.sstride, sp.scratch, stream, 4);
   if (rc) return rc;
-  gather_source_kernel<<<ceil_div(ns, 256), 256, 0, stream>>>(b.src_g0, b.src0, b.sstride, ns,
-                                                             b.src_vals[0]);
+  gather_source_kernel<<<ceil_div(ns, 256), 256, 0, stream>>>(b.src_g0, b.src0, b.sstride, ns, sp.vals[0]);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }

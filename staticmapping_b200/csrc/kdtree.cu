@@ -452,6 +452,17 @@ __global__ void kd_compact_buckets_kernel(const double* __restrict__ coord, int6
   if (pid) pid[e] = id;
 }
 
+// bucket slot s of the blocked tree (FloatTree): the point of leaf_order[s]
+__global__ void fill_buckets_kernel(const double* __restrict__ coord, int64_t cstride,
+                                    const uint32_t* __restrict__ leaf_order, int n, BucketPoint* __restrict__ bpts) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n) return;
+  const uint32_t id = leaf_order[s];
+  BucketPoint p;
+  p.x = coord[id]; p.y = coord[cstride + id]; p.z = coord[2 * cstride + id]; p.id = id;
+  bpts[s] = p;
+}
+
 // keys32: the coordinates are exactly representable as float (clouds that entered as float): the float
 // bit pattern orders them like the double one and the sort needs 4 byte passes instead of 8
 __global__ void kd_keys_kernel(const double* __restrict__ coord, int64_t cstride, int n,
@@ -485,7 +496,7 @@ int kd_num_levels(int n, int bucket) {
   return L;  // all nodes of level L are leaves; heap has 2^(L+1)-1 slots
 }
 
-size_t KdWorkspace::bytes_needed(int n, int bucket) {
+static size_t kd_workspace_bytes(int n, int bucket) {
   const int levels = kd_num_levels(n, bucket);
   const int64_t ls = (n + 63) & ~63;
   size_t b = 0;
@@ -499,10 +510,11 @@ size_t KdWorkspace::bytes_needed(int n, int bucket) {
   return b + 4096;
 }
 
-void KdWorkspace::carve(void* base, int n, int bucket) {
+int KdWorkspace::carve(DevBuf& buf, int n, int bucket) {
+  SMB_RC(buf.reserve(kd_workspace_bytes(n, bucket)));
   const int levels = kd_num_levels(n, bucket);
   lstride = (n + 63) & ~63;
-  char* p = (char*)base;
+  char* p = (char*)buf.p;
   auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) & ~(size_t)255; return r; };
   keys[0] = (uint64_t*)take(3 * lstride * sizeof(uint64_t));
   keys[1] = (uint64_t*)take(3 * lstride * sizeof(uint64_t));
@@ -514,14 +526,30 @@ void KdWorkspace::carve(void* base, int n, int bucket) {
   bounds[0] = (double*)take(((size_t)1 << levels) * 6 * sizeof(double));
   bounds[1] = (double*)take(((size_t)1 << levels) * 6 * sizeof(double));
   level_dim = (int*)take(((size_t)1 << levels) * sizeof(int));
+  return 0;
+}
+
+// entries of the compact layout's cut[] / dim[]: 2^levels - 1 inner-capable nodes, rounded up to a multiple of
+// 16 because bulk copies move multiples of 16 bytes
+static size_t kd_compact_node_slots(int levels) {
+  const size_t n = (size_t)1 << levels;
+  return n < 16 ? 16 : n;
+}
+
+// node[] of the compact layout, behind cut[] in the same allocation
+static double2* compact_node_array(const KdCompactTree& t) {
+  return reinterpret_cast<double2*>((double*)t.cut.p + kd_compact_node_slots(t.levels));
 }
 
 // coord: SoA [3][cstride] doubles (already centred).  Writes nodes (heap layout,
 // 2^(levels+1)-1 entries) and leaf_order[n] (point ids in bucket order).
 int kd_build(const double* coord, int64_t cstride, int n, int bucket, KdWorkspace& ws,
-             KdNode* nodes, uint32_t* leaf_order, cudaStream_t stream, double* ccut, uint8_t* cdim,
-             bool coords_are_float, double2* cnode) {
+             KdNode* nodes, uint32_t* leaf_order, cudaStream_t stream, const KdCompactTree* compact,
+             bool coords_are_float) {
   if (n <= 0) return -1;
+  double* ccut = compact ? (double*)compact->cut.p : nullptr;
+  uint8_t* cdim = compact ? (uint8_t*)compact->dim.p : nullptr;
+  double2* cnode = compact ? compact_node_array(*compact) : nullptr;
   const int levels = kd_num_levels(n, bucket);
   const int64_t ls = ws.lstride;
   kd_keys_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(coord, cstride, n, ws.keys[0],
@@ -567,18 +595,48 @@ int kd_build(const double* coord, int64_t cstride, int n, int bucket, KdWorkspac
   return 0;
 }
 
-size_t kd_compact_node_slots(int levels) {
-  const size_t n = (size_t)1 << levels;      // 2^levels - 1 inner-capable nodes, rounded up
-  return n < 16 ? 16 : n;                    // bulk copies move multiples of 16 bytes
+int KdCompactTree::reserve(int n, int bucket, Payload payload) {
+  levels = kd_num_levels(n, bucket);
+  const size_t slots = kd_compact_node_slots(levels), entries = (size_t)8 << levels;
+  SMB_RC(nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
+  SMB_RC(leaf_order.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(cut.reserve(slots * (sizeof(double) + sizeof(double2))));
+  SMB_RC(dim.reserve(slots));
+  SMB_RC(pb.reserve(entries * 3 * sizeof(double)));
+  return payload == kNormals ? pn.reserve(entries * sizeof(BucketNormal)) : pid.reserve(entries * sizeof(int32_t));
 }
 
-int kd_compact_buckets(const double* coord, int64_t cstride, const double* nrm, int64_t nstride,
-                       const uint32_t* leaf_order, int n, int bucket, int levels, double* pb,
-                       BucketNormal* pn, int32_t* pid, cudaStream_t stream) {
+int KdCompactTree::build(const double* coord, const double* nrm, int64_t cstride, int n, int bucket,
+                         KdWorkspace& ws, cudaStream_t stream) const {
   if (bucket > 8) return -1;
+  SMB_RC(kd_build(coord, cstride, n, bucket, ws, (KdNode*)nodes.p, (uint32_t*)leaf_order.p, stream, this));
   const int64_t total = (int64_t)8 << levels;
-  kd_compact_buckets_kernel<<<ceil_div(total, 256), 256, 0, stream>>>(coord, cstride, nrm, nstride, leaf_order, n,
-                                                                     bucket, levels, pb, pn, pid);
+  kd_compact_buckets_kernel<<<ceil_div(total, 256), 256, 0, stream>>>(
+      coord, cstride, nrm, cstride, (const uint32_t*)leaf_order.p, n, bucket, levels, (double*)pb.p,
+      (BucketNormal*)pn.p, (int32_t*)pid.p);
+  SMB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+KdCompact KdCompactTree::view() const {
+  return {(const double*)cut.p, (const uint8_t*)dim.p, compact_node_array(*this), (const double*)pb.p,
+          (const BucketNormal*)pn.p, (const int32_t*)pid.p, levels, 0};
+}
+
+int FloatTree::build(const float* pts, int n, DevBuf& kdws, cudaStream_t stream) {
+  const int levels = kd_num_levels(n, 8);
+  const int64_t stride = ((int64_t)n + 63) & ~(int64_t)63;
+  SMB_RC(soa.reserve((size_t)(3 * stride) * sizeof(double)));
+  SMB_RC(nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
+  SMB_RC(order.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(bpts.reserve((size_t)(n + 8) * sizeof(BucketPoint)));
+  KdWorkspace ws;
+  SMB_RC(ws.carve(kdws, n, 8));
+  SMB_RC(ndt_float_to_soa(pts, n, (double*)soa.p, stride, stream));
+  SMB_RC(kd_build((const double*)soa.p, stride, n, 8, ws, (KdNode*)nodes.p, (uint32_t*)order.p, stream, nullptr,
+                  true));       // the cloud entered as float: 32-bit sort keys
+  fill_buckets_kernel<<<ceil_div(n, 256), 256, 0, stream>>>((const double*)soa.p, stride, (const uint32_t*)order.p, n,
+                                                            (BucketPoint*)bpts.p);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }

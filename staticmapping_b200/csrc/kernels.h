@@ -33,6 +33,15 @@ struct DevBuf {
 
 // ---- radix_sort.cu ---------------------------------------------------------------------
 size_t radix_sort_scratch_bytes(int n, int batch);
+// One sort of up to `stride` (key, value) pairs: the ping-pong buffers and the scratch, carved from one
+// allocation of bytes(stride, n) bytes.
+struct RadixPairs {
+  uint64_t* keys[2];
+  uint32_t* vals[2];
+  uint32_t* scratch;
+  static size_t bytes(int64_t stride, int n);
+  void carve(void* base, int64_t stride);
+};
 int radix_sort_pairs_u64(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b, uint32_t* vals_b,
                          int n, int batch, int64_t stride, uint32_t* scratch,
                          cudaStream_t stream, int passes = 8);
@@ -50,16 +59,9 @@ struct KdWorkspace {
   double* bounds[2];
   int* level_dim;
   int64_t lstride;
-  static size_t bytes_needed(int n, int bucket);
-  void carve(void* base, int n, int bucket);
+  int carve(DevBuf& buf, int n, int bucket);   // grows buf to what (n, bucket) needs, then carves it
 };
-// ccut / cdim (optional): the compact search layout's node arrays, see KdCompact
-// coords_are_float: every coordinate is exactly a float (clouds uploaded as float): 32-bit sort keys
-int kd_build(const double* coord, int64_t cstride, int n, int bucket, KdWorkspace& ws,
-             KdNode* nodes, uint32_t* leaf_order, cudaStream_t stream, double* ccut = nullptr,
-             uint8_t* cdim = nullptr, bool coords_are_float = false, double2* cnode = nullptr);
-
-// Compact search layout of the same tree, shaped for a shared-memory resident traversal:
+// Compact search layout of a tree built by kd_build, shaped for a shared-memory resident traversal:
 //   cut[h], dim[h]  heap order (children of h: 2h+1, 2h+2) for the levels above the deepest
 //                   leaf level; dim 3 = leaf.  8 + 1 bytes per node: the 14 inner levels of a
 //                   ~107 k-point target are 144 KB and are staged into shared memory with bulk
@@ -77,12 +79,33 @@ struct KdCompact {
   const BucketNormal* pn;
   const int32_t* pid;
   int levels;
+  int pad;                // set too: IcpBuffers embeds this struct, and its bytes are a graph key
 };
-size_t kd_compact_node_slots(int levels);     // entries of cut[] / dim[] (multiple of 16)
-inline size_t kd_compact_bucket_entries(int levels) { return (size_t)8 << levels; }
-int kd_compact_buckets(const double* coord, int64_t cstride, const double* nrm, int64_t nstride,
-                       const uint32_t* leaf_order, int n, int bucket, int levels, double* pb,
-                       BucketNormal* pn, int32_t* pid, cudaStream_t stream);
+// The device buffers of one tree in the compact layout, with its blocked node array and leaf order.  reserve()
+// sizes them for (n, bucket) with one payload per padded entry, the normals (pn) or the original ids (pid);
+// they only grow, so a tree of the same size keeps its pointers.  build() fills them.
+struct KdCompactTree {
+  enum Payload { kNormals, kIds };
+  DevBuf nodes, leaf_order, cut, dim, pb, pn, pid;   // cut: cut[] then node[]
+  int levels = 0;
+  int reserve(int n, int bucket, Payload payload);
+  // coord / nrm: SoA [3][cstride]; nrm only with the kNormals payload
+  int build(const double* coord, const double* nrm, int64_t cstride, int n, int bucket, KdWorkspace& ws,
+            cudaStream_t stream) const;
+  KdCompact view() const;
+};
+// compact (optional): also write its node arrays
+// coords_are_float: every coordinate is exactly a float (clouds uploaded as float): 32-bit sort keys
+int kd_build(const double* coord, int64_t cstride, int n, int bucket, KdWorkspace& ws, KdNode* nodes,
+             uint32_t* leaf_order, cudaStream_t stream, const KdCompactTree* compact = nullptr,
+             bool coords_are_float = false);
+
+// k-d tree over a packed float cloud (fitness scores, GICP correspondences, the type-1 score): the cloud as
+// SoA doubles, the blocked node array, the leaf order and the buckets; kdws is the build workspace.
+struct FloatTree {
+  DevBuf soa, nodes, order, bpts;
+  int build(const float* pts, int n, DevBuf& kdws, cudaStream_t stream);
+};
 
 // ---- icp.cu ----------------------------------------------------------------------------
 constexpr int kKnnItemSlack = 4096;   // a warp's item list may extend past the last query of the last batch
@@ -129,19 +152,12 @@ struct IcpBuffers {
   // tree: build-time node array (blocked layout), leaf order, and the compact search layout
   KdNode* nodes;
   uint32_t* leaf_order;
-  double* ccut;           // writable views of kc.cut / kc.dim / kc.pb / kc.pn (filled by the prologue)
-  uint8_t* cdim;
-  double2* cnode;
-  double* cpb;
-  BucketNormal* cpn;
   KdCompact kc;
   // source
   double* src_raw;        // [3][sstride] as uploaded
   double* src_g0;         // [3][sstride] after G0, caller order
   double* src0;           // [3][sstride] after G0, Morton order (what the iterations read)
-  uint64_t* src_keys[2];  // Morton keys (ping-pong)
-  uint32_t* src_vals[2];  // permutation (ping-pong)
-  uint32_t* src_scratch;  // radix scratch
+  RadixPairs src_sort;    // Morton keys and the permutation
   int64_t sstride;
   // per-iteration
   int32_t* slot;          // [n_source] padded bucket entry of the match (kc.pb / kc.pn index)
@@ -160,8 +176,9 @@ struct IcpBuffers {
 };
 
 int icp_accum_blocks(int n_source);
+// builds the target tree into `tree`, whose view is b.kc
 int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_dev,
-                 KdWorkspace& ws, cudaStream_t stream);
+                 KdWorkspace& ws, const KdCompactTree& tree, cudaStream_t stream);
 // events (optional): 4 per iteration — before A, after A, after B, after C
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
                            cudaStream_t stream, cudaEvent_t* events);
@@ -169,9 +186,6 @@ void icp_finish_launch(const IcpBuffers& b, const IcpParams& p, int nblocks_b, c
 // stand-alone k-NN over an already built tree (compact layout incl. pid): ids = original indices
 int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, double max_error2,
               int32_t* ids, double* d2, cudaStream_t stream, int queries_per_cta = 0, int4* items = nullptr);
-int kd_fill_buckets(const double* coord, int64_t cstride, const double* nrm, int64_t nstride,
-                    const uint32_t* leaf_order, int n, BucketPoint* bpts, BucketNormal* bnrm,
-                    cudaStream_t stream);
 
 // ---- ndt.cu ------------------------------------------------------------------------------
 struct NdtGrid {            // VoxelGridCovariance bookkeeping (_impl.hpp:88-103)
@@ -270,11 +284,18 @@ int gicp_cost(const float* src, int ns, const float* tgt, const GicpCostParams& 
               long long* host_flag_dev, long long seq, cudaStream_t stream);
 
 // ---- normals.cu ------------------------------------------------------------------------
-int normals_scratch_blocks(int n);
-int normals_run(const double* coord, int64_t cstride, int n, KdWorkspace& ws, KdNode* nodes,
-                uint32_t* leaf_order, double* tmp_pts, double* tmp_nrm, uint32_t* keep,
-                uint32_t* block_sums, double* out_pts, double* out_nrm, uint32_t* m_dev,
-                cudaStream_t stream);
+// The device buffers of CalculateNormals over n points, sized by reserve(n): the input cloud, the bucket-7 tree
+// with its workspace, the per-leaf scratch, and the AoS 3xM outputs with their count M.
+struct NormalsPipeline {
+  DevBuf coord, nodes, order, kdws, tmp_pts, tmp_nrm, keep, bsum, out_pts, out_nrm, count;
+  int64_t stride = 0;
+  int reserve(int n);
+  double* input() const { return (double*)coord.p; }   // SoA [3][stride], filled by the caller
+  // runs the pipeline on the first n points of input() and waits for M
+  int run(int n, cudaStream_t stream, uint32_t* m);
+  const double* points() const { return (const double*)out_pts.p; }
+  const double* normals() const { return (const double*)out_nrm.p; }
+};
 
 }  // namespace smb
 

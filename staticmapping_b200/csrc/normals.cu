@@ -142,28 +142,41 @@ int normals_debug_leaf_host(const double* members, int count, double* mean, doub
   return leaf_plane_fit(d, count, mean, unit) ? 1 : 0;
 }
 
-// coord: SoA [3][cstride] (un-centred input).  Outputs are AoS 3xM (Eigen layout) in
-// device memory; *m_dev receives M.  tmp_pts/tmp_nrm: AoS 3xN scratch; keep: N u32.
-int normals_run(const double* coord, int64_t cstride, int n, KdWorkspace& ws, KdNode* nodes,
-                uint32_t* leaf_order, double* tmp_pts, double* tmp_nrm, uint32_t* keep,
-                uint32_t* block_sums, double* out_pts, double* out_nrm, uint32_t* m_dev,
-                cudaStream_t stream) {
+int NormalsPipeline::reserve(int n) {
   const int levels = kd_num_levels(n, 7);
-  int rc = kd_build(coord, cstride, n, 7, ws, nodes, leaf_order, stream);
-  if (rc) return rc;
-  SMB_CUDA_OK(cudaMemsetAsync(keep, 0, (size_t)n * sizeof(uint32_t), stream));
-  const int total = (1 << (levels + 1)) - 1;
-  normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(coord, cstride, nodes, leaf_order, n,
-                                                               levels, tmp_pts, tmp_nrm, keep);
-  const int nblk = ceil_div(n, kCTile);
-  compact_count_kernel<<<nblk, kCT, 0, stream>>>(keep, n, block_sums);
-  radix_scan_kernel_launch(block_sums, nblk, 1, stream);
-  compact_scatter_kernel<<<nblk, kCT, 0, stream>>>(keep, n, block_sums, tmp_pts, tmp_nrm, out_pts,
-                                                   out_nrm, m_dev, nblk);
-  SMB_CUDA_OK(cudaGetLastError());
-  return 0;
+  const size_t aos = (size_t)3 * (size_t)n * sizeof(double);
+  stride = ((int64_t)n + 63) & ~(int64_t)63;
+  SMB_RC(coord.reserve((size_t)3 * stride * sizeof(double)));
+  SMB_RC(nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
+  SMB_RC(order.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(tmp_pts.reserve(aos)); SMB_RC(tmp_nrm.reserve(aos));
+  SMB_RC(keep.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(bsum.reserve((size_t)(ceil_div(n, kCTile) + 1) * sizeof(uint32_t)));
+  SMB_RC(out_pts.reserve(aos)); SMB_RC(out_nrm.reserve(aos));
+  return count.reserve(sizeof(uint32_t));
 }
 
-int normals_scratch_blocks(int n) { return ceil_div(n, kCTile); }
+int NormalsPipeline::run(int n, cudaStream_t stream, uint32_t* m) {
+  const int levels = kd_num_levels(n, 7);
+  uint32_t* block_sums = (uint32_t*)bsum.p;
+  KdWorkspace ws;
+  SMB_RC(ws.carve(kdws, n, 7));
+  SMB_RC(kd_build(input(), stride, n, 7, ws, (KdNode*)nodes.p, (uint32_t*)order.p, stream));
+  SMB_CUDA_OK(cudaMemsetAsync(keep.p, 0, (size_t)n * sizeof(uint32_t), stream));
+  const int total = (1 << (levels + 1)) - 1;
+  normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(input(), stride, (const KdNode*)nodes.p,
+                                                               (const uint32_t*)order.p, n, levels, (double*)tmp_pts.p,
+                                                               (double*)tmp_nrm.p, (uint32_t*)keep.p);
+  const int nblk = ceil_div(n, kCTile);
+  compact_count_kernel<<<nblk, kCT, 0, stream>>>((const uint32_t*)keep.p, n, block_sums);
+  radix_scan_kernel_launch(block_sums, nblk, 1, stream);
+  compact_scatter_kernel<<<nblk, kCT, 0, stream>>>((const uint32_t*)keep.p, n, block_sums, (const double*)tmp_pts.p,
+                                                   (const double*)tmp_nrm.p, (double*)out_pts.p, (double*)out_nrm.p,
+                                                   (uint32_t*)count.p, nblk);
+  SMB_CUDA_OK(cudaGetLastError());
+  SMB_CUDA_OK(cudaMemcpyAsync(m, count.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+  SMB_CUDA_OK(cudaStreamSynchronize(stream));
+  return 0;
+}
 
 }  // namespace smb

@@ -218,6 +218,18 @@ size_t radix_sort_scratch_bytes(int n, int batch) {
   return ((size_t)batch * count + (size_t)batch * ((count + kScanChunk - 1) / kScanChunk) + 8) * sizeof(uint32_t);
 }
 
+size_t RadixPairs::bytes(int64_t stride, int n) {
+  return (size_t)stride * (2 * sizeof(uint64_t) + 2 * sizeof(uint32_t)) + radix_sort_scratch_bytes(n, 1);
+}
+
+void RadixPairs::carve(void* base, int64_t stride) {
+  keys[0] = (uint64_t*)base;
+  keys[1] = keys[0] + stride;
+  vals[0] = (uint32_t*)(keys[1] + stride);
+  vals[1] = vals[0] + stride;
+  scratch = vals[1] + stride;
+}
+
 // Sorts keys_a/vals_a (layout [batch][stride]); keys_b/vals_b are ping-pong buffers.
 // `passes` 8-bit digits are sorted starting from bit 0 (8 = full 64-bit keys); for an even
 // number of passes the sorted data ends in the *_a buffers, otherwise in *_b.

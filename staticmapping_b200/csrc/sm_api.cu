@@ -200,10 +200,6 @@ struct GraphCache {
   void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; key.clear(); }
 };
 
-// k-d tree over a packed float cloud, built by build_tree_f32: the cloud as SoA doubles, the
-// blocked node array, the leaf order and the buckets
-struct FloatTree { DevBuf soa, nodes, order, bpts; };
-
 }  // namespace
 }  // namespace smb
 
@@ -234,9 +230,9 @@ struct sm_handle {
 
   // IcpFast, and the ICP chain of type 1: SoA double clouds, the tree, the iteration buffers
   struct {
-    DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, tgt, nrm, src_raw, src0, src_g0, src_sort, nodes,
-        leaf_order, ccut, cdim, cpb, cpn, slot, d2, hist, cand_terms, cand_key, cand_cnt, partials, mean_partials,
-        state, guess;
+    DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, tgt, nrm, src_raw, src0, src_g0, src_sort, slot, d2,
+        hist, cand_terms, cand_key, cand_cnt, partials, mean_partials, state, guess;
+    KdCompactTree tree;
     int64_t sstride = 0, tstride = 0;
     bool up_src = false, up_tgt = false;
     IcpState* host_state = nullptr;  // pinned
@@ -263,11 +259,13 @@ struct sm_handle {
     long long seq = 0;
   } ndt_gicp;
 
-  // IcpUsingPointMatcher stand-in (type 1): raw float clouds -> filtered double clouds
+  // IcpUsingPointMatcher stand-in (type 1): raw float clouds -> filtered double clouds.  The normals
+  // pipeline has its own k-d workspace: h->kdws.p is part of the IcpFast graph keys.
   struct {
     int64_t n_src = 0, n_tgt = 0;
     bool src_dirty = false, tgt_dirty = false, score_tree_dirty = true;
-    DevBuf coord, nodes, order, kdws, tmp_pts, tmp_nrm, keep, bsum, outp, outn, cnt, src, score_buf;
+    NormalsPipeline normals;
+    DevBuf cnt, src, score_buf;       // sampling counts, the sampled source, the score's sort and I/O
   } pm;
 
   ~sm_handle() {
@@ -427,7 +425,11 @@ int set_target(sm_handle* h, const double* pts, const double* nrm, int64_t n, bo
 int ndt_align(sm_handle* h, const double* guess, double* result);
 int ndt_gicp_align(sm_handle* h, const double* guess, double* result);
 int pm_align(sm_handle* h, const double* guess, double* result);
-int build_tree_f32(sm_handle* h, const float* pts, int n, FloatTree& tree);
+int build_tree_f32(sm_handle* h, const float* pts, int n, FloatTree& t) {
+  if (kd_num_levels(n, 8) > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "cloud too large");
+  H_RC(t.build(pts, n, h->kdws, h->stream));
+  return 0;
+}
 
 // one chunk of iterations + the asynchronous read-back of the state record
 int icp_enqueue_chunk(sm_handle* h) {
@@ -478,13 +480,8 @@ int icp_begin(sm_handle* h, const double* guess) {
   H_RC(f.tgt.reserve((size_t)(3 * f.tstride) * sizeof(double)));
   H_RC(f.src0.reserve((size_t)(3 * f.sstride) * sizeof(double)));
   H_RC(f.src_g0.reserve((size_t)(3 * f.sstride) * sizeof(double)));
-  H_RC(f.src_sort.reserve((size_t)f.sstride * 24 + radix_sort_scratch_bytes(ns, 1) + 1024));
-  H_RC(f.nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
-  H_RC(f.leaf_order.reserve((size_t)nt * sizeof(uint32_t)));
-  H_RC(f.ccut.reserve(kd_compact_node_slots(levels) * (sizeof(double) + sizeof(double2))));   // cut[] then node[]
-  H_RC(f.cdim.reserve(kd_compact_node_slots(levels)));
-  H_RC(f.cpb.reserve(kd_compact_bucket_entries(levels) * 3 * sizeof(double)));
-  H_RC(f.cpn.reserve(kd_compact_bucket_entries(levels) * sizeof(BucketNormal)));
+  H_RC(f.src_sort.reserve(RadixPairs::bytes(f.sstride, ns)));
+  H_RC(f.tree.reserve(nt, 8, KdCompactTree::kNormals));
   const size_t slot_bytes = (((size_t)ns * sizeof(int32_t) + 64 + 255) / 256) * 256;
   H_RC(f.slot.reserve(slot_bytes + ((size_t)ns + kKnnItemSlack) * sizeof(int4)));
   H_RC(f.d2.reserve((size_t)ns * sizeof(double)));
@@ -496,23 +493,17 @@ int icp_begin(sm_handle* h, const double* guess) {
   H_RC(f.mean_partials.reserve((size_t)ceil_div(nt, 1024) * 4 * sizeof(double)));
   H_RC(f.state.reserve(sizeof(IcpState)));
   H_RC(f.guess.reserve(16 * sizeof(double)));
-  H_RC(h->kdws.reserve(KdWorkspace::bytes_needed(nt, 8)));
   KdWorkspace& ws = r.ws;
-  ws.carve(h->kdws.p, nt, 8);
+  H_RC(ws.carve(h->kdws, nt, 8));
 
   IcpBuffers& b = r.b;
   b.tgt = (double*)f.tgt.p; b.tgt_raw = (double*)f.tgt_raw.p; b.nrm = (double*)f.nrm.p;
   b.tstride = f.tstride;
-  b.nodes = (KdNode*)f.nodes.p; b.leaf_order = (uint32_t*)f.leaf_order.p;
-  b.ccut = (double*)f.ccut.p; b.cdim = (uint8_t*)f.cdim.p;
-  b.cnode = reinterpret_cast<double2*>(b.ccut + kd_compact_node_slots(levels));
-  b.cpb = (double*)f.cpb.p; b.cpn = (BucketNormal*)f.cpn.p;
-  b.kc.cut = b.ccut; b.kc.dim = b.cdim; b.kc.node = b.cnode; b.kc.pb = b.cpb; b.kc.pn = b.cpn; b.kc.pid = nullptr; b.kc.levels = levels;
+  b.nodes = (KdNode*)f.tree.nodes.p; b.leaf_order = (uint32_t*)f.tree.leaf_order.p;
+  b.kc = f.tree.view();
   b.src_raw = (double*)f.src_raw.p; b.src0 = (double*)f.src0.p; b.sstride = f.sstride;
   b.src_g0 = (double*)f.src_g0.p;
-  b.src_keys[0] = (uint64_t*)f.src_sort.p; b.src_keys[1] = b.src_keys[0] + f.sstride;
-  b.src_vals[0] = (uint32_t*)(b.src_keys[1] + f.sstride); b.src_vals[1] = b.src_vals[0] + f.sstride;
-  b.src_scratch = b.src_vals[1] + f.sstride;
+  b.src_sort.carve(f.src_sort.p, f.sstride);
   b.slot = (int32_t*)f.slot.p;
   b.knn_items = reinterpret_cast<int4*>((char*)f.slot.p + slot_bytes);
   b.d2 = (double*)f.d2.p; b.hist = (uint32_t*)f.hist.p;
@@ -541,10 +532,10 @@ int icp_begin(sm_handle* h, const double* guess) {
   key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.guess.p); key_append(r.key, h->kdws.p);
   if (r.graphs) {
     H_RC(run_graphed(h, f.g_prologue, r.key, [&]() {
-      return icp_prologue(b, p, (const double*)f.guess.p, ws, h->stream);
+      return icp_prologue(b, p, (const double*)f.guess.p, ws, f.tree, h->stream);
     }));
   } else {
-    H_RC(icp_prologue(b, p, (const double*)f.guess.p, ws, h->stream));
+    H_RC(icp_prologue(b, p, (const double*)f.guess.p, ws, f.tree, h->stream));
   }
   H_CUDA(cudaEventRecord(h->ev[1], h->stream));
   r.launches = 2 + 1 + 24 + levels * 5 + 1 + 1 + 2 + 13;
@@ -626,30 +617,14 @@ int pm_align(sm_handle* h, const double* guess, double* result) {
     return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
   cudaStream_t s = h->stream;
   if (h->pm.tgt_dirty) {
-    const int64_t n = h->pm.n_tgt, cs = pad64(n);
-    const int levels = kd_num_levels((int)n, 7);
-    const size_t aos = (size_t)3 * (size_t)n * sizeof(double);
-    H_RC(h->pm.coord.reserve((size_t)3 * cs * sizeof(double)));
-    H_RC(h->pm.nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
-    H_RC(h->pm.order.reserve((size_t)n * sizeof(uint32_t)));
-    H_RC(h->pm.kdws.reserve(KdWorkspace::bytes_needed((int)n, 7)));
-    H_RC(h->pm.tmp_pts.reserve(aos)); H_RC(h->pm.tmp_nrm.reserve(aos));
-    H_RC(h->pm.keep.reserve((size_t)n * sizeof(uint32_t)));
-    H_RC(h->pm.bsum.reserve((size_t)(normals_scratch_blocks((int)n) + 1) * sizeof(uint32_t)));
-    H_RC(h->pm.outp.reserve(aos)); H_RC(h->pm.outn.reserve(aos));
-    H_RC(h->pm.cnt.reserve(((size_t)ceil_div(h->pm.n_src > n ? h->pm.n_src : n, 256) + 8) * sizeof(uint32_t)));
-    H_RC(ndt_float_to_soa((const float*)h->f32.tgt.p, (int)n, (double*)h->pm.coord.p, cs, s));
-    KdWorkspace ws;
-    ws.carve(h->pm.kdws.p, (int)n, 7);
-    uint32_t* mdev = (uint32_t*)h->pm.cnt.p;
-    H_RC(normals_run((const double*)h->pm.coord.p, cs, (int)n, ws, (KdNode*)h->pm.nodes.p, (uint32_t*)h->pm.order.p,
-                     (double*)h->pm.tmp_pts.p, (double*)h->pm.tmp_nrm.p, (uint32_t*)h->pm.keep.p,
-                     (uint32_t*)h->pm.bsum.p, (double*)h->pm.outp.p, (double*)h->pm.outn.p, mdev, s));
+    const int n = (int)h->pm.n_tgt;
+    NormalsPipeline& np = h->pm.normals;
+    H_RC(np.reserve(n));
+    H_RC(ndt_float_to_soa((const float*)h->f32.tgt.p, n, np.input(), np.stride, s));
     uint32_t m = 0;
-    H_CUDA(cudaMemcpyAsync(&m, mdev, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    H_CUDA(cudaStreamSynchronize(s));
+    H_RC(np.run(n, s, &m));
     if (m == 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: no target point survived the surface-normal filter");
-    H_RC(set_target(h, (const double*)h->pm.outp.p, (const double*)h->pm.outn.p, (int64_t)m, true));
+    H_RC(set_target(h, np.points(), np.normals(), (int64_t)m, true));
     h->pm.tgt_dirty = false;
   }
   if (h->pm.src_dirty) {
@@ -687,22 +662,19 @@ int pm_align(sm_handle* h, const double* guess, double* result) {
       h->pm.score_tree_dirty = false;
     }
     const int64_t st = pad64(ns);
-    const size_t scratch = radix_sort_scratch_bytes(ns, 1);
-    H_RC(h->pm.score_buf.reserve((size_t)st * 24 + scratch + 16 * sizeof(double) + 8 * sizeof(double) + 1024));
-    uint64_t* k0 = (uint64_t*)h->pm.score_buf.p;
-    uint64_t* k1 = k0 + st;
-    uint32_t* v0 = (uint32_t*)(k1 + st);
-    uint32_t* v1 = v0 + st;
-    uint32_t* scr = v1 + st;
-    double* Tdev = (double*)((char*)scr + ((scratch + 255) & ~(size_t)255));
+    H_RC(h->pm.score_buf.reserve(256 + RadixPairs::bytes(st, ns)));
+    double* Tdev = (double*)h->pm.score_buf.p;      // 16 doubles of pose, 8 of output, then the sort
     double* outdev = Tdev + 16;
+    RadixPairs sp;
+    sp.carve((char*)h->pm.score_buf.p + 256, st);
     for (int i = 0; i < 16; ++i) h->host_guess[i] = result[i];      // pinned staging
     H_CUDA(cudaMemcpyAsync(Tdev, h->host_guess, 16 * sizeof(double), cudaMemcpyHostToDevice, s));
     const double eps = (double)h->icp.knn_epsilon;
     pm_score_knn_kernel<<<ceil_div(ns, 256), 256, 0, s>>>((const float*)h->f32.src.p, ns, Tdev, (const KdNode*)h->f32.target_tree.nodes.p,
-                                                       (const BucketPoint*)h->f32.target_tree.bpts.p, (1.0 + eps) * (1.0 + eps), k0, v0);
-    H_RC(radix_sort_pairs_u64(k0, v0, k1, v1, ns, 1, st, scr, s, 8));
-    pm_score_reduce_kernel<<<1, 1024, 0, s>>>(k0, ns, h->icp.dist_outlier_ratio, outdev);
+                                                       (const BucketPoint*)h->f32.target_tree.bpts.p, (1.0 + eps) * (1.0 + eps),
+                                                       sp.keys[0], sp.vals[0]);
+    H_RC(radix_sort_pairs_u64(sp.keys[0], sp.vals[0], sp.keys[1], sp.vals[1], ns, 1, st, sp.scratch, s, 8));
+    pm_score_reduce_kernel<<<1, 1024, 0, s>>>(sp.keys[0], ns, h->icp.dist_outlier_ratio, outdev);
     H_CUDA(cudaGetLastError());
     H_CUDA(cudaMemcpyAsync(h->host_sums, outdev, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
     H_CUDA(cudaStreamSynchronize(s));
@@ -714,15 +686,22 @@ int pm_align(sm_handle* h, const double* guess, double* result) {
 }
 
 // ---- Ndt ---------------------------------------------------------------------------------
-int load_cloud_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride, bool on_device, DevBuf& dst) {
+// the packed float source or target cloud (Ndt, NdtWithGicp, type 1)
+int set_input_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride, bool target, bool on_device) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
   if (!xyz || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInput: empty cloud");
   if (stride < 12 || n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInput: bad stride / size");
   H_CUDA(cudaSetDevice(h->device));
+  DevBuf& dst = target ? h->f32.tgt : h->f32.src;
   H_RC(dst.reserve((size_t)n * 12 + 64));
   H_CUDA(cudaMemcpy2DAsync(dst.p, 12, xyz, (size_t)stride, 12, (size_t)n,
                            on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
   if (!on_device) H_CUDA(cudaStreamSynchronize(h->stream));
+  if (target) {
+    h->n_target = n; h->has_target = true; h->pm.n_tgt = n; h->pm.tgt_dirty = true; h->pm.score_tree_dirty = true;
+  } else {
+    h->n_source = n; h->has_source = true; h->pm.n_src = n; h->pm.src_dirty = true;
+  }
   return 0;
 }
 
@@ -739,26 +718,6 @@ struct NdtRunOut {
   int iterations = 0, evaluations = 0, launches = 0;
   float ms_grid = 0, ms_iter = 0, ms_fit = 0;
 };
-
-// k-d tree over a packed float cloud
-int build_tree_f32(sm_handle* h, const float* pts, int n, FloatTree& t) {
-  const int levels = kd_num_levels(n, 8);
-  if (levels > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "cloud too large");
-  const int64_t stride = pad64(n);
-  H_RC(t.soa.reserve((size_t)(3 * stride) * sizeof(double)));
-  H_RC(t.nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
-  H_RC(t.order.reserve((size_t)n * sizeof(uint32_t)));
-  H_RC(t.bpts.reserve((size_t)(n + 8) * sizeof(BucketPoint)));
-  H_RC(h->kdws.reserve(KdWorkspace::bytes_needed(n, 8)));
-  KdWorkspace kws;
-  kws.carve(h->kdws.p, n, 8);
-  H_RC(ndt_float_to_soa(pts, n, (double*)t.soa.p, stride, h->stream));
-  H_RC(kd_build((const double*)t.soa.p, stride, n, 8, kws, (KdNode*)t.nodes.p, (uint32_t*)t.order.p, h->stream,
-                nullptr, nullptr, true));        // the cloud entered as float: 32-bit sort keys
-  H_RC(kd_fill_buckets((const double*)t.soa.p, stride, nullptr, 0, (const uint32_t*)t.order.p, n,
-                       (BucketPoint*)t.bpts.p, nullptr, h->stream));
-  return 0;
-}
 
 // pcl::Registration::getFitnessScore over h->f32.target_tree
 int fitness_score(sm_handle* h, const float* src, int ns, const float* tgt, const float* T, NdtWorkspace& ws,
@@ -1098,24 +1057,16 @@ int sm_set_input_target_device(sm_handle* h, const double* p, const double* nrm,
 }
 
 int sm_set_input_source_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride) {
-  int rc = load_cloud_f32(h, xyz, n, stride, false, h->f32.src);
-  if (rc == 0) { h->n_source = n; h->has_source = true; h->pm.n_src = n; h->pm.src_dirty = true; }
-  return rc;
+  return set_input_f32(h, xyz, n, stride, false, false);
 }
 int sm_set_input_target_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride) {
-  int rc = load_cloud_f32(h, xyz, n, stride, false, h->f32.tgt);
-  if (rc == 0) { h->n_target = n; h->has_target = true; h->pm.n_tgt = n; h->pm.tgt_dirty = true; h->pm.score_tree_dirty = true; }
-  return rc;
+  return set_input_f32(h, xyz, n, stride, true, false);
 }
 int sm_set_input_source_f32_device(sm_handle* h, const float* xyz, int64_t n, int64_t stride) {
-  int rc = load_cloud_f32(h, xyz, n, stride, true, h->f32.src);
-  if (rc == 0) { h->n_source = n; h->has_source = true; h->pm.n_src = n; h->pm.src_dirty = true; }
-  return rc;
+  return set_input_f32(h, xyz, n, stride, false, true);
 }
 int sm_set_input_target_f32_device(sm_handle* h, const float* xyz, int64_t n, int64_t stride) {
-  int rc = load_cloud_f32(h, xyz, n, stride, true, h->f32.tgt);
-  if (rc == 0) { h->n_target = n; h->has_target = true; h->pm.n_tgt = n; h->pm.tgt_dirty = true; h->pm.score_tree_dirty = true; }
-  return rc;
+  return set_input_f32(h, xyz, n, stride, true, true);
 }
 
 int sm_align(sm_handle* h, const double* guess, double* result) {
@@ -1499,31 +1450,15 @@ int sm_calculate_normals(int device, const double* points, int64_t n, double* ou
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
   SMB_CUDA_OK(cudaSetDevice(device));
   cudaStream_t s = nullptr;
-  const int64_t cs = pad64(n);
-  const int levels = kd_num_levels((int)n, 7);
-  DevBuf stage, coord, nodes, order, kdws, tmp_pts, tmp_nrm, keep, bsum, outp, outn, mdev;
-  const size_t aos = (size_t)3 * (size_t)n * sizeof(double);
-  SMB_RC(coord.reserve((size_t)3 * cs * sizeof(double)));
-  SMB_RC(nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
-  SMB_RC(order.reserve((size_t)n * sizeof(uint32_t)));
-  SMB_RC(kdws.reserve(KdWorkspace::bytes_needed((int)n, 7)));
-  SMB_RC(tmp_pts.reserve(aos)); SMB_RC(tmp_nrm.reserve(aos));
-  SMB_RC(keep.reserve((size_t)n * sizeof(uint32_t)));
-  SMB_RC(bsum.reserve((size_t)(normals_scratch_blocks((int)n) + 1) * sizeof(uint32_t)));
-  SMB_RC(outp.reserve(aos)); SMB_RC(outn.reserve(aos));
-  SMB_RC(mdev.reserve(sizeof(uint32_t)));
-  SMB_RC(upload_soa(points, n, false, stage, (double*)coord.p, cs, s));
-  KdWorkspace ws;
-  ws.carve(kdws.p, (int)n, 7);
-  SMB_RC(normals_run((const double*)coord.p, cs, (int)n, ws, (KdNode*)nodes.p, (uint32_t*)order.p,
-                     (double*)tmp_pts.p, (double*)tmp_nrm.p, (uint32_t*)keep.p, (uint32_t*)bsum.p,
-                     (double*)outp.p, (double*)outn.p, (uint32_t*)mdev.p, s));
+  NormalsPipeline np;
+  DevBuf stage;
+  SMB_RC(np.reserve((int)n));
+  SMB_RC(upload_soa(points, n, false, stage, np.input(), np.stride, s));
   uint32_t m = 0;
-  SMB_CUDA_OK(cudaMemcpyAsync(&m, mdev.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  SMB_RC(np.run((int)n, s, &m));
   if (m > 0) {
-    SMB_CUDA_OK(cudaMemcpyAsync(out_points, outp.p, (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));
-    SMB_CUDA_OK(cudaMemcpyAsync(out_normals, outn.p, (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));
+    SMB_CUDA_OK(cudaMemcpyAsync(out_points, np.points(), (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));
+    SMB_CUDA_OK(cudaMemcpyAsync(out_normals, np.normals(), (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));
     SMB_CUDA_OK(cudaStreamSynchronize(s));
   }
   *m_out = (int64_t)m;
@@ -1559,36 +1494,23 @@ static int knn1_impl(int device, const double* target, int64_t nt, const double*
   const int64_t ts = pad64(nt), qs = pad64(nq > 0 ? nq : 1);
   const int levels = kd_num_levels((int)nt, bucket);
   if (levels > 24) return SM_ERR_BAD_ARGUMENT;
-  DevBuf stage, tgt, qry, nodes, order, kdws, ids_d, d2_d, ccut, cdim, cpb, cpid, items;
+  DevBuf stage, tgt, qry, kdws, ids_d, d2_d, items;
+  KdCompactTree tree;
   SMB_RC(stage.reserve((size_t)3 * (size_t)(nt > nq ? nt : nq) * sizeof(double)));   // shared by both uploads
   SMB_RC(tgt.reserve((size_t)3 * ts * sizeof(double)));
   SMB_RC(qry.reserve((size_t)3 * qs * sizeof(double)));
-  SMB_RC(nodes.reserve((size_t)blocked_node_slots(levels) * sizeof(KdNode)));
-  SMB_RC(order.reserve((size_t)nt * sizeof(uint32_t)));
-  SMB_RC(kdws.reserve(KdWorkspace::bytes_needed((int)nt, bucket)));
-  SMB_RC(ccut.reserve(kd_compact_node_slots(levels) * (sizeof(double) + sizeof(double2))));
-  SMB_RC(cdim.reserve(kd_compact_node_slots(levels)));
-  SMB_RC(cpb.reserve(kd_compact_bucket_entries(levels) * 3 * sizeof(double)));
-  SMB_RC(cpid.reserve(kd_compact_bucket_entries(levels) * sizeof(int32_t)));
+  SMB_RC(tree.reserve((int)nt, bucket, KdCompactTree::kIds));
+  KdWorkspace ws;
+  SMB_RC(ws.carve(kdws, (int)nt, bucket));
   SMB_RC(ids_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(int32_t)));
   SMB_RC(d2_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(double)));
   SMB_RC(items.reserve(((size_t)nq + kKnnItemSlack) * sizeof(int4)));
   SMB_RC(upload_soa(target, nt, false, stage, (double*)tgt.p, ts, s));
   SMB_CUDA_OK(cudaStreamSynchronize(s));
-  KdWorkspace ws;
-  ws.carve(kdws.p, (int)nt, bucket);
-  SMB_RC(kd_build((const double*)tgt.p, ts, (int)nt, bucket, ws, (KdNode*)nodes.p, (uint32_t*)order.p, s,
-                  (double*)ccut.p, (uint8_t*)cdim.p, false,
-                  reinterpret_cast<double2*>((double*)ccut.p + kd_compact_node_slots(levels))));
-  SMB_RC(kd_compact_buckets((const double*)tgt.p, ts, nullptr, 0, (const uint32_t*)order.p, (int)nt, bucket, levels,
-                            (double*)cpb.p, nullptr, (int32_t*)cpid.p, s));
+  SMB_RC(tree.build((const double*)tgt.p, nullptr, ts, (int)nt, bucket, ws, s));
   if (nq > 0) {
-    KdCompact kc;
-    kc.cut = (const double*)ccut.p; kc.dim = (const uint8_t*)cdim.p; kc.pb = (const double*)cpb.p;
-    kc.node = reinterpret_cast<const double2*>(kc.cut + kd_compact_node_slots(levels));
-    kc.pn = nullptr; kc.pid = (const int32_t*)cpid.p; kc.levels = levels;
     SMB_RC(upload_soa(query, nq, false, stage, (double*)qry.p, qs, s));
-    SMB_RC(knn_query(kc, (const double*)qry.p, qs, (int)nq, (1.0 + epsilon) * (1.0 + epsilon), (int32_t*)ids_d.p,
+    SMB_RC(knn_query(tree.view(), (const double*)qry.p, qs, (int)nq, (1.0 + epsilon) * (1.0 + epsilon), (int32_t*)ids_d.p,
                      (double*)d2_d.p, s, queries_per_cta, (int4*)items.p));
     SMB_CUDA_OK(cudaMemcpyAsync(ids, ids_d.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     SMB_CUDA_OK(cudaMemcpyAsync(d2, d2_d.p, (size_t)nq * sizeof(double), cudaMemcpyDeviceToHost, s));

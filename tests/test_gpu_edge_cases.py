@@ -63,6 +63,29 @@ def test_icp_reuse_handle_with_changing_sizes():
         assert dt <= 1e-4 and dr <= 1e-4 and m.GetAlignInfo()["iterations"] == o["iterations"]
 
 
+def _pm_align(m, src, tgt):
+    m.SetInputSource(smb.InnerCloud(src))
+    m.SetInputTarget(smb.InnerCloud(tgt))
+    ok, res = m.Align(np.eye(4))
+    info = m.GetAlignInfo()
+    return ok, res, m.GetFitnessScore(), info["iterations"], list(info["aux"][:4])
+
+
+def test_icp_pm_reuse_handle_with_changing_sizes():
+    # one type-1 handle keeps its normals pipeline, sampling and score buffers across targets and sources that
+    # grow and then shrink: every step must give exactly what a fresh handle gives
+    src_all, sub_all, _ = scenes.lidar_pair(pair=1)
+    rng = np.random.default_rng(5)
+    m = smb.IcpUsingPointMatcher()
+    for ns, nt in [(1500, 6000), (4000, 25000), (src_all.shape[0], sub_all.shape[0]), (3000, 15000), (800, 3000)]:
+        src = src_all[np.sort(rng.choice(src_all.shape[0], ns, replace=False))].astype(np.float32)
+        tgt = sub_all[np.sort(rng.choice(sub_all.shape[0], nt, replace=False))].astype(np.float32)
+        reused = _pm_align(m, src, tgt)
+        fresh = _pm_align(smb.IcpUsingPointMatcher(), src, tgt)
+        assert reused[0] == fresh[0] and np.array_equal(reused[1], fresh[1]), (ns, nt)
+        assert reused[2:] == fresh[2:], (ns, nt, reused[2:], fresh[2:])
+
+
 def test_normals_tiny_inputs():
     rng = np.random.default_rng(0)
     for n in (1, 2, 3, 6, 7, 8, 13):
