@@ -76,6 +76,7 @@ class IcpFastB200 : public Interface {
 
   // icp_fast.cc:455-529
   bool Align(const Eigen::Matrix4d& guess, Eigen::Matrix4d& result) override {  // NOLINT
+    PrepareBatch();
     const int rc = sm_align(handle_, guess.data(), result.data());  // both column-major
     Check(rc);
     this->final_score_ = sm_get_fitness_score(handle_);
@@ -84,13 +85,23 @@ class IcpFastB200 : public Interface {
 
   // hooks of AlignBatch (below)
   sm_handle* handle() const { return handle_; }
-  void PrepareBatch() {}
+  // Enable/DisableInnerCompensation are not virtual (interface.h:89-91): the flag is read at every Align
+  // (icp_fast.cc:487, :509)
+  void PrepareBatch() { Check(sm_set_inner_compensation(handle_, InnerCompensation(this, 0) ? 1 : 0)); }
   void SetFinalScore(double score) { this->final_score_ = score; }
 
  private:
   void Check(int rc) const {
     CHECK_GE(rc, 0) << "sm_b200: " << sm_last_error(handle_);   // reference aborts via glog
   }
+  // Interface::inner_compensation_ (interface.h:115).  An Interface without that member (a reduced stand-in of
+  // the header) still compiles the adapter, with the flag off.
+  template <typename Self>
+  static auto InnerCompensation(const Self* self, int) -> decltype(static_cast<bool>(self->inner_compensation_)) {
+    return self->inner_compensation_;
+  }
+  template <typename Self>
+  static bool InnerCompensation(const Self*, long) { return false; }
 
   sm_handle* handle_ = nullptr;
   struct {

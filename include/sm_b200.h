@@ -83,6 +83,17 @@ int sm_set_option(sm_handle* h, const char* name, const char* text);
 /* Interface::PrintOptions (interface.cc:115-137): writes one "name -> value\n" line per option
  * sm_set_option accepts for the handle's type. */
 int sm_print_options(sm_handle* h, char* buf, int64_t buf_len);
+/* Interface::EnableInnerCompensation / DisableInnerCompensation (interface.h:89-91, interface.cc:34-36):
+ * enable != 0 switches IcpFast::Align to its in-loop motion compensation from the next Align on (sm_align,
+ * sm_align_async, sm_align_batch and sm_align_pairs alike).  Every handle type accepts it; only SM_TYPE_FAST_ICP
+ * reads it, as in the reference.  In every iteration source point i (f_i = i / N, its column in
+ * sm_set_input_source) is moved by InterpolateTransform(Identity, T_iter, f_i) (icp_fast.cc:487-488) instead of
+ * T_iter, and its match's Jacobian column is scaled by f_i (:284-289).  Deviation: the reference's
+ * EigenPointCloud::ApplyMotionCompensation (cloud_types.cc:306-318) declares a local `transform` that shadows the
+ * parameter and interpolates towards that uninitialised local (undefined behaviour); the engine interpolates
+ * towards T_iter, which is what the code evidently intends.  Not an XML option: sm_print_options does not list
+ * it. */
+int sm_set_inner_compensation(sm_handle* h, int32_t enable);
 /* Interface::GetType (interface.h:106). */
 int sm_get_type(const sm_handle* h);
 

@@ -119,9 +119,16 @@ int sm_debug_gicp_host(int32_t op, const double* in, double* out);
  * when rank(covariance) + 1 < 3. */
 int sm_debug_normals_leaf(const double* members_3k, int32_t count, double* mean_3, double* normal_3, int32_t* kept);
 
-/* sm_motion_compensation's arithmetic on the host (csrc/motion.cu make_params + motion_point): packed
+/* sm_motion_compensation's arithmetic on the host (csrc/motion_dev.cuh make_motion_params + motion_point): packed
  * {x, y, z, intensity, factor} float records in and out; SM_ERR_BAD_ARGUMENT if a factor is outside [0, 1]. */
 int sm_debug_motion_host(const float* points_5n, int64_t n, const double* delta_4x4, float* out_5n);
+
+/* IcpFast's inner compensation on the host (csrc/motion.cu icp_deskew_kernel and icp.cu's compensated phase B, the
+ * same __host__ __device__ code): the n points (3xN, the source after G0, caller order, f_i = i / n) de-skewed with
+ * InterpolateTransform(Identity, T_iter, f_i) into out_points_3n; if targets_3n, normals_3n and out_terms_7n are
+ * given, each point's match against (target i, normal i) as {f_i F[6], residual} (icp_fast.cc:268-302, :284-289). */
+int sm_debug_inner_compensation_host(const double* T_iter_4x4, const double* points_3n, const double* targets_3n,
+                                     const double* normals_3n, int64_t n, double* out_points_3n, double* out_terms_7n);
 
 /* One leaf of VoxelGridCovariance::applyFilter (voxel_grid_covariance_omp_impl.hpp:209-366; csrc/ndt.cu finish_leaf
  * compiled for the host): the n points of a voxel in input order -> mean, inverse covariance (zero when the leaf has

@@ -42,6 +42,7 @@ SIGNATURES = {
     "sm_destroy": (C.c_int, [_VP]),
     "sm_set_option": (C.c_int, [_VP, C.c_char_p, C.c_char_p]),
     "sm_print_options": (C.c_int, [_VP, C.c_char_p, C.c_int64]),
+    "sm_set_inner_compensation": (C.c_int, [_VP, C.c_int32]),
     "sm_get_type": (C.c_int, [_VP]),
     "sm_set_input_source": (C.c_int, [_VP, _VP, C.c_int64]),
     "sm_set_input_target": (C.c_int, [_VP, _VP, _VP, C.c_int64]),
@@ -81,6 +82,7 @@ SIGNATURES = {
     "sm_debug_gicp_outer": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "sm_debug_gicp_host": (C.c_int, [C.c_int32, _VP, _VP]),
     "sm_debug_motion_host": (C.c_int, [_VP, C.c_int64, _DP, _VP]),
+    "sm_debug_inner_compensation_host": (C.c_int, [_DP, _VP, _VP, _VP, C.c_int64, _VP, _VP]),
     "sm_debug_icp_host": (C.c_int, [C.c_int32, _VP, C.c_int64, _VP]),
     "sm_debug_ndt_leaf": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_double, _VP, _VP, _VP, _VP, _VP]),
     "sm_debug_ndt_term": (C.c_int, [_VP, C.c_double, C.c_float, C.c_int32, _VP, _VP, _VP, _VP, _VP]),

@@ -17,6 +17,7 @@
 #include "icp_dev.cuh"
 #include "knn_smem.cuh"
 #include "linalg_dev.cuh"
+#include "motion_dev.cuh"
 
 #include <nvtx3/nvToolsExt.h>
 
@@ -138,9 +139,20 @@ __global__ void gather_source_kernel(const double* __restrict__ in, double* __re
 #endif
 // Phase A, one query per thread (a single alignment in flight: 469 CTAs, all resident at once, the
 // kernel lasts as long as its longest search).
-template <bool kAllSmem>
+// the query of source point i: T_iter (x) src0_i, or with inner compensation the de-skewed point of the iteration
+template <bool kComp>
+__device__ __forceinline__ void load_query(const IcpBuffers& b, const double* T, const double* __restrict__ deskewed,
+                                           int i, double& x, double& y, double& z) {
+  if constexpr (kComp) {
+    x = deskewed[i]; y = deskewed[b.sstride + i]; z = deskewed[2 * b.sstride + i];
+  } else {
+    transform_point(T, b.src0[i], b.src0[b.sstride + i], b.src0[2 * b.sstride + i], x, y, z);
+  }
+}
+
+template <bool kAllSmem, bool kComp>
 __global__ void __launch_bounds__(kKnnCtaThreads, SMB_KNN_MIN_CTAS)
-icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta) {
+icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __restrict__ deskewed) {
   extern __shared__ __align__(128) unsigned char knn_smem[];
   if (b.state->done) return;
   uint64_t* bar; double* T;
@@ -150,7 +162,7 @@ icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta) {
   const int begin = blockIdx.x * per_cta, end = min(begin + per_cta, p.n_source);
   int i = begin + threadIdx.x;
   double px = 0.0, py = 0.0, pz = 0.0;
-  if (i < end) transform_point(T, b.src0[i], b.src0[b.sstride + i], b.src0[2 * b.sstride + i], px, py, pz);
+  if (i < end) load_query<kComp>(b, T, deskewed, i, px, py, pz);
   mbar_wait(bar, 0);      // every thread waits: the CTA must not retire while the copy engine writes its smem
   while (i < end) {
     int slot; double d2;
@@ -160,7 +172,7 @@ icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta) {
     // fire-and-forget reduction straight into the 2048-bin global histogram (L2-resident)
     if (finite_d2(d2)) atomicAdd(&b.hist[dist_bin(d2)], 1u);
     i += kKnnCtaThreads;
-    if (i < end) transform_point(T, b.src0[i], b.src0[b.sstride + i], b.src0[2 * b.sstride + i], px, py, pz);
+    if (i < end) load_query<kComp>(b, T, deskewed, i, px, py, pz);
   }
 }
 
@@ -168,9 +180,9 @@ icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta) {
 // visits, then the lanes of every warp pull the parked searches of their batch (knn_batch_cta, knn_smem.cuh).
 // The one-query-per-thread form spends its time in passes in which a few lanes finish long searches
 // (11.7 of 32 lanes busy on average, 18.0 here).
-template <bool kAllSmem>
+template <bool kAllSmem, bool kComp>
 __global__ void __launch_bounds__(kKnnCtaThreads, SMB_KNN_MIN_CTAS)
-icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta) {
+icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __restrict__ deskewed) {
   extern __shared__ __align__(128) unsigned char knn_smem[];
   if (b.state->done) return;
   uint64_t* bar; double* T;
@@ -181,9 +193,7 @@ icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta) {
   mbar_wait(bar, 0);      // every thread waits: the CTA must not retire while the copy engine writes its smem
   knn_batch_cta<kAllSmem>(
       tree, begin, end, per_cta, p.max_error2, b.knn_items,
-      [&](int i, double& x, double& y, double& z) {
-        transform_point(T, b.src0[i], b.src0[b.sstride + i], b.src0[2 * b.sstride + i], x, y, z);
-      },
+      [&](int i, double& x, double& y, double& z) { load_query<kComp>(b, T, deskewed, i, x, y, z); },
       [&](int i, int best, double head) { b.slot[i] = best; b.d2[i] = head; },
       [&](int i, double& head, int& best) { head = __ldcg(b.d2 + i); best = __ldcg(b.slot + i); },
       [&](int i, int slot, double d2) {
@@ -195,8 +205,11 @@ icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta) {
 }
 
 // -------------------------------------------------------------------------------- phase B
+// kComp: inner compensation (icp_fast.cc:284-289): the points are the iteration's de-skewed ones and every
+// match's Jacobian column is scaled by the point's factor, both for the sums and for the parked candidates
+template <bool kComp>
 __global__ void __launch_bounds__(kAccThreads)
-icp_accum_kernel(IcpBuffers b, IcpParams p) {
+icp_accum_kernel(IcpBuffers b, IcpParams p, const double* __restrict__ deskewed) {
   __shared__ uint32_t warp_tot[8];
   __shared__ BinSel sel_sm;
   __shared__ double T[16];
@@ -208,6 +221,7 @@ icp_accum_kernel(IcpBuffers b, IcpParams p) {
   //     points of the thread at once (these reads overlap the histogram read of select_bin)
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
   double d2[kAccItems], sx[kAccItems], sy[kAccItems], sz[kAccItems];
+  [[maybe_unused]] double fac[kAccItems];
   int slot[kAccItems];
 #pragma unroll
   for (int r = 0; r < kAccItems; ++r) {
@@ -215,9 +229,11 @@ icp_accum_kernel(IcpBuffers b, IcpParams p) {
     const bool in = i < p.n_source;
     d2[r] = in ? b.d2[i] : inf;
     slot[r] = in ? b.slot[i] : -1;
-    sx[r] = in ? b.src0[i] : 0.0;
-    sy[r] = in ? b.src0[b.sstride + i] : 0.0;
-    sz[r] = in ? b.src0[2 * b.sstride + i] : 0.0;
+    const double* src = kComp ? deskewed : b.src0;
+    sx[r] = in ? src[i] : 0.0;
+    sy[r] = in ? src[b.sstride + i] : 0.0;
+    sz[r] = in ? src[2 * b.sstride + i] : 0.0;
+    if constexpr (kComp) fac[r] = in ? source_factor(b.src_sort.vals[0][i], p.n_source) : 0.0;
   }
   if (b.state->done) return;
   if (threadIdx.x < 16) T[threadIdx.x] = b.state->T_iter[threadIdx.x];
@@ -245,12 +261,16 @@ icp_accum_kernel(IcpBuffers b, IcpParams p) {
   double F[kAccItems][6], dot[kAccItems], sq[kAccItems];
 #pragma unroll
   for (int r = 0; r < kAccItems; ++r) {
-    double px, py, pz;
-    transform_point(T, sx[r], sy[r], sz[r], px, py, pz);
     BucketPoint q; BucketNormal n;
     q.x = qxy[r].x; q.y = qxy[r].y; q.z = qz[r];
     n.x = nxy[r].x; n.y = nxy[r].y; n.z = nz[r];
-    match_terms(px, py, pz, q, n, F[r], dot[r]);
+    if constexpr (kComp) {
+      compensated_match_terms(sx[r], sy[r], sz[r], q, n, fac[r], F[r], dot[r]);
+    } else {
+      double px, py, pz;
+      transform_point(T, sx[r], sy[r], sz[r], px, py, pz);
+      match_terms(px, py, pz, q, n, F[r], dot[r]);
+    }
     sq[r] = sqrt(use[r] ? d2[r] : 0.0);
     add_terms_if(acc, F[r], dot[r], sq[r], use[r] && bin[r] < sel.bin);
     is_cand[r] = use[r] && bin[r] == sel.bin;
@@ -379,9 +399,27 @@ int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_de
   return 0;
 }
 
-// Iterations start_iteration .. start_iteration+count-1 of one Align: three launches each.
+// Iterations start_iteration .. start_iteration+count-1 of one Align: three launches each, four with inner
+// compensation (the de-skew of the source goes first).
+template <bool kComp>
+void icp_enqueue_search(const IcpBuffers& b, const IcpParams& p, int grid, int per, size_t smem, cudaStream_t stream,
+                        const double* deskewed) {
+  if (per > kKnnCtaThreads) {
+    if (p.tree_levels <= kKnnSmemLevels)
+      icp_knn_batch_kernel<true, kComp><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per, deskewed);
+    else
+      icp_knn_batch_kernel<false, kComp><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per, deskewed);
+  } else if (p.tree_levels <= kKnnSmemLevels) {
+    icp_knn_kernel<true, kComp><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per, deskewed);
+  } else {
+    icp_knn_kernel<false, kComp><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per, deskewed);
+  }
+}
+
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
-                           cudaStream_t stream, cudaEvent_t* events) {
+                           cudaStream_t stream, cudaEvent_t* events, double* deskewed) {
+  const bool comp = p.inner_compensation != 0;
+  if (comp && !deskewed) return -1;
   const int nb = icp_accum_blocks(p.n_source);
   int grid, per;
   knn_geometry(p.n_source, p.knn_queries_per_cta, &grid, &per);
@@ -389,21 +427,19 @@ int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_it
   for (int it = 0; it < count; ++it) {
     nvtxRangePushA("Iteration");                 // REGISTER_BLOCK("Iteration"), icp_fast.cc:484
     if (events) cudaEventRecord(events[4 * it + 0], stream);
-    nvtxRangePushA("FindClosests");              // icp_fast.cc:169-180
-    if (per > kKnnCtaThreads) {
-      if (p.tree_levels <= kKnnSmemLevels)
-        icp_knn_batch_kernel<true><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per);
-      else
-        icp_knn_batch_kernel<false><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per);
-    } else if (p.tree_levels <= kKnnSmemLevels) {
-      icp_knn_kernel<true><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per);
-    } else {
-      icp_knn_kernel<false><<<grid, kKnnCtaThreads, smem, stream>>>(b, p, per);
+    if (comp) {
+      nvtxRangePushA("ApplyMotionCompensation");   // icp_fast.cc:487-488
+      icp_deskew_launch(b, p, deskewed, stream);
+      nvtxRangePop();
     }
+    nvtxRangePushA("FindClosests");              // icp_fast.cc:169-180
+    if (comp) icp_enqueue_search<true>(b, p, grid, per, smem, stream, deskewed);
+    else icp_enqueue_search<false>(b, p, grid, per, smem, stream, nullptr);
     nvtxRangePop();
     if (events) cudaEventRecord(events[4 * it + 1], stream);
     nvtxRangePushA("ErrorElements");             // icp_fast.cc:92-167 (+ the sums of ComputePointToPlane)
-    icp_accum_kernel<<<nb, kAccThreads, 0, stream>>>(b, p);
+    if (comp) icp_accum_kernel<true><<<nb, kAccThreads, 0, stream>>>(b, p, deskewed);
+    else icp_accum_kernel<false><<<nb, kAccThreads, 0, stream>>>(b, p, nullptr);
     nvtxRangePop();
     if (events) cudaEventRecord(events[4 * it + 2], stream);
     nvtxRangePushA("ComputePointToPlane");       // icp_fast.cc:256-323

@@ -272,6 +272,15 @@ __host__ __device__ __forceinline__ void match_terms(double px, double py, doubl
   F[3] = n.x; F[4] = n.y; F[5] = n.z;
   dot = (px - q.x) * n.x + (py - q.y) * n.y + (pz - q.z) * n.z;
 }
+// IcpFast with inner compensation (icp_fast.cc:284-289): the Jacobian column of the match scaled by the point's
+// factor f (wF and F both, so A sums (f F)(f F)^T and b sums (f F) * dot); the residual is not scaled
+__host__ __device__ __forceinline__ void compensated_match_terms(double px, double py, double pz, const BucketPoint& q,
+                                                                 const BucketNormal& n, double f, double* F,
+                                                                 double& dot) {
+  match_terms(px, py, pz, q, n, F, dot);
+#pragma unroll
+  for (int r = 0; r < 6; ++r) F[r] = F[r] * f;
+}
 __host__ __device__ __forceinline__ void add_terms(double* acc, const double* F, double dot, double d2) {
   int k = 0;
 #pragma unroll

@@ -141,7 +141,9 @@ struct IcpParams {
   int disable_convergence;
   int tree_levels;         // kd_num_levels(n_target, 8): depth of the root-to-leaf path
   int knn_queries_per_cta; // phase A: 0 = one query per thread, else queries per 256-thread CTA
+  int inner_compensation;  // 1: IcpFast::EnableInnerCompensation, the source is de-skewed in every iteration
 };
+static_assert(sizeof(IcpParams) == 40, "inner_compensation takes the tail padding: kernel argument offsets stay put");
 
 struct IcpBuffers {
   // target (caller order, SoA, centred in place by the prologue)
@@ -180,12 +182,17 @@ int icp_accum_blocks(int n_source);
 int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_dev,
                  KdWorkspace& ws, const KdCompactTree& tree, cudaStream_t stream);
 // events (optional): 4 per iteration — before A, after A, after B, after C
+// deskewed: [3][sstride] doubles, the de-skewed source of the iteration; needed when p.inner_compensation
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
-                           cudaStream_t stream, cudaEvent_t* events);
+                           cudaStream_t stream, cudaEvent_t* events, double* deskewed = nullptr);
 void icp_finish_launch(const IcpBuffers& b, const IcpParams& p, int nblocks_b, cudaStream_t stream);
 // stand-alone k-NN over an already built tree (compact layout incl. pid): ids = original indices
 int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, double max_error2,
               int32_t* ids, double* d2, cudaStream_t stream, int queries_per_cta = 0, int4* items = nullptr);
+
+// ---- motion.cu ---------------------------------------------------------------------------
+// one iteration's de-skewed source of IcpFast with inner compensation: out = Interp(T_iter, f_i) (x) src0_i
+void icp_deskew_launch(const IcpBuffers& b, const IcpParams& p, double* out, cudaStream_t stream);
 
 // ---- ndt.cu ------------------------------------------------------------------------------
 struct NdtGrid {            // VoxelGridCovariance bookkeeping (_impl.hpp:88-103)

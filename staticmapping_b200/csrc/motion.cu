@@ -17,49 +17,18 @@
 #include "../../include/sm_b200.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "icp_dev.cuh"
+#include "motion_dev.cuh"
 
 namespace smb {
 namespace {
 
-struct MotionParams {
-  double qb[4];       // Quaternion(R_delta): w, x, y, z
-  double t[3];        // translation of delta
-  double d;           // dot(q_a, q_b) with q_a = identity
-  double theta;       // acos(|d|)       (unused when lerp)
-  double sin_theta;   // sin(theta)
-  int lerp;           // |d| >= 1 - eps: Eigen falls back to linear weights
-};
-
 // one point: InterpolateTransform(Identity, delta, factor) applied to (x, y, z), written as float
 __host__ __device__ __forceinline__ void motion_point(const MotionParams& P, float x, float y, float z, float factor,
                                                       float* o) {
-  const double t = (double)factor;
-  double scale0, scale1;
-  if (P.lerp) {
-    scale0 = 1.0 - t; scale1 = t;
-  } else {
-    scale0 = sin((1.0 - t) * P.theta) / P.sin_theta;
-    scale1 = sin(t * P.theta) / P.sin_theta;
-  }
-  if (P.d < 0.0) scale1 = -scale1;
-  // coeffs = scale0 * q_a + scale1 * q_b with q_a = (1, 0, 0, 0)
-  const double qw = scale0 * 1.0 + scale1 * P.qb[0];
-  const double qx = scale0 * 0.0 + scale1 * P.qb[1];
-  const double qy = scale0 * 0.0 + scale1 * P.qb[2];
-  const double qz = scale0 * 0.0 + scale1 * P.qb[3];
-  // QuaternionBase::toRotationMatrix (no normalisation, like Eigen)
-  const double tx = 2.0 * qx, ty = 2.0 * qy, tz = 2.0 * qz;
-  const double twx = tx * qw, twy = ty * qw, twz = tz * qw;
-  const double txx = tx * qx, txy = ty * qx, txz = tz * qx;
-  const double tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
-  const double r00 = 1.0 - (tyy + tzz), r01 = txy - twz, r02 = txz + twy;
-  const double r10 = txy + twz, r11 = 1.0 - (txx + tzz), r12 = tyz - twx;
-  const double r20 = txz - twy, r21 = tyz + twx, r22 = 1.0 - (txx + tyy);
-  const double px = (double)x, py = (double)y, pz = (double)z;
-  const double ox = ((r00 * px + r01 * py) + r02 * pz) + P.t[0] * t;
-  const double oy = ((r10 * px + r11 * py) + r12 * pz) + P.t[1] * t;
-  const double oz = ((r20 * px + r21 * py) + r22 * pz) + P.t[2] * t;
-  o[0] = (float)ox; o[1] = (float)oy; o[2] = (float)oz;
+  double d[3];
+  motion_point_d(P, x, y, z, factor, d);
+  o[0] = (float)d[0]; o[1] = (float)d[1]; o[2] = (float)d[2];
 }
 
 __global__ void __launch_bounds__(256)
@@ -76,48 +45,27 @@ motion_compensation_kernel(const char* __restrict__ in, char* __restrict__ out, 
   o[3] = intensity; o[4] = factor;
 }
 
-// Eigen::Quaternion(Matrix3) (quaternionbase_assign_impl); m column-major 4x4
-void rotation_to_quaternion_host(const double* T, double* q) {
-  auto m = [&](int r, int c) { return T[r + 4 * c]; };
-  double t = m(0, 0) + m(1, 1) + m(2, 2);
-  if (t > 0.0) {
-    t = sqrt(t + 1.0);
-    q[0] = 0.5 * t;
-    t = 0.5 / t;
-    q[1] = (m(2, 1) - m(1, 2)) * t;
-    q[2] = (m(0, 2) - m(2, 0)) * t;
-    q[3] = (m(1, 0) - m(0, 1)) * t;
-  } else {
-    int i = 0;
-    if (m(1, 1) > m(0, 0)) i = 1;
-    if (m(2, 2) > m(i, i)) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    t = sqrt(m(i, i) - m(j, j) - m(k, k) + 1.0);
-    q[1 + i] = 0.5 * t;
-    t = 0.5 / t;
-    q[0] = (m(k, j) - m(j, k)) * t;
-    q[1 + j] = (m(j, i) + m(i, j)) * t;
-    q[1 + k] = (m(k, i) + m(i, k)) * t;
-  }
-}
-
-MotionParams make_params(const double* delta) {
-  MotionParams P;
-  rotation_to_quaternion_host(delta, P.qb);
-  for (int k = 0; k < 3; ++k) P.t[k] = delta[12 + k];
-  // q_a = Quaternion(Identity) = (1, 0, 0, 0); coeffs dot product in Eigen's (x, y, z, w) order
-  P.d = ((0.0 * P.qb[1] + 0.0 * P.qb[2]) + 0.0 * P.qb[3]) + 1.0 * P.qb[0];
-  const double one = 1.0 - 2.220446049250313e-16;
-  const double abs_d = fabs(P.d);
-  P.lerp = abs_d >= one ? 1 : 0;
-  P.theta = P.lerp ? 0.0 : acos(abs_d);
-  P.sin_theta = P.lerp ? 1.0 : sin(P.theta);
-  return P;
+// IcpFast with inner compensation (icp_fast.cc:487-488): step_cloud.ApplyMotionCompensation(T_iter) instead of
+// ApplyTransform(T_iter).  Every source point gets its own InterpolateTransform(Identity, T_iter, f_i), f_i = i / N
+// of its caller column i; the result stays in double.  T_iter lives in device state, so the quaternion, theta and
+// sin(theta) are formed per CTA from it; the output is read by both the k-NN search (phase A) and phase B.
+__global__ void __launch_bounds__(256)
+icp_deskew_kernel(IcpBuffers b, IcpParams p, double* __restrict__ out) {
+  __shared__ MotionParams P;
+  if (b.state->done) return;
+  if (threadIdx.x == 0) P = make_motion_params(b.state->T_iter);
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.n_source) return;
+  const float factor = (float)source_factor(b.src_sort.vals[0][i], p.n_source);   // InterpolateTransform's float
+  double o[3];
+  motion_point_d(P, b.src0[i], b.src0[b.sstride + i], b.src0[2 * b.sstride + i], factor, o);
+  out[i] = o[0]; out[b.sstride + i] = o[1]; out[2 * b.sstride + i] = o[2];
 }
 
 int run(const char* dev_in, char* dev_out, int64_t n, int64_t stride, const double* delta, int* dev_bad,
         cudaStream_t s) {
-  const MotionParams P = make_params(delta);
+  const MotionParams P = make_motion_params(delta);
   SMB_CUDA_OK(cudaMemsetAsync(dev_bad, 0, sizeof(int), s));
   motion_compensation_kernel<<<ceil_div(n, 256), 256, 0, s>>>(dev_in, dev_out, stride, (int)n, P, dev_bad);
   SMB_CUDA_OK(cudaGetLastError());
@@ -125,6 +73,11 @@ int run(const char* dev_in, char* dev_out, int64_t n, int64_t stride, const doub
 }
 
 }  // namespace
+
+void icp_deskew_launch(const IcpBuffers& b, const IcpParams& p, double* out, cudaStream_t stream) {
+  icp_deskew_kernel<<<ceil_div(p.n_source, 256), 256, 0, stream>>>(b, p, out);
+}
+
 }  // namespace smb
 
 using namespace smb;
@@ -149,10 +102,10 @@ int sm_motion_compensation_device(int device, const float* dev_points, int64_t n
   return host_bad ? SM_ERR_BAD_ARGUMENT : SM_OK;
 }
 
-// test hook (include/sm_b200_debug.h): make_params + motion_point on the host, packed 5-float records
+// test hook (include/sm_b200_debug.h): make_motion_params + motion_point on the host, packed 5-float records
 int sm_debug_motion_host(const float* points, int64_t n, const double* delta_4x4, float* out) {
   if (!points || !out || !delta_4x4 || n < 0) return SM_ERR_BAD_ARGUMENT;
-  const MotionParams P = make_params(delta_4x4);
+  const MotionParams P = make_motion_params(delta_4x4);
   int bad = 0;
   for (int64_t i = 0; i < n; ++i) {
     const float* p = points + 5 * i;
@@ -161,6 +114,25 @@ int sm_debug_motion_host(const float* points, int64_t n, const double* delta_4x4
     out[5 * i + 3] = p[3]; out[5 * i + 4] = p[4];
   }
   return bad ? SM_ERR_BAD_ARGUMENT : SM_OK;
+}
+
+// test hook (include/sm_b200_debug.h): the arithmetic of icp_deskew_kernel and of phase B's compensated match
+// terms on the host
+int sm_debug_inner_compensation_host(const double* T_iter_4x4, const double* points_3n, const double* targets_3n,
+                                     const double* normals_3n, int64_t n, double* out_points_3n, double* out_terms_7n) {
+  if (!T_iter_4x4 || !points_3n || n <= 0 || n > (1 << 30) || !out_points_3n) return SM_ERR_BAD_ARGUMENT;
+  const MotionParams P = make_motion_params(T_iter_4x4);
+  for (int64_t i = 0; i < n; ++i) {
+    const double f = source_factor((uint32_t)i, (int)n);
+    double* o = out_points_3n + 3 * i;
+    motion_point_d(P, points_3n[3 * i], points_3n[3 * i + 1], points_3n[3 * i + 2], (float)f, o);
+    if (!targets_3n || !normals_3n || !out_terms_7n) continue;
+    BucketPoint q; BucketNormal nr;
+    q.x = targets_3n[3 * i]; q.y = targets_3n[3 * i + 1]; q.z = targets_3n[3 * i + 2]; q.id = 0;
+    nr.x = normals_3n[3 * i]; nr.y = normals_3n[3 * i + 1]; nr.z = normals_3n[3 * i + 2]; nr.pad = 0.0;
+    dev::compensated_match_terms(o[0], o[1], o[2], q, nr, f, out_terms_7n + 7 * i, out_terms_7n[7 * i + 6]);
+  }
+  return SM_OK;
 }
 
 int sm_motion_compensation(int device, const float* points, int64_t n, int64_t stride_bytes,

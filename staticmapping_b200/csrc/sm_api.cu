@@ -224,6 +224,7 @@ struct sm_handle {
   int64_t n_source = 0, n_target = 0;
   bool has_source = false, has_target = false;
   IcpOptions icp;
+  bool inner_compensation = false;  // Interface::EnableInnerCompensation; only IcpFast reads it
   ndt::Options ndt;
   NdtGicpOptions ng;
   DevBuf kdws;                     // k-d tree build workspace of every tree below
@@ -232,6 +233,7 @@ struct sm_handle {
   struct {
     DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, tgt, nrm, src_raw, src0, src_g0, src_sort, slot, d2,
         hist, cand_terms, cand_key, cand_cnt, partials, mean_partials, state, guess;
+    DevBuf deskewed;                 // [3][sstride]: the source of the iteration, with inner compensation only
     KdCompactTree tree;
     int64_t sstride = 0, tstride = 0;
     bool up_src = false, up_tgt = false;
@@ -240,6 +242,7 @@ struct sm_handle {
     // in-flight Align (sm_align_async .. sm_align_wait)
     struct {
       IcpBuffers b; IcpParams p; KdWorkspace ws; std::string key;
+      double* deskewed = nullptr;
       bool graphs = false, active = false;
       int enqueued = 0, launches = 0, max_it = 0;
     } run;
@@ -450,13 +453,13 @@ int icp_enqueue_chunk(sm_handle* h) {
     const int first_chunk = r.enqueued == 0 ? 1 : 0;
     key_append(ikey, chunk); key_append(ikey, first_chunk);
     H_RC(run_graphed(h, f.g_iterations, ikey, [&]() {
-      return icp_enqueue_iterations(r.b, p, r.enqueued, chunk, h->stream, nullptr);
+      return icp_enqueue_iterations(r.b, p, r.enqueued, chunk, h->stream, nullptr, r.deskewed);
     }));
   } else {
-    H_RC(icp_enqueue_iterations(r.b, p, r.enqueued, chunk, h->stream, evs));
+    H_RC(icp_enqueue_iterations(r.b, p, r.enqueued, chunk, h->stream, evs, r.deskewed));
   }
   r.enqueued += chunk;
-  r.launches += 3 * chunk;
+  r.launches += (p.inner_compensation ? 4 : 3) * chunk;
   H_CUDA(cudaMemcpyAsync(f.host_state, f.state.p, sizeof(IcpState), cudaMemcpyDeviceToHost, h->stream));
   return 0;
 }
@@ -522,6 +525,14 @@ int icp_begin(sm_handle* h, const double* guess) {
   p.disable_convergence = h->icp.disable_convergence_check ? 1 : 0;
   p.knn_queries_per_cta = h->icp.knn_queries_per_cta;
   p.tree_levels = levels;
+  // EnableInnerCompensation: IcpFast::Align reads it (icp_fast.cc:487, :509); type 1 runs the IcpFast chain but,
+  // like IcpUsingPointMatcher, ignores it
+  p.inner_compensation = (h->type == SM_TYPE_FAST_ICP && h->inner_compensation) ? 1 : 0;
+  r.deskewed = nullptr;
+  if (p.inner_compensation) {
+    H_RC(f.deskewed.reserve((size_t)(3 * f.sstride) * sizeof(double)));
+    r.deskewed = (double*)f.deskewed.p;
+  }
   if (levels > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "target too large (tree deeper than 24 levels)");
 
   memcpy(h->host_guess, guess, 16 * sizeof(double));   // pinned: the caller's array may go away
@@ -530,6 +541,7 @@ int icp_begin(sm_handle* h, const double* guess) {
   r.graphs = h->icp.use_graphs && !h->icp.profile_kernels;
   r.key.clear();
   key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.guess.p); key_append(r.key, h->kdws.p);
+  key_append(r.key, r.deskewed);   // p.inner_compensation is part of p
   if (r.graphs) {
     H_RC(run_graphed(h, f.g_prologue, r.key, [&]() {
       return icp_prologue(b, p, (const double*)f.guess.p, ws, f.tree, h->stream);
@@ -1025,6 +1037,12 @@ int sm_set_option(sm_handle* h, const char* name, const char* text) {
     return SM_OK;
   }
   return fail(h, SM_ERR_UNKNOWN_OPTION, std::string("Init an unknown option of this matcher! ") + name);
+}
+
+int sm_set_inner_compensation(sm_handle* h, int32_t enable) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  h->inner_compensation = enable != 0;
+  return SM_OK;
 }
 
 int sm_print_options(sm_handle* h, char* buf, int64_t buf_len) {

@@ -155,11 +155,15 @@ class Interface:
         print(text, end="")
         return text
 
+    # interface.cc:34-36; takes effect from the next Align.  IcpFast de-skews the source in every
+    # iteration (icp_fast.cc:487-491); the other types keep the flag without effect, as in the reference.
     def EnableInnerCompensation(self):
-        self._inner_compensation = True   # no caller in the reference (SURVEY Appendix A)
+        self._inner_compensation = True
+        self._check(self._lib.sm_set_inner_compensation(self._h, 1), "EnableInnerCompensation")
 
     def DisableInnerCompensation(self):
         self._inner_compensation = False
+        self._check(self._lib.sm_set_inner_compensation(self._h, 0), "DisableInnerCompensation")
 
     # --- data ----------------------------------------------------------------------------
     def SetInputSource(self, cloud: EigenCloud):
