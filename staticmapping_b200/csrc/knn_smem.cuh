@@ -12,10 +12,10 @@
 //     CTA per SM and no room for the kernels of other alignments in flight;
 //   * leaves carry no payload: a leaf's bucket is (in-level index << (levels - level)) in the
 //     padded bucket array, one bucket = x[8] y[8] z[8] = 12 aligned 16-byte loads;
-//   * the heap index of a reached leaf encodes its whole path, so the far-side tests of a frame
-//     are re-derived from it after the bucket, deepest level first, as the recursion would test
-//     them (knn1_frames): no per-level bookkeeping during a descent, and the frame stack is
-//     touched only by nested far visits.
+//   * no stack, and no local memory for the search state: the heap index of the reached leaf encodes the whole path, and
+//     the pending far sides of a query are siblings of that path's nodes, at most one per level, so
+//     the search state is the leaf plus a `pending` and a `turns` bit per level, in registers.  The
+//     rd / off[] of a popped far child are replayed exactly over the turns above it (knn_pop).
 // The visit ORDER and every comparison are those of libnabo's recurseKnn, so index sets and
 // squared distances are bit-identical to the oracle for any epsilon (tests/test_gpu_icp.py).
 #ifndef SM_B200_KNN_SMEM_CUH_
@@ -44,9 +44,6 @@ namespace dev {
 #else
 #define SMB_KNN_Q(t, reg, d) (reg)
 #endif
-#ifndef SMB_KNN_PAIR_PREFETCH
-#define SMB_KNN_PAIR_PREFETCH 0
-#endif
 constexpr int kKnnCtaThreads = SMB_KNN_THREADS;        // threads (= traversal slots) per CTA
 constexpr int kKnnSmemLevels = SMB_KNN_SMEM_LEVELS;    // tree levels staged in shared memory: 2^11 * 9 B = 18 KB
 constexpr int kKnnCtasPerSm = 1024 / kKnnCtaThreads;   // 64 registers per thread -> 1024 threads per SM
@@ -60,8 +57,8 @@ struct SmemTree {
   const double2* g_node;    // global, packed {cut, dim} of heap node h at slot h + 1 (one 16-byte load per node)
   const double* pb;         // padded buckets
   int levels;
-  double* sq;               // this thread's query: sq[d * kKnnCtaThreads] (shared memory, d = 0..2)
-  double* so;               // this thread's off[] of the recursion, same layout
+  double* sq;               // this thread's query: sq[d * kKnnCtaThreads] (shared memory, d = 0..2), and
+                            // its off[] of the recursion right behind it: sq[(3 + d) * kKnnCtaThreads]
 };
 
 // ---- mbarrier + bulk async copy (TMA engine, non-tensor form) --------------------------------
@@ -126,7 +123,6 @@ __device__ __forceinline__ SmemTree stage_tree(const KdCompact& t, unsigned char
   st.s_cut = s_cut; st.s_dim = s_dim; st.n_smem = slots;
   st.g_cut = t.cut; st.g_dim = t.dim; st.g_node = t.node; st.pb = t.pb; st.levels = t.levels;
   st.sq = *extra_out + 16 + threadIdx.x;
-  st.so = st.sq + 3 * kKnnCtaThreads;
   return st;
 }
 
@@ -216,80 +212,88 @@ __device__ __forceinline__ void scan_bucket(const double* __restrict__ pb, int b
 #endif
 }
 
-constexpr int kKnnMaxStack = 32;
-constexpr int kKnnMaxLevels = 24;        // sm_api rejects deeper trees
+// Far-side state of a query, with no stack.  Pushes during a descent come in increasing level order and a
+// pop takes the deepest pending entry, so everything still pending after a pop at level j lies above j and
+// the next descent pushes only below it: at most one pending far child per level, the sibling of the current
+// path's node one level down.  The whole state is therefore the current leaf (hp1 = heap index + 1, ll = its
+// level: hp1 >> (ll - a) is the path node of level a, plus one), a `pending` bit per level and a `turns` bit
+// per level (the path went to the FAR child there).  rd and off[] change only at turns, so those of a popped
+// far child are replayed exactly over the turns above it (knn_pop).  Bit a of a mask = path level a.
+constexpr int kKnnMaxLevels = 24;        // sm_api rejects deeper trees (the masks have one bit per level)
+
+// A path node: from the staged levels in shared memory when it is one of them, else one packed record (L1).
+__device__ __forceinline__ void path_node(const SmemTree& t, int n, double& cut, int& dim) {
+  if (n < t.n_smem) { cut = t.s_cut[n]; dim = t.s_dim[n]; }
+  else ldg_node(t.g_node, n, cut, dim);
+}
 
 // The coordinate of the query / the recursion's off[] along a node's cut dimension are read from
 // per-thread shared-memory columns indexed by that dimension (one LDS instead of a three-way select
 // on register pairs: the descent loop of a far visit shrank from 69 to ~30 SASS instructions a level).
-struct KnnStackEntry {
-  double rd;
-  double o[3];
-  int h, pad;
-};
-
-// recurseKnn on the subtree rooted at heap node h with the recursion's rd at entry; its off[] is in
-// t.so.  Near child first; a far child is pushed if it passes rd_new*(1+eps)^2 < head now (the head
-// only shrinks) and re-tested when popped, which is when the recursion tests it.  Far subtrees start
-// deep in the tree: nodes come through the read-only path (L1).
-__device__ __forceinline__ void visit_subtree(const SmemTree& t, double qx, double qy, double qz, double me2,
-                                              int h, double rd, double& head, int& best) {
-  KnnStackEntry stack[kKnnMaxStack];
-  int sp = 0;
-  while (true) {
-    int l = 31 - __clz(h + 1);
-#if SMB_KNN_PAIR_PREFETCH
-    double cut = 0.0; int cd = 3;
-    if (l < t.levels) ldg_node(t.g_node, h, cut, cd);
-#endif
-    while (l < t.levels) {
-#if SMB_KNN_PAIR_PREFETCH
-      if (cd == 3) break;
-      Double4 ch = {0.0, 0.0, 0.0, 0.0};                       // both children, fetched while this node is decided
-      if (l + 1 < t.levels) ch = ldg_nc_f64x4(t.g_node + 2 * (h + 1));
-#else
+//
+// Pop: the deepest pending level j, and the rd / off[] the recursion had for its far child, replayed from
+// rd = 0, off = 0 over the turn levels above j and then j itself with the recursion's own operations
+// (rd += -old_off^2 + new_off^2, off[cd] = new_off), so rd is bit-identical to what the recursion computed
+// when it pushed that child; re-tested with the head of this moment, which is when the recursion tests it.
+// On success h is the far child, rd its rd, its off[] in t.sq, and the path turns at j.  false: nothing left.
+__device__ __forceinline__ bool knn_pop(const SmemTree& t, double me2, double head, int hp1, int ll,
+                                        uint32_t& pending, uint32_t& turns, int& h, double& rd) {
+  while (pending != 0u) {
+    const int j = 31 - __clz(pending);
+    pending &= ~(1u << j);
+    const uint32_t upto = (turns & ((1u << j) - 1u)) | (1u << j);
+    t.sq[3 * kKnnCtaThreads] = 0.0; t.sq[4 * kKnnCtaThreads] = 0.0; t.sq[5 * kKnnCtaThreads] = 0.0;
+    double r = 0.0;
+    uint32_t steps = upto;
+    do {
+      const int a = __ffs(steps) - 1;
+      steps &= steps - 1u;
       double cut; int cd;
-      ldg_node(t.g_node, h, cut, cd);
-      if (cd == 3) break;
-#endif
-      const double q = t.sq[cd * kKnnCtaThreads];
-      const double old_off = t.so[cd * kKnnCtaThreads];
-      const double new_off = dsub(q, cut);
-      const double rd_new = dadd(rd, dadd(-dmul(old_off, old_off), dmul(new_off, new_off)));
-      const int right = q > cut ? 1 : 0;              // == (q - cut > 0) for IEEE doubles
-      if (dmul(rd_new, me2) < head && sp < kKnnMaxStack) {
-        KnnStackEntry& e = stack[sp++];
-        e.rd = rd_new;
-        e.o[0] = t.so[0]; e.o[1] = t.so[kKnnCtaThreads]; e.o[2] = t.so[2 * kKnnCtaThreads];
-        e.o[cd] = new_off;
-        e.h = 2 * h + 2 - right;
-      }
-      h = 2 * h + 1 + right;
-      ++l;
-#if SMB_KNN_PAIR_PREFETCH
-      cut = right ? ch.c : ch.a;
-      cd = (int)__double_as_longlong(right ? ch.d : ch.b);
-#endif
+      path_node(t, (hp1 >> (ll - a)) - 1, cut, cd);
+      const double old_off = t.sq[(3 + cd) * kKnnCtaThreads];
+      const double new_off = dsub(t.sq[cd * kKnnCtaThreads], cut);
+      r = dadd(r, dadd(-dmul(old_off, old_off), dmul(new_off, new_off)));
+      t.sq[(3 + cd) * kKnnCtaThreads] = new_off;
+    } while (steps != 0u);
+    if (dmul(r, me2) < head) {
+      h = ((hp1 >> (ll - j - 1)) ^ 1) - 1;             // sibling of the path node of level j + 1
+      rd = r;
+      turns = upto;
+      return true;
     }
-    scan_bucket(t.pb, (h + 1 - (1 << l)) << (t.levels - l), SMB_KNN_Q(t, qx, 0), SMB_KNN_Q(t, qy, 1), SMB_KNN_Q(t, qz, 2), head, best);
-    bool found = false;
-    while (sp > 0) {
-      const KnnStackEntry& e = stack[--sp];
-      if (dmul(e.rd, me2) < head) {
-        h = e.h; rd = e.rd;
-        t.so[0] = e.o[0]; t.so[kKnnCtaThreads] = e.o[1]; t.so[2 * kKnnCtaThreads] = e.o[2];
-        found = true;
-        break;
-      }
-    }
-    if (!found) break;
   }
+  return false;
+}
+
+// recurseKnn's descent from heap node h (rd at entry, off[] in its t.sq column): near child first down to a leaf; a far
+// child that passes rd_new*(1+eps)^2 < head now (the head only shrinks) sets the pending bit of its parent's
+// level.  Far subtrees start deep in the tree: nodes come through the read-only path (L1).  Leaves the new
+// path in hp1 / ll and returns the leaf's bucket.
+__device__ __forceinline__ int knn_descend(const SmemTree& t, double me2, double head, int h, double rd,
+                                           uint32_t& pending, int& hp1, int& ll) {
+  int l = 31 - __clz(h + 1);
+  while (l < t.levels) {
+    double cut; int cd;
+    ldg_node(t.g_node, h, cut, cd);
+    if (cd == 3) break;
+    const double q = t.sq[cd * kKnnCtaThreads];
+    const double old_off = t.sq[(3 + cd) * kKnnCtaThreads];
+    const double new_off = dsub(q, cut);
+    const double rd_new = dadd(rd, dadd(-dmul(old_off, old_off), dmul(new_off, new_off)));
+    const int right = q > cut ? 1 : 0;              // == (q - cut > 0) for IEEE doubles
+    if (dmul(rd_new, me2) < head) pending |= 1u << l;
+    h = 2 * h + 1 + right;
+    ++l;
+  }
+  hp1 = h + 1; ll = l;
+  return (h + 1 - (1 << l)) << (t.levels - l);
 }
 
 // First visit of a query: the descent from the root (staged levels from shared memory, the rest one
 // packed record per level), the first bucket, and the mask of the path levels whose far side passes
-// with the head that bucket left.  Path node of level a: ((hp1) >> (ll-a)) - 1.  rd = 0 and off = 0
-// along the whole root path, so rd_new(a) = 0 + (-(0*0) + new_off^2) = new_off^2 exactly.
+// with the head that bucket left, each tested exactly (node re-read: shared memory or L1).  rd = 0 and
+// off = 0 along the whole root path, so rd_new(a) = 0 + (-(0*0) + off^2) = off^2 exactly, and the pop
+// re-tests every level of the mask with the head of its moment.
 template <bool kAllSmem>
 __device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, double qy, double qz, double me2,
                                                double& head, int& best, int& hp1_out, int& ll_out, uint32_t& mask_out) {
@@ -297,20 +301,12 @@ __device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, dou
   best = -1;
   t.sq[0] = qx; t.sq[kKnnCtaThreads] = qy; t.sq[2 * kKnnCtaThreads] = qz;
   const int lsm = kAllSmem ? t.levels : min(t.levels, kKnnSmemLevels);    // levels staged in shared memory
-  // lb[a]: the squared distance to the cutting plane of path level a, rounded DOWN to float while the
-  // descent has the node in hand.  RN(lb * me2) <= RN(off^2 * me2), so "lb * me2 < head" holds whenever the
-  // exact test does: the mask below is a superset of the levels that pass, and every level of it is
-  // re-tested exactly (node re-read) at the moment the recursion would test it.  The array lives in local
-  // memory; all lanes of a warp store / load the same level together (one 128-byte line per access).
-  float lb[kKnnMaxLevels];
   int h = 0, l = 0;
   bool leaf = false;
   while (l < lsm) {
     const int cd = t.s_dim[h];
     if (cd == 3) { leaf = true; break; }
-    const double q = t.sq[cd * kKnnCtaThreads], off = dsub(q, t.s_cut[h]);
-    lb[l] = __double2float_rd(dmul(off, off));
-    h = 2 * h + 1 + (off > 0.0 ? 1 : 0);              // == (q > cut) for IEEE doubles
+    h = 2 * h + 1 + (t.sq[cd * kKnnCtaThreads] > t.s_cut[h] ? 1 : 0);
     ++l;
   }
   if (!kAllSmem && !leaf) {
@@ -318,18 +314,19 @@ __device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, dou
       double cut; int cd;
       ldg_node(t.g_node, h, cut, cd);
       if (cd == 3) break;
-      const double q = t.sq[cd * kKnnCtaThreads], off = dsub(q, cut);
-      lb[l] = __double2float_rd(dmul(off, off));
-      h = 2 * h + 1 + (off > 0.0 ? 1 : 0);
+      h = 2 * h + 1 + (t.sq[cd * kKnnCtaThreads] > cut ? 1 : 0);
       ++l;
     }
   }
   scan_bucket(t.pb, (h + 1 - (1 << l)) << (t.levels - l), qx, qy, qz, head, best);
   const int hp1 = h + 1, ll = l;
   uint32_t mask = 0u;
-#pragma unroll 4
-  for (int a = 0; a < ll; ++a)
-    if (dmul((double)lb[a], me2) < head) mask |= 1u << a;
+  for (int a = 0; a < ll; ++a) {
+    double cut; int cd;
+    path_node(t, (hp1 >> (ll - a)) - 1, cut, cd);
+    const double off = dsub(t.sq[cd * kKnnCtaThreads], cut);
+    if (dmul(dmul(off, off), me2) < head) mask |= 1u << a;
+  }
   hp1_out = hp1; ll_out = ll; mask_out = mask;
 }
 
@@ -337,23 +334,11 @@ __device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, dou
 template <bool kAllSmem>
 __device__ __forceinline__ void knn1_smem(const SmemTree& t, double qx, double qy, double qz, double me2,
                                           int& best_out, double& d2_out) {
-  double head; int best, hp1, ll; uint32_t mask;
-  knn_root_visit<kAllSmem>(t, qx, qy, qz, me2, head, best, hp1, ll, mask);
-  // the levels of the mask deepest first, each re-tested with the head of that moment
-  while (mask != 0u) {
-    const int a = 31 - __clz(mask);
-    mask &= ~(1u << a);
-    const int n = (hp1 >> (ll - a)) - 1;
-    double cut; int cd;
-    ldg_node(t.g_node, n, cut, cd);
-    const double off = dsub(t.sq[cd * kKnnCtaThreads], cut);
-    const double rd_new = dmul(off, off);
-    if (dmul(rd_new, me2) < head) {
-      t.so[0] = 0.0; t.so[kKnnCtaThreads] = 0.0; t.so[2 * kKnnCtaThreads] = 0.0;
-      t.so[cd * kKnnCtaThreads] = off;
-      const int near_p1 = hp1 >> (ll - a - 1);       // path node of level a+1, plus one
-      visit_subtree(t, qx, qy, qz, me2, (near_p1 ^ 1) - 1, rd_new, head, best);
-    }
+  double head, rd; int best, hp1, ll, h; uint32_t pending, turns = 0u;
+  knn_root_visit<kAllSmem>(t, qx, qy, qz, me2, head, best, hp1, ll, pending);
+  while (knn_pop(t, me2, head, hp1, ll, pending, turns, h, rd)) {
+    const int bucket = knn_descend(t, me2, head, h, rd, pending, hp1, ll);
+    scan_bucket(t.pb, bucket, SMB_KNN_Q(t, qx, 0), SMB_KNN_Q(t, qy, 1), SMB_KNN_Q(t, qz, 2), head, best);
   }
   best_out = best;
   d2_out = head;
@@ -361,94 +346,48 @@ __device__ __forceinline__ void knn1_smem(const SmemTree& t, double qx, double q
 
 // ---- far visits of a batch of queries, one WARP working through a list ---------------------------
 // A query whose root visit left far-side candidates (knn_root_visit's mask != 0) is parked as a
-// KnnItem; the lanes of the warp then pull items from the list.  Every pass of the loop below is ONE
-// bucket visit per busy lane — the next subtree of the lane's query (a nested far child popped from its
-// stack, else the next root-path level of the mask, both re-tested with the head of that moment exactly
-// as recurseKnn tests them), the descent into it with far children pushed, the bucket — and a lane
-// whose query is finished takes the next item in the same pass.  The per-query visit order is the
-// recursion's; only WHICH lane runs a query and when is different, so results are bit-identical.
-// Static one-query-per-lane scheduling leaves 13 of 32 lanes busy (the visit count per query is 1..29,
-// mean 2.9); here the bucket scans and descents of a pass run with most lanes busy.
+// KnnItem (its leaf and mask; a parked query has no turns); the lanes of the warp then pull items from
+// the list.  Every pass of the loop below is ONE bucket visit per busy lane — the next subtree of the
+// lane's query (knn_pop, as knn1_smem pops it), the descent into it, the bucket — and a lane whose query
+// is finished takes the next item in the same pass.  The per-query visit order is the recursion's; only
+// WHICH lane runs a query and when is different, so results are bit-identical.  Static one-query-per-lane
+// scheduling leaves 13 of 32 lanes busy (the visit count per query is 1..29, mean 2.9); here the bucket
+// scans and descents of a pass run with most lanes busy.
 struct KnnItem { int i, hp1, ll; uint32_t mask; };      // 16 bytes
 
 template <typename LoadQuery, typename StoreResult>
 __device__ __forceinline__ void knn_far_phase(const SmemTree& t, double me2, const int4* __restrict__ items,
                                               int n_items, LoadQuery load_query, StoreResult store_result) {
   const unsigned lt = (1u << (threadIdx.x & 31)) - 1u;
-  KnnStackEntry stack[kKnnMaxStack];
-  int sp = 0, next = 0;
-  bool have = false;
-  int qi = 0, hp1 = 1, ll = 0, best = -1;
-  uint32_t mask = 0u;
-  double head = 0.0, qx = 0.0, qy = 0.0, qz = 0.0;
+  int next = 0;
+  int qi = -1, hp1 = 1, ll = 0, best = -1;            // qi < 0: the lane has no query
+  uint32_t pending = 0u, turns = 0u;
+  double head = 0.0;
   while (true) {
-    const unsigned need = __ballot_sync(0xffffffffu, !have);
-    if (!have) {
+    const unsigned need = __ballot_sync(0xffffffffu, qi < 0);
+    if (qi < 0) {
       const int idx = next + __popc(need & lt);
       if (idx < n_items) {
         const int4 it = __ldcg(items + idx);
-        qi = it.x; hp1 = it.y; ll = it.z; mask = (uint32_t)it.w;
+        qi = it.x; hp1 = it.y; ll = it.z; pending = (uint32_t)it.w; turns = 0u;
+        double qx, qy, qz;
         load_query(qi, qx, qy, qz, head, best);
         t.sq[0] = qx; t.sq[kKnnCtaThreads] = qy; t.sq[2 * kKnnCtaThreads] = qz;
-        sp = 0;
-        have = true;
       }
     }
     next += __popc(need);
-    if (!__any_sync(0xffffffffu, have)) break;
+    if (!__any_sync(0xffffffffu, qi >= 0)) break;
     bool go = false;
     int h = 0;
     double rd = 0.0;
-    if (have) {
-      while (sp > 0) {                                 // nested far children first (the recursion is inside them)
-        const KnnStackEntry& e = stack[--sp];
-        if (dmul(e.rd, me2) < head) {
-          h = e.h; rd = e.rd;
-          t.so[0] = e.o[0]; t.so[kKnnCtaThreads] = e.o[1]; t.so[2 * kKnnCtaThreads] = e.o[2];
-          go = true;
-          break;
-        }
-      }
-      while (!go && mask != 0u) {                      // then the root path, deepest level first
-        const int a = 31 - __clz(mask);
-        mask &= ~(1u << a);
-        const int n = (hp1 >> (ll - a)) - 1;
-        double cut; int cd;
-        ldg_node(t.g_node, n, cut, cd);
-        const double off = dsub(t.sq[cd * kKnnCtaThreads], cut);
-        const double rd_new = dmul(off, off);
-        if (dmul(rd_new, me2) < head) {
-          t.so[0] = 0.0; t.so[kKnnCtaThreads] = 0.0; t.so[2 * kKnnCtaThreads] = 0.0;
-          t.so[cd * kKnnCtaThreads] = off;
-          h = ((hp1 >> (ll - a - 1)) ^ 1) - 1;         // sibling of the path node of level a + 1
-          rd = rd_new;
-          go = true;
-        }
-      }
-      if (!go) { store_result(qi, best, head); have = false; }
+    if (qi >= 0) {
+      go = knn_pop(t, me2, head, hp1, ll, pending, turns, h, rd);
+      if (!go) { store_result(qi, best, head); qi = -1; }
     }
     if (go) {
-      int l = 31 - __clz(h + 1);
-      while (l < t.levels) {
-        double cut; int cd;
-        ldg_node(t.g_node, h, cut, cd);
-        if (cd == 3) break;
-        const double q = t.sq[cd * kKnnCtaThreads];
-        const double old_off = t.so[cd * kKnnCtaThreads];
-        const double new_off = dsub(q, cut);
-        const double rd_new = dadd(rd, dadd(-dmul(old_off, old_off), dmul(new_off, new_off)));
-        const int right = q > cut ? 1 : 0;
-        if (dmul(rd_new, me2) < head && sp < kKnnMaxStack) {
-          KnnStackEntry& e = stack[sp++];
-          e.rd = rd_new;
-          e.o[0] = t.so[0]; e.o[1] = t.so[kKnnCtaThreads]; e.o[2] = t.so[2 * kKnnCtaThreads];
-          e.o[cd] = new_off;
-          e.h = 2 * h + 2 - right;
-        }
-        h = 2 * h + 1 + right;
-        ++l;
-      }
-      scan_bucket(t.pb, (h + 1 - (1 << l)) << (t.levels - l), qx, qy, qz, head, best);
+      const int bucket = knn_descend(t, me2, head, h, rd, pending, hp1, ll);
+      // the query from its shared-memory column: six registers fewer across the loop, no spills
+      scan_bucket(t.pb, bucket, t.sq[0], t.sq[kKnnCtaThreads], t.sq[2 * kKnnCtaThreads], head, best);
     }
   }
 }
@@ -467,9 +406,10 @@ __device__ __forceinline__ void knn_batch_cta(const SmemTree& tree, int begin, i
                                               Unpark unpark, Finish finish) {
   const int warp = threadIdx.x >> 5;
   const unsigned lt = (1u << (threadIdx.x & 31)) - 1u;
-  const int qpt = min(kKnnMaxQpt, per_cta / kKnnCtaThreads);
-  for (int base = begin; base < end; base += kKnnCtaThreads * qpt) {
-    const int qb = min(qpt, (begin + per_cta - base) / kKnnCtaThreads);
+  // qb: the batch's queries per thread, min(qpt, what is left of the range) with qpt = min(kKnnMaxQpt,
+  // per_cta / 256); what is left never exceeds per_cta / 256, so qpt itself need not be held across the far phase
+  for (int base = begin, qb; base < end; base += kKnnCtaThreads * qb) {
+    qb = min(kKnnMaxQpt, (begin + per_cta - base) / kKnnCtaThreads);
     int4* items = items_all + base + warp * 32 * qb;
     int count = 0;
     for (int j = 0; j < qb; ++j) {
