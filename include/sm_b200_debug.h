@@ -23,8 +23,8 @@
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
  *                              (queries_per_cta > 256: lockstep root visits, then the lanes of a warp pull parked
  *                              searches), so that path's index sets and squared distances meet the oracle's directly
- *     sm_debug_ndt_grid        the NDT target grid as ndt_build_grid leaves it: voxel keys, leaves, size guard
- *     sm_debug_ndt_derivatives the 44 sums of ndt_eval (computeDerivatives) at given pose vectors, both term forms
+ *     sm_debug_ndt_grid        the NDT target grid as NdtStage::build_grid leaves it: voxel keys, leaves, size guard
+ *     sm_debug_ndt_derivatives the 44 sums of NdtStage::eval (computeDerivatives) at given pose vectors, both forms
  *     sm_debug_float_tree_knn  the float tree's exact searches: knn1 (eps = 0) and the 20-NN of the covariances
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
@@ -151,19 +151,20 @@ int sm_debug_ndt_term(const double* p_6, double outlier_ratio, float resolution,
                       const float* x_orig_3, const float* x_trans_3, const double* voxel_mean_3,
                       const double* voxel_icov_9, double* out43);
 
-/* ---- the device stages of Ndt and NdtWithGicp, each run by the product's own launch functions (csrc/ndt.cu,
- * csrc/gicp.cu, csrc/kdtree.cu) on buffers of the hook's own.  Clouds are packed float xyz; 4x4 matrices are
- * column-major; every output array is sized by the caller for the worst case stated. */
+/* ---- the device stages of Ndt and NdtWithGicp, each run by the owner sm_align runs it with (NdtStage in
+ * csrc/ndt.cu, ApproxVoxelGrid and gicp::Stage in csrc/gicp.cu, FloatTree in csrc/kdtree.cu) on buffers of the
+ * hook's own.  Clouds are packed float xyz; 4x4 matrices are column-major; every output array is sized by the
+ * caller for the worst case stated. */
 
-/* ndt_build_grid (VoxelGridCovariance::filter(true)): the voxels in the device's order (ascending voxel index as
+/* NdtStage::build_grid (VoxelGridCovariance::filter(true)): the voxels in the device's order (ascending voxel index as
  * a 32-bit unsigned key), each array holding up to n entries.  overflow = 1: the target's box holds more than
  * INT32_MAX voxels (voxel_grid_covariance_omp_impl.hpp:74-84) and the grid is unusable. */
 int sm_debug_ndt_grid(int device, const float* target_3n, int64_t n, float resolution, int32_t* n_voxels,
                       int32_t* overflow, int32_t* key, int32_t* nr_points, int32_t* searchable, double* mean_3,
                       double* icov_9, float* centroid_3);
 
-/* ndt_build_grid, then ndt_eval (computeDerivatives) at each of the n_poses pose vectors p, with the evaluation
- * parameters sm_debug_ndt_term builds; f64_math = 1: the stock-PCL double term math.  sums_44k[44 k ..]: score,
+/* NdtStage::build_grid, then NdtStage::eval (computeDerivatives) at each of the n_poses pose vectors p, with the
+ * evaluation parameters sm_debug_ndt_term builds; f64_math = 1: the stock-PCL double term math.  sums_44k[44 k ..]: score,
  * gradient[6], Hessian[36] row-major, neighbour count. */
 int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, const float* source_3n, int64_t ns,
                       float resolution, double outlier_ratio, int32_t f64_math, const double* p_6k, int32_t n_poses,
@@ -175,17 +176,17 @@ int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, con
 int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const double* query_3m, int64_t nq,
                             int32_t k, int32_t* ids, double* d2);
 
-/* approx_voxel_grid + approx_voxel_grid_emit (pcl::ApproximateVoxelGrid): *m_out points into out_3n (capacity n). */
+/* ApproxVoxelGrid::filter (pcl::ApproximateVoxelGrid): *m_out points into out_3n (capacity n). */
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,
                                int64_t* m_out);
 
-/* the cloud's own float tree + gicp_covariances (computeCovariances, k = 20, epsilon 1e-3): n row-major 3x3;
+/* the cloud's own float tree + gicp::Stage::covariances (computeCovariances, k = 20, epsilon 1e-3): n row-major 3x3;
  * zeros for fewer than 20 points, as the GICP stage leaves them. */
 int sm_debug_gicp_covariances(int device, const float* cloud_3n, int64_t n, double* covs_9n);
 
-/* One GICP outer iteration's device work: the covariances of both clouds, gicp_correspond for transformation_
- * with R = rot(transformation_ * guess) formed as the outer loop forms it, then gicp_cost at each of the n_states
- * states x (T = guess with applyState(x)), in sequence on one last-block ticket.  match[ns]: target index or -1;
+/* One GICP outer iteration's device work (gicp::Stage): the covariances of both clouds, the correspondences for
+ * transformation_ with R = rot(transformation_ * guess) from gicp::outer_rotation, then the cost at each of the
+ * n_states states x (T = guess with applyState(x)), in sequence on one last-block ticket.  match[ns]: target index or -1;
  * maha_9n: the Mahalanobis matrix of each matched source point (row-major); *count: matches;
  * sums_13k[13 k ..]: sum res^T M res, sum M res[3], sum (guess p)(M res)^T[9] row-major. */
 int sm_debug_gicp_step(int device, const float* source_3n, int64_t ns, const float* target_3n, int64_t nt,

@@ -16,6 +16,7 @@
 //                       the 3x3 matrix R that computeRDerivative contracts; 13 double sums.
 // Compiled with -fmad=false (same operation order as oracle/gicp_oracle.cc).
 #include "common.cuh"
+#include "gicp_host.h"
 #include "icp_dev.cuh"
 #include "kernels.h"
 #include "linalg_dev.cuh"
@@ -424,17 +425,16 @@ void gicp_debug_cost_terms_host(const float* T, const float* base, const float* 
   cost_terms(T, base, ps, pt, M, acc13);
 }
 
-size_t approx_ws_bytes(int n) {
+// pcl::ApproximateVoxelGrid::filter: keys, runs and centroids, then (with the run count on the host to size the
+// sort) the runs in emission order
+int ApproxVoxelGrid::filter(const float* pts, int n, float leaf, DevBuf& out, int* m_out, cudaStream_t stream) {
   const int64_t st = (n + 63) & ~63;
-  return (size_t)(4 * st * sizeof(uint64_t) + 4 * st * sizeof(uint32_t) + (st + 64) * sizeof(uint32_t) +
-                  3 * st * sizeof(float) + radix_sort_scratch_bytes(n, 1) + 8192);
-}
-
-// out: packed float xyz (capacity n points); *n_out_dev: number of output points (device)
-int approx_voxel_grid(const float* pts, int n, float leaf, void* ws_base, float* out, uint32_t* n_out_dev,
-                      cudaStream_t stream) {
-  const int64_t st = (n + 63) & ~63;
-  char* p = (char*)ws_base;
+  SMB_RC(ws.reserve((size_t)(4 * st * sizeof(uint64_t) + 4 * st * sizeof(uint32_t) + (st + 64) * sizeof(uint32_t) +
+                             3 * st * sizeof(float) + radix_sort_scratch_bytes(n, 1) + 8192)));
+  SMB_RC(out.reserve((size_t)n * 12 + 64));
+  SMB_RC(counter.reserve(64));
+  uint32_t* n_out_dev = (uint32_t*)counter.p;
+  char* p = (char*)ws.p;
   auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) & ~(size_t)255; return r; };
   uint64_t* keys0 = (uint64_t*)take(st * 8); uint64_t* keys1 = (uint64_t*)take(st * 8);
   uint64_t* ekey0 = (uint64_t*)take(st * 8); uint64_t* ekey1 = (uint64_t*)take(st * 8);
@@ -445,65 +445,81 @@ int approx_voxel_grid(const float* pts, int n, float leaf, void* ws_base, float*
   uint32_t* scratch = (uint32_t*)take(radix_sort_scratch_bytes(n, 1) + 4096);
   const float inv = 1.0f / leaf;
   approx_key_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(pts, n, inv, keys0, ord0);
-  int rc = radix_sort_pairs_u64(keys0, ord0, keys1, ord1, n, 1, st, scratch, stream, 2);
-  if (rc) return rc;
+  SMB_RC(radix_sort_pairs_u64(keys0, ord0, keys1, ord1, n, 1, st, scratch, stream, 2));
   const int nblk = ceil_div(n, kRTile);
   approx_heads_count_kernel<<<nblk, kRT, 0, stream>>>(pts, ord0, keys0, n, inv, scratch);
   radix_scan_kernel_launch(scratch, nblk, 1, stream);
   approx_heads_scatter_kernel<<<nblk, kRT, 0, stream>>>(pts, ord0, keys0, n, inv, scratch, nblk, run_start, n_out_dev);
   approx_run_kernel<<<ceil_div(n, 128), 128, 0, stream>>>(pts, ord0, keys0, run_start, n_out_dev, n, centroid, ekey0, eval0);
-  // runs beyond n_runs must sort last: pre-fill is not needed because only the first n_runs keys
-  // are read back, but the sort works on n entries -> set the tail keys to the maximum
+  SMB_CUDA_OK(cudaGetLastError());
+  uint32_t m = 0;
+  SMB_CUDA_OK(cudaMemcpyAsync(&m, n_out_dev, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+  SMB_CUDA_OK(cudaStreamSynchronize(stream));
+  *m_out = (int)m;
+  if (m == 0) return 0;
+  SMB_RC(radix_sort_pairs_u64(ekey0, eval0, ekey1, eval1, (int)m, 1, st, scratch, stream, 4));
+  approx_emit_kernel<<<ceil_div(m, 256), 256, 0, stream>>>(centroid, eval0, n_out_dev, (float*)out.p);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-// second half (needs the run count on the host to size the sort): order the runs by emission key
-int approx_voxel_grid_emit(int n, int n_runs, void* ws_base, float* out, const uint32_t* n_out_dev,
-                           cudaStream_t stream) {
-  const int64_t st = (n + 63) & ~63;
-  char* p = (char*)ws_base;
-  auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) & ~(size_t)255; return r; };
-  take(st * 8); take(st * 8);
-  uint64_t* ekey0 = (uint64_t*)take(st * 8); uint64_t* ekey1 = (uint64_t*)take(st * 8);
-  take(st * 4); take(st * 4);
-  uint32_t* eval0 = (uint32_t*)take(st * 4); uint32_t* eval1 = (uint32_t*)take(st * 4);
-  take((st + 64) * 4);
-  float* centroid = (float*)take(3 * st * 4);
-  uint32_t* scratch = (uint32_t*)take(radix_sort_scratch_bytes(n, 1) + 4096);
-  if (n_runs <= 0) return 0;
-  int rc = radix_sort_pairs_u64(ekey0, eval0, ekey1, eval1, n_runs, 1, st, scratch, stream, 4);
-  if (rc) return rc;
-  approx_emit_kernel<<<ceil_div(n_runs, 256), 256, 0, stream>>>(centroid, eval0, n_out_dev, out);
+static int cost_blocks(int ns) { return ceil_div(ns, 256); }
+
+int gicp::Stage::reserve(int ns, int nt, cudaStream_t stream) {
+  SMB_RC(cov_s.reserve((size_t)ns * 9 * sizeof(double)));
+  SMB_RC(cov_t.reserve((size_t)nt * 9 * sizeof(double)));
+  SMB_RC(maha.reserve((size_t)ns * 9 * sizeof(double)));
+  SMB_RC(match.reserve((size_t)ns * sizeof(int32_t)));
+  SMB_RC(partials.reserve((size_t)(cost_blocks(ns) + 1) * kCostSums * sizeof(double) + 256));
+  SMB_RC(counter.reserve(64));
+  sums = (double*)partials.p + (size_t)cost_blocks(ns) * kCostSums;
+  ticket = (uint32_t*)counter.p + 8;
+  SMB_CUDA_OK(cudaMemsetAsync(ticket, 0, sizeof(uint32_t), stream));
+  seq = 0;
+  return 0;
+}
+
+int gicp::Stage::covariances(const gicp::Options& o, const float* cloud, int n, const FloatTree& t, const DevBuf& out,
+                             cudaStream_t stream) const {
+  if (o.k_correspondences > n) {   // gicp_omp_impl.hpp:61-65: PCL_ERROR and the covariances stay unset
+    SMB_CUDA_OK(cudaMemsetAsync(out.p, 0, (size_t)n * 9 * sizeof(double), stream));
+    return 0;
+  }
+  gicp_knn20_cov_kernel<<<ceil_div(n, 64), 64, 0, stream>>>(cloud, n, (const KdNode*)t.nodes.p,
+                                                           (const BucketPoint*)t.bpts.p, o.gicp_epsilon,
+                                                           (double*)out.p);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-int gicp_covariances(const float* cloud, int n, const KdNode* nodes, const BucketPoint* bpts, double eps,
-                     double* covs, cudaStream_t stream) {
-  gicp_knn20_cov_kernel<<<ceil_div(n, 64), 64, 0, stream>>>(cloud, n, nodes, bpts, eps, covs);
-  SMB_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-int gicp_correspond(const float* src, int ns, const float* tgt, const GicpIterParams& P, const KdNode* nodes,
-                    const BucketPoint* bpts, const double* cov_s, const double* cov_t, int32_t* match,
-                    double* maha, uint32_t* count, cudaStream_t stream) {
+int gicp::Stage::correspond(const gicp::Options& o, const float* src, int ns, const float* tgt, const FloatTree& tt,
+                            const float* guess, const float* transformation, const double* R, cudaStream_t stream,
+                            int* m) {
+  GicpIterParams P;
+  for (int i = 0; i < 16; ++i) { P.guess[i] = guess[i]; P.transformation[i] = transformation[i]; }
+  for (int q = 0; q < 9; ++q) P.R[q] = R[q];
+  P.dist_threshold = o.corr_dist_threshold * o.corr_dist_threshold;
+  uint32_t* count = (uint32_t*)counter.p;
   SMB_CUDA_OK(cudaMemsetAsync(count, 0, sizeof(uint32_t), stream));
-  gicp_correspond_kernel<<<ceil_div(ns, 128), 128, 0, stream>>>(src, ns, tgt, P, nodes, bpts, cov_s, cov_t,
-                                                               match, maha, count);
+  gicp_correspond_kernel<<<ceil_div(ns, 128), 128, 0, stream>>>(src, ns, tgt, P, (const KdNode*)tt.nodes.p,
+                                                               (const BucketPoint*)tt.bpts.p, (const double*)cov_s.p,
+                                                               (const double*)cov_t.p, (int32_t*)match.p,
+                                                               (double*)maha.p, count);
   SMB_CUDA_OK(cudaGetLastError());
+  uint32_t mu = 0;
+  SMB_CUDA_OK(cudaMemcpyAsync(&mu, count, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+  SMB_CUDA_OK(cudaStreamSynchronize(stream));
+  *m = (int)mu;
   return 0;
 }
 
-int gicp_cost_blocks(int ns) { return ceil_div(ns, 256); }
-
-int gicp_cost(const float* src, int ns, const float* tgt, const GicpCostParams& P, const int32_t* match,
-              const double* maha, double* partials, double* sums, uint32_t* ticket, double* host_sums_dev,
-              long long* host_flag_dev, long long seq, cudaStream_t stream) {
-  const int nb = gicp_cost_blocks(ns);
-  gicp_cost_kernel<<<nb, 256, 0, stream>>>(src, ns, tgt, P, match, maha, partials, sums, ticket, host_sums_dev,
-                                          host_flag_dev, seq);
+int gicp::Stage::cost(const float* src, int ns, const float* tgt, const float* T, const float* base, double* host_sums,
+                      long long* host_seq, cudaStream_t stream) {
+  GicpCostParams P;
+  for (int i = 0; i < 16; ++i) { P.T[i] = T[i]; P.base[i] = base[i]; }
+  gicp_cost_kernel<<<cost_blocks(ns), 256, 0, stream>>>(src, ns, tgt, P, (const int32_t*)match.p, (const double*)maha.p,
+                                                       (double*)partials.p, sums, ticket, host_sums, host_seq,
+                                                       host_seq ? ++seq : 0);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -276,9 +276,19 @@ struct Minimizer {
 //       (column-major float 4x4) and R = rot(transformation_ * guess) in double, row-major; m = correspondences
 //   cost(T, S): the sums of one functor evaluation (:255-377) for T = base with applyState(x):
 //       S[0] = sum res^T M res, S[1..3] = sum M res, S[4..12] = sum (base p)(M res)^T row-major
-// both return < 0 on error (propagated as -1).  The device path passes lambdas around the kernels (sm_api.cu
-// gicp_run); the test hook sm_debug_gicp_outer passes a caller's functions, so this control flow — start vector,
-// f / g assembly, BFGS driver, convergence test, final composition — is exercised on the host.
+// both return < 0 on error (propagated as -1).  The device path passes lambdas around Stage's correspond and
+// cost (gicp_run of the C ABI); the test hook sm_debug_gicp_outer passes a caller's functions, so this control flow —
+// start vector, f / g assembly, BFGS driver, convergence test, final composition — is exercised on the host.
+// transform_R = transformation_ * guess in double (:423-429): its rotation, row-major, for the correspondences
+inline void outer_rotation(const float* transformation, const float* guess, double* R) {
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      double s = 0.0;
+      for (int k = 0; k < 4; ++k) s += (double)transformation[i + 4 * k] * (double)guess[k + 4 * j];
+      R[i * 3 + j] = s;
+    }
+}
+
 struct OuterOut {
   float final_T[16];
   int iterations = 0;
@@ -293,12 +303,7 @@ inline int outer_loop(const Options& o, const float* guess, Correspond correspon
   bool converged = false, callback_error = false;
   while (!converged) {
     double R[9];
-    for (int i = 0; i < 3; ++i)          // transform_R = transformation_ * guess in double (:423-429)
-      for (int j = 0; j < 3; ++j) {
-        double s = 0.0;
-        for (int k = 0; k < 4; ++k) s += (double)transformation[i + 4 * k] * (double)guess[k + 4 * j];
-        R[i * 3 + j] = s;
-      }
+    outer_rotation(transformation, guess, R);
     int m = 0;
     if (correspond(transformation, R, &m) < 0) return -1;
     for (int i = 0; i < 16; ++i) previous[i] = transformation[i];
@@ -366,6 +371,30 @@ inline int outer_loop(const Options& o, const float* guess, Correspond correspon
   out->bfgs_evals = evals;
   return 0;
 }
+
+// The device side of the GICP stage (gicp.cu): the source's float tree, both clouds' covariances, the matches with
+// their Mahalanobis matrices, and the cost kernel's partial sums, ticket and sequence number.  reserve() sizes the
+// buffers for ns source / nt target points, zeroes the ticket (each cost evaluation's last block resets it) and
+// restarts the sequence.
+struct Stage {
+  FloatTree source_tree;
+  DevBuf cov_s, cov_t, maha, match, partials, counter;   // counter: the match count, then the ticket
+  double* sums = nullptr;      // device: the 13 sums of the last cost evaluation
+  uint32_t* ticket = nullptr;
+  long long seq = 0;
+  int reserve(int ns, int nt, cudaStream_t stream);
+  // computeCovariances (:59-131) over the cloud's own tree t into out; zeros below k_correspondences points, where
+  // the reference logs an error and leaves them unset
+  int covariances(const Options& o, const float* cloud, int n, const FloatTree& t, const DevBuf& out,
+                  cudaStream_t stream) const;
+  // the per-point part of one outer iteration (:430-461) over the target's tree tt; waits for the match count m
+  int correspond(const Options& o, const float* src, int ns, const float* tgt, const FloatTree& tt, const float* guess,
+                 const float* transformation, const double* R, cudaStream_t stream, int* m);
+  // one functor evaluation (:255-377) at T; with host_sums / host_seq (device views of mapped pinned memory) the
+  // kernel also writes the 13 sums there, then the sequence number ++seq
+  int cost(const float* src, int ns, const float* tgt, const float* T, const float* base, double* host_sums,
+           long long* host_seq, cudaStream_t stream);
+};
 
 }  // namespace gicp
 }  // namespace smb

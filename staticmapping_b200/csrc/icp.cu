@@ -26,12 +26,14 @@ using namespace dev;
 namespace {
 
 // ------------------------------------------------------------------------------ prologue
+constexpr int kMeanChunk = 1024;   // target points per mean_partial_kernel block (4 per thread), 4 doubles out each
+
 __global__ void __launch_bounds__(256)
 mean_partial_kernel(const double* __restrict__ raw, int64_t stride, int n,
                     double* __restrict__ partials) {
   __shared__ double sm[3][8];
   double s[3] = {0.0, 0.0, 0.0};
-  const int base = blockIdx.x * 1024;
+  const int base = blockIdx.x * kMeanChunk;
   for (int r = 0; r < 4; ++r) {
     const int i = base + r * 256 + threadIdx.x;
     if (i < n) { s[0] += raw[i]; s[1] += raw[stride + i]; s[2] += raw[2 * stride + i]; }
@@ -343,7 +345,58 @@ knn_query_batch_kernel(KdCompact kc, const double* __restrict__ query, int64_t q
 
 }  // namespace
 
-int icp_accum_blocks(int n_source) { return ceil_div(n_source, kAccTile); }
+static int icp_accum_blocks(int n_source) { return ceil_div(n_source, kAccTile); }
+
+// a warp's item list may extend past the last query of the last batch
+size_t knn_items_bytes(int nq) { return ((size_t)nq + 4096) * sizeof(int4); }
+
+constexpr int kSumWords = 32;    // one record of normal-equation sums: kNumSums padded to 32 doubles
+constexpr int kCandWords = 8;    // one quantile-bin candidate: 6 Jacobian terms, the residual, sqrt(d2)
+// hist: the two histograms, 64 words of padding, then the iteration's sums record
+constexpr size_t kHistSumsOffset = (2 * kHistBins + 64) * sizeof(uint32_t);
+// slot: the per-point match slots, padded to 256 bytes, then the parked-search items
+static size_t slot_bytes(int ns) { return (((size_t)ns * sizeof(int32_t) + 64 + 255) / 256) * 256; }
+
+int IcpFastBuffers::reserve(int ns, int nt, int64_t sstride, int64_t tstride, bool inner_compensation) {
+  this->ns = ns; this->sstride = sstride; this->tstride = tstride;
+  const int nb = icp_accum_blocks(ns);
+  SMB_RC(tgt.reserve((size_t)(3 * tstride) * sizeof(double)));
+  SMB_RC(src0.reserve((size_t)(3 * sstride) * sizeof(double)));
+  SMB_RC(src_g0.reserve((size_t)(3 * sstride) * sizeof(double)));
+  SMB_RC(src_sort.reserve(RadixPairs::bytes(sstride, ns)));
+  SMB_RC(tree.reserve(nt, 8, KdCompactTree::kNormals));
+  SMB_RC(slot.reserve(slot_bytes(ns) + knn_items_bytes(ns)));
+  SMB_RC(d2.reserve((size_t)ns * sizeof(double)));
+  SMB_RC(hist.reserve(kHistSumsOffset + kSumWords * sizeof(double)));
+  SMB_RC(cand_terms.reserve((size_t)nb * kAccTile * kCandWords * sizeof(double)));
+  SMB_RC(cand_key.reserve((size_t)nb * kAccTile * sizeof(unsigned long long)));
+  SMB_RC(cand_cnt.reserve((size_t)nb * sizeof(uint32_t)));
+  SMB_RC(partials.reserve((size_t)nb * kSumWords * sizeof(double)));
+  SMB_RC(mean_partials.reserve((size_t)ceil_div(nt, kMeanChunk) * 4 * sizeof(double)));
+  SMB_RC(state.reserve(sizeof(IcpState)));
+  SMB_RC(guess.reserve(16 * sizeof(double)));
+  if (inner_compensation) SMB_RC(deskewed.reserve((size_t)(3 * sstride) * sizeof(double)));
+  return 0;
+}
+
+void IcpFastBuffers::fill(IcpBuffers& b, const double* tgt_raw, const double* nrm, const double* src_raw) const {
+  b.tgt = (double*)tgt.p; b.tgt_raw = (double*)tgt_raw; b.nrm = (double*)nrm;
+  b.tstride = tstride;
+  b.nodes = (KdNode*)tree.nodes.p; b.leaf_order = (uint32_t*)tree.leaf_order.p;
+  b.kc = tree.view();
+  b.src_raw = (double*)src_raw; b.src0 = (double*)src0.p; b.sstride = sstride;
+  b.src_g0 = (double*)src_g0.p;
+  b.src_sort.carve(src_sort.p, sstride);
+  b.slot = (int32_t*)slot.p;
+  b.knn_items = reinterpret_cast<int4*>((char*)slot.p + slot_bytes(ns));
+  b.d2 = (double*)d2.p; b.hist = (uint32_t*)hist.p;
+  b.hist2 = b.hist + kHistBins;
+  b.sums = (double*)((char*)hist.p + kHistSumsOffset);
+  b.cand_terms = (double*)cand_terms.p;
+  b.cand_key = (unsigned long long*)cand_key.p; b.cand_cnt = (uint32_t*)cand_cnt.p;
+  b.partials = (double*)partials.p; b.mean_partials = (double*)mean_partials.p;
+  b.state = (IcpState*)state.p;
+}
 
 // Launch geometry of the search kernels: `per_cta` consecutive queries per 256-thread CTA.
 // queries_per_cta == 0: one query per thread (120 000 queries = 469 CTAs, ~3 per SM, all
@@ -380,7 +433,7 @@ int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq,
 int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_dev,
                  KdWorkspace& ws, const KdCompactTree& tree, cudaStream_t stream) {
   const int nt = p.n_target, ns = p.n_source;
-  const int nparts = ceil_div(nt, 1024);
+  const int nparts = ceil_div(nt, kMeanChunk);
   mean_partial_kernel<<<nparts, 256, 0, stream>>>(b.tgt_raw, b.tstride, nt, b.mean_partials);
   center_kernel<<<ceil_div(nt, 256), 256, 0, stream>>>(b.tgt_raw, b.tgt, b.tstride, nt,
                                                       b.mean_partials, nparts, b.state);
@@ -399,8 +452,14 @@ int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_de
   return 0;
 }
 
+// kernel launches of icp_prologue with a target tree of `levels` levels: centring 2, tree build 27 + 5 per level,
+// init and G0 2, Morton sort and gather 13
+int icp_prologue_launches(int levels) { return 2 + 1 + 24 + levels * 5 + 1 + 1 + 2 + 13; }
+
 // Iterations start_iteration .. start_iteration+count-1 of one Align: three launches each, four with inner
 // compensation (the de-skew of the source goes first).
+int icp_iteration_launches(bool inner_compensation) { return inner_compensation ? 4 : 3; }
+
 template <bool kComp>
 void icp_enqueue_search(const IcpBuffers& b, const IcpParams& p, int grid, int per, size_t smem, cudaStream_t stream,
                         const double* deskewed) {

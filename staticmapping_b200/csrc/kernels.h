@@ -108,7 +108,6 @@ struct FloatTree {
 };
 
 // ---- icp.cu ----------------------------------------------------------------------------
-constexpr int kKnnItemSlack = 4096;   // a warp's item list may extend past the last query of the last batch
 constexpr int kHistBins = 2048;
 
 // Device-resident state of one IcpFast::Align call (one per handle).
@@ -163,7 +162,7 @@ struct IcpBuffers {
   int64_t sstride;
   // per-iteration
   int32_t* slot;          // [n_source] padded bucket entry of the match (kc.pb / kc.pn index)
-  int4* knn_items;        // [n_source + kKnnItemSlack] parked searches of the k-NN kernel's second phase (16 B each)
+  int4* knn_items;        // [knn_items_bytes(n_source)] parked searches of the k-NN kernel's second phase (16 B each)
   double* d2;             // [n_source]
   uint32_t* hist;         // [kHistBins] first-level histogram of dist^2 (phase A)
   uint32_t* hist2;        // [kHistBins] second-level histogram inside the quantile bin (phase B)
@@ -177,14 +176,30 @@ struct IcpBuffers {
   IcpState* state;
 };
 
-int icp_accum_blocks(int n_source);
+size_t knn_items_bytes(int nq);   // the parked searches of the batched k-NN kernels for nq queries
+
+// The device buffers of IcpFast's iterations and its target tree.  reserve() sizes them for ns source / nt target
+// points in SoA clouds of strides sstride / tstride (deskewed with inner compensation only); they only grow, so
+// clouds of the same size keep their pointers and the captured graphs.  fill() lays them out as IcpBuffers.
+struct IcpFastBuffers {
+  DevBuf tgt, src0, src_g0, src_sort, slot, d2, hist, cand_terms, cand_key, cand_cnt, partials, mean_partials, state,
+      guess, deskewed;
+  KdCompactTree tree;
+  int ns = 0;
+  int64_t sstride = 0, tstride = 0;
+  int reserve(int ns, int nt, int64_t sstride, int64_t tstride, bool inner_compensation);
+  void fill(IcpBuffers& b, const double* tgt_raw, const double* nrm, const double* src_raw) const;
+};
+
 // builds the target tree into `tree`, whose view is b.kc
 int icp_prologue(const IcpBuffers& b, const IcpParams& p, const double* guess_dev,
                  KdWorkspace& ws, const KdCompactTree& tree, cudaStream_t stream);
+int icp_prologue_launches(int tree_levels);
 // events (optional): 4 per iteration — before A, after A, after B, after C
 // deskewed: [3][sstride] doubles, the de-skewed source of the iteration; needed when p.inner_compensation
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
                            cudaStream_t stream, cudaEvent_t* events, double* deskewed = nullptr);
+int icp_iteration_launches(bool inner_compensation);
 void icp_finish_launch(const IcpBuffers& b, const IcpParams& p, int nblocks_b, cudaStream_t stream);
 // stand-alone k-NN over an already built tree (compact layout incl. pid): ids = original indices
 int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, double max_error2,
@@ -220,7 +235,6 @@ struct NdtEvalParams {      // everything one computeDerivatives call needs, by 
   double j_ang_d[8][3];     // the same tables in double (stock PCL keeps them as Vector3d)
   double h_ang_d[15][3];
 };
-uint32_t ndt_table_size(int nt);
 // host build of the leaf plane fit of normals.cu (test hook sm_debug_normals_leaf): 1 kept, 0 dropped, < 0 bad count
 int normals_debug_leaf_host(const double* members, int count, double* mean, double* unit);
 // host build of one target-grid leaf of ndt.cu (test hook sm_debug_ndt_leaf)
@@ -229,7 +243,6 @@ void ndt_debug_leaf_host(const float* pts, int n, int min_points, double eig_mul
 // host build of the per-(point, voxel) derivative term of ndt.cu (test hook sm_debug_ndt_term)
 void ndt_debug_term_host(const NdtEvalParams& P, const float* x_orig, const float* x_trans, const double* mean,
                          const double* icov, double* out43);
-int ndt_blocks(int n);
 struct NdtWorkspace {
   uint64_t* keys[2];
   uint32_t* order[2];
@@ -246,14 +259,23 @@ struct NdtWorkspace {
   float* sorted_pts;        // target points gathered into voxel order (packed xyz)
   NdtGrid* grid;
   int64_t stride;
-  static size_t bytes_needed(int nt, int ns);
-  void carve(void* base, int nt, int ns);
 };
-int ndt_build_grid(const float* tgt, int nt, float resolution, NdtWorkspace& ws, cudaStream_t stream);
-int ndt_eval(const float* src, int ns, const NdtEvalParams& P, NdtWorkspace& ws, cudaStream_t stream);
+// The NDT target grid and the evaluation sums of one Align, carved from one allocation sized by reserve() for nt
+// target / ns source points.  eval reads computeDerivatives' 44 sums (score, gradient, Hessian row-major, neighbour
+// count) back into host memory, fitness getFitnessScore's 2 (squared-distance sum, count) through sums2.
+struct NdtStage {
+  DevBuf buf;
+  NdtWorkspace ws;
+  int reserve(int nt, int ns);
+  int build_grid(const float* tgt, int nt, float resolution, cudaStream_t stream);   // setInputTarget -> init()
+  static constexpr int kGridLaunches = 12 + 12;
+  int eval(const float* src, int ns, const NdtEvalParams& P, double* sums44, cudaStream_t stream);
+  static constexpr int kEvalLaunches = 2;
+  int fitness(const float* src, int ns, const float* tgt, const float* T, const FloatTree& t, double* sums2,
+              cudaStream_t stream, double* score);
+  static int fitness_launches(int nt);   // with the build of the target's float tree
+};
 int ndt_float_to_soa(const float* pts, int n, double* soa, int64_t stride, cudaStream_t stream);
-int ndt_fitness(const float* src, int ns, const NdtEvalParams& P, const KdNode* nodes,
-                const BucketPoint* bpts, const float* tgt, NdtWorkspace& ws, cudaStream_t stream);
 
 // ---- gicp.cu -----------------------------------------------------------------------------
 struct GicpIterParams {     // one outer GICP iteration (gicp_omp_impl.hpp:414-461)
@@ -274,25 +296,15 @@ void gicp_debug_approx_cell_host(const float* p, float inv, int* ixyz, uint32_t*
 void gicp_debug_mahalanobis_host(const double* R, const double* C1, const double* C2, double* out9);
 void gicp_debug_cost_terms_host(const float* T, const float* base, const float* ps, const float* pt, const double* M,
                                 double* acc13);
-size_t approx_ws_bytes(int n);
-int approx_voxel_grid(const float* pts, int n, float leaf, void* ws_base, float* out, uint32_t* n_out_dev,
-                      cudaStream_t stream);
-int approx_voxel_grid_emit(int n, int n_runs, void* ws_base, float* out, const uint32_t* n_out_dev,
-                           cudaStream_t stream);
-int gicp_covariances(const float* cloud, int n, const KdNode* nodes, const BucketPoint* bpts, double eps,
-                     double* covs, cudaStream_t stream);
-int gicp_correspond(const float* src, int ns, const float* tgt, const GicpIterParams& P, const KdNode* nodes,
-                    const BucketPoint* bpts, const double* cov_s, const double* cov_t, int32_t* match,
-                    double* maha, uint32_t* count, cudaStream_t stream);
+// pcl::ApproximateVoxelGrid::filter of packed float clouds into out (grown to room for n points): the workspace and
+// the output count m, which filter() reads back between its two halves.
+struct ApproxVoxelGrid {
+  DevBuf ws, counter;
+  int filter(const float* pts, int n, float leaf, DevBuf& out, int* m, cudaStream_t stream);
+};
 // test hook sm_debug_float_tree_knn: knn1 (eps = 0, k = 1) or knn_k (k = 20) over t for nq AoS double queries
 int float_tree_debug_knn(const FloatTree& t, const double* q, int nq, int k, int32_t* ids, double* d2,
                          cudaStream_t stream);
-int gicp_cost_blocks(int ns);
-// ticket: a zeroed u32; host_sums_dev / host_flag_dev: device views of mapped pinned host memory (13 doubles and a
-// sequence word the kernel sets to `seq` after the sums), or null
-int gicp_cost(const float* src, int ns, const float* tgt, const GicpCostParams& P, const int32_t* match,
-              const double* maha, double* partials, double* sums, uint32_t* ticket, double* host_sums_dev,
-              long long* host_flag_dev, long long seq, cudaStream_t stream);
 
 // ---- normals.cu ------------------------------------------------------------------------
 // The device buffers of CalculateNormals over n points, sized by reserve(n): the input cloud, the bucket-7 tree

@@ -18,6 +18,8 @@
 //                         target through the same k-d tree as the ICP path (eps = 0).
 // Compiled with -fmad=false: the per-leaf and per-(point, voxel) arithmetic is bit-identical
 // to the oracle's written-out operation order.
+#include <limits>
+
 #include "common.cuh"
 #include "icp_dev.cuh"
 #include "kernels.h"
@@ -633,9 +635,15 @@ void ndt_debug_term_host(const NdtEvalParams& P, const float* x_orig, const floa
                         : update_derivatives(P, x_orig, x_trans, leaf, out43 + 1, out43 + 7);
 }
 
-int ndt_blocks(int n) { return ceil_div(n, kNdtThreads); }
+static int ndt_blocks(int n) { return ceil_div(n, kNdtThreads); }
 
-size_t NdtWorkspace::bytes_needed(int nt, int ns) {
+static uint32_t ndt_table_size(int nt) {
+  uint32_t s = 1024;
+  while (s < 2u * (uint32_t)(nt > 0 ? nt : 1)) s <<= 1;   // voxels <= points; load factor <= 0.5
+  return s;
+}
+
+static size_t workspace_bytes(int nt, int ns) {
   const int64_t st = (nt + 63) & ~63;
   size_t b = 0;
   b += 2 * st * sizeof(uint64_t) + 2 * st * sizeof(uint32_t);              // keys / order ping-pong
@@ -649,35 +657,31 @@ size_t NdtWorkspace::bytes_needed(int nt, int ns) {
   return b + 8192;
 }
 
-uint32_t ndt_table_size(int nt) {
-  uint32_t s = 1024;
-  while (s < 2u * (uint32_t)(nt > 0 ? nt : 1)) s <<= 1;   // voxels <= points; load factor <= 0.5
-  return s;
-}
-
-void NdtWorkspace::carve(void* base, int nt, int ns) {
+int NdtStage::reserve(int nt, int ns) {
+  SMB_RC(buf.reserve(workspace_bytes(nt, ns)));
   const int64_t st = (nt + 63) & ~63;
-  char* p = (char*)base;
+  char* p = (char*)buf.p;
   auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) & ~(size_t)255; return r; };
-  stride = st;
-  keys[0] = (uint64_t*)take(st * sizeof(uint64_t)); keys[1] = (uint64_t*)take(st * sizeof(uint64_t));
-  order[0] = (uint32_t*)take(st * sizeof(uint32_t)); order[1] = (uint32_t*)take(st * sizeof(uint32_t));
-  scratch = (uint32_t*)take(radix_sort_scratch_bytes(nt, 1) + 4096);
-  voxel_start = (uint32_t*)take((st + 64) * sizeof(uint32_t));
-  voxel_key = (int*)take(st * sizeof(int));
-  leaves = (NdtLeaf*)take(st * sizeof(NdtLeaf));
-  table_size = ndt_table_size(nt);
-  table_key = (int*)take((size_t)table_size * sizeof(int));
-  table_val = (int*)take((size_t)table_size * sizeof(int));
-  partials = (double*)take((size_t)(ndt_blocks(ns) + 8) * kNdtSums * sizeof(double));
-  sums = (double*)take(64 * sizeof(double));
-  minmax = (float*)take(1024 * 6 * sizeof(float));
-  sorted_pts = (float*)take(3 * st * sizeof(float));
-  grid = (NdtGrid*)take(sizeof(NdtGrid));
+  ws.stride = st;
+  ws.keys[0] = (uint64_t*)take(st * sizeof(uint64_t)); ws.keys[1] = (uint64_t*)take(st * sizeof(uint64_t));
+  ws.order[0] = (uint32_t*)take(st * sizeof(uint32_t)); ws.order[1] = (uint32_t*)take(st * sizeof(uint32_t));
+  ws.scratch = (uint32_t*)take(radix_sort_scratch_bytes(nt, 1) + 4096);
+  ws.voxel_start = (uint32_t*)take((st + 64) * sizeof(uint32_t));
+  ws.voxel_key = (int*)take(st * sizeof(int));
+  ws.leaves = (NdtLeaf*)take(st * sizeof(NdtLeaf));
+  ws.table_size = ndt_table_size(nt);
+  ws.table_key = (int*)take((size_t)ws.table_size * sizeof(int));
+  ws.table_val = (int*)take((size_t)ws.table_size * sizeof(int));
+  ws.partials = (double*)take((size_t)(ndt_blocks(ns) + 8) * kNdtSums * sizeof(double));
+  ws.sums = (double*)take(64 * sizeof(double));
+  ws.minmax = (float*)take(1024 * 6 * sizeof(float));
+  ws.sorted_pts = (float*)take(3 * st * sizeof(float));
+  ws.grid = (NdtGrid*)take(sizeof(NdtGrid));
+  return 0;
 }
 
 // VoxelGridCovariance::filter(true) for the target (ndt_omp.h:117-122,271-278)
-int ndt_build_grid(const float* tgt, int nt, float resolution, NdtWorkspace& ws, cudaStream_t stream) {
+int NdtStage::build_grid(const float* tgt, int nt, float resolution, cudaStream_t stream) {
   const int nparts = nt < 256 * 512 ? ceil_div(nt, 256) : 512;
   ndt_minmax_partial_kernel<<<nparts, 256, 0, stream>>>(tgt, nt, ws.minmax);
   ndt_grid_params_kernel<<<1, 256, 0, stream>>>(ws.minmax, nparts, resolution, ws.grid);
@@ -702,12 +706,14 @@ int ndt_build_grid(const float* tgt, int nt, float resolution, NdtWorkspace& ws,
 }
 
 // computeDerivatives: out[44] = score, gradient, hessian (row-major), neighbour count
-int ndt_eval(const float* src, int ns, const NdtEvalParams& P, NdtWorkspace& ws, cudaStream_t stream) {
+int NdtStage::eval(const float* src, int ns, const NdtEvalParams& P, double* sums44, cudaStream_t stream) {
   const int nb = ndt_blocks(ns);
   ndt_derivatives_kernel<<<nb, kNdtThreads, 0, stream>>>(src, ns, P, ws.grid, ws.leaves, ws.table_key,
                                                         ws.table_val, ws.table_size - 1, ws.partials);
   ndt_reduce_kernel<<<1, 1024, 0, stream>>>(ws.partials, nb, kNdtSums, ws.sums);
   SMB_CUDA_OK(cudaGetLastError());
+  SMB_CUDA_OK(cudaMemcpyAsync(sums44, ws.sums, kNdtSums * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  SMB_CUDA_OK(cudaStreamSynchronize(stream));
   return 0;
 }
 
@@ -717,14 +723,23 @@ int ndt_float_to_soa(const float* pts, int n, double* soa, int64_t stride, cudaS
   return 0;
 }
 
-// getFitnessScore: sums[0] = sum of squared NN distances (float each), sums[1] = count
-int ndt_fitness(const float* src, int ns, const NdtEvalParams& P, const KdNode* nodes,
-                const BucketPoint* bpts, const float* tgt, NdtWorkspace& ws, cudaStream_t stream) {
+// getFitnessScore: the mean over the matched points of the squared NN distance (float each); sums2 stages the sum
+// and the count
+int NdtStage::fitness(const float* src, int ns, const float* tgt, const float* T, const FloatTree& t, double* sums2,
+                      cudaStream_t stream, double* score) {
+  NdtEvalParams P;
+  memset(&P, 0, sizeof(P));
+  for (int i = 0; i < 16; ++i) P.T[i] = T[i];
   const int nb = ceil_div(ns, 256);
-  ndt_fitness_kernel<<<nb, 256, 0, stream>>>(src, ns, P, nodes, bpts, tgt, ws.partials);
+  ndt_fitness_kernel<<<nb, 256, 0, stream>>>(src, ns, P, (const KdNode*)t.nodes.p, (const BucketPoint*)t.bpts.p, tgt,
+                                            ws.partials);
   ndt_reduce_kernel<<<1, 1024, 0, stream>>>(ws.partials, nb, 2, ws.sums);
   SMB_CUDA_OK(cudaGetLastError());
+  SMB_CUDA_OK(cudaMemcpyAsync(sums2, ws.sums, 2 * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  SMB_CUDA_OK(cudaStreamSynchronize(stream));
+  *score = sums2[1] > 0.0 ? sums2[0] / sums2[1] : std::numeric_limits<double>::max();
   return 0;
 }
+int NdtStage::fitness_launches(int nt) { return 24 + kd_num_levels(nt, 8) * 5 + 6; }
 
 }  // namespace smb

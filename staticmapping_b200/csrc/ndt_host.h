@@ -7,6 +7,7 @@
 #define SM_B200_NDT_HOST_H_
 
 #include <math.h>
+#include <string.h>
 
 #include <algorithm>
 #include <limits>
@@ -23,14 +24,6 @@ struct Options {                 // defaults of the reference (ndt.cc:31, ndt_om
   double transformation_epsilon = 0.1;
   int max_iterations = 35;
 };
-
-inline void gauss_constants(const Options& o, double* d1, double* d2) {
-  const double c1 = 10.0 * (1 - o.outlier_ratio);
-  const double c2 = o.outlier_ratio / pow((double)o.resolution, 3);
-  const double d3 = -log(c2);
-  *d1 = -log(c1 + c2) - d3;
-  *d2 = -2 * log((-log(c1 * exp(-0.5) + c2) - d3) / *d1);
-}
 
 inline void angle_tables(const double* p, NdtEvalParams* P) {
   double cx, cy, cz, sx, sy, sz;
@@ -97,6 +90,26 @@ inline void transform_from_p(const double* p, float* T) {
   }
   T[15] = 1.0f;
 }
+// The parameters of computeDerivatives for o: Gauss constants (:86-93), radius, term math (f64_math: stock PCL's
+// double form, else pclomp's float form); at pose vector p also its transform and angle tables, which newton_loop
+// sets otherwise.
+inline NdtEvalParams eval_params(const Options& o, bool f64_math, const double* p = nullptr) {
+  NdtEvalParams P;
+  memset(&P, 0, sizeof(P));
+  const double c1 = 10.0 * (1 - o.outlier_ratio);
+  const double c2 = o.outlier_ratio / pow((double)o.resolution, 3);
+  const double d3 = -log(c2);
+  P.gauss_d1 = -log(c1 + c2) - d3;
+  P.gauss_d2 = -2 * log((-log(c1 * exp(-0.5) + c2) - d3) / P.gauss_d1);
+  P.radius = o.resolution;
+  P.f64_math = f64_math ? 1 : 0;
+  if (p) {
+    angle_tables(p, &P);
+    transform_from_p(p, P.T);
+  }
+  return P;
+}
+
 // translation + rotation().eulerAngles(0,1,2), single precision (Eigen 3.3 EulerAngles.h)
 inline void p_from_transform(const float* T, double* p) {
   const float pi = 3.14159265358979323846f;
@@ -157,9 +170,10 @@ inline void svd_solve6(const double* A, const double* b, double* x) {
 // an evaluation callback: eval(P, p, sums) runs computeDerivatives for the pose vector p (P.T and the angle tables
 // of P are built from it) and fills
 // sums[0] = score, sums[1..6] = gradient, sums[7..42] = Hessian (row-major), sums[43] = neighbour count over all
-// points; it returns < 0 on error (propagated).  P comes in with the Gauss constants, radius and f64_math set.
-// The device path passes a lambda around ndt_eval_sync (sm_api.cu ndt_run); the test hook sm_debug_ndt_newton passes a
-// caller-supplied function, so this control flow is exercised on the host against an independent restatement.
+// points; it returns < 0 on error (propagated).  P comes in from eval_params without a pose.
+// The device path passes a lambda around NdtStage::eval (ndt_run of the C ABI); the test hook sm_debug_ndt_newton
+// passes a caller-supplied function, so this control flow is exercised on the host against an independent
+// restatement.
 struct NewtonOut {
   float final_T[16];           // final_transformation_, column-major
   int iterations = 0;          // nr_iterations_

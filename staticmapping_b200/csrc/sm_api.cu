@@ -18,7 +18,6 @@
 #include "common.cuh"
 #include "icp_dev.cuh"
 #include "kernels.h"
-#include "linalg_dev.cuh"
 #include "gicp_host.h"
 #include "ndt_host.h"
 
@@ -162,11 +161,6 @@ pm_score_reduce_kernel(const uint64_t* __restrict__ keys, int n, float ratio, do
   }
 }
 
-__global__ void debug_solve6_kernel(const double* __restrict__ A, const double* __restrict__ b, double* __restrict__ x,
-                                    int* __restrict__ path) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) *path = la::solve_possibly_underdetermined(A, b, x);
-}
-
 enum OptKind { kOptInt, kOptFloat, kOptDouble, kOptBool };
 struct OptionDef { const char* name; OptKind kind; size_t offset; };
 
@@ -190,6 +184,18 @@ struct NdtGicpOptions {                  // ndt_gicp.h:71-75
   bool using_voxel_filter = true;
   bool use_ndt = true;
 };
+
+// The handle's mapped pinned block: what the device hands back to the host.  The GICP cost kernel writes its sums
+// and then the sequence word straight into it; the other fields arrive with a read-back and a synchronisation.
+struct HostBlock {
+  double ndt_sums[44];     // one NDT evaluation (score, gradient, Hessian row-major, neighbours) or the fitness pass
+  int ndt_overflow;        // the NDT grid's size guard, read back with the first evaluation
+  double gicp_sums[13];    // one GICP cost evaluation
+  long long gicp_seq;      // its sequence number, written after the sums
+  double pm_score[3];      // the type-1 score pass: mean kept distance, kept, valid
+  double spare[2];
+};
+static_assert(sizeof(HostBlock) == 64 * sizeof(double), "the mapped pinned block is 64 doubles");
 
 // A captured launch sequence, replayed while the key (all pointers and sizes baked into the
 // kernel arguments) is unchanged: one cudaGraphLaunch instead of ~100 kernel launches.
@@ -216,8 +222,8 @@ struct sm_handle {
   cudaEvent_t ev_up[4] = {nullptr, nullptr, nullptr, nullptr};
   std::vector<cudaEvent_t> prof_events;
   double* host_guess = nullptr;    // pinned, 16 doubles
-  double* host_sums = nullptr;     // pinned + mapped, 64 doubles; word 60 doubles as the GICP evaluation flag
-  double* host_sums_dev = nullptr; // its device view
+  HostBlock* host = nullptr;       // pinned + mapped
+  HostBlock* host_dev = nullptr;   // its device view
   std::string error;
   double final_score = 0.0;
   sm_align_info info;
@@ -229,12 +235,10 @@ struct sm_handle {
   NdtGicpOptions ng;
   DevBuf kdws;                     // k-d tree build workspace of every tree below
 
-  // IcpFast, and the ICP chain of type 1: SoA double clouds, the tree, the iteration buffers
+  // IcpFast, and the ICP chain of type 1: the uploaded SoA double clouds, the iteration buffers and the tree
   struct {
-    DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, tgt, nrm, src_raw, src0, src_g0, src_sort, slot, d2,
-        hist, cand_terms, cand_key, cand_cnt, partials, mean_partials, state, guess;
-    DevBuf deskewed;                 // [3][sstride]: the source of the iteration, with inner compensation only
-    KdCompactTree tree;
+    DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, nrm, src_raw;
+    IcpFastBuffers bufs;
     int64_t sstride = 0, tstride = 0;
     bool up_src = false, up_tgt = false;
     IcpState* host_state = nullptr;  // pinned
@@ -248,18 +252,19 @@ struct sm_handle {
     } run;
   } fast;
 
-  // Ndt, NdtWithGicp and type 1: packed float clouds (12 bytes per point), the NDT workspace and the
+  // Ndt, NdtWithGicp and type 1: packed float clouds (12 bytes per point), the NDT stage and the
   // target's tree (fitness scores, GICP correspondences, the type-1 score)
   struct {
-    DevBuf src, tgt, ndt_ws;
+    DevBuf src, tgt;
+    NdtStage ndt;
     FloatTree target_tree;
   } f32;
 
   // NdtWithGicp
   struct {
-    DevBuf src_filt, tgt_filt, approx_ws, cov_s, cov_t, maha, match, partials, counter;
-    FloatTree source_tree;
-    long long seq = 0;
+    DevBuf src_filt, tgt_filt;
+    ApproxVoxelGrid approx;
+    gicp::Stage gicp;
   } ndt_gicp;
 
   // IcpUsingPointMatcher stand-in (type 1): raw float clouds -> filtered double clouds.  The normals
@@ -276,7 +281,7 @@ struct sm_handle {
     for (cudaEvent_t e : ev_up) if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : prof_events) cudaEventDestroy(e);
     if (fast.host_state) cudaFreeHost(fast.host_state);
-    if (host_sums) cudaFreeHost(host_sums);
+    if (host) cudaFreeHost(host);
     if (host_guess) cudaFreeHost(host_guess);
     if (own_stream) cudaStreamDestroy(own_stream);
   }
@@ -459,8 +464,8 @@ int icp_enqueue_chunk(sm_handle* h) {
     H_RC(icp_enqueue_iterations(r.b, p, r.enqueued, chunk, h->stream, evs, r.deskewed));
   }
   r.enqueued += chunk;
-  r.launches += (p.inner_compensation ? 4 : 3) * chunk;
-  H_CUDA(cudaMemcpyAsync(f.host_state, f.state.p, sizeof(IcpState), cudaMemcpyDeviceToHost, h->stream));
+  r.launches += icp_iteration_launches(p.inner_compensation != 0) * chunk;
+  H_CUDA(cudaMemcpyAsync(f.host_state, f.bufs.state.p, sizeof(IcpState), cudaMemcpyDeviceToHost, h->stream));
   return 0;
 }
 
@@ -479,43 +484,15 @@ int icp_begin(sm_handle* h, const double* guess) {
   NvtxRange nvtx_align("IcpFast::Align");
   const int ns = (int)h->n_source, nt = (int)h->n_target;
   const int levels = kd_num_levels(nt, 8);
-  const int nb = icp_accum_blocks(ns);
-  H_RC(f.tgt.reserve((size_t)(3 * f.tstride) * sizeof(double)));
-  H_RC(f.src0.reserve((size_t)(3 * f.sstride) * sizeof(double)));
-  H_RC(f.src_g0.reserve((size_t)(3 * f.sstride) * sizeof(double)));
-  H_RC(f.src_sort.reserve(RadixPairs::bytes(f.sstride, ns)));
-  H_RC(f.tree.reserve(nt, 8, KdCompactTree::kNormals));
-  const size_t slot_bytes = (((size_t)ns * sizeof(int32_t) + 64 + 255) / 256) * 256;
-  H_RC(f.slot.reserve(slot_bytes + ((size_t)ns + kKnnItemSlack) * sizeof(int4)));
-  H_RC(f.d2.reserve((size_t)ns * sizeof(double)));
-  H_RC(f.hist.reserve((2 * kHistBins + 64) * sizeof(uint32_t) + 32 * sizeof(double)));
-  H_RC(f.cand_terms.reserve((size_t)nb * 512 * 8 * sizeof(double)));
-  H_RC(f.cand_key.reserve((size_t)nb * 512 * sizeof(unsigned long long)));
-  H_RC(f.cand_cnt.reserve((size_t)nb * sizeof(uint32_t)));
-  H_RC(f.partials.reserve((size_t)nb * 32 * sizeof(double)));
-  H_RC(f.mean_partials.reserve((size_t)ceil_div(nt, 1024) * 4 * sizeof(double)));
-  H_RC(f.state.reserve(sizeof(IcpState)));
-  H_RC(f.guess.reserve(16 * sizeof(double)));
+  // EnableInnerCompensation: IcpFast::Align reads it (icp_fast.cc:487, :509); type 1 runs the IcpFast chain but,
+  // like IcpUsingPointMatcher, ignores it
+  const bool comp = h->type == SM_TYPE_FAST_ICP && h->inner_compensation;
+  H_RC(f.bufs.reserve(ns, nt, f.sstride, f.tstride, comp));
   KdWorkspace& ws = r.ws;
   H_RC(ws.carve(h->kdws, nt, 8));
 
   IcpBuffers& b = r.b;
-  b.tgt = (double*)f.tgt.p; b.tgt_raw = (double*)f.tgt_raw.p; b.nrm = (double*)f.nrm.p;
-  b.tstride = f.tstride;
-  b.nodes = (KdNode*)f.tree.nodes.p; b.leaf_order = (uint32_t*)f.tree.leaf_order.p;
-  b.kc = f.tree.view();
-  b.src_raw = (double*)f.src_raw.p; b.src0 = (double*)f.src0.p; b.sstride = f.sstride;
-  b.src_g0 = (double*)f.src_g0.p;
-  b.src_sort.carve(f.src_sort.p, f.sstride);
-  b.slot = (int32_t*)f.slot.p;
-  b.knn_items = reinterpret_cast<int4*>((char*)f.slot.p + slot_bytes);
-  b.d2 = (double*)f.d2.p; b.hist = (uint32_t*)f.hist.p;
-  b.hist2 = b.hist + kHistBins;
-  b.sums = (double*)(b.hist + 2 * kHistBins + 64);
-  b.cand_terms = (double*)f.cand_terms.p;
-  b.cand_key = (unsigned long long*)f.cand_key.p; b.cand_cnt = (uint32_t*)f.cand_cnt.p;
-  b.partials = (double*)f.partials.p; b.mean_partials = (double*)f.mean_partials.p;
-  b.state = (IcpState*)f.state.p;
+  f.bufs.fill(b, (const double*)f.tgt_raw.p, (const double*)f.nrm.p, (const double*)f.src_raw.p);
   IcpParams& p = r.p;
   p.n_source = ns; p.n_target = nt;
   p.max_iteration = h->icp.max_iteration;
@@ -525,32 +502,26 @@ int icp_begin(sm_handle* h, const double* guess) {
   p.disable_convergence = h->icp.disable_convergence_check ? 1 : 0;
   p.knn_queries_per_cta = h->icp.knn_queries_per_cta;
   p.tree_levels = levels;
-  // EnableInnerCompensation: IcpFast::Align reads it (icp_fast.cc:487, :509); type 1 runs the IcpFast chain but,
-  // like IcpUsingPointMatcher, ignores it
-  p.inner_compensation = (h->type == SM_TYPE_FAST_ICP && h->inner_compensation) ? 1 : 0;
-  r.deskewed = nullptr;
-  if (p.inner_compensation) {
-    H_RC(f.deskewed.reserve((size_t)(3 * f.sstride) * sizeof(double)));
-    r.deskewed = (double*)f.deskewed.p;
-  }
+  p.inner_compensation = comp ? 1 : 0;
+  r.deskewed = comp ? (double*)f.bufs.deskewed.p : nullptr;
   if (levels > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "target too large (tree deeper than 24 levels)");
 
   memcpy(h->host_guess, guess, 16 * sizeof(double));   // pinned: the caller's array may go away
-  H_CUDA(cudaMemcpyAsync(f.guess.p, h->host_guess, 16 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  H_CUDA(cudaMemcpyAsync(f.bufs.guess.p, h->host_guess, 16 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   H_CUDA(cudaEventRecord(h->ev[0], h->stream));
   r.graphs = h->icp.use_graphs && !h->icp.profile_kernels;
   r.key.clear();
-  key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.guess.p); key_append(r.key, h->kdws.p);
+  key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.bufs.guess.p); key_append(r.key, h->kdws.p);
   key_append(r.key, r.deskewed);   // p.inner_compensation is part of p
   if (r.graphs) {
     H_RC(run_graphed(h, f.g_prologue, r.key, [&]() {
-      return icp_prologue(b, p, (const double*)f.guess.p, ws, f.tree, h->stream);
+      return icp_prologue(b, p, (const double*)f.bufs.guess.p, ws, f.bufs.tree, h->stream);
     }));
   } else {
-    H_RC(icp_prologue(b, p, (const double*)f.guess.p, ws, f.tree, h->stream));
+    H_RC(icp_prologue(b, p, (const double*)f.bufs.guess.p, ws, f.bufs.tree, h->stream));
   }
   H_CUDA(cudaEventRecord(h->ev[1], h->stream));
-  r.launches = 2 + 1 + 24 + levels * 5 + 1 + 1 + 2 + 13;
+  r.launches = icp_prologue_launches(levels);
   r.enqueued = 0;
   r.max_it = p.max_iteration > 0 ? p.max_iteration : 1;
   H_RC(icp_enqueue_chunk(h));
@@ -688,11 +659,11 @@ int pm_align(sm_handle* h, const double* guess, double* result) {
     H_RC(radix_sort_pairs_u64(sp.keys[0], sp.vals[0], sp.keys[1], sp.vals[1], ns, 1, st, sp.scratch, s, 8));
     pm_score_reduce_kernel<<<1, 1024, 0, s>>>(sp.keys[0], ns, h->icp.dist_outlier_ratio, outdev);
     H_CUDA(cudaGetLastError());
-    H_CUDA(cudaMemcpyAsync(h->host_sums, outdev, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    H_CUDA(cudaMemcpyAsync(h->host->pm_score, outdev, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
     H_CUDA(cudaStreamSynchronize(s));
-    if (!(h->host_sums[1] > 0.0)) return fail(h, SM_ERR_NOTHING_TO_MINIMIZE, "Align: no matched point for the score");
-    h->final_score = exp(-h->host_sums[0]);
-    h->info.aux[1] = h->host_sums[1];     // matches kept by the trim in the score pass
+    if (!(h->host->pm_score[1] > 0.0)) return fail(h, SM_ERR_NOTHING_TO_MINIMIZE, "Align: no matched point for the score");
+    h->final_score = exp(-h->host->pm_score[0]);
+    h->info.aux[1] = h->host->pm_score[1];     // matches kept by the trim in the score pass
   }
   return h->final_score < (double)h->icp.accept_min_score ? 0 : 1;
 }
@@ -717,13 +688,6 @@ int set_input_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride, boo
   return 0;
 }
 
-int ndt_eval_sync(sm_handle* h, const float* src, int ns, const NdtEvalParams& P, NdtWorkspace& ws) {
-  H_RC(ndt_eval(src, ns, P, ws, h->stream));
-  H_CUDA(cudaMemcpyAsync(h->host_sums, ws.sums, 44 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  H_CUDA(cudaStreamSynchronize(h->stream));
-  return 0;
-}
-
 struct NdtRunOut {
   float final_T[16];
   double fitness = 0, trans_probability = 0, mean_neighbors = 0;
@@ -731,49 +695,29 @@ struct NdtRunOut {
   float ms_grid = 0, ms_iter = 0, ms_fit = 0;
 };
 
-// pcl::Registration::getFitnessScore over h->f32.target_tree
-int fitness_score(sm_handle* h, const float* src, int ns, const float* tgt, const float* T, NdtWorkspace& ws,
-                  double* out) {
-  NdtEvalParams P;
-  memset(&P, 0, sizeof(P));
-  for (int i = 0; i < 16; ++i) P.T[i] = T[i];
-  const FloatTree& t = h->f32.target_tree;
-  H_RC(ndt_fitness(src, ns, P, (const KdNode*)t.nodes.p, (const BucketPoint*)t.bpts.p, tgt, ws, h->stream));
-  H_CUDA(cudaMemcpyAsync(h->host_sums, ws.sums, 2 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  H_CUDA(cudaStreamSynchronize(h->stream));
-  *out = h->host_sums[1] > 0.0 ? h->host_sums[0] / h->host_sums[1] : std::numeric_limits<double>::max();
-  return 0;
-}
-
 // pcl::Registration::align -> NormalDistributionsTransform::computeTransformation
 // (ndt_omp_impl.hpp:81-171) -> getFitnessScore, on device clouds src/tgt (packed float xyz).
 int ndt_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, const ndt::Options& o,
             bool f64_math, const double* guess, NdtRunOut* out) {
-  H_RC(h->f32.ndt_ws.reserve(NdtWorkspace::bytes_needed(nt, ns)));
-  NdtWorkspace ws;
-  ws.carve(h->f32.ndt_ws.p, nt, ns);
+  NdtStage& st = h->f32.ndt;
+  H_RC(st.reserve(nt, ns));
   H_CUDA(cudaEventRecord(h->ev[0], h->stream));
-  H_RC(ndt_build_grid(tgt, nt, o.resolution, ws, h->stream));        // setInputTarget -> init()
-  // the grid's size guard arrives with the first evaluation's sums (word 44 of the pinned block is free)
-  volatile int* overflow = reinterpret_cast<volatile int*>(h->host_sums + 44);
+  H_RC(st.build_grid(tgt, nt, o.resolution, h->stream));        // setInputTarget -> init()
+  // the grid's size guard arrives with the first evaluation's sums
+  volatile int* overflow = &h->host->ndt_overflow;
   *overflow = 0;
-  H_CUDA(cudaMemcpyAsync((void*)overflow, &ws.grid->overflow, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  H_CUDA(cudaMemcpyAsync((void*)overflow, &st.ws.grid->overflow, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   H_CUDA(cudaEventRecord(h->ev[1], h->stream));
-  NdtEvalParams P;
-  memset(&P, 0, sizeof(P));
-  ndt::gauss_constants(o, &P.gauss_d1, &P.gauss_d2);
-  P.radius = o.resolution;
-  P.f64_math = f64_math ? 1 : 0;
+  NdtEvalParams P = ndt::eval_params(o, f64_math);
   // the Newton loop itself is host code shared with the test hook sm_debug_ndt_newton (ndt_host.h newton_loop);
   // one evaluation = computeDerivatives on the device, 44 sums handed back through mapped pinned memory
   ndt::NewtonOut nw;
-  int launches = 12 + 12;
+  int launches = NdtStage::kGridLaunches;
   const int nrc = ndt::newton_loop(o, guess, ns, P, [&](const NdtEvalParams& Pe, const double*, double* sums) -> int {
-    const int rc = ndt_eval_sync(h, src, ns, Pe, ws);
-    if (rc < 0) return rc;
+    H_RC(st.eval(src, ns, Pe, h->host->ndt_sums, h->stream));
     if (*overflow) return SM_ERR_BAD_ARGUMENT;
-    for (int i = 0; i < 44; ++i) sums[i] = h->host_sums[i];
-    launches += 2;
+    for (int i = 0; i < 44; ++i) sums[i] = h->host->ndt_sums[i];
+    launches += NdtStage::kEvalLaunches;
     return 0;
   }, &nw);
   // the reference clears the grid and goes on to search a tree that was never given a cloud (undefined behaviour)
@@ -783,20 +727,18 @@ int ndt_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, co
   H_RC(nrc);
   float* final_T = out->final_T;
   for (int i = 0; i < 16; ++i) final_T[i] = nw.final_T[i];
-  const int nr_iterations = nw.iterations, evals = nw.evaluations;
-  const double score = nw.score, nb_sum = nw.nb_sum;
   H_CUDA(cudaEventRecord(h->ev[2], h->stream));
   // getFitnessScore (ndt.cc:60): exact 1-NN over the full target (PCL builds this search
   // tree in setInputTarget; the reference calls that on every Align)
   H_RC(build_tree_f32(h, tgt, nt, h->f32.target_tree));
-  H_RC(fitness_score(h, src, ns, tgt, final_T, ws, &out->fitness));
+  H_RC(st.fitness(src, ns, tgt, final_T, h->f32.target_tree, h->host->ndt_sums, h->stream, &out->fitness));
   H_CUDA(cudaEventRecord(h->ev[3], h->stream));
   H_CUDA(cudaEventSynchronize(h->ev[3]));
-  out->iterations = nr_iterations;
-  out->evaluations = evals;
-  out->trans_probability = score / (double)ns;
-  out->mean_neighbors = evals ? nb_sum / evals : 0.0;
-  out->launches = launches + 24 + kd_num_levels(nt, 8) * 5 + 6;
+  out->iterations = nw.iterations;
+  out->evaluations = nw.evaluations;
+  out->trans_probability = nw.score / (double)ns;
+  out->mean_neighbors = nw.evaluations ? nw.nb_sum / nw.evaluations : 0.0;
+  out->launches = launches + NdtStage::fitness_launches(nt);
   cudaEventElapsedTime(&out->ms_grid, h->ev[0], h->ev[1]);
   cudaEventElapsedTime(&out->ms_iter, h->ev[1], h->ev[2]);
   cudaEventElapsedTime(&out->ms_fit, h->ev[2], h->ev[3]);
@@ -826,86 +768,42 @@ int ndt_align(sm_handle* h, const double* guess, double* result) {
 }
 
 // ---- NdtWithGicp ---------------------------------------------------------------------------
-// pcl::ApproximateVoxelGrid::filter (ndt_gicp.cc:59-70)
-int approx_filter(sm_handle* h, const float* pts, int n, float leaf, DevBuf& out, int* m_out) {
-  auto& g = h->ndt_gicp;
-  H_RC(g.approx_ws.reserve(approx_ws_bytes(n)));
-  H_RC(out.reserve((size_t)n * 12 + 64));
-  H_RC(g.counter.reserve(64));
-  uint32_t* cnt = (uint32_t*)g.counter.p;
-  H_RC(approx_voxel_grid(pts, n, leaf, g.approx_ws.p, (float*)out.p, cnt, h->stream));
-  uint32_t m = 0;
-  H_CUDA(cudaMemcpyAsync(&m, cnt, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
-  H_CUDA(cudaStreamSynchronize(h->stream));
-  H_RC(approx_voxel_grid_emit(n, (int)m, g.approx_ws.p, (float*)out.p, cnt, h->stream));
-  *m_out = (int)m;
-  return 0;
-}
-
 // GeneralizedIterativeClosestPoint::computeTransformation (gicp_omp_impl.hpp:381-514) with the
 // BFGS inner solver on the host; the target tree must be built in h->f32.target_tree.
 int gicp_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, const float* guess,
              const gicp::Options& o, float* final_T, int* iterations, int* bfgs_evals) {
-  auto& g = h->ndt_gicp;
+  gicp::Stage& g = h->ndt_gicp.gicp;
   const FloatTree& tt = h->f32.target_tree;
   H_RC(build_tree_f32(h, src, ns, g.source_tree));
-  H_RC(g.cov_s.reserve((size_t)ns * 9 * sizeof(double)));
-  H_RC(g.cov_t.reserve((size_t)nt * 9 * sizeof(double)));
-  H_RC(g.maha.reserve((size_t)ns * 9 * sizeof(double)));
-  H_RC(g.match.reserve((size_t)ns * sizeof(int32_t)));
-  H_RC(g.partials.reserve((size_t)(gicp_cost_blocks(ns) + 1) * 13 * sizeof(double) + 256));
-  H_RC(g.counter.reserve(64));
-  double* sums_dev = (double*)g.partials.p + (size_t)gicp_cost_blocks(ns) * 13;
-  uint32_t* ticket_dev = (uint32_t*)g.counter.p + 8;
-  H_CUDA(cudaMemsetAsync(ticket_dev, 0, sizeof(uint32_t), h->stream));
-  *reinterpret_cast<volatile long long*>(h->host_sums + 60) = 0;
-  g.seq = 0;
-  if (o.k_correspondences <= nt)   // :61-65: otherwise PCL_ERROR and the covariances stay unset
-    H_RC(gicp_covariances(tgt, nt, (const KdNode*)tt.nodes.p, (const BucketPoint*)tt.bpts.p, o.gicp_epsilon,
-                          (double*)g.cov_t.p, h->stream));
-  else H_CUDA(cudaMemsetAsync(g.cov_t.p, 0, (size_t)nt * 9 * sizeof(double), h->stream));
-  if (o.k_correspondences <= ns)
-    H_RC(gicp_covariances(src, ns, (const KdNode*)g.source_tree.nodes.p,
-                          (const BucketPoint*)g.source_tree.bpts.p, o.gicp_epsilon,
-                          (double*)g.cov_s.p, h->stream));
-  else H_CUDA(cudaMemsetAsync(g.cov_s.p, 0, (size_t)ns * 9 * sizeof(double), h->stream));
+  H_RC(g.reserve(ns, nt, h->stream));
+  volatile long long* seq_word = &h->host->gicp_seq;
+  *seq_word = 0;
+  H_RC(g.covariances(o, tgt, nt, tt, g.cov_t, h->stream));
+  H_RC(g.covariances(o, src, ns, g.source_tree, g.cov_s, h->stream));
   // the outer loop, the BFGS driver and the assembly of f / g from the 13 sums are host code shared with the test
   // hook sm_debug_gicp_outer (gicp_host.h outer_loop); the two callbacks are the device work
   gicp::OuterOut go;
   bool cuda_error = false;
   const int grc = gicp::outer_loop(
       o, guess,
-      [&](const float* transformation, const double* R, int* m_out) -> int {
-        GicpIterParams IP;
-        for (int i = 0; i < 16; ++i) { IP.guess[i] = guess[i]; IP.transformation[i] = transformation[i]; }
-        for (int q = 0; q < 9; ++q) IP.R[q] = R[q];
-        IP.dist_threshold = o.corr_dist_threshold * o.corr_dist_threshold;
-        if (gicp_correspond(src, ns, tgt, IP, (const KdNode*)tt.nodes.p, (const BucketPoint*)tt.bpts.p,
-                            (const double*)g.cov_s.p, (const double*)g.cov_t.p, (int32_t*)g.match.p,
-                            (double*)g.maha.p, (uint32_t*)g.counter.p, h->stream) != 0) { cuda_error = true; return -1; }
-        uint32_t m_u = 0;
-        if (cudaMemcpyAsync(&m_u, g.counter.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream) != cudaSuccess ||
-            cudaStreamSynchronize(h->stream) != cudaSuccess) { cuda_error = true; return -1; }
-        *m_out = (int)m_u;
+      [&](const float* transformation, const double* R, int* m) -> int {
+        if (g.correspond(o, src, ns, tgt, tt, guess, transformation, R, h->stream, m) != 0) { cuda_error = true; return -1; }
         return 0;
       },
       [&](const float* T, double* S) -> int {
-        GicpCostParams CP;
-        for (int i = 0; i < 16; ++i) { CP.T[i] = T[i]; CP.base[i] = guess[i]; }
         // the kernel's last block writes the 13 sums and then the sequence word into mapped pinned memory
-        volatile long long* flag = reinterpret_cast<volatile long long*>(h->host_sums + 60);
-        const long long seq = ++g.seq;
-        if (gicp_cost(src, ns, tgt, CP, (const int32_t*)g.match.p, (const double*)g.maha.p,
-                      (double*)g.partials.p, sums_dev, ticket_dev, h->host_sums_dev,
-                      reinterpret_cast<long long*>(h->host_sums_dev + 60), seq, h->stream) != 0) { cuda_error = true; return -1; }
-        for (long spins = 0; *flag != seq; ++spins) {
+        if (g.cost(src, ns, tgt, T, guess, h->host_dev->gicp_sums, &h->host_dev->gicp_seq, h->stream) != 0) {
+          cuda_error = true;
+          return -1;
+        }
+        for (long spins = 0; *seq_word != g.seq; ++spins) {
           if ((spins & 0xfff) == 0xfff && cudaStreamQuery(h->stream) != cudaErrorNotReady) {
-            if (*flag == seq) break;
-            if (cudaStreamSynchronize(h->stream) != cudaSuccess || *flag != seq) { cuda_error = true; return -1; }   // the kernel failed
+            if (*seq_word == g.seq) break;
+            if (cudaStreamSynchronize(h->stream) != cudaSuccess || *seq_word != g.seq) { cuda_error = true; return -1; }   // the kernel failed
           }
         }
         std::atomic_thread_fence(std::memory_order_acquire);
-        for (int q = 0; q < 13; ++q) S[q] = h->host_sums[q];
+        for (int q = 0; q < 13; ++q) S[q] = h->host->gicp_sums[q];
         return 0;
       },
       &go);
@@ -924,9 +822,9 @@ int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
   const float* tgt = (const float*)h->f32.tgt.p;
   int ns = (int)h->n_source, nt = (int)h->n_target;
   if (h->ng.using_voxel_filter) {
-    auto& g = h->ndt_gicp;
-    H_RC(approx_filter(h, src, ns, h->ng.voxel_resolution, g.src_filt, &ns));
-    H_RC(approx_filter(h, tgt, nt, h->ng.voxel_resolution, g.tgt_filt, &nt));
+    auto& g = h->ndt_gicp;    // pcl::ApproximateVoxelGrid::filter (ndt_gicp.cc:59-70)
+    H_RC(g.approx.filter(src, ns, h->ng.voxel_resolution, g.src_filt, &ns, h->stream));
+    H_RC(g.approx.filter(tgt, nt, h->ng.voxel_resolution, g.tgt_filt, &nt, h->stream));
     src = (const float*)g.src_filt.p;
     tgt = (const float*)g.tgt_filt.p;
   }
@@ -956,10 +854,9 @@ int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
     int it = 0, evals = 0;
     H_CUDA(cudaEventRecord(h->ev[0], h->stream));
     H_RC(gicp_run(h, src, ns, tgt, nt, ndt_guess, gicp::Options(), final_T, &it, &evals));
-    H_RC(h->f32.ndt_ws.reserve(NdtWorkspace::bytes_needed(nt, ns)));
-    NdtWorkspace ws;
-    ws.carve(h->f32.ndt_ws.p, nt, ns);
-    H_RC(fitness_score(h, src, ns, tgt, final_T, ws, &icp_score));
+    NdtStage& st = h->f32.ndt;
+    H_RC(st.reserve(nt, ns));
+    H_RC(st.fitness(src, ns, tgt, final_T, h->f32.target_tree, h->host->ndt_sums, h->stream, &icp_score));
     H_CUDA(cudaEventRecord(h->ev[1], h->stream));
     H_CUDA(cudaEventSynchronize(h->ev[1]));
     cudaEventElapsedTime(&h->info.ms_iterations, h->ev[0], h->ev[1]);
@@ -1003,8 +900,8 @@ int sm_create(int type, int device, sm_handle** out) {
   if (cudaSetDevice(device) != cudaSuccess ||
       cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaMallocHost((void**)&h->fast.host_state, sizeof(IcpState)) != cudaSuccess ||
-      cudaHostAlloc((void**)&h->host_sums, 64 * sizeof(double), cudaHostAllocMapped) != cudaSuccess ||
-      cudaHostGetDevicePointer((void**)&h->host_sums_dev, h->host_sums, 0) != cudaSuccess ||
+      cudaHostAlloc((void**)&h->host, sizeof(HostBlock), cudaHostAllocMapped) != cudaSuccess ||
+      cudaHostGetDevicePointer((void**)&h->host_dev, h->host, 0) != cudaSuccess ||
       cudaMallocHost((void**)&h->host_guess, 16 * sizeof(double)) != cudaSuccess) {
     delete h;
     return SM_ERR_CUDA;
@@ -1199,259 +1096,6 @@ int sm_align_pairs(sm_handle* const* handles, int32_t n_handles, const sm_pair* 
   return worst < 0 ? worst : SM_OK;
 }
 
-int sm_debug_solve6(int device, const double* A, const double* b, double* x, int32_t* path) {
-  if (!A || !b || !x || !path) return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
-  DevBuf buf;
-  SMB_RC(buf.reserve(64 * sizeof(double)));
-  double* d = (double*)buf.p;
-  SMB_CUDA_OK(cudaMemcpy(d, A, 36 * sizeof(double), cudaMemcpyHostToDevice));
-  SMB_CUDA_OK(cudaMemcpy(d + 36, b, 6 * sizeof(double), cudaMemcpyHostToDevice));
-  debug_solve6_kernel<<<1, 32>>>(d, d + 36, d + 42, reinterpret_cast<int*>(d + 48));
-  int p = 0;
-  SMB_CUDA_OK(cudaMemcpy(x, d + 42, 6 * sizeof(double), cudaMemcpyDeviceToHost));
-  SMB_CUDA_OK(cudaMemcpy(&p, d + 48, sizeof(int), cudaMemcpyDeviceToHost));
-  *path = p;
-  return SM_OK;
-}
-
-// test hook: csrc/linalg_dev.cuh's solver (the code icp_finish_kernel runs when its Cholesky certificate is not
-// conclusive) compiled for the HOST, so the product's transcription is checked against numpy without a GPU
-int sm_debug_solve6_host(const double* A, const double* b, double* x, int32_t* path) {
-  if (!A || !b || !x || !path) return SM_ERR_BAD_ARGUMENT;
-  *path = la::solve_possibly_underdetermined(A, b, x);
-  return SM_OK;
-}
-
-// test hook: the NDT Newton loop of the product (ndt_host.h newton_loop, the function ndt_run drives the device
-// with) over a caller-supplied evaluation — no GPU involved
-int sm_debug_ndt_newton(sm_debug_ndt_eval fn, void* user, const double* guess_4x4, int32_t n_source, float resolution,
-                        double step_size, double outlier_ratio, double transformation_epsilon, int32_t max_iterations,
-                        double* final_4x4, int32_t* iterations, int32_t* evaluations, double* score) {
-  if (!fn || !guess_4x4 || !final_4x4 || !iterations || !evaluations || !score || n_source <= 0)
-    return SM_ERR_BAD_ARGUMENT;
-  ndt::Options o;
-  o.resolution = resolution; o.step_size = step_size; o.outlier_ratio = outlier_ratio;
-  o.transformation_epsilon = transformation_epsilon; o.max_iterations = max_iterations;
-  NdtEvalParams P;
-  memset(&P, 0, sizeof(P));
-  ndt::gauss_constants(o, &P.gauss_d1, &P.gauss_d2);
-  P.radius = o.resolution;
-  ndt::NewtonOut nw;
-  const int rc = ndt::newton_loop(o, guess_4x4, n_source, P, [&](const NdtEvalParams& Pe, const double* p6, double* sums) -> int {
-    double T[16];
-    for (int i = 0; i < 16; ++i) T[i] = (double)Pe.T[i];
-    return fn(T, p6, sums, user);
-  }, &nw);
-  if (rc < 0) return rc;
-  for (int i = 0; i < 16; ++i) final_4x4[i] = (double)nw.final_T[i];
-  *iterations = nw.iterations; *evaluations = nw.evaluations; *score = nw.score;
-  return SM_OK;
-}
-
-// test hook: the GICP outer loop of the product (gicp_host.h outer_loop: start vector, f / g from the 13 sums, BFGS
-// driver, convergence test, final composition — the function gicp_run drives the device with) over a caller's
-// correspondence and cost functions; no GPU involved
-int sm_debug_gicp_outer(sm_debug_gicp_correspond correspond, sm_debug_gicp_cost cost, void* user, const double* guess_4x4,
-                        double* final_4x4, int32_t* iterations, int32_t* bfgs_evaluations) {
-  if (!correspond || !cost || !guess_4x4 || !final_4x4 || !iterations || !bfgs_evaluations) return SM_ERR_BAD_ARGUMENT;
-  float guess[16];
-  for (int i = 0; i < 16; ++i) guess[i] = (float)guess_4x4[i];
-  gicp::OuterOut go;
-  const int rc = gicp::outer_loop(
-      gicp::Options(), guess,
-      [&](const float* transformation, const double* R, int* m) -> int {
-        double T[16];
-        for (int i = 0; i < 16; ++i) T[i] = (double)transformation[i];
-        int32_t mm = 0;
-        const int r = correspond(T, R, &mm, user);
-        *m = (int)mm;
-        return r;
-      },
-      [&](const float* Tf, double* S) -> int {
-        double T[16];
-        for (int i = 0; i < 16; ++i) T[i] = (double)Tf[i];
-        return cost(T, S, user);
-      },
-      &go);
-  if (rc < 0) return SM_ERR_CUDA;
-  for (int i = 0; i < 16; ++i) final_4x4[i] = (double)go.final_T[i];
-  *iterations = go.iterations;
-  *bfgs_evaluations = go.bfgs_evals;
-  return SM_OK;
-}
-
-// test hook: the leaf routine of CalculateNormals (normals.cu leaf_plane_fit) compiled for the host
-int sm_debug_normals_leaf(const double* members_3k, int32_t count, double* mean3, double* normal3, int32_t* kept) {
-  if (!members_3k || !mean3 || !normal3 || !kept) return SM_ERR_BAD_ARGUMENT;
-  const int r = normals_debug_leaf_host(members_3k, count, mean3, normal3);
-  if (r < 0) return SM_ERR_BAD_ARGUMENT;
-  *kept = r;
-  return SM_OK;
-}
-
-// test hook: the voxel index of a point as the three voxelisations compute it, compiled for the host
-int sm_debug_voxel_index(int32_t op, const float* p3, float param, int32_t min_b, int64_t* out4) {
-  if (!p3 || !out4) return SM_ERR_BAD_ARGUMENT;
-  switch (op) {
-    case 0: {   // submap filter (filter_voxel_grid.cc:50-52): lround(x / voxel); out[3] = 0 when the point is dropped
-      long long ix[3] = {0, 0, 0};
-      const bool ok = vf_debug_index_host(p3, param, ix);
-      out4[0] = ix[0]; out4[1] = ix[1]; out4[2] = ix[2]; out4[3] = ok ? 1 : 0;
-      return SM_OK;
-    }
-    case 1:     // NDT grid (voxel_grid_covariance_omp_impl.hpp:218-220): int(floor(x * inv) - float(min_b)), per axis
-      for (int d = 0; d < 3; ++d) out4[d] = ndt_debug_voxel_coord_host(p3[d], param, min_b);
-      out4[3] = 1;
-      return SM_OK;
-    case 2: {   // ApproximateVoxelGrid: floor(x * inv) per axis and the 512-slot hash
-      int ix[3]; uint32_t slot = 0;
-      gicp_debug_approx_cell_host(p3, param, ix, &slot);
-      out4[0] = ix[0]; out4[1] = ix[1]; out4[2] = ix[2]; out4[3] = (int64_t)slot;
-      return SM_OK;
-    }
-    default: return SM_ERR_BAD_ARGUMENT;
-  }
-}
-
-// test hook: the per-point arithmetic of the GICP kernels (gicp.cu mahalanobis / cost_terms) compiled for the host
-int sm_debug_gicp_point(int32_t op, const double* in, double* out) {
-  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
-  switch (op) {
-    case 0: gicp_debug_mahalanobis_host(in, in + 9, in + 18, out); return SM_OK;   // in = R[9], C1[9], C2[9] row-major
-    case 1: {   // in = T[16], base[16] (col-major, cast to float), p_src[3], p_tgt[3] (cast to float), M[9]
-      float T[16], base[16], ps[3], pt[3];
-      for (int i = 0; i < 16; ++i) { T[i] = (float)in[i]; base[i] = (float)in[16 + i]; }
-      for (int i = 0; i < 3; ++i) { ps[i] = (float)in[32 + i]; pt[i] = (float)in[35 + i]; }
-      gicp_debug_cost_terms_host(T, base, ps, pt, in + 38, out);
-      return SM_OK;
-    }
-    default: return SM_ERR_BAD_ARGUMENT;
-  }
-}
-
-// test hook: the host pieces of the GICP stage other than the minimiser (csrc/gicp_host.h), no GPU involved
-int sm_debug_gicp_host(int32_t op, const double* in, double* out) {
-  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
-  switch (op) {
-    case 0: {   // applyState (gicp_omp_impl.hpp:516-527): in = T[16] col-major (cast to float), x[6]; out = T'[16]
-      float T[16];
-      for (int i = 0; i < 16; ++i) T[i] = (float)in[i];
-      gicp::apply_state(T, in + 16);
-      for (int i = 0; i < 16; ++i) out[i] = (double)T[i];
-      return SM_OK;
-    }
-    case 1:     // computeRDerivative (:133-183): in = x[6], R[9] row-major; out[0..2] = g[3..5]
-      { double g[6] = {0, 0, 0, 0, 0, 0}; gicp::r_derivative(in, in + 6, g); out[0] = g[3]; out[1] = g[4]; out[2] = g[5]; }
-      return SM_OK;
-    default: return SM_ERR_BAD_ARGUMENT;
-  }
-}
-
-// test hook: the per-match contribution to the point-to-plane normal equations (icp_dev.cuh match_terms /
-// add_terms, the functions icp_accum_kernel and icp_finish_kernel call) and the pose-update helpers of
-// linalg_dev.cuh, compiled for the HOST
-int sm_debug_icp_host(int32_t op, const double* in, int64_t n, double* out) {
-  if (!in || !out || n < 0) return SM_ERR_BAD_ARGUMENT;
-  switch (op) {
-    case 0: {   // in = n records {p[3], q[3], normal[3], d2}; out = the 29 sums, matches added in order
-      for (int k = 0; k < dev::kNumSums; ++k) out[k] = 0.0;
-      for (int64_t i = 0; i < n; ++i) {
-        const double* r = in + 10 * i;
-        BucketPoint q; q.x = r[3]; q.y = r[4]; q.z = r[5];
-        BucketNormal nn; nn.x = r[6]; nn.y = r[7]; nn.z = r[8];
-        double F[6], dot;
-        dev::match_terms(r[0], r[1], r[2], q, nn, F, dot);
-        dev::add_terms(out, F, dot, r[9]);
-      }
-      return SM_OK;
-    }
-    case 1: la::angle_axis_to_rotation(in[0], in + 1, out); return SM_OK;          // out = R[9] row-major
-    case 2: la::rotation_to_quaternion(in, out); return SM_OK;                     // in = R[9], out = {w, x, y, z}
-    case 3: out[0] = la::quaternion_angular_distance(in, in + 4); return SM_OK;    // in = two quaternions
-    case 4: la::mul4(in, in + 16, out); return SM_OK;                              // column-major 4x4 product
-    default: return SM_ERR_BAD_ARGUMENT;
-  }
-}
-
-// test hook: one leaf of the NDT target grid (ndt.cu finish_leaf: covariance, eigen-inflation, inverse) on the host
-int sm_debug_ndt_leaf(const float* points_3n, int32_t n, int32_t min_points, double eig_mult, double* mean3,
-                      double* icov9, float* centroid3, int32_t* nr_points, int32_t* searchable) {
-  if (!points_3n || n <= 0 || !mean3 || !icov9 || !centroid3 || !nr_points || !searchable) return SM_ERR_BAD_ARGUMENT;
-  int np = 0, se = 0;
-  ndt_debug_leaf_host(points_3n, n, min_points, eig_mult, mean3, icov9, centroid3, &np, &se);
-  *nr_points = np; *searchable = se;
-  return SM_OK;
-}
-
-// test hook: the per-(point, voxel) derivative term of ndt.cu (update_derivatives / update_derivatives_f64, the
-// functions ndt_derivatives_kernel calls) compiled for the HOST, with the evaluation parameters built by the
-// product's own host code (ndt_host.h) for pose vector p — no GPU involved
-int sm_debug_ndt_term(const double* p6, double outlier_ratio, float resolution, int32_t f64_math, const float* x_orig,
-                      const float* x_trans, const double* mean3, const double* icov9, double* out43) {
-  if (!p6 || !x_orig || !x_trans || !mean3 || !icov9 || !out43) return SM_ERR_BAD_ARGUMENT;
-  ndt::Options o;
-  o.outlier_ratio = outlier_ratio;
-  o.resolution = resolution;
-  NdtEvalParams P;
-  memset(&P, 0, sizeof(P));
-  ndt::gauss_constants(o, &P.gauss_d1, &P.gauss_d2);
-  ndt::angle_tables(p6, &P);
-  ndt::transform_from_p(p6, P.T);
-  P.radius = resolution;
-  P.f64_math = f64_math ? 1 : 0;
-  ndt_debug_term_host(P, x_orig, x_trans, mean3, icov9, out43);
-  return SM_OK;
-}
-
-// test hook (include/sm_b200_debug.h): the scalar host pieces of the NDT Newton loop, no GPU involved
-int sm_debug_ndt_host(int32_t op, const double* in, double* out) {
-  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
-  switch (op) {
-    case 0: ndt::svd_solve6(in, in + 36, out); return SM_OK;
-    case 1: {
-      float T[16];
-      ndt::transform_from_p(in, T);
-      for (int i = 0; i < 16; ++i) out[i] = (double)T[i];
-      return SM_OK;
-    }
-    case 2: {
-      float T[16];
-      for (int i = 0; i < 16; ++i) T[i] = (float)in[i];
-      ndt::p_from_transform(T, out);
-      return SM_OK;
-    }
-    case 3: {
-      ndt::Options o;
-      o.outlier_ratio = in[0];
-      o.resolution = (float)in[1];
-      ndt::gauss_constants(o, &out[0], &out[1]);
-      return SM_OK;
-    }
-    default: return SM_ERR_BAD_ARGUMENT;
-  }
-}
-
-int sm_debug_bfgs_minimize(sm_debug_fdf fn, void* user, double* x, double grad_tol, int32_t max_iterations,
-                           int32_t* iterations, int32_t* evaluations, int32_t* status) {
-  if (!fn || !x || !iterations || !evaluations || !status) return SM_ERR_BAD_ARGUMENT;
-  int evals = 0;
-  gicp::Minimizer mz;
-  mz.fdf = [&](const double* xx, double* f, double* g) -> int { ++evals; return fn(xx, f, g, user); };
-  mz.init(x);
-  int result = gicp::kRunning, inner = 0;
-  do {                                   // gicp_omp_impl.hpp:225-240
-    ++inner;
-    result = mz.one_step(x);
-    if (result) break;
-    result = mz.test_gradient(grad_tol);
-  } while (result == gicp::kRunning && inner < max_iterations);
-  *iterations = inner; *evaluations = evals; *status = mz.failed ? gicp::kError : result;
-  return SM_OK;
-}
-
 double sm_get_fitness_score(const sm_handle* h) { return h ? h->final_score : 0.0; }
 
 int sm_get_align_info(const sm_handle* h, sm_align_info* out) {
@@ -1533,7 +1177,7 @@ static int knn1_impl(int device, const double* target, int64_t nt, const double*
   SMB_RC(ws.carve(kdws, (int)nt, bucket));
   SMB_RC(ids_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(int32_t)));
   SMB_RC(d2_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(double)));
-  SMB_RC(items.reserve(((size_t)nq + kKnnItemSlack) * sizeof(int4)));
+  SMB_RC(items.reserve(knn_items_bytes((int)nq)));
   SMB_RC(upload_soa(target, nt, false, stage, (double*)tgt.p, ts, s));
   SMB_CUDA_OK(cudaStreamSynchronize(s));
   SMB_RC(tree.build((const double*)tgt.p, nullptr, ts, (int)nt, bucket, ws, s));
@@ -1545,211 +1189,6 @@ static int knn1_impl(int device, const double* target, int64_t nt, const double*
     SMB_CUDA_OK(cudaMemcpyAsync(d2, d2_d.p, (size_t)nq * sizeof(double), cudaMemcpyDeviceToHost, s));
   }
   SMB_CUDA_OK(cudaStreamSynchronize(s));
-  return SM_OK;
-}
-
-// ---- test hooks of the Ndt / NdtWithGicp device stages (include/sm_b200_debug.h) ------------------------------------
-// Each runs the product's own launch functions on buffers of its own, on the default stream, with no handle.
-static int debug_set_device(int device) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  if (device < 0 || device >= ndev) return SM_ERR_BAD_ARGUMENT;
-  SMB_CUDA_OK(cudaSetDevice(device));
-  return SM_OK;
-}
-
-// a packed float xyz cloud of n points copied into buf
-static int debug_upload_f32(const float* pts, int64_t n, DevBuf& buf) {
-  SMB_RC(buf.reserve((size_t)n * 12 + 64));
-  SMB_CUDA_OK(cudaMemcpy(buf.p, pts, (size_t)n * 12, cudaMemcpyHostToDevice));
-  return SM_OK;
-}
-
-static bool debug_cloud_ok(const float* pts, int64_t n) { return pts && n > 0 && n <= (1 << 24); }
-
-// ndt_build_grid over the target, with a workspace sized for ns source points
-static int debug_ndt_build(const float* target, int64_t nt, int64_t ns, float resolution, DevBuf& tgt, DevBuf& wsbuf,
-                           NdtWorkspace& ws, NdtGrid* grid) {
-  SMB_RC(debug_upload_f32(target, nt, tgt));
-  SMB_RC(wsbuf.reserve(NdtWorkspace::bytes_needed((int)nt, (int)ns)));
-  ws.carve(wsbuf.p, (int)nt, (int)ns);
-  SMB_RC(ndt_build_grid((const float*)tgt.p, (int)nt, resolution, ws, nullptr));
-  SMB_CUDA_OK(cudaMemcpy(grid, ws.grid, sizeof(NdtGrid), cudaMemcpyDeviceToHost));
-  return SM_OK;
-}
-
-int sm_debug_ndt_grid(int device, const float* target_3n, int64_t n, float resolution, int32_t* n_voxels,
-                      int32_t* overflow, int32_t* key, int32_t* nr_points, int32_t* searchable, double* mean_3,
-                      double* icov_9, float* centroid_3) {
-  if (!debug_cloud_ok(target_3n, n) || !(resolution > 0.0f) || !n_voxels || !overflow || !key || !nr_points ||
-      !searchable || !mean_3 || !icov_9 || !centroid_3)
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
-  DevBuf tgt, wsbuf;
-  NdtWorkspace ws;
-  NdtGrid g;
-  SMB_RC(debug_ndt_build(target_3n, n, 1, resolution, tgt, wsbuf, ws, &g));
-  const int nv = g.n_voxels;
-  std::vector<int> keys((size_t)nv);
-  std::vector<NdtLeaf> leaves((size_t)nv);
-  SMB_CUDA_OK(cudaMemcpy(keys.data(), ws.voxel_key, (size_t)nv * sizeof(int), cudaMemcpyDeviceToHost));
-  SMB_CUDA_OK(cudaMemcpy(leaves.data(), ws.leaves, (size_t)nv * sizeof(NdtLeaf), cudaMemcpyDeviceToHost));
-  *n_voxels = nv;
-  *overflow = g.overflow;
-  for (int v = 0; v < nv; ++v) {
-    const NdtLeaf& l = leaves[(size_t)v];
-    key[v] = keys[(size_t)v]; nr_points[v] = l.nr_points; searchable[v] = l.searchable;
-    for (int d = 0; d < 3; ++d) { mean_3[3 * v + d] = l.mean[d]; centroid_3[3 * v + d] = l.centroid[d]; }
-    for (int q = 0; q < 9; ++q) icov_9[9 * v + q] = l.icov[q];
-  }
-  return SM_OK;
-}
-
-int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, const float* source_3n, int64_t ns,
-                      float resolution, double outlier_ratio, int32_t f64_math, const double* p_6k, int32_t n_poses,
-                      double* sums_44k) {
-  if (!debug_cloud_ok(target_3n, nt) || !debug_cloud_ok(source_3n, ns) || !(resolution > 0.0f) || !p_6k ||
-      n_poses <= 0 || !sums_44k)
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
-  DevBuf tgt, src, wsbuf;
-  NdtWorkspace ws;
-  NdtGrid g;
-  SMB_RC(debug_ndt_build(target_3n, nt, ns, resolution, tgt, wsbuf, ws, &g));
-  SMB_RC(debug_upload_f32(source_3n, ns, src));
-  ndt::Options o;                      // the evaluation parameters as sm_debug_ndt_term builds them
-  o.outlier_ratio = outlier_ratio;
-  o.resolution = resolution;
-  for (int k = 0; k < n_poses; ++k) {
-    NdtEvalParams P;
-    memset(&P, 0, sizeof(P));
-    ndt::gauss_constants(o, &P.gauss_d1, &P.gauss_d2);
-    ndt::angle_tables(p_6k + 6 * k, &P);
-    ndt::transform_from_p(p_6k + 6 * k, P.T);
-    P.radius = resolution;
-    P.f64_math = f64_math ? 1 : 0;
-    SMB_RC(ndt_eval((const float*)src.p, (int)ns, P, ws, nullptr));
-    SMB_CUDA_OK(cudaMemcpy(sums_44k + 44 * (int64_t)k, ws.sums, 44 * sizeof(double), cudaMemcpyDeviceToHost));
-  }
-  return SM_OK;
-}
-
-int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const double* query_3m, int64_t nq,
-                            int32_t k, int32_t* ids, double* d2) {
-  if (!debug_cloud_ok(cloud_3n, n) || !query_3m || nq <= 0 || nq > (1 << 24) || (k != 1 && k != 20) || !ids || !d2 ||
-      kd_num_levels((int)n, 8) > 24)
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
-  DevBuf cloud, kdws, q, ids_d, d2_d;
-  FloatTree t;
-  SMB_RC(debug_upload_f32(cloud_3n, n, cloud));
-  SMB_RC(t.build((const float*)cloud.p, (int)n, kdws, nullptr));
-  SMB_RC(q.reserve((size_t)nq * 3 * sizeof(double)));
-  SMB_RC(ids_d.reserve((size_t)nq * k * sizeof(int32_t)));
-  SMB_RC(d2_d.reserve((size_t)nq * k * sizeof(double)));
-  SMB_CUDA_OK(cudaMemcpy(q.p, query_3m, (size_t)nq * 3 * sizeof(double), cudaMemcpyHostToDevice));
-  SMB_RC(float_tree_debug_knn(t, (const double*)q.p, (int)nq, k, (int32_t*)ids_d.p, (double*)d2_d.p, nullptr));
-  SMB_CUDA_OK(cudaMemcpy(ids, ids_d.p, (size_t)nq * k * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  SMB_CUDA_OK(cudaMemcpy(d2, d2_d.p, (size_t)nq * k * sizeof(double), cudaMemcpyDeviceToHost));
-  return SM_OK;
-}
-
-int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,
-                               int64_t* m_out) {
-  if (!debug_cloud_ok(points_3n, n) || !(leaf > 0.0f) || !out_3n || !m_out) return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
-  DevBuf pts, wsbuf, out, counter;
-  SMB_RC(debug_upload_f32(points_3n, n, pts));
-  SMB_RC(wsbuf.reserve(approx_ws_bytes((int)n)));
-  SMB_RC(out.reserve((size_t)n * 12 + 64));
-  SMB_RC(counter.reserve(64));
-  uint32_t* cnt = (uint32_t*)counter.p;
-  SMB_RC(approx_voxel_grid((const float*)pts.p, (int)n, leaf, wsbuf.p, (float*)out.p, cnt, nullptr));
-  uint32_t m = 0;
-  SMB_CUDA_OK(cudaMemcpy(&m, cnt, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-  SMB_RC(approx_voxel_grid_emit((int)n, (int)m, wsbuf.p, (float*)out.p, cnt, nullptr));
-  SMB_CUDA_OK(cudaMemcpy(out_3n, out.p, (size_t)m * 12, cudaMemcpyDeviceToHost));
-  *m_out = (int64_t)m;
-  return SM_OK;
-}
-
-// GICP covariances of a cloud as gicp_run forms them: its own float tree, gicp_covariances, zeros below k points
-static int debug_gicp_cov(const float* cloud_dev, int64_t n, FloatTree& t, DevBuf& kdws, DevBuf& cov) {
-  const gicp::Options o;
-  SMB_RC(t.build(cloud_dev, (int)n, kdws, nullptr));
-  SMB_RC(cov.reserve((size_t)n * 9 * sizeof(double)));
-  if (o.k_correspondences <= n)
-    SMB_RC(gicp_covariances(cloud_dev, (int)n, (const KdNode*)t.nodes.p, (const BucketPoint*)t.bpts.p, o.gicp_epsilon,
-                            (double*)cov.p, nullptr));
-  else SMB_CUDA_OK(cudaMemset(cov.p, 0, (size_t)n * 9 * sizeof(double)));
-  return SM_OK;
-}
-
-int sm_debug_gicp_covariances(int device, const float* cloud_3n, int64_t n, double* covs_9n) {
-  if (!debug_cloud_ok(cloud_3n, n) || !covs_9n || kd_num_levels((int)n, 8) > 24) return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
-  DevBuf cloud, kdws, cov;
-  FloatTree t;
-  SMB_RC(debug_upload_f32(cloud_3n, n, cloud));
-  SMB_RC(debug_gicp_cov((const float*)cloud.p, n, t, kdws, cov));
-  SMB_CUDA_OK(cudaMemcpy(covs_9n, cov.p, (size_t)n * 9 * sizeof(double), cudaMemcpyDeviceToHost));
-  return SM_OK;
-}
-
-int sm_debug_gicp_step(int device, const float* source_3n, int64_t ns, const float* target_3n, int64_t nt,
-                       const double* guess_4x4, const double* transformation_4x4, const double* x_6k, int32_t n_states,
-                       int32_t* match, double* maha_9n, int32_t* count, double* sums_13k) {
-  if (!debug_cloud_ok(source_3n, ns) || !debug_cloud_ok(target_3n, nt) || !guess_4x4 || !transformation_4x4 ||
-      !x_6k || n_states <= 0 || !match || !maha_9n || !count || !sums_13k || kd_num_levels((int)ns, 8) > 24 ||
-      kd_num_levels((int)nt, 8) > 24)
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
-  const gicp::Options o;
-  DevBuf src, tgt, kdws, cov_s, cov_t, maha_d, match_d, partials, counter;
-  FloatTree st, tt;
-  SMB_RC(debug_upload_f32(source_3n, ns, src));
-  SMB_RC(debug_upload_f32(target_3n, nt, tgt));
-  SMB_RC(debug_gicp_cov((const float*)tgt.p, nt, tt, kdws, cov_t));
-  SMB_RC(debug_gicp_cov((const float*)src.p, ns, st, kdws, cov_s));
-  SMB_RC(maha_d.reserve((size_t)ns * 9 * sizeof(double)));
-  SMB_RC(match_d.reserve((size_t)ns * sizeof(int32_t)));
-  SMB_RC(partials.reserve((size_t)(gicp_cost_blocks((int)ns) + 1) * 13 * sizeof(double) + 256));
-  SMB_RC(counter.reserve(64));
-  SMB_CUDA_OK(cudaMemset(counter.p, 0, 64));
-  double* sums_dev = (double*)partials.p + (size_t)gicp_cost_blocks((int)ns) * 13;
-  uint32_t* ticket_dev = (uint32_t*)counter.p + 8;
-  float guess[16];
-  GicpIterParams IP;
-  for (int i = 0; i < 16; ++i) {
-    guess[i] = (float)guess_4x4[i];
-    IP.guess[i] = guess[i];
-    IP.transformation[i] = (float)transformation_4x4[i];
-  }
-  for (int i = 0; i < 3; ++i)          // R = rot(transformation_ * guess) in double, as gicp::outer_loop forms it
-    for (int j = 0; j < 3; ++j) {
-      double s = 0.0;
-      for (int k = 0; k < 4; ++k) s += (double)IP.transformation[i + 4 * k] * (double)guess[k + 4 * j];
-      IP.R[i * 3 + j] = s;
-    }
-  IP.dist_threshold = o.corr_dist_threshold * o.corr_dist_threshold;
-  SMB_RC(gicp_correspond((const float*)src.p, (int)ns, (const float*)tgt.p, IP, (const KdNode*)tt.nodes.p,
-                         (const BucketPoint*)tt.bpts.p, (const double*)cov_s.p, (const double*)cov_t.p,
-                         (int32_t*)match_d.p, (double*)maha_d.p, (uint32_t*)counter.p, nullptr));
-  uint32_t m = 0;
-  SMB_CUDA_OK(cudaMemcpy(&m, counter.p, sizeof(uint32_t), cudaMemcpyDeviceToHost));
-  SMB_CUDA_OK(cudaMemcpy(match, match_d.p, (size_t)ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
-  SMB_CUDA_OK(cudaMemcpy(maha_9n, maha_d.p, (size_t)ns * 9 * sizeof(double), cudaMemcpyDeviceToHost));
-  *count = (int32_t)m;
-  // the evaluations share one ticket, as the BFGS evaluations of an outer iteration do: each relies on the
-  // previous one's last block having reset it
-  for (int k = 0; k < n_states; ++k) {
-    GicpCostParams CP;
-    for (int i = 0; i < 16; ++i) { CP.T[i] = guess[i]; CP.base[i] = guess[i]; }
-    gicp::apply_state(CP.T, x_6k + 6 * k);
-    SMB_RC(gicp_cost((const float*)src.p, (int)ns, (const float*)tgt.p, CP, (const int32_t*)match_d.p,
-                     (const double*)maha_d.p, (double*)partials.p, sums_dev, ticket_dev, nullptr, nullptr, 0, nullptr));
-    SMB_CUDA_OK(cudaMemcpy(sums_13k + 13 * (int64_t)k, sums_dev, 13 * sizeof(double), cudaMemcpyDeviceToHost));
-  }
   return SM_OK;
 }
 

@@ -1,0 +1,439 @@
+// Test hooks of include/sm_b200_debug.h: the product's host code driven by a caller's callbacks, its device math
+// compiled for the host, and its Ndt / NdtWithGicp device stages run on buffers of their own.
+#include "../../include/sm_b200.h"
+#include "../../include/sm_b200_debug.h"
+
+#include <vector>
+
+#include "common.cuh"
+#include "icp_dev.cuh"
+#include "kernels.h"
+#include "linalg_dev.cuh"
+#include "gicp_host.h"
+#include "ndt_host.h"
+
+namespace smb {
+namespace {
+
+__global__ void debug_solve6_kernel(const double* __restrict__ A, const double* __restrict__ b, double* __restrict__ x,
+                                    int* __restrict__ path) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) *path = la::solve_possibly_underdetermined(A, b, x);
+}
+
+}  // namespace
+}  // namespace smb
+
+using namespace smb;
+
+extern "C" {
+
+int sm_debug_solve6(int device, const double* A, const double* b, double* x, int32_t* path) {
+  if (!A || !b || !x || !path) return SM_ERR_BAD_ARGUMENT;
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
+  SMB_CUDA_OK(cudaSetDevice(device));
+  DevBuf buf;
+  SMB_RC(buf.reserve(64 * sizeof(double)));
+  double* d = (double*)buf.p;
+  SMB_CUDA_OK(cudaMemcpy(d, A, 36 * sizeof(double), cudaMemcpyHostToDevice));
+  SMB_CUDA_OK(cudaMemcpy(d + 36, b, 6 * sizeof(double), cudaMemcpyHostToDevice));
+  debug_solve6_kernel<<<1, 32>>>(d, d + 36, d + 42, reinterpret_cast<int*>(d + 48));
+  int p = 0;
+  SMB_CUDA_OK(cudaMemcpy(x, d + 42, 6 * sizeof(double), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(&p, d + 48, sizeof(int), cudaMemcpyDeviceToHost));
+  *path = p;
+  return SM_OK;
+}
+
+// test hook: csrc/linalg_dev.cuh's solver (the code icp_finish_kernel runs when its Cholesky certificate is not
+// conclusive) compiled for the HOST, so the product's transcription is checked against numpy without a GPU
+int sm_debug_solve6_host(const double* A, const double* b, double* x, int32_t* path) {
+  if (!A || !b || !x || !path) return SM_ERR_BAD_ARGUMENT;
+  *path = la::solve_possibly_underdetermined(A, b, x);
+  return SM_OK;
+}
+
+// test hook: the NDT Newton loop of the product (ndt_host.h newton_loop, the function ndt_run drives the device
+// with) over a caller-supplied evaluation — no GPU involved
+int sm_debug_ndt_newton(sm_debug_ndt_eval fn, void* user, const double* guess_4x4, int32_t n_source, float resolution,
+                        double step_size, double outlier_ratio, double transformation_epsilon, int32_t max_iterations,
+                        double* final_4x4, int32_t* iterations, int32_t* evaluations, double* score) {
+  if (!fn || !guess_4x4 || !final_4x4 || !iterations || !evaluations || !score || n_source <= 0)
+    return SM_ERR_BAD_ARGUMENT;
+  ndt::Options o;
+  o.resolution = resolution; o.step_size = step_size; o.outlier_ratio = outlier_ratio;
+  o.transformation_epsilon = transformation_epsilon; o.max_iterations = max_iterations;
+  NdtEvalParams P = ndt::eval_params(o, false);
+  ndt::NewtonOut nw;
+  const int rc = ndt::newton_loop(o, guess_4x4, n_source, P, [&](const NdtEvalParams& Pe, const double* p6, double* sums) -> int {
+    double T[16];
+    for (int i = 0; i < 16; ++i) T[i] = (double)Pe.T[i];
+    return fn(T, p6, sums, user);
+  }, &nw);
+  if (rc < 0) return rc;
+  for (int i = 0; i < 16; ++i) final_4x4[i] = (double)nw.final_T[i];
+  *iterations = nw.iterations; *evaluations = nw.evaluations; *score = nw.score;
+  return SM_OK;
+}
+
+// test hook: the GICP outer loop of the product (gicp_host.h outer_loop: start vector, f / g from the 13 sums, BFGS
+// driver, convergence test, final composition — the function gicp_run drives the device with) over a caller's
+// correspondence and cost functions; no GPU involved
+int sm_debug_gicp_outer(sm_debug_gicp_correspond correspond, sm_debug_gicp_cost cost, void* user, const double* guess_4x4,
+                        double* final_4x4, int32_t* iterations, int32_t* bfgs_evaluations) {
+  if (!correspond || !cost || !guess_4x4 || !final_4x4 || !iterations || !bfgs_evaluations) return SM_ERR_BAD_ARGUMENT;
+  float guess[16];
+  for (int i = 0; i < 16; ++i) guess[i] = (float)guess_4x4[i];
+  gicp::OuterOut go;
+  const int rc = gicp::outer_loop(
+      gicp::Options(), guess,
+      [&](const float* transformation, const double* R, int* m) -> int {
+        double T[16];
+        for (int i = 0; i < 16; ++i) T[i] = (double)transformation[i];
+        int32_t mm = 0;
+        const int r = correspond(T, R, &mm, user);
+        *m = (int)mm;
+        return r;
+      },
+      [&](const float* Tf, double* S) -> int {
+        double T[16];
+        for (int i = 0; i < 16; ++i) T[i] = (double)Tf[i];
+        return cost(T, S, user);
+      },
+      &go);
+  if (rc < 0) return SM_ERR_CUDA;
+  for (int i = 0; i < 16; ++i) final_4x4[i] = (double)go.final_T[i];
+  *iterations = go.iterations;
+  *bfgs_evaluations = go.bfgs_evals;
+  return SM_OK;
+}
+
+// test hook: the leaf routine of CalculateNormals (normals.cu leaf_plane_fit) compiled for the host
+int sm_debug_normals_leaf(const double* members_3k, int32_t count, double* mean3, double* normal3, int32_t* kept) {
+  if (!members_3k || !mean3 || !normal3 || !kept) return SM_ERR_BAD_ARGUMENT;
+  const int r = normals_debug_leaf_host(members_3k, count, mean3, normal3);
+  if (r < 0) return SM_ERR_BAD_ARGUMENT;
+  *kept = r;
+  return SM_OK;
+}
+
+// test hook: the voxel index of a point as the three voxelisations compute it, compiled for the host
+int sm_debug_voxel_index(int32_t op, const float* p3, float param, int32_t min_b, int64_t* out4) {
+  if (!p3 || !out4) return SM_ERR_BAD_ARGUMENT;
+  switch (op) {
+    case 0: {   // submap filter (filter_voxel_grid.cc:50-52): lround(x / voxel); out[3] = 0 when the point is dropped
+      long long ix[3] = {0, 0, 0};
+      const bool ok = vf_debug_index_host(p3, param, ix);
+      out4[0] = ix[0]; out4[1] = ix[1]; out4[2] = ix[2]; out4[3] = ok ? 1 : 0;
+      return SM_OK;
+    }
+    case 1:     // NDT grid (voxel_grid_covariance_omp_impl.hpp:218-220): int(floor(x * inv) - float(min_b)), per axis
+      for (int d = 0; d < 3; ++d) out4[d] = ndt_debug_voxel_coord_host(p3[d], param, min_b);
+      out4[3] = 1;
+      return SM_OK;
+    case 2: {   // ApproximateVoxelGrid: floor(x * inv) per axis and the 512-slot hash
+      int ix[3]; uint32_t slot = 0;
+      gicp_debug_approx_cell_host(p3, param, ix, &slot);
+      out4[0] = ix[0]; out4[1] = ix[1]; out4[2] = ix[2]; out4[3] = (int64_t)slot;
+      return SM_OK;
+    }
+    default: return SM_ERR_BAD_ARGUMENT;
+  }
+}
+
+// test hook: the per-point arithmetic of the GICP kernels (gicp.cu mahalanobis / cost_terms) compiled for the host
+int sm_debug_gicp_point(int32_t op, const double* in, double* out) {
+  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
+  switch (op) {
+    case 0: gicp_debug_mahalanobis_host(in, in + 9, in + 18, out); return SM_OK;   // in = R[9], C1[9], C2[9] row-major
+    case 1: {   // in = T[16], base[16] (col-major, cast to float), p_src[3], p_tgt[3] (cast to float), M[9]
+      float T[16], base[16], ps[3], pt[3];
+      for (int i = 0; i < 16; ++i) { T[i] = (float)in[i]; base[i] = (float)in[16 + i]; }
+      for (int i = 0; i < 3; ++i) { ps[i] = (float)in[32 + i]; pt[i] = (float)in[35 + i]; }
+      gicp_debug_cost_terms_host(T, base, ps, pt, in + 38, out);
+      return SM_OK;
+    }
+    default: return SM_ERR_BAD_ARGUMENT;
+  }
+}
+
+// test hook: the host pieces of the GICP stage other than the minimiser (csrc/gicp_host.h), no GPU involved
+int sm_debug_gicp_host(int32_t op, const double* in, double* out) {
+  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
+  switch (op) {
+    case 0: {   // applyState (gicp_omp_impl.hpp:516-527): in = T[16] col-major (cast to float), x[6]; out = T'[16]
+      float T[16];
+      for (int i = 0; i < 16; ++i) T[i] = (float)in[i];
+      gicp::apply_state(T, in + 16);
+      for (int i = 0; i < 16; ++i) out[i] = (double)T[i];
+      return SM_OK;
+    }
+    case 1:     // computeRDerivative (:133-183): in = x[6], R[9] row-major; out[0..2] = g[3..5]
+      { double g[6] = {0, 0, 0, 0, 0, 0}; gicp::r_derivative(in, in + 6, g); out[0] = g[3]; out[1] = g[4]; out[2] = g[5]; }
+      return SM_OK;
+    default: return SM_ERR_BAD_ARGUMENT;
+  }
+}
+
+// test hook: the per-match contribution to the point-to-plane normal equations (icp_dev.cuh match_terms /
+// add_terms, the functions icp_accum_kernel and icp_finish_kernel call) and the pose-update helpers of
+// linalg_dev.cuh, compiled for the HOST
+int sm_debug_icp_host(int32_t op, const double* in, int64_t n, double* out) {
+  if (!in || !out || n < 0) return SM_ERR_BAD_ARGUMENT;
+  switch (op) {
+    case 0: {   // in = n records {p[3], q[3], normal[3], d2}; out = the 29 sums, matches added in order
+      for (int k = 0; k < dev::kNumSums; ++k) out[k] = 0.0;
+      for (int64_t i = 0; i < n; ++i) {
+        const double* r = in + 10 * i;
+        BucketPoint q; q.x = r[3]; q.y = r[4]; q.z = r[5];
+        BucketNormal nn; nn.x = r[6]; nn.y = r[7]; nn.z = r[8];
+        double F[6], dot;
+        dev::match_terms(r[0], r[1], r[2], q, nn, F, dot);
+        dev::add_terms(out, F, dot, r[9]);
+      }
+      return SM_OK;
+    }
+    case 1: la::angle_axis_to_rotation(in[0], in + 1, out); return SM_OK;          // out = R[9] row-major
+    case 2: la::rotation_to_quaternion(in, out); return SM_OK;                     // in = R[9], out = {w, x, y, z}
+    case 3: out[0] = la::quaternion_angular_distance(in, in + 4); return SM_OK;    // in = two quaternions
+    case 4: la::mul4(in, in + 16, out); return SM_OK;                              // column-major 4x4 product
+    default: return SM_ERR_BAD_ARGUMENT;
+  }
+}
+
+// test hook: one leaf of the NDT target grid (ndt.cu finish_leaf: covariance, eigen-inflation, inverse) on the host
+int sm_debug_ndt_leaf(const float* points_3n, int32_t n, int32_t min_points, double eig_mult, double* mean3,
+                      double* icov9, float* centroid3, int32_t* nr_points, int32_t* searchable) {
+  if (!points_3n || n <= 0 || !mean3 || !icov9 || !centroid3 || !nr_points || !searchable) return SM_ERR_BAD_ARGUMENT;
+  int np = 0, se = 0;
+  ndt_debug_leaf_host(points_3n, n, min_points, eig_mult, mean3, icov9, centroid3, &np, &se);
+  *nr_points = np; *searchable = se;
+  return SM_OK;
+}
+
+// test hook: the per-(point, voxel) derivative term of ndt.cu (update_derivatives / update_derivatives_f64, the
+// functions ndt_derivatives_kernel calls) compiled for the HOST, with the evaluation parameters built by the
+// product's own host code (ndt_host.h) for pose vector p — no GPU involved
+int sm_debug_ndt_term(const double* p6, double outlier_ratio, float resolution, int32_t f64_math, const float* x_orig,
+                      const float* x_trans, const double* mean3, const double* icov9, double* out43) {
+  if (!p6 || !x_orig || !x_trans || !mean3 || !icov9 || !out43) return SM_ERR_BAD_ARGUMENT;
+  ndt::Options o;
+  o.outlier_ratio = outlier_ratio;
+  o.resolution = resolution;
+  ndt_debug_term_host(ndt::eval_params(o, f64_math != 0, p6), x_orig, x_trans, mean3, icov9, out43);
+  return SM_OK;
+}
+
+// test hook (include/sm_b200_debug.h): the scalar host pieces of the NDT Newton loop, no GPU involved
+int sm_debug_ndt_host(int32_t op, const double* in, double* out) {
+  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
+  switch (op) {
+    case 0: ndt::svd_solve6(in, in + 36, out); return SM_OK;
+    case 1: {
+      float T[16];
+      ndt::transform_from_p(in, T);
+      for (int i = 0; i < 16; ++i) out[i] = (double)T[i];
+      return SM_OK;
+    }
+    case 2: {
+      float T[16];
+      for (int i = 0; i < 16; ++i) T[i] = (float)in[i];
+      ndt::p_from_transform(T, out);
+      return SM_OK;
+    }
+    case 3: {
+      ndt::Options o;
+      o.outlier_ratio = in[0];
+      o.resolution = (float)in[1];
+      const NdtEvalParams P = ndt::eval_params(o, false);
+      out[0] = P.gauss_d1; out[1] = P.gauss_d2;
+      return SM_OK;
+    }
+    default: return SM_ERR_BAD_ARGUMENT;
+  }
+}
+
+int sm_debug_bfgs_minimize(sm_debug_fdf fn, void* user, double* x, double grad_tol, int32_t max_iterations,
+                           int32_t* iterations, int32_t* evaluations, int32_t* status) {
+  if (!fn || !x || !iterations || !evaluations || !status) return SM_ERR_BAD_ARGUMENT;
+  int evals = 0;
+  gicp::Minimizer mz;
+  mz.fdf = [&](const double* xx, double* f, double* g) -> int { ++evals; return fn(xx, f, g, user); };
+  mz.init(x);
+  int result = gicp::kRunning, inner = 0;
+  do {                                   // gicp_omp_impl.hpp:225-240
+    ++inner;
+    result = mz.one_step(x);
+    if (result) break;
+    result = mz.test_gradient(grad_tol);
+  } while (result == gicp::kRunning && inner < max_iterations);
+  *iterations = inner; *evaluations = evals; *status = mz.failed ? gicp::kError : result;
+  return SM_OK;
+}
+
+// ---- test hooks of the Ndt / NdtWithGicp device stages (include/sm_b200_debug.h) ------------------------------------
+// Each runs the product's own launch functions on buffers of its own, on the default stream, with no handle.
+static int debug_set_device(int device) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
+  if (device < 0 || device >= ndev) return SM_ERR_BAD_ARGUMENT;
+  SMB_CUDA_OK(cudaSetDevice(device));
+  return SM_OK;
+}
+
+// a packed float xyz cloud of n points copied into buf
+static int debug_upload_f32(const float* pts, int64_t n, DevBuf& buf) {
+  SMB_RC(buf.reserve((size_t)n * 12 + 64));
+  SMB_CUDA_OK(cudaMemcpy(buf.p, pts, (size_t)n * 12, cudaMemcpyHostToDevice));
+  return SM_OK;
+}
+
+static bool debug_cloud_ok(const float* pts, int64_t n) { return pts && n > 0 && n <= (1 << 24); }
+
+// the NDT grid of the target, in a stage sized for ns source points
+static int debug_ndt_build(const float* target, int64_t nt, int64_t ns, float resolution, DevBuf& tgt, NdtStage& st,
+                           NdtGrid* grid) {
+  SMB_RC(debug_upload_f32(target, nt, tgt));
+  SMB_RC(st.reserve((int)nt, (int)ns));
+  SMB_RC(st.build_grid((const float*)tgt.p, (int)nt, resolution, nullptr));
+  SMB_CUDA_OK(cudaMemcpy(grid, st.ws.grid, sizeof(NdtGrid), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
+int sm_debug_ndt_grid(int device, const float* target_3n, int64_t n, float resolution, int32_t* n_voxels,
+                      int32_t* overflow, int32_t* key, int32_t* nr_points, int32_t* searchable, double* mean_3,
+                      double* icov_9, float* centroid_3) {
+  if (!debug_cloud_ok(target_3n, n) || !(resolution > 0.0f) || !n_voxels || !overflow || !key || !nr_points ||
+      !searchable || !mean_3 || !icov_9 || !centroid_3)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DevBuf tgt;
+  NdtStage st;
+  NdtGrid g;
+  SMB_RC(debug_ndt_build(target_3n, n, 1, resolution, tgt, st, &g));
+  const int nv = g.n_voxels;
+  std::vector<int> keys((size_t)nv);
+  std::vector<NdtLeaf> leaves((size_t)nv);
+  SMB_CUDA_OK(cudaMemcpy(keys.data(), st.ws.voxel_key, (size_t)nv * sizeof(int), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(leaves.data(), st.ws.leaves, (size_t)nv * sizeof(NdtLeaf), cudaMemcpyDeviceToHost));
+  *n_voxels = nv;
+  *overflow = g.overflow;
+  for (int v = 0; v < nv; ++v) {
+    const NdtLeaf& l = leaves[(size_t)v];
+    key[v] = keys[(size_t)v]; nr_points[v] = l.nr_points; searchable[v] = l.searchable;
+    for (int d = 0; d < 3; ++d) { mean_3[3 * v + d] = l.mean[d]; centroid_3[3 * v + d] = l.centroid[d]; }
+    for (int q = 0; q < 9; ++q) icov_9[9 * v + q] = l.icov[q];
+  }
+  return SM_OK;
+}
+
+int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, const float* source_3n, int64_t ns,
+                      float resolution, double outlier_ratio, int32_t f64_math, const double* p_6k, int32_t n_poses,
+                      double* sums_44k) {
+  if (!debug_cloud_ok(target_3n, nt) || !debug_cloud_ok(source_3n, ns) || !(resolution > 0.0f) || !p_6k ||
+      n_poses <= 0 || !sums_44k)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DevBuf tgt, src;
+  NdtStage st;
+  NdtGrid g;
+  SMB_RC(debug_ndt_build(target_3n, nt, ns, resolution, tgt, st, &g));
+  SMB_RC(debug_upload_f32(source_3n, ns, src));
+  ndt::Options o;                      // the evaluation parameters as sm_debug_ndt_term builds them
+  o.outlier_ratio = outlier_ratio;
+  o.resolution = resolution;
+  for (int k = 0; k < n_poses; ++k) {
+    SMB_RC(st.eval((const float*)src.p, (int)ns, ndt::eval_params(o, f64_math != 0, p_6k + 6 * k), sums_44k + 44 * (int64_t)k,
+                   nullptr));
+  }
+  return SM_OK;
+}
+
+int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const double* query_3m, int64_t nq,
+                            int32_t k, int32_t* ids, double* d2) {
+  if (!debug_cloud_ok(cloud_3n, n) || !query_3m || nq <= 0 || nq > (1 << 24) || (k != 1 && k != 20) || !ids || !d2 ||
+      kd_num_levels((int)n, 8) > 24)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DevBuf cloud, kdws, q, ids_d, d2_d;
+  FloatTree t;
+  SMB_RC(debug_upload_f32(cloud_3n, n, cloud));
+  SMB_RC(t.build((const float*)cloud.p, (int)n, kdws, nullptr));
+  SMB_RC(q.reserve((size_t)nq * 3 * sizeof(double)));
+  SMB_RC(ids_d.reserve((size_t)nq * k * sizeof(int32_t)));
+  SMB_RC(d2_d.reserve((size_t)nq * k * sizeof(double)));
+  SMB_CUDA_OK(cudaMemcpy(q.p, query_3m, (size_t)nq * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  SMB_RC(float_tree_debug_knn(t, (const double*)q.p, (int)nq, k, (int32_t*)ids_d.p, (double*)d2_d.p, nullptr));
+  SMB_CUDA_OK(cudaMemcpy(ids, ids_d.p, (size_t)nq * k * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(d2, d2_d.p, (size_t)nq * k * sizeof(double), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
+int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,
+                               int64_t* m_out) {
+  if (!debug_cloud_ok(points_3n, n) || !(leaf > 0.0f) || !out_3n || !m_out) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DevBuf pts, out;
+  ApproxVoxelGrid filter;
+  SMB_RC(debug_upload_f32(points_3n, n, pts));
+  int m = 0;
+  SMB_RC(filter.filter((const float*)pts.p, (int)n, leaf, out, &m, nullptr));
+  SMB_CUDA_OK(cudaMemcpy(out_3n, out.p, (size_t)m * 12, cudaMemcpyDeviceToHost));
+  *m_out = (int64_t)m;
+  return SM_OK;
+}
+
+int sm_debug_gicp_covariances(int device, const float* cloud_3n, int64_t n, double* covs_9n) {
+  if (!debug_cloud_ok(cloud_3n, n) || !covs_9n || kd_num_levels((int)n, 8) > 24) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DevBuf cloud, kdws;
+  gicp::Stage g;                       // the cloud as the stage's source
+  SMB_RC(debug_upload_f32(cloud_3n, n, cloud));
+  SMB_RC(g.source_tree.build((const float*)cloud.p, (int)n, kdws, nullptr));
+  SMB_RC(g.reserve((int)n, (int)n, nullptr));
+  SMB_RC(g.covariances(gicp::Options(), (const float*)cloud.p, (int)n, g.source_tree, g.cov_s, nullptr));
+  SMB_CUDA_OK(cudaMemcpy(covs_9n, g.cov_s.p, (size_t)n * 9 * sizeof(double), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
+int sm_debug_gicp_step(int device, const float* source_3n, int64_t ns, const float* target_3n, int64_t nt,
+                       const double* guess_4x4, const double* transformation_4x4, const double* x_6k, int32_t n_states,
+                       int32_t* match, double* maha_9n, int32_t* count, double* sums_13k) {
+  if (!debug_cloud_ok(source_3n, ns) || !debug_cloud_ok(target_3n, nt) || !guess_4x4 || !transformation_4x4 ||
+      !x_6k || n_states <= 0 || !match || !maha_9n || !count || !sums_13k || kd_num_levels((int)ns, 8) > 24 ||
+      kd_num_levels((int)nt, 8) > 24)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  const gicp::Options o;
+  DevBuf src, tgt, kdws;
+  FloatTree tt;
+  gicp::Stage g;
+  SMB_RC(debug_upload_f32(source_3n, ns, src));
+  SMB_RC(debug_upload_f32(target_3n, nt, tgt));
+  SMB_RC(tt.build((const float*)tgt.p, (int)nt, kdws, nullptr));
+  SMB_RC(g.source_tree.build((const float*)src.p, (int)ns, kdws, nullptr));
+  SMB_RC(g.reserve((int)ns, (int)nt, nullptr));
+  SMB_RC(g.covariances(o, (const float*)tgt.p, (int)nt, tt, g.cov_t, nullptr));
+  SMB_RC(g.covariances(o, (const float*)src.p, (int)ns, g.source_tree, g.cov_s, nullptr));
+  float guess[16], transformation[16];
+  for (int i = 0; i < 16; ++i) { guess[i] = (float)guess_4x4[i]; transformation[i] = (float)transformation_4x4[i]; }
+  double R[9];
+  gicp::outer_rotation(transformation, guess, R);
+  int m = 0;
+  SMB_RC(g.correspond(o, (const float*)src.p, (int)ns, (const float*)tgt.p, tt, guess, transformation, R, nullptr, &m));
+  SMB_CUDA_OK(cudaMemcpy(match, g.match.p, (size_t)ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(maha_9n, g.maha.p, (size_t)ns * 9 * sizeof(double), cudaMemcpyDeviceToHost));
+  *count = (int32_t)m;
+  // the evaluations share one ticket, as the BFGS evaluations of an outer iteration do: each relies on the
+  // previous one's last block having reset it
+  for (int k = 0; k < n_states; ++k) {
+    float T[16];
+    for (int i = 0; i < 16; ++i) T[i] = guess[i];
+    gicp::apply_state(T, x_6k + 6 * k);
+    SMB_RC(g.cost((const float*)src.p, (int)ns, (const float*)tgt.p, T, guess, nullptr, nullptr, nullptr));
+    SMB_CUDA_OK(cudaMemcpy(sums_13k + 13 * (int64_t)k, g.sums, 13 * sizeof(double), cudaMemcpyDeviceToHost));
+  }
+  return SM_OK;
+}
+
+}  // extern "C"
