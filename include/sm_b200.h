@@ -262,7 +262,9 @@ int sm_voxel_grid_filter(int device, const float* points, int64_t n, int64_t str
  * (data::InnerPointType = 20).  descriptor: p*q + l*t floats, l = ceil(sqrt(max_distance / r)) — [u1; v1],
  * the first left / right singular vectors of the p*q x l*t signature matrix (:148-152); A_out (optional):
  * that matrix as counts, row-major.  Returns 1 (true), 0 for an empty cloud (setInputCloud returns false,
- * :130-133), SM_ERR_BAD_ARGUMENT for r < 1e-6 (:64-67) or a too small `capacity`.
+ * :130-133), SM_ERR_BAD_ARGUMENT for r < 1e-6 (:64-67), l*t > 8192, p*q > 256 (the first singular pair is
+ * solved on the host in time cubic in p*q) or a too small `capacity`.  A is zero when the max_distance gate
+ * drops every point, and so is the descriptor.
  * Two orientations are Eigen-internal in the reference and fixed here: each of the first two PCA axes has
  * its component of largest magnitude positive, and so has u1 (v1 follows).  sm_m2dp_match does not depend
  * on the second; the first decides which points the reference's |.| projections fold together.

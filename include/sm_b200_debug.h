@@ -9,6 +9,7 @@
  *     sm_debug_gicp_outer      the GICP outer loop (csrc/gicp_host.h outer_loop, gicp_omp_impl.hpp:381-514, :187-246)
  *     sm_debug_ndt_host        6x6 Jacobi-SVD solve, pose <-> 6-vector with Eigen's eulerAngles(0,1,2), Gauss constants
  *     sm_debug_gicp_host       applyState, computeRDerivative
+ *     sm_debug_m2dp_host       M2DP's two eigenproblems: PCA axes from the float covariance, [u1; v1] from A and A A^T
  *   device math of the product compiled for the host (the same __host__ __device__ source the kernels call)
  *     sm_debug_solve6_host     SolvePossiblyUnderdeterminedLinearSystem (csrc/linalg_dev.cuh, icp_fast.cc:204-254)
  *     sm_debug_icp_host        per-match normal-equation terms, AngleAxis / quaternion / angularDistance helpers
@@ -29,7 +30,9 @@
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
  *     sm_debug_gicp_step       correspondences, Mahalanobis matrices and cost sums of one GICP outer iteration
- *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose */
+ *     sm_debug_m2dp_stages     every intermediate of M2dpStage: mean, covariance, axes, view axes, A, A A^T, descriptor
+ *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
+ *   each stage of M2DP meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
 #define SM_B200_DEBUG_H_
 
@@ -192,6 +195,23 @@ int sm_debug_gicp_covariances(int device, const float* cloud_3n, int64_t n, doub
 int sm_debug_gicp_step(int device, const float* source_3n, int64_t ns, const float* target_3n, int64_t nt,
                        const double* guess_4x4, const double* transformation_4x4, const double* x_6k, int32_t n_states,
                        int32_t* match, double* maha_9n, int32_t* count, double* sums_13k);
+
+/* The host routines of M2dp::setInputCloud (csrc/m2dp.cu), no GPU needed:
+ *   op 0: m2dp_axes       in = cov_6 (float xx xy xz yy yz zz)    out = E[9] (E[k * 3 + j]: component k of axis j)
+ *         axes by descending eigenvalue, each of the first two with its largest-magnitude component positive,
+ *         third = first x second in float; the identity when an entry is not finite
+ *   op 1: m2dp_descriptor in = A (rows x cols int32, row-major), gram = A A^T (rows x rows)
+ *                                                                  out = [u1; v1] (rows + cols floats), zero if A is */
+int sm_debug_m2dp_host(int32_t op, const float* cov_6, const int32_t* A, const double* gram, int32_t rows, int32_t cols,
+                       float* out);
+
+/* M2dpStage::run as sm_m2dp runs it (arguments as for sm_m2dp, n >= 1), then m2dp_descriptor: the float mean, the six
+ * double covariance sums and the six float entries sum / float(n - 1), E[9], the view axes {xa[3], ya[3]} of each of
+ * the rows = p * q views (6 * rows floats), A (rows x cols counts), A A^T (rows x rows) and the descriptor
+ * (rows + cols floats), with cols = ceil(sqrt(max_distance / r)) * t. */
+int sm_debug_m2dp_stages(int device, const float* points, int64_t n, int64_t stride_bytes, double r, double max_distance,
+                         int32_t t, int32_t p, int32_t q, float* mean_3, double* cov_sums_6, float* cov_6, float* E_9,
+                         float* views_6r, int32_t* A, double* gram, float* descriptor);
 
 #ifdef __cplusplus
 }

@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include <utility>
+#include <vector>
 
 #include "common.cuh"
 
@@ -319,6 +320,33 @@ struct NormalsPipeline {
   const double* points() const { return (const double*)out_pts.p; }
   const double* normals() const { return (const double*)out_nrm.p; }
 };
+
+// ---- m2dp.cu -----------------------------------------------------------------------------
+struct M2dpView { float xa[3], ya[3]; };   // x_axis, y_axis of one view (m2dp.cc:73-83), not normalised
+static_assert(sizeof(M2dpView) == 6 * sizeof(float), "the test hook copies views as 6 floats each");
+// The device work of M2dp::setInputCloud over n >= 1 records of stride_bytes (float xyz first): the buffers, carved
+// from one allocation, and the mean, covariance, histogram and Gram kernels with the host steps between them.  run()
+// leaves every intermediate in host memory: the float mean, the six double covariance sums (xx xy xz yy yz zz) and
+// the float covariance entries sum / float(n - 1), the axes E = m2dp_axes(cov), the view axes, A (rows x cols counts,
+// row-major) and G = A A^T.
+struct M2dpStage {
+  DevBuf buf;
+  int rows = 0, cols = 0, l = 0;
+  float mean[3];
+  double cov_sums[6];
+  float cov[6];
+  float E[9];                // E[k * 3 + j]: component k of axis j
+  std::vector<M2dpView> views;
+  std::vector<int> A;
+  std::vector<double> G;
+  int run(const float* points, int64_t n, int64_t stride_bytes, double r, double max_distance, int t, int p, int q,
+          cudaStream_t stream);
+};
+// the PCA axes from the six float covariance entries: descending eigenvalue, largest-magnitude component positive,
+// third = first x second in float; the identity when an entry is not finite
+void m2dp_axes(const float* cov6, float* E9);
+// [u1; v1] (rows + cols floats) from A and G = A A^T; zero when A is
+void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* out);
 
 }  // namespace smb
 

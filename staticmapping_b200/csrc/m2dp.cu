@@ -12,17 +12,26 @@
 //   setInputCloud (:129-153)   A (64 x 512 counts), first singular vectors -> [u1; v1]
 //
 // H100 formulation: the work is N x 64 (point, view) bin updates — integer scatter, no
-// contraction.  One CTA owns a chunk of points and a GROUP of 8 views whose 8 x 512 histogram
-// lives in shared memory (16 KB): the point is loaded and projected once per CTA-thread, the
-// eight views hit shared-memory atomics only (the reference's |.| folds everything into the first
-// quadrant, so a view touches ~128 distinct bins: global atomics would serialise in L2), and the
-// non-empty bins are flushed to the global matrix with one atomic each at the end.  Sums for the
-// PCA are double block reductions.  A A^T (64 x 64, exact in double: counts < 2^31) is formed on the
-// device; the two tiny eigenproblems run on the host by power iteration (an algorithm deliberately
-// different from the oracle's Jacobi sweeps).  Sign conventions: see oracle/m2dp_oracle.cc — they
-// live inside Eigen in the reference and are fixed the same way on both sides here.
+// contraction.  One CTA owns a chunk of points and a GROUP of up to 8 views whose histograms
+// live in shared memory (8 x 512 x 4 B = 16 KB by default; fewer views per CTA when a histogram
+// is wider, so that a group always fits the 48 KB a block gets without opting in): the point is
+// loaded and projected once per CTA-thread, the views hit shared-memory atomics only (the
+// reference's |.| folds everything into the first quadrant, so a view touches ~128 distinct bins:
+// global atomics would serialise in L2), and the non-empty bins are flushed to the global matrix
+// with one atomic each at the end.  Sums for the PCA are double block reductions.  A A^T (64 x 64,
+// exact in double: counts < 2^31) is formed on the device; the two small symmetric eigenproblems
+// run on the host by cyclic Jacobi in double, whose error does not grow as the leading eigenvalues
+// close in (a square patch has lambda1 ~ lambda2, and M2DP is meant to be invariant in that frame).
+// Sign conventions: see oracle/m2dp_oracle.cc — they live inside Eigen in the reference and are
+// fixed the same way on both sides here.
+//
+// The pieces: M2dpStage (device buffers and kernels, with the host steps between them),
+// m2dp_axes (covariance -> axes) and m2dp_descriptor (A and A A^T -> [u1; v1]); sm_m2dp and the
+// test hooks of csrc/sm_debug.cu call these.
 #include <math.h>
+#include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "../../include/sm_b200.h"
@@ -36,12 +45,12 @@ constexpr int kViewsPerCta = 8;
 constexpr int kHistThreads = 256;
 constexpr int kPointsPerCta = 4096;
 
-struct M2dpView { float xa[3], ya[3]; };
 struct M2dpParams {
   float mean[3];
   float E[9];             // E[k * 3 + j]: component k of axis j
   double r, max_distance, angle_step;
   int l, t, cols, n_views;
+  int views_per_cta;      // hist_views_per_cta(cols)
 };
 
 __global__ void __launch_bounds__(256)
@@ -90,15 +99,15 @@ m2dp_cov_kernel(const char* __restrict__ pts, int64_t stride, int64_t n, float c
   }
 }
 
-// grid: (point chunks, view groups).  Dynamic shared memory: kViewsPerCta * cols ints.
+// grid: (point chunks, view groups of P.views_per_cta).  Dynamic shared memory: views_per_cta * cols ints.
 __global__ void __launch_bounds__(kHistThreads)
 m2dp_hist_kernel(const char* __restrict__ pts, int64_t stride, int64_t n, M2dpParams P,
                  const M2dpView* __restrict__ views, int* __restrict__ A) {
   extern __shared__ int hist[];
   __shared__ M2dpView sv[kViewsPerCta];
-  const int v0 = blockIdx.y * kViewsPerCta;
-  const int nv = min(kViewsPerCta, P.n_views - v0);
-  for (int k = threadIdx.x; k < kViewsPerCta * P.cols; k += kHistThreads) hist[k] = 0;
+  const int v0 = blockIdx.y * P.views_per_cta;
+  const int nv = min(P.views_per_cta, P.n_views - v0);
+  for (int k = threadIdx.x; k < nv * P.cols; k += kHistThreads) hist[k] = 0;
   if (threadIdx.x < nv) sv[threadIdx.x] = views[v0 + threadIdx.x];
   __syncthreads();
   const int64_t base = (int64_t)blockIdx.x * kPointsPerCta;
@@ -132,6 +141,15 @@ m2dp_hist_kernel(const char* __restrict__ pts, int64_t stride, int64_t n, M2dpPa
   }
 }
 
+// views per histogram CTA: up to 8, as many histograms of cols counts as the kernel's dynamic shared memory holds
+// without opting in (48 KB less its static part: 8 views up to cols = 1530, one view for the widest, 8192)
+int hist_views_per_cta(int cols, int* vpc) {
+  cudaFuncAttributes fa;
+  SMB_CUDA_OK(cudaFuncGetAttributes(&fa, m2dp_hist_kernel));
+  *vpc = std::max(1, std::min(kViewsPerCta, fa.maxDynamicSharedSizeBytes / (int)(cols * sizeof(int))));
+  return 0;
+}
+
 // G = A A^T (rows x rows) in double; one block per (a, b-tile)
 __global__ void __launch_bounds__(256)
 m2dp_gram_kernel(const int* __restrict__ A, int rows, int cols, double* __restrict__ G) {
@@ -150,27 +168,45 @@ m2dp_gram_kernel(const int* __restrict__ A, int rows, int cols, double* __restri
   }
 }
 
-// dominant eigenpair of a symmetric PSD matrix by power iteration (host, double)
-double power_iteration(const std::vector<double>& M, int n, std::vector<double>& v) {
-  v.assign((size_t)n, 1.0 / sqrt((double)n));
-  for (int k = 0; k < n; ++k) v[(size_t)k] *= 1.0 + 1e-3 * k;      // not orthogonal to anything by accident
-  std::vector<double> w((size_t)n);
-  double lambda = 0.0;
-  for (int it = 0; it < 20000; ++it) {
-    double norm = 0.0;
-    for (int i = 0; i < n; ++i) {
-      double s = 0.0;
-      for (int j = 0; j < n; ++j) s += M[(size_t)i * n + j] * v[(size_t)j];
-      w[(size_t)i] = s; norm += s * s;
-    }
-    norm = sqrt(norm);
-    if (!(norm > 0.0)) return 0.0;
-    double diff = 0.0;
-    for (int i = 0; i < n; ++i) { const double nv = w[(size_t)i] / norm; diff += fabs(nv - v[(size_t)i]); v[(size_t)i] = nv; }
-    lambda = norm;
-    if (diff < 1e-15 * n) break;
+// Eigen-decomposition of the symmetric n x n matrix a (row-major, double) by cyclic Jacobi rotations: on return
+// a[j * n + j] is an eigenvalue and row j of vt its unit eigenvector.  A rotation is skipped once its off-diagonal
+// entry is below the rounding of its two diagonal entries (|a_pq| <= eps sqrt(|a_pp a_qq|)), and the sweeps stop
+// when one skips them all.  Each rotation is orthogonal, so the computed pairs belong to a matrix within a few
+// roundings of a whatever the eigenvalue gaps; an eigenvector's error is then that over its gap, the conditioning
+// of the problem itself, with no iteration count that depends on the gap as power iteration's does.
+void jacobi_eigen(std::vector<double>& a, int n, std::vector<double>& vt) {
+  vt.assign((size_t)n * n, 0.0);
+  for (int i = 0; i < n; ++i) vt[(size_t)i * n + i] = 1.0;
+  for (int sweep = 0; sweep < 64; ++sweep) {
+    bool rotated = false;
+    for (int p = 0; p < n - 1; ++p)
+      for (int q = p + 1; q < n; ++q) {
+        double* ap = &a[(size_t)p * n];
+        double* aq = &a[(size_t)q * n];
+        const double apq = ap[q], app = ap[p], aqq = aq[q];
+        if (!(fabs(apq) > 2.2e-16 * sqrt(fabs(app) * fabs(aqq)))) continue;
+        rotated = true;
+        const double theta = (aqq - app) / (2.0 * apq);
+        const double t = fabs(theta) > 1e150 ? 0.5 / theta
+                                             : (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < n; ++k) {               // rows p and q, mirrored into columns p and q
+          if (k == p || k == q) continue;
+          const double akp = ap[k], akq = aq[k];
+          ap[k] = a[(size_t)k * n + p] = c * akp - s * akq;
+          aq[k] = a[(size_t)k * n + q] = s * akp + c * akq;
+        }
+        ap[p] = app - t * apq; aq[q] = aqq + t * apq;
+        ap[q] = aq[p] = 0.0;
+        double* vp = &vt[(size_t)p * n];
+        double* vq = &vt[(size_t)q * n];
+        for (int k = 0; k < n; ++k) {
+          const double x = vp[k], y = vq[k];
+          vp[k] = c * x - s * y; vq[k] = s * x + c * y;
+        }
+      }
+    if (!rotated) break;
   }
-  return lambda;
 }
 
 void orient(double* v, int n) {    // component of largest magnitude positive
@@ -180,14 +216,121 @@ void orient(double* v, int n) {    // component of largest magnitude positive
 }
 
 }  // namespace
+
+// axes of the float covariance matrix, descending eigenvalue (pcl::PCA::initCompute), third = first x second in float
+void m2dp_axes(const float* c, float* E) {
+  double e[2][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}};   // no finite covariance (one point: 0 / 0): the input frame
+  bool finite = true;
+  for (int k = 0; k < 6; ++k) finite = finite && isfinite(c[k]);
+  if (finite) {
+    std::vector<double> a = {c[0], c[1], c[2], c[1], c[3], c[4], c[2], c[4], c[5]}, vt;
+    jacobi_eigen(a, 3, vt);
+    int order[3] = {0, 1, 2};
+    std::stable_sort(order, order + 3, [&](int x, int y) { return a[(size_t)x * 4] > a[(size_t)y * 4]; });
+    for (int j = 0; j < 2; ++j)
+      for (int k = 0; k < 3; ++k) e[j][k] = vt[(size_t)order[j] * 3 + k];
+  }
+  orient(e[0], 3); orient(e[1], 3);
+  for (int k = 0; k < 3; ++k) { E[k * 3 + 0] = (float)e[0][k]; E[k * 3 + 1] = (float)e[1][k]; }
+  E[0 * 3 + 2] = E[1 * 3 + 0] * E[2 * 3 + 1] - E[2 * 3 + 0] * E[1 * 3 + 1];
+  E[1 * 3 + 2] = E[2 * 3 + 0] * E[0 * 3 + 1] - E[0 * 3 + 0] * E[2 * 3 + 1];
+  E[2 * 3 + 2] = E[0 * 3 + 0] * E[1 * 3 + 1] - E[1 * 3 + 0] * E[0 * 3 + 1];
+}
+
+// first singular pair of A (rows x cols) from G = A A^T: u1 = dominant eigenvector of G, sigma1^2 its eigenvalue,
+// v1 = A^T u1 / sigma1; out = [u1; v1] in float, all zero when A is
+void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* out) {
+  std::vector<double> a(G, G + (size_t)rows * rows), vt;
+  jacobi_eigen(a, rows, vt);
+  int top = 0;
+  for (int k = 1; k < rows; ++k) if (a[(size_t)k * rows + k] > a[(size_t)top * rows + top]) top = k;
+  const double lambda = a[(size_t)top * rows + top];
+  if (!(lambda > 0.0)) {
+    for (int k = 0; k < rows + cols; ++k) out[k] = 0.f;
+    return;
+  }
+  std::vector<double> u(vt.begin() + (size_t)top * rows, vt.begin() + (size_t)(top + 1) * rows);
+  orient(u.data(), rows);
+  const double sigma = sqrt(lambda);
+  for (int k = 0; k < rows; ++k) out[k] = (float)u[(size_t)k];
+  for (int c = 0; c < cols; ++c) {
+    double sacc = 0.0;
+    for (int a_ = 0; a_ < rows; ++a_) sacc += (double)A[(size_t)a_ * cols + c] * u[(size_t)a_];
+    out[rows + c] = (float)(sacc / sigma);
+  }
+}
+
+int M2dpStage::run(const float* points, int64_t n, int64_t stride_bytes, double r, double max_distance, int t, int p,
+                   int q, cudaStream_t s) {
+  l = (int)ceil(sqrt(max_distance / r));
+  rows = p * q; cols = l * t;
+  const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
+  const size_t bytes = in_bytes + 256 + 16 * sizeof(double) + (size_t)rows * sizeof(M2dpView) + 256 +
+                       (size_t)rows * cols * sizeof(int) + 256 + (size_t)rows * rows * sizeof(double) + 256;
+  SMB_RC(buf.reserve(bytes));
+  char* cur = (char*)buf.p;
+  auto take = [&](size_t b) { char* ptr = cur; cur += (b + 255) & ~(size_t)255; return ptr; };
+  char* d_in = take(in_bytes);
+  double* d_sums = (double*)take(16 * sizeof(double));
+  M2dpView* d_views = (M2dpView*)take((size_t)rows * sizeof(M2dpView));
+  int* d_A = (int*)take((size_t)rows * cols * sizeof(int));
+  double* d_G = (double*)take((size_t)rows * rows * sizeof(double));
+  SMB_CUDA_OK(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s));
+  SMB_CUDA_OK(cudaMemsetAsync(d_sums, 0, 16 * sizeof(double), s));
+  SMB_CUDA_OK(cudaMemsetAsync(d_A, 0, (size_t)rows * cols * sizeof(int), s));
+  const int red_blocks = (int)std::min<int64_t>(4 * kNumSMs, (n + 255) / 256);
+  m2dp_mean_kernel<<<red_blocks, 256, 0, s>>>(d_in, stride_bytes, n, d_sums);
+  double h[3];
+  SMB_CUDA_OK(cudaMemcpyAsync(h, d_sums, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  M2dpParams P;
+  for (int d = 0; d < 3; ++d) P.mean[d] = mean[d] = (float)(h[d] / (double)n);
+  m2dp_cov_kernel<<<red_blocks, 256, 0, s>>>(d_in, stride_bytes, n, P.mean[0], P.mean[1], P.mean[2], d_sums + 8);
+  SMB_CUDA_OK(cudaMemcpyAsync(cov_sums, d_sums + 8, 6 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  const double denom = (double)(float)(n - 1);
+  for (int k = 0; k < 6; ++k) cov[k] = (float)(cov_sums[k] / denom);
+  m2dp_axes(cov, E);
+  memcpy(P.E, E, sizeof(E));
+  P.r = r; P.max_distance = max_distance; P.angle_step = (M_PI * 2.) / t;
+  P.l = l; P.t = t; P.cols = cols; P.n_views = rows;
+  SMB_RC(hist_views_per_cta(cols, &P.views_per_cta));
+  views.resize((size_t)rows);               // view axes (m2dp.cc:73-83), float like the reference
+  const double theta_step = M_PI / p, phi_step = M_PI_2 / q;
+  for (int pi = 0; pi < p; ++pi)
+    for (int qi = 0; qi < q; ++qi) {
+      const double theta = pi * theta_step, phi = qi * phi_step;
+      const float mx = (float)(cos(theta) * cos(phi)), my = (float)(cos(theta) * sin(phi)), mz = (float)sin(theta);
+      const float sgl = fabsf(mx);
+      M2dpView& v = views[(size_t)(pi * q + qi)];
+      v.xa[0] = 1.f - sgl * mx; v.xa[1] = 0.f - sgl * my; v.xa[2] = 0.f - sgl * mz;
+      v.ya[0] = my * v.xa[2] - mz * v.xa[1]; v.ya[1] = mz * v.xa[0] - mx * v.xa[2]; v.ya[2] = mx * v.xa[1] - my * v.xa[0];
+    }
+  SMB_CUDA_OK(cudaMemcpyAsync(d_views, views.data(), (size_t)rows * sizeof(M2dpView), cudaMemcpyHostToDevice, s));
+  const dim3 grid((unsigned)((n + kPointsPerCta - 1) / kPointsPerCta),
+                  (unsigned)((rows + P.views_per_cta - 1) / P.views_per_cta));
+  m2dp_hist_kernel<<<grid, kHistThreads, (size_t)P.views_per_cta * cols * sizeof(int), s>>>(d_in, stride_bytes, n, P,
+                                                                                           d_views, d_A);
+  m2dp_gram_kernel<<<dim3((unsigned)rows, (unsigned)rows), 256, 0, s>>>(d_A, rows, cols, d_G);
+  SMB_CUDA_OK(cudaGetLastError());
+  A.resize((size_t)rows * cols);
+  G.resize((size_t)rows * rows);
+  SMB_CUDA_OK(cudaMemcpyAsync(A.data(), d_A, A.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(G.data(), d_G, G.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
+}
+
 }  // namespace smb
 
 using namespace smb;
 
+// At most 8192 bins per view and 256 views: the eigenproblem of A A^T (p*q x p*q) is solved on the host by Jacobi,
+// whose cost grows as (p*q)^3: about 2 ms at the default 64 views, 0.8 s at 256, 13 s at 512 (one CPU core).
 extern "C" int64_t sm_m2dp_descriptor_length(double r, double max_distance, int32_t t, int32_t p, int32_t q) {
   if (r < 1.e-6 || !(max_distance > 0.0) || t <= 0 || p <= 0 || q <= 0) return SM_ERR_BAD_ARGUMENT;
   const double l = ceil(sqrt(max_distance / r));
-  if (!(l >= 1.0) || l * t > 8192.0 || (double)p * q > 4096.0) return SM_ERR_BAD_ARGUMENT;
+  if (!(l >= 1.0) || l * t > 8192.0 || (double)p * q > 256.0) return SM_ERR_BAD_ARGUMENT;
   return (int64_t)p * q + (int64_t)l * t;
 }
 
@@ -200,93 +343,10 @@ extern "C" int sm_m2dp(int device, const float* points, int64_t n, int64_t strid
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
   SMB_CUDA_OK(cudaSetDevice(device));
-  const int rows = p * q, l = (int)ceil(sqrt(max_distance / r)), cols = l * t;
-  const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
-  const size_t bytes = in_bytes + 256 + 16 * sizeof(double) + (size_t)rows * sizeof(M2dpView) + 256 +
-                       (size_t)rows * cols * sizeof(int) + 256 + (size_t)rows * rows * sizeof(double) + 256;
-  DevBuf buf;
-  SMB_RC(buf.reserve(bytes));
-  char* cur = (char*)buf.p;
-  auto take = [&](size_t b) { char* ptr = cur; cur += (b + 255) & ~(size_t)255; return ptr; };
-  char* d_in = take(in_bytes);
-  double* d_sums = (double*)take(16 * sizeof(double));
-  M2dpView* d_views = (M2dpView*)take((size_t)rows * sizeof(M2dpView));
-  int* d_A = (int*)take((size_t)rows * cols * sizeof(int));
-  double* d_G = (double*)take((size_t)rows * rows * sizeof(double));
-  cudaStream_t s = nullptr;
-  SMB_CUDA_OK(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s));
-  SMB_CUDA_OK(cudaMemsetAsync(d_sums, 0, 16 * sizeof(double), s));
-  SMB_CUDA_OK(cudaMemsetAsync(d_A, 0, (size_t)rows * cols * sizeof(int), s));
-  const int red_blocks = (int)std::min<int64_t>(4 * kNumSMs, (n + 255) / 256);
-  m2dp_mean_kernel<<<red_blocks, 256, 0, s>>>(d_in, stride_bytes, n, d_sums);
-  double h[16];
-  SMB_CUDA_OK(cudaMemcpyAsync(h, d_sums, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  M2dpParams P;
-  for (int d = 0; d < 3; ++d) P.mean[d] = (float)(h[d] / (double)n);
-  m2dp_cov_kernel<<<red_blocks, 256, 0, s>>>(d_in, stride_bytes, n, P.mean[0], P.mean[1], P.mean[2], d_sums + 8);
-  SMB_CUDA_OK(cudaMemcpyAsync(h, d_sums + 8, 6 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  {   // axes of the float covariance matrix, descending eigenvalue (pcl::PCA::initCompute)
-    const double denom = (double)(float)(n - 1);
-    const float c0 = (float)(h[0] / denom), c1 = (float)(h[1] / denom), c2 = (float)(h[2] / denom),
-                c3 = (float)(h[3] / denom), c4 = (float)(h[4] / denom), c5 = (float)(h[5] / denom);
-    std::vector<double> C = {c0, c1, c2, c1, c3, c4, c2, c4, c5};
-    std::vector<double> e0, e1;
-    const double l0 = power_iteration(C, 3, e0);
-    std::vector<double> D = C;                                     // deflate the first axis
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) D[(size_t)i * 3 + j] -= l0 * e0[(size_t)i] * e0[(size_t)j];
-    power_iteration(D, 3, e1);
-    double dot = 0.0;                                              // re-orthogonalise against the first axis
-    for (int i = 0; i < 3; ++i) dot += e0[(size_t)i] * e1[(size_t)i];
-    double nrm = 0.0;
-    for (int i = 0; i < 3; ++i) { e1[(size_t)i] -= dot * e0[(size_t)i]; nrm += e1[(size_t)i] * e1[(size_t)i]; }
-    nrm = sqrt(nrm);
-    if (nrm > 0) for (int i = 0; i < 3; ++i) e1[(size_t)i] /= nrm;
-    orient(e0.data(), 3); orient(e1.data(), 3);
-    for (int k = 0; k < 3; ++k) { P.E[k * 3 + 0] = (float)e0[(size_t)k]; P.E[k * 3 + 1] = (float)e1[(size_t)k]; }
-    P.E[0 * 3 + 2] = P.E[1 * 3 + 0] * P.E[2 * 3 + 1] - P.E[2 * 3 + 0] * P.E[1 * 3 + 1];
-    P.E[1 * 3 + 2] = P.E[2 * 3 + 0] * P.E[0 * 3 + 1] - P.E[0 * 3 + 0] * P.E[2 * 3 + 1];
-    P.E[2 * 3 + 2] = P.E[0 * 3 + 0] * P.E[1 * 3 + 1] - P.E[1 * 3 + 0] * P.E[0 * 3 + 1];
-  }
-  P.r = r; P.max_distance = max_distance; P.angle_step = (M_PI * 2.) / t;
-  P.l = l; P.t = t; P.cols = cols; P.n_views = rows;
-  {   // view axes (m2dp.cc:73-83), float like the reference
-    std::vector<M2dpView> hv((size_t)rows);
-    const double theta_step = M_PI / p, phi_step = M_PI_2 / q;
-    for (int pi = 0; pi < p; ++pi)
-      for (int qi = 0; qi < q; ++qi) {
-        const double theta = pi * theta_step, phi = qi * phi_step;
-        const float mx = (float)(cos(theta) * cos(phi)), my = (float)(cos(theta) * sin(phi)), mz = (float)sin(theta);
-        const float sgl = fabsf(mx);
-        M2dpView& v = hv[(size_t)(pi * q + qi)];
-        v.xa[0] = 1.f - sgl * mx; v.xa[1] = 0.f - sgl * my; v.xa[2] = 0.f - sgl * mz;
-        v.ya[0] = my * v.xa[2] - mz * v.xa[1]; v.ya[1] = mz * v.xa[0] - mx * v.xa[2]; v.ya[2] = mx * v.xa[1] - my * v.xa[0];
-      }
-    SMB_CUDA_OK(cudaMemcpyAsync(d_views, hv.data(), (size_t)rows * sizeof(M2dpView), cudaMemcpyHostToDevice, s));
-    SMB_CUDA_OK(cudaStreamSynchronize(s));          // hv goes out of scope
-  }
-  const dim3 grid((unsigned)((n + kPointsPerCta - 1) / kPointsPerCta), (unsigned)((rows + kViewsPerCta - 1) / kViewsPerCta));
-  m2dp_hist_kernel<<<grid, kHistThreads, (size_t)kViewsPerCta * cols * sizeof(int), s>>>(d_in, stride_bytes, n, P, d_views, d_A);
-  m2dp_gram_kernel<<<dim3((unsigned)rows, (unsigned)rows), 256, 0, s>>>(d_A, rows, cols, d_G);
-  SMB_CUDA_OK(cudaGetLastError());
-  std::vector<int> A((size_t)rows * cols);
-  std::vector<double> G((size_t)rows * rows);
-  SMB_CUDA_OK(cudaMemcpyAsync(A.data(), d_A, A.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaMemcpyAsync(G.data(), d_G, G.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  if (A_out) memcpy(A_out, A.data(), A.size() * sizeof(int));
-  // first singular pair: u1 = dominant eigenvector of A A^T, sigma1^2 its eigenvalue, v1 = A^T u1 / sigma1
-  std::vector<double> u;
-  const double lambda = power_iteration(G, rows, u);
-  orient(u.data(), rows);
-  const double sigma = sqrt(lambda > 0 ? lambda : 0.0);
-  for (int k = 0; k < rows; ++k) descriptor[k] = (float)u[(size_t)k];
-  for (int c = 0; c < cols; ++c) {
-    double sacc = 0.0;
-    for (int a = 0; a < rows; ++a) sacc += (double)A[(size_t)a * cols + c] * u[(size_t)a];
-    descriptor[rows + c] = sigma > 0 ? (float)(sacc / sigma) : 0.f;
-  }
+  M2dpStage st;
+  SMB_RC(st.run(points, n, stride_bytes, r, max_distance, t, p, q, nullptr));
+  if (A_out) memcpy(A_out, st.A.data(), st.A.size() * sizeof(int));
+  m2dp_descriptor(st.A.data(), st.G.data(), st.rows, st.cols, descriptor);
   return 1;
 }
 

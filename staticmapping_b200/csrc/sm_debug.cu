@@ -1,7 +1,9 @@
 // Test hooks of include/sm_b200_debug.h: the product's host code driven by a caller's callbacks, its device math
-// compiled for the host, and its Ndt / NdtWithGicp device stages run on buffers of their own.
+// compiled for the host, and its Ndt / NdtWithGicp / M2DP device stages run on buffers of their own.
 #include "../../include/sm_b200.h"
 #include "../../include/sm_b200_debug.h"
+
+#include <string.h>
 
 #include <vector>
 
@@ -433,6 +435,44 @@ int sm_debug_gicp_step(int device, const float* source_3n, int64_t ns, const flo
     SMB_RC(g.cost((const float*)src.p, (int)ns, (const float*)tgt.p, T, guess, nullptr, nullptr, nullptr));
     SMB_CUDA_OK(cudaMemcpy(sums_13k + 13 * (int64_t)k, g.sums, 13 * sizeof(double), cudaMemcpyDeviceToHost));
   }
+  return SM_OK;
+}
+
+// test hook: the host routines of M2DP (m2dp.cu m2dp_axes / m2dp_descriptor), no GPU involved
+int sm_debug_m2dp_host(int32_t op, const float* cov_6, const int32_t* A, const double* gram, int32_t rows, int32_t cols,
+                       float* out) {
+  if (!out) return SM_ERR_BAD_ARGUMENT;
+  switch (op) {
+    case 0:
+      if (!cov_6) return SM_ERR_BAD_ARGUMENT;
+      m2dp_axes(cov_6, out);
+      return SM_OK;
+    case 1:
+      if (!A || !gram || rows <= 0 || cols <= 0) return SM_ERR_BAD_ARGUMENT;
+      m2dp_descriptor(A, gram, rows, cols, out);
+      return SM_OK;
+    default: return SM_ERR_BAD_ARGUMENT;
+  }
+}
+
+// test hook: M2dpStage exactly as sm_m2dp runs it, every intermediate copied out, then m2dp_descriptor
+int sm_debug_m2dp_stages(int device, const float* points, int64_t n, int64_t stride_bytes, double r, double max_distance,
+                         int32_t t, int32_t p, int32_t q, float* mean_3, double* cov_sums_6, float* cov_6, float* E_9,
+                         float* views_6r, int32_t* A, double* gram, float* descriptor) {
+  if (!points || n <= 0 || n > (1ll << 30) || stride_bytes < 12 || stride_bytes % 4 || !mean_3 || !cov_sums_6 ||
+      !cov_6 || !E_9 || !views_6r || !A || !gram || !descriptor || sm_m2dp_descriptor_length(r, max_distance, t, p, q) < 0)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  M2dpStage st;
+  SMB_RC(st.run(points, n, stride_bytes, r, max_distance, t, p, q, nullptr));
+  memcpy(mean_3, st.mean, sizeof(st.mean));
+  memcpy(cov_sums_6, st.cov_sums, sizeof(st.cov_sums));
+  memcpy(cov_6, st.cov, sizeof(st.cov));
+  memcpy(E_9, st.E, sizeof(st.E));
+  memcpy(views_6r, st.views.data(), st.views.size() * sizeof(M2dpView));
+  memcpy(A, st.A.data(), st.A.size() * sizeof(int));
+  memcpy(gram, st.G.data(), st.G.size() * sizeof(double));
+  m2dp_descriptor(st.A.data(), st.G.data(), st.rows, st.cols, descriptor);
   return SM_OK;
 }
 

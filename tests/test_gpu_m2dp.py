@@ -33,6 +33,23 @@ def test_descriptor_matches_oracle(pair):
     assert abs(np.linalg.norm(got[:64]) - 1.0) < 1e-5 and abs(np.linalg.norm(got[64:]) - 1.0) < 1e-5
 
 
+def test_descriptor_matches_oracle_behind_the_distance_gate():
+    # a submap four times as wide as the default one, with max_distance = 20 m: about half of it is dropped
+    pts = _cloud(0) * np.float32(4.0)
+    want, A_o, axes = O.m2dp(pts, max_distance=20.0, with_matrix=True)
+    m = smb.M2dp(max_distance=20.0)
+    assert m.setInputCloud(smb.InnerCloud(pts)) is True
+    got = m.getFinalDescriptor()
+    assert got.shape == want.shape == (4 * 16 + 15 * 16,)
+    A_g = m.signature_matrix
+    assert 0.2 * 64 * pts.shape[0] < A_o.sum() < 0.8 * 64 * pts.shape[0]
+    assert abs(int(A_g.sum()) - int(A_o.sum())) <= 2e-3 * A_o.sum()    # the two means may gate a border point apart
+    moved = np.abs(A_g.astype(np.int64) - A_o).sum() / 2
+    assert moved <= 2e-3 * A_o.sum(), moved
+    assert np.abs(got - want).max() < 2e-3
+    assert smb.matchTwoM2dpDescriptors(got, want) > 0.99999
+
+
 def test_full_size_submap_and_strided_records():
     src, sub, P = scenes.full_size_pair(0)
     pts = sub.astype(np.float32)
