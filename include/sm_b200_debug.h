@@ -31,6 +31,9 @@
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
  *     sm_debug_gicp_step       correspondences, Mahalanobis matrices and cost sums of one GICP outer iteration
  *     sm_debug_m2dp_stages     every intermediate of M2dpStage: mean, covariance, axes, view axes, A, A A^T, descriptor
+ *     sm_debug_radix_sort      radix_sort_pairs_u64 as the tree build, the voxel filters and the NDT grid call it
+ *     sm_debug_kd_tree         every array a k-d tree owner (KdCompactTree, NormalsPipeline, FloatTree) fills, after
+ *                              an optional earlier build into the same owner
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
  *   each stage of M2DP meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
@@ -212,6 +215,33 @@ int sm_debug_m2dp_host(int32_t op, const float* cov_6, const int32_t* A, const d
 int sm_debug_m2dp_stages(int device, const float* points, int64_t n, int64_t stride_bytes, double r, double max_distance,
                          int32_t t, int32_t p, int32_t q, float* mean_3, double* cov_sums_6, float* cov_6, float* E_9,
                          float* views_6r, int32_t* A, double* gram, float* descriptor);
+
+/* ---- the two device stages every matcher builds on, run through the functions and owners the matchers call */
+
+/* radix_sort_pairs_u64 (csrc/radix_sort.cu) over `batch` independent arrays [batch][stride] of n (key, value) pairs,
+ * the low 8 * passes bits of the keys ordered (stable), with scratch sized by radix_sort_scratch_bytes(n, batch).
+ * Both ping-pong buffers start as copies of the caller's arrays, entries n..stride-1 of each batch included, and
+ * keys_out / vals_out ([batch][stride]) receive the buffer holding the result, so a write past n shows. */
+int sm_debug_radix_sort(int device, const uint64_t* keys, const uint32_t* vals, int64_t n, int32_t batch, int64_t stride,
+                        int32_t passes, uint64_t* keys_out, uint32_t* vals_out);
+
+/* One k-d tree owner, built as the matchers build it: with n_first > 0 first over the first cloud, then over the cloud,
+ * into the SAME owner, workspace and input buffers (a reused handle).  variant:
+ *   0  KdCompactTree with the normals payload (IcpFast's target): double clouds, normals_3n required, bucket 2..8
+ *   1  KdCompactTree with the ids payload (sm_knn1): double clouds, bucket 2..8
+ *   2  NormalsPipeline (CalculateNormals): double clouds, bucket 7
+ *   3  FloatTree (Ndt fitness, GICP, type-1 score): packed float clouds, bucket 8
+ * levels must equal kd_num_levels(n, bucket), L below; the arrays the owner fills are copied out, unwritten slots as
+ * the device holds them:
+ *   nodes    blocked_node_slots(L) 16-byte KdNode records          order  n leaf-order ids
+ *   variants 0 / 1:  cut, dim  2^L - 1 entries (heap order)          node_2l  2^L {cut, dim as int64} records
+ *                    pb  (8 << L) * 3 doubles                        pn  (8 << L) * 4 doubles (0) / pid  8 << L (1)
+ *   variant 3:       bpts  n 32-byte {x, y, z, id} records
+ * Arrays of other variants may be NULL. */
+int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* first_3n, const double* first_normals_3n,
+                     int64_t n_first, const void* cloud_3n, const double* normals_3n, int64_t n, int32_t levels,
+                     void* nodes, uint32_t* order, double* cut, uint8_t* dim, double* node_2l, double* pb, double* pn,
+                     int32_t* pid, void* bpts);
 
 #ifdef __cplusplus
 }

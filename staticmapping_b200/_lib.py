@@ -99,6 +99,9 @@ SIGNATURES = {
     "sm_debug_m2dp_host": (C.c_int, [C.c_int32, _VP, _VP, _VP, C.c_int32, C.c_int32, _VP]),
     "sm_debug_m2dp_stages": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_int32,
                                        C.c_int32, C.c_int32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "sm_debug_radix_sort": (C.c_int, [C.c_int, _VP, _VP, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _VP, _VP]),
+    "sm_debug_kd_tree": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _VP, _VP, C.c_int64, _VP, _VP, C.c_int64, C.c_int32,
+                                   _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

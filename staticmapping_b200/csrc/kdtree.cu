@@ -228,8 +228,9 @@ kd_part_scatter_kernel(const uint32_t* __restrict__ lists, uint32_t* __restrict_
 // ONE CTA: the same four steps per level (nodes, side flags, stable partition of the three lists), with
 // __syncthreads between them instead of four launches per level.  For a 106 784-point target the global
 // passes stop at level 6 (segments of <= 1 669 points) and 64 CTAs do levels 6..13: 56 launches become 25.
-// The tree is the same one (same medians, same tie rule, same implicit bounds): it is checked through the
-// bit-exact k-NN tests and the CalculateNormals leaf counts.
+// The tree is the same one (same medians, same tie rule, same implicit bounds).  tests/test_gpu_kdtree_stages.py
+// compares every array each tree owner fills with a numpy model of the build (tests/kd_tree_model.py), node for
+// node, at n = capacity and capacity + 1 for every bucket size and past the unfused partition scan.
 constexpr int kSubThreads = 512;
 constexpr int kSubItems = 4;
 constexpr int kSubMax = kSubThreads * kSubItems;     // 2048 points

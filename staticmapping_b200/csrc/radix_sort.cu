@@ -116,7 +116,9 @@ radix_scan_chunks_kernel(uint32_t* __restrict__ data, int count, int nchunks, ui
   if (!is_last) return;
   __threadfence();
   if (threadIdx.x == 0) *ticket = 0;                 // ready for the next pass
-  for (int bb = w; bb < (int)gridDim.y; bb += 32) {  // one warp per batch; nchunks is small (<= 2^18 keys -> 32)
+  // one warp per batch, 32 chunk totals per pass with the running carry; one chunk per 16 tiles of 2048 keys, so
+  // 2^20 keys make 32 chunks and larger sorts take more than one pass
+  for (int bb = w; bb < (int)gridDim.y; bb += 32) {
     uint32_t carry = 0;
     for (int base = 0; base < nchunks; base += 32) {
       const int k = base + lane;

@@ -476,4 +476,115 @@ int sm_debug_m2dp_stages(int device, const float* points, int64_t n, int64_t str
   return SM_OK;
 }
 
+// ---- test hooks of the shared build stages: the radix sort and the k-d tree owners ----------------------------------
+int sm_debug_radix_sort(int device, const uint64_t* keys, const uint32_t* vals, int64_t n, int32_t batch, int64_t stride,
+                        int32_t passes, uint64_t* keys_out, uint32_t* vals_out) {
+  if (!keys || !vals || !keys_out || !vals_out || n <= 0 || n > (1 << 30) || batch < 1 || batch > 16 || stride < n ||
+      stride > (1 << 30) || passes < 1 || passes > 8)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  const size_t words = (size_t)batch * (size_t)stride;
+  DevBuf k, v, scratch;
+  SMB_RC(k.reserve(2 * words * sizeof(uint64_t)));
+  SMB_RC(v.reserve(2 * words * sizeof(uint32_t)));
+  SMB_RC(scratch.reserve(radix_sort_scratch_bytes((int)n, batch)));
+  uint64_t* ka = (uint64_t*)k.p;
+  uint32_t* va = (uint32_t*)v.p;
+  for (int h = 0; h < 2; ++h) {   // both ping-pong halves start as the caller's arrays, the padding past n included
+    SMB_CUDA_OK(cudaMemcpy(ka + h * words, keys, words * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    SMB_CUDA_OK(cudaMemcpy(va + h * words, vals, words * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  }
+  SMB_RC(radix_sort_pairs_u64(ka, va, ka + words, va + words, (int)n, batch, stride, (uint32_t*)scratch.p, nullptr,
+                              passes));
+  const size_t res = passes % 2 == 0 ? 0 : words;   // an odd number of passes ends in the second half
+  SMB_CUDA_OK(cudaMemcpy(keys_out, ka + res, words * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(vals_out, va + res, words * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
+// n AoS double points -> SoA [3][stride] doubles at dev
+static int debug_soa(const double* aos, int64_t n, int64_t stride, double* dev) {
+  std::vector<double> soa((size_t)(3 * stride), 0.0);
+  for (int64_t i = 0; i < n; ++i)
+    for (int d = 0; d < 3; ++d) soa[(size_t)(d * stride + i)] = aos[3 * i + d];
+  SMB_CUDA_OK(cudaMemcpy(dev, soa.data(), soa.size() * sizeof(double), cudaMemcpyHostToDevice));
+  return SM_OK;
+}
+
+namespace {
+// the owners of the four tree variants, and the buffers that outlive one build in a handle
+struct DebugKdOwners {
+  KdCompactTree tree;
+  NormalsPipeline np;
+  FloatTree ft;
+  DevBuf coord, nrm, kdws;
+};
+}  // namespace
+
+// one build of `cloud` into the owner of `variant`, as sm_align / sm_knn1 / sm_calculate_normals run it
+static int debug_kd_build(DebugKdOwners& o, int variant, int bucket, const void* cloud, const double* normals,
+                          int64_t n) {
+  const int64_t stride = (n + 63) & ~(int64_t)63;
+  if (variant <= 1) {
+    SMB_RC(o.coord.reserve((size_t)(3 * stride) * sizeof(double)));
+    SMB_RC(debug_soa((const double*)cloud, n, stride, (double*)o.coord.p));
+    if (variant == 0) {
+      SMB_RC(o.nrm.reserve((size_t)(3 * stride) * sizeof(double)));
+      SMB_RC(debug_soa(normals, n, stride, (double*)o.nrm.p));
+    }
+    SMB_RC(o.tree.reserve((int)n, bucket, variant == 0 ? KdCompactTree::kNormals : KdCompactTree::kIds));
+    KdWorkspace ws;
+    SMB_RC(ws.carve(o.kdws, (int)n, bucket));
+    SMB_RC(o.tree.build((const double*)o.coord.p, variant == 0 ? (const double*)o.nrm.p : nullptr, stride, (int)n,
+                        bucket, ws, nullptr));
+  } else if (variant == 2) {
+    SMB_RC(o.np.reserve((int)n));
+    SMB_RC(debug_soa((const double*)cloud, n, o.np.stride, o.np.input()));
+    uint32_t m = 0;
+    SMB_RC(o.np.run((int)n, nullptr, &m));
+  } else {
+    SMB_RC(debug_upload_f32((const float*)cloud, n, o.coord));
+    SMB_RC(o.ft.build((const float*)o.coord.p, (int)n, o.kdws, nullptr));
+  }
+  SMB_CUDA_OK(cudaDeviceSynchronize());
+  return SM_OK;
+}
+
+int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* first_3n, const double* first_normals_3n,
+                     int64_t n_first, const void* cloud_3n, const double* normals_3n, int64_t n, int32_t levels,
+                     void* nodes, uint32_t* order, double* cut, uint8_t* dim, double* node_2l, double* pb, double* pn,
+                     int32_t* pid, void* bpts) {
+  if (variant < 0 || variant > 3 || !cloud_3n || n <= 0 || n > (1 << 30) || n_first < 0 || n_first > (1 << 30) ||
+      (n_first > 0 && !first_3n) || !nodes || !order)
+    return SM_ERR_BAD_ARGUMENT;
+  if (variant <= 1 && (bucket < 2 || bucket > 8 || !cut || !dim || !node_2l || !pb)) return SM_ERR_BAD_ARGUMENT;
+  if (variant == 0 && (!normals_3n || !pn || (n_first > 0 && !first_normals_3n))) return SM_ERR_BAD_ARGUMENT;
+  if (variant == 1 && !pid) return SM_ERR_BAD_ARGUMENT;
+  if ((variant == 2 && bucket != 7) || (variant == 3 && (bucket != 8 || !bpts))) return SM_ERR_BAD_ARGUMENT;
+  const int lv = kd_num_levels((int)n, bucket);
+  if (lv != levels || lv > 24 || (n_first > 0 && kd_num_levels((int)n_first, bucket) > 24)) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DebugKdOwners o;
+  if (n_first > 0) SMB_RC(debug_kd_build(o, variant, bucket, first_3n, first_normals_3n, n_first));
+  SMB_RC(debug_kd_build(o, variant, bucket, cloud_3n, normals_3n, n));
+  const DevBuf& nd = variant <= 1 ? o.tree.nodes : variant == 2 ? o.np.nodes : o.ft.nodes;
+  const DevBuf& od = variant <= 1 ? o.tree.leaf_order : variant == 2 ? o.np.order : o.ft.order;
+  SMB_CUDA_OK(cudaMemcpy(nodes, nd.p, (size_t)blocked_node_slots(lv) * sizeof(KdNode), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(order, od.p, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  if (variant <= 1) {
+    const KdCompact kc = o.tree.view();
+    const size_t inner = ((size_t)1 << lv) - 1, entries = (size_t)8 << lv;
+    if (kc.levels != lv) return SM_ERR_BAD_ARGUMENT;
+    SMB_CUDA_OK(cudaMemcpy(cut, kc.cut, inner * sizeof(double), cudaMemcpyDeviceToHost));
+    SMB_CUDA_OK(cudaMemcpy(dim, kc.dim, inner, cudaMemcpyDeviceToHost));
+    SMB_CUDA_OK(cudaMemcpy(node_2l, kc.node, (inner + 1) * sizeof(double2), cudaMemcpyDeviceToHost));
+    SMB_CUDA_OK(cudaMemcpy(pb, kc.pb, entries * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+    if (variant == 0) SMB_CUDA_OK(cudaMemcpy(pn, kc.pn, entries * sizeof(BucketNormal), cudaMemcpyDeviceToHost));
+    else SMB_CUDA_OK(cudaMemcpy(pid, kc.pid, entries * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  } else if (variant == 3) {
+    SMB_CUDA_OK(cudaMemcpy(bpts, o.ft.bpts.p, (size_t)n * sizeof(BucketPoint), cudaMemcpyDeviceToHost));
+  }
+  return SM_OK;
+}
+
 }  // extern "C"
