@@ -158,6 +158,10 @@ class FloatCloudMatcherB200 : public Interface {
 class NdtB200 : public FloatCloudMatcherB200<SM_TYPE_NDT> {   // registers no option, like Ndt
  public:
   explicit NdtB200(int device = 0) : FloatCloudMatcherB200<SM_TYPE_NDT>(device) {}
+  // pclomp setNeighborhoodSearchMethod (ndt_omp.h:184) with pclomp's NeighborSearchMethod values (sm_ndt_search_method);
+  // the engine keeps it for every later Align and AlignBatch.  The reference's Ndt sets KDTREE (ndt.cc:33), the
+  // default.  A value outside 0..3 CHECK-fails.
+  void SetNeighborhoodSearchMethod(int method) { CheckRc(sm_set_ndt_search_method(handle_, method)); }
 };
 
 class NdtWithGicpB200 : public FloatCloudMatcherB200<SM_TYPE_NDT_WITH_GICP> {

@@ -94,6 +94,32 @@ int sm_print_options(sm_handle* h, char* buf, int64_t buf_len);
  * towards T_iter, which is what the code evidently intends.  Not an XML option: sm_print_options does not list
  * it. */
 int sm_set_inner_compensation(sm_handle* h, int32_t enable);
+/* pclomp::NormalDistributionsTransform::setNeighborhoodSearchMethod (registrators/pclomp/ndt_omp.h:184), the
+ * neighbour search of the per-point derivative evaluation (switch at ndt_omp_impl.hpp:233-246).  Values are
+ * pclomp's NeighborSearchMethod (ndt_omp.h:52-57).  The reference's Ndt sets KDTREE (ndt.cc:33), the default here;
+ * pclomp's own default is DIRECT7 (ndt_omp_impl.hpp:74).
+ *   KDTREE    radius search over the voxel centroids (radius = resolution), sorted by distance; a voxel whose
+ *             covariance failed the eigenvalue test stays searchable with a zero inverse covariance.
+ *   DIRECT26 / DIRECT7 / DIRECT1  VoxelGridCovariance::getNeighborhoodAtPoint / 7 / 1
+ *             (voxel_grid_covariance_omp_impl.hpp:373-441): the query cell is int(floor(x / resolution)) per axis, a
+ *             float division (the grid itself is built with a multiplication by 1 / resolution), and the voxels at
+ *             fixed offsets from it are taken in list order, without a distance test or a sort, when they lie in the
+ *             target's voxel box and hold >= 6 points with a valid covariance.  DIRECT1: the query cell;
+ *             DIRECT7: it and its 6 face neighbours; DIRECT26: the 26 surrounding cells WITHOUT the query cell
+ *             (pcl::getAllNeighborCellIndices of stock PCL, restated from upstream PCL).  A point whose
+ *             floor(x / resolution) is not finite or lies more than one cell outside the box on some axis has no
+ *             neighbour (the reference's int conversion is undefined there).
+ * Applies from the next Align on (sm_align and sm_align_batch alike).  SM_TYPE_NDT only: every other type returns
+ * SM_ERR_UNSUPPORTED_TYPE (the NDT stage of NdtWithGicp is stock pcl::NormalDistributionsTransform, which has no
+ * such setter); a method outside 0..3 returns SM_ERR_BAD_ARGUMENT and leaves the setting unchanged.  Not an XML
+ * option (the reference's Ndt registers none): sm_print_options does not list it. */
+enum sm_ndt_search_method {
+  SM_NDT_KDTREE = 0,
+  SM_NDT_DIRECT26 = 1,
+  SM_NDT_DIRECT7 = 2,
+  SM_NDT_DIRECT1 = 3
+};
+int sm_set_ndt_search_method(sm_handle* h, int32_t method);
 /* Interface::GetType (interface.h:106). */
 int sm_get_type(const sm_handle* h);
 

@@ -19,6 +19,7 @@
  *     sm_debug_voxel_index     the voxel index of a point in the submap filter, the NDT grid and ApproximateVoxelGrid
  *     sm_debug_motion_host     InterpolateTransform(Identity, delta, factor) applied to a point
  *     sm_debug_normals_leaf    the leaf plane fit of CalculateNormals (cloud_types.cc:73-103)
+ *     sm_debug_ndt_direct_neighbors  the NDT derivative kernel's DIRECT26 / DIRECT7 / DIRECT1 neighbour searches
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -26,6 +27,7 @@
  *                              searches), so that path's index sets and squared distances meet the oracle's directly
  *     sm_debug_ndt_grid        the NDT target grid as NdtStage::build_grid leaves it: voxel keys, leaves, size guard
  *     sm_debug_ndt_derivatives the 44 sums of NdtStage::eval (computeDerivatives) at given pose vectors, both forms
+ *     sm_debug_ndt_derivatives_search  the same with each of pclomp's four neighbour searches
  *     sm_debug_float_tree_knn  the float tree's exact searches: knn1 (eps = 0) and the 20-NN of the covariances
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
@@ -175,6 +177,23 @@ int sm_debug_ndt_grid(int device, const float* target_3n, int64_t n, float resol
 int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, const float* source_3n, int64_t ns,
                       float resolution, double outlier_ratio, int32_t f64_math, const double* p_6k, int32_t n_poses,
                       double* sums_44k);
+
+/* sm_debug_ndt_derivatives (pclomp's float term math) with the neighbour search of sm_set_ndt_search_method:
+ * search_method 0 KDTREE, 1 DIRECT26, 2 DIRECT7, 3 DIRECT1. */
+int sm_debug_ndt_derivatives_search(int device, const float* target_3n, int64_t nt, const float* source_3n,
+                                    int64_t ns, float resolution, double outlier_ratio, int32_t search_method,
+                                    const double* p_6k, int32_t n_poses, double* sums_44k);
+
+/* The direct neighbour searches of the derivative kernel (csrc/ndt.cu for_each_direct_cell and its leaf test,
+ * voxel_grid_covariance_omp_impl.hpp:373-441) compiled for the host, no GPU needed: for each point {x, y, z} (the
+ * transformed source point), search_method 1 DIRECT26 / 2 DIRECT7 / 3 DIRECT1, cells of `resolution` in the box
+ * min_b_3 .. min_b_3 + div_b_3 - 1, and the grid's leaves (leaf_key: leaf index, leaf_nr_points: nr_points, -1 for
+ * a failed covariance), counts_n[i] neighbours whose leaf indices are keys_26n[26 i ..], in the order the kernel
+ * visits them. */
+int sm_debug_ndt_direct_neighbors(int32_t search_method, const float* points_3n, int64_t n, float resolution,
+                                  const int32_t* min_b_3, const int32_t* div_b_3, const int32_t* leaf_key,
+                                  const int32_t* leaf_nr_points, int64_t n_leaves, int32_t* counts_n,
+                                  int32_t* keys_26n);
 
 /* FloatTree::build over the cloud, then for each double query {x, y, z}: k = 1, knn1 with eps = 0 (the fitness
  * score and the GICP correspondences); k = 20, knn_k (the GICP covariances), ascending (d2, id), unused entries

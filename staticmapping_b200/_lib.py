@@ -43,6 +43,7 @@ SIGNATURES = {
     "sm_set_option": (C.c_int, [_VP, C.c_char_p, C.c_char_p]),
     "sm_print_options": (C.c_int, [_VP, C.c_char_p, C.c_int64]),
     "sm_set_inner_compensation": (C.c_int, [_VP, C.c_int32]),
+    "sm_set_ndt_search_method": (C.c_int, [_VP, C.c_int32]),
     "sm_get_type": (C.c_int, [_VP]),
     "sm_set_input_source": (C.c_int, [_VP, _VP, C.c_int64]),
     "sm_set_input_target": (C.c_int, [_VP, _VP, _VP, C.c_int64]),
@@ -91,6 +92,10 @@ SIGNATURES = {
     "sm_debug_ndt_grid": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_float, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "sm_debug_ndt_derivatives": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_float, C.c_double,
                                            C.c_int32, _VP, C.c_int32, _VP]),
+    "sm_debug_ndt_derivatives_search": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_float, C.c_double,
+                                                  C.c_int32, _VP, C.c_int32, _VP]),
+    "sm_debug_ndt_direct_neighbors": (C.c_int, [C.c_int32, _VP, C.c_int64, C.c_float, _VP, _VP, _VP, _VP, C.c_int64,
+                                                _VP, _VP]),
     "sm_debug_float_tree_knn": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, _VP, _VP]),
     "sm_debug_approx_voxel_grid": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_float, _VP, _VP]),
     "sm_debug_gicp_covariances": (C.c_int, [C.c_int, _VP, C.c_int64, _VP]),

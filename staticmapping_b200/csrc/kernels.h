@@ -236,6 +236,13 @@ struct NdtEvalParams {      // everything one computeDerivatives call needs, by 
   double j_ang_d[8][3];     // the same tables in double (stock PCL keeps them as Vector3d)
   double h_ang_d[15][3];
 };
+// pclomp's NeighborSearchMethod (ndt_omp.h:52-57), same values as sm_ndt_search_method
+enum NdtSearch : int { kNdtKdtree = 0, kNdtDirect26 = 1, kNdtDirect7 = 2, kNdtDirect1 = 3 };
+// host build of the direct neighbour searches of ndt.cu (test hook sm_debug_ndt_direct_neighbors): the keys of the
+// in-box offset cells of point x in offset order, at most 26; returns their number
+int ndt_debug_direct_cells_host(int search, const float* x, float leaf, const NdtGrid& g, int* keys26);
+// the leaf test the kernel applies to those cells: nr_points >= min_points_per_voxel_
+bool ndt_debug_direct_leaf_accepted_host(int nr_points);
 // host build of the leaf plane fit of normals.cu (test hook sm_debug_normals_leaf): 1 kept, 0 dropped, < 0 bad count
 int normals_debug_leaf_host(const double* members, int count, double* mean, double* unit);
 // host build of one target-grid leaf of ndt.cu (test hook sm_debug_ndt_leaf)
@@ -270,7 +277,7 @@ struct NdtStage {
   int reserve(int nt, int ns);
   int build_grid(const float* tgt, int nt, float resolution, cudaStream_t stream);   // setInputTarget -> init()
   static constexpr int kGridLaunches = 12 + 12;
-  int eval(const float* src, int ns, const NdtEvalParams& P, double* sums44, cudaStream_t stream);
+  int eval(const float* src, int ns, const NdtEvalParams& P, int search, double* sums44, cudaStream_t stream);
   static constexpr int kEvalLaunches = 2;
   int fitness(const float* src, int ns, const float* tgt, const float* T, const FloatTree& t, double* sums2,
               cudaStream_t stream, double* score);

@@ -347,6 +347,59 @@ __device__ __forceinline__ int hash_lookup(const int* __restrict__ table_key, co
   return -1;
 }
 
+// ---- direct neighbour searches (pclomp DIRECT26 / DIRECT7 / DIRECT1) ------------------------
+constexpr int kMinPointsPerVoxel = 6;   // min_points_per_voxel_ (voxel_grid_covariance_omp.h)
+
+// Offset k of the method's list (voxel_grid_covariance_omp_impl.hpp:405-441).  DIRECT26 is
+// pcl::getAllNeighborCellIndices() of stock PCL, which is not vendored; restated from upstream PCL: the 13 "half"
+// offsets (i, j, -1) for i = -1..1, j = -1..1 (i outer), (i, -1, 0) for i = -1..1, (-1, 0, 0), then those 13
+// negated.  It holds no (0, 0, 0): DIRECT26 never visits the query's own cell.
+template <int kSearch>
+__host__ __device__ __forceinline__ void direct_offset(int k, int* o) {
+  if (kSearch == kNdtDirect26) {
+    const int h = k < 13 ? k : k - 13, s = k < 13 ? 1 : -1;
+    if (h < 9) { o[0] = h / 3 - 1; o[1] = h % 3 - 1; o[2] = -1; }
+    else if (h < 12) { o[0] = h - 10; o[1] = -1; o[2] = 0; }
+    else { o[0] = -1; o[1] = 0; o[2] = 0; }
+    o[0] *= s; o[1] *= s; o[2] *= s;
+  } else {   // DIRECT7: (0,0,0), (+1,0,0), (-1,0,0), (0,+1,0), (0,-1,0), (0,0,+1), (0,0,-1); DIRECT1: k = 0 only
+    o[0] = o[1] = o[2] = 0;
+    if (k > 0) o[(k - 1) / 2] = (k & 1) ? 1 : -1;
+  }
+}
+
+// VoxelGridCovariance::getNeighborhoodAtPoint (voxel_grid_covariance_omp_impl.hpp:373-403) up to the leaf test:
+// visit(key) for each offset cell of point x that lies in the grid's box, in list order, key = the cell's leaf
+// index ((ijk + d - min_b) . divb_mul, the index build_grid gives it).  The caller keeps a cell whose leaf exists and
+// has nr_points >= 6 (:394-395), so a leaf that failed the eigenvalue test (nr_points = -1) is never a neighbour
+// here, while the KDTREE search keeps it with icov = 0.
+// ijk = int(floor(x / leaf_size)), a float DIVISION (:379-381): the grid build multiplies by 1 / leaf_size, and the
+// two disagree for points on or near a cell face when the resolution is not a power of two.
+// Undefined input: the reference's static_cast<int> of a non-finite or out-of-range floor is undefined behaviour.
+// Here a point has no neighbour when floor(x / leaf) is not finite or outside [min_b - 1, max_b + 1] on some axis.
+// Wherever the reference is defined this is its result (no offset in {-1, 0, 1} reaches the box from there), and
+// ijk + d cannot overflow.
+template <int kSearch, class Visit>
+__host__ __device__ __forceinline__ void for_each_direct_cell(const float* x, float leaf, const NdtGrid& g,
+                                                              Visit visit) {
+  int rel[3];
+  for (int d = 0; d < 3; ++d) {
+    const float f = floorf(x[d] / leaf);
+    const double lo = (double)g.min_b[d] - 1.0, hi = (double)g.min_b[d] + (double)g.div_b[d];   // max_b + 1
+    if (!((double)f >= lo && (double)f <= hi)) return;
+    rel[d] = (int)f - g.min_b[d];
+  }
+  const int count = kSearch == kNdtDirect26 ? 26 : (kSearch == kNdtDirect7 ? 7 : 1);
+#pragma unroll 1
+  for (int k = 0; k < count; ++k) {
+    int o[3];
+    direct_offset<kSearch>(k, o);
+    const int a = rel[0] + o[0], b = rel[1] + o[1], c = rel[2] + o[2];
+    if (a < 0 || b < 0 || c < 0 || a >= g.div_b[0] || b >= g.div_b[1] || c >= g.div_b[2]) continue;
+    visit(a * g.mul[0] + b * g.mul[1] + c * g.mul[2]);
+  }
+}
+
 // ---- derivatives ----------------------------------------------------------------------------
 __device__ __forceinline__ float dist2f(float qx, float qy, float qz, const float* c) {
   const float dx = qx - c[0], dy = qy - c[1], dz = qz - c[2];
@@ -469,6 +522,8 @@ __host__ __device__ __forceinline__ double update_derivatives_f64(const NdtEvalP
   return score_inc;
 }
 
+// kSearch: pclomp's neighbour search (ndt_omp_impl.hpp:233-246); KDTREE is the radius search the reference selects
+template <int kSearch>
 __global__ void __launch_bounds__(kNdtThreads)
 ndt_derivatives_kernel(const float* __restrict__ src, int n, NdtEvalParams P,
                        const NdtGrid* __restrict__ grid, const NdtLeaf* __restrict__ leaves,
@@ -479,7 +534,36 @@ ndt_derivatives_kernel(const float* __restrict__ src, int n, NdtEvalParams P,
 #pragma unroll
   for (int k = 0; k < kNdtSums; ++k) acc[k] = 0.0;
   const int i = blockIdx.x * kNdtThreads + threadIdx.x;
-  if (i < n) {
+  if (kSearch != kNdtKdtree && i < n) {
+    const NdtGrid g = *grid;
+    const float xo[3] = {src[3 * (int64_t)i], src[3 * (int64_t)i + 1], src[3 * (int64_t)i + 2]};
+    float xt[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) xt[r] = ((P.T[r] * xo[0] + P.T[r + 4] * xo[1]) + P.T[r + 8] * xo[2]) + P.T[r + 12];
+    double score_pt = 0.0, grad_pt[6], hess_pt[36];
+#pragma unroll
+    for (int q = 0; q < 6; ++q) grad_pt[q] = 0.0;
+#pragma unroll
+    for (int q = 0; q < 36; ++q) hess_pt[q] = 0.0;
+    int nc = 0;
+    // neighbours in offset order, no distance test and no sort (voxel_grid_covariance_omp_impl.hpp:383-400)
+    for_each_direct_cell<kSearch>(xt, P.radius, g, [&](int key) {
+      const int v = hash_lookup(table_key, table_val, table_mask, key);   // the table holds leaves of >= 6 points
+      if (v < 0) return;
+      const NdtLeaf leaf = leaves[v];
+      if (leaf.nr_points < kMinPointsPerVoxel) return;                     // nr_points = -1: failed covariance
+      ++nc;
+      score_pt += P.f64_math ? update_derivatives_f64(P, xo, xt, leaf, grad_pt, hess_pt)
+                             : update_derivatives(P, xo, xt, leaf, grad_pt, hess_pt);
+    });
+    acc[0] = score_pt;
+#pragma unroll
+    for (int q = 0; q < 6; ++q) acc[1 + q] = grad_pt[q];
+#pragma unroll
+    for (int q = 0; q < 36; ++q) acc[7 + q] = hess_pt[q];
+    acc[43] = (double)nc;
+  }
+  if (kSearch == kNdtKdtree && i < n) {
     const NdtGrid g = *grid;
     const float xo[3] = {src[3 * (int64_t)i], src[3 * (int64_t)i + 1], src[3 * (int64_t)i + 2]};
     float xt[3];
@@ -600,6 +684,17 @@ ndt_fitness_kernel(const float* __restrict__ src, int n, NdtEvalParams P, const 
 // host build of the per-axis voxel coordinate of the NDT grid (test hook sm_debug_voxel_index op 1)
 int ndt_debug_voxel_coord_host(float v, float inv_leaf, int min_b) { return voxel_coord(v, inv_leaf, min_b); }
 
+// host build of the direct searches' cell walk (test hook sm_debug_ndt_direct_neighbors)
+int ndt_debug_direct_cells_host(int search, const float* x, float leaf, const NdtGrid& g, int* keys26) {
+  int m = 0;
+  auto keep = [&](int key) { keys26[m++] = key; };
+  if (search == kNdtDirect26) for_each_direct_cell<kNdtDirect26>(x, leaf, g, keep);
+  else if (search == kNdtDirect7) for_each_direct_cell<kNdtDirect7>(x, leaf, g, keep);
+  else if (search == kNdtDirect1) for_each_direct_cell<kNdtDirect1>(x, leaf, g, keep);
+  return m;
+}
+bool ndt_debug_direct_leaf_accepted_host(int nr_points) { return nr_points >= kMinPointsPerVoxel; }
+
 // Host build of one leaf of the target grid (test hook sm_debug_ndt_leaf): the running sums are formed here in input
 // order (the kernel forms them with one warp per voxel, in the same order), the rest is finish_leaf.
 void ndt_debug_leaf_host(const float* pts, int n, int min_points, double eig_mult, double* mean3, double* icov9,
@@ -706,10 +801,15 @@ int NdtStage::build_grid(const float* tgt, int nt, float resolution, cudaStream_
 }
 
 // computeDerivatives: out[44] = score, gradient, hessian (row-major), neighbour count
-int NdtStage::eval(const float* src, int ns, const NdtEvalParams& P, double* sums44, cudaStream_t stream) {
+int NdtStage::eval(const float* src, int ns, const NdtEvalParams& P, int search, double* sums44,
+                   cudaStream_t stream) {
   const int nb = ndt_blocks(ns);
-  ndt_derivatives_kernel<<<nb, kNdtThreads, 0, stream>>>(src, ns, P, ws.grid, ws.leaves, ws.table_key,
-                                                        ws.table_val, ws.table_size - 1, ws.partials);
+  auto kernel = search == kNdtDirect26 ? ndt_derivatives_kernel<kNdtDirect26>
+              : search == kNdtDirect7  ? ndt_derivatives_kernel<kNdtDirect7>
+              : search == kNdtDirect1  ? ndt_derivatives_kernel<kNdtDirect1>
+                                       : ndt_derivatives_kernel<kNdtKdtree>;
+  kernel<<<nb, kNdtThreads, 0, stream>>>(src, ns, P, ws.grid, ws.leaves, ws.table_key, ws.table_val,
+                                         ws.table_size - 1, ws.partials);
   ndt_reduce_kernel<<<1, 1024, 0, stream>>>(ws.partials, nb, kNdtSums, ws.sums);
   SMB_CUDA_OK(cudaGetLastError());
   SMB_CUDA_OK(cudaMemcpyAsync(sums44, ws.sums, kNdtSums * sizeof(double), cudaMemcpyDeviceToHost, stream));

@@ -23,6 +23,7 @@ struct Options {                 // defaults of the reference (ndt.cc:31, ndt_om
   double outlier_ratio = 0.55;
   double transformation_epsilon = 0.1;
   int max_iterations = 35;
+  int search = kNdtKdtree;       // setNeighborhoodSearchMethod (ndt_omp.h:184); the reference sets KDTREE (ndt.cc:33)
 };
 
 inline void angle_tables(const double* p, NdtEvalParams* P) {

@@ -714,7 +714,7 @@ int ndt_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, co
   ndt::NewtonOut nw;
   int launches = NdtStage::kGridLaunches;
   const int nrc = ndt::newton_loop(o, guess, ns, P, [&](const NdtEvalParams& Pe, const double*, double* sums) -> int {
-    H_RC(st.eval(src, ns, Pe, h->host->ndt_sums, h->stream));
+    H_RC(st.eval(src, ns, Pe, o.search, h->host->ndt_sums, h->stream));
     if (*overflow) return SM_ERR_BAD_ARGUMENT;
     for (int i = 0; i < 44; ++i) sums[i] = h->host->ndt_sums[i];
     launches += NdtStage::kEvalLaunches;
@@ -835,7 +835,7 @@ int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
   for (int i = 0; i < 16; ++i) ndt_guess[i] = (float)guess[i];
   double ndt_score = 0.9;
   if (h->ng.use_ndt) {                    // ndt_gicp.cc:82-88, configuration :44-47
-    ndt::Options no;
+    ndt::Options no;                      // stock pcl::NormalDistributionsTransform: KDTREE only
     no.transformation_epsilon = 0.01; no.step_size = 0.1; no.resolution = 1.0f; no.max_iterations = 35;
     NdtRunOut r;
     const int rc = ndt_run(h, src, ns, tgt, nt, no, true, guess, &r);
@@ -950,6 +950,16 @@ int sm_set_option(sm_handle* h, const char* name, const char* text) {
 int sm_set_inner_compensation(sm_handle* h, int32_t enable) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
   h->inner_compensation = enable != 0;
+  return SM_OK;
+}
+
+int sm_set_ndt_search_method(sm_handle* h, int32_t method) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  if (h->type != SM_TYPE_NDT)
+    return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetNeighborhoodSearchMethod: registrator::Ndt (type 5) only");
+  if (method < SM_NDT_KDTREE || method > SM_NDT_DIRECT1)
+    return fail(h, SM_ERR_BAD_ARGUMENT, "SetNeighborhoodSearchMethod: method must be 0..3");
+  h->ndt.search = method;
   return SM_OK;
 }
 

@@ -5,6 +5,7 @@
 
 #include <string.h>
 
+#include <map>
 #include <vector>
 
 #include "common.cuh"
@@ -345,8 +346,57 @@ int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, con
   o.outlier_ratio = outlier_ratio;
   o.resolution = resolution;
   for (int k = 0; k < n_poses; ++k) {
-    SMB_RC(st.eval((const float*)src.p, (int)ns, ndt::eval_params(o, f64_math != 0, p_6k + 6 * k), sums_44k + 44 * (int64_t)k,
-                   nullptr));
+    SMB_RC(st.eval((const float*)src.p, (int)ns, ndt::eval_params(o, f64_math != 0, p_6k + 6 * k), kNdtKdtree,
+                   sums_44k + 44 * (int64_t)k, nullptr));
+  }
+  return SM_OK;
+}
+
+int sm_debug_ndt_derivatives_search(int device, const float* target_3n, int64_t nt, const float* source_3n,
+                                    int64_t ns, float resolution, double outlier_ratio, int32_t search_method,
+                                    const double* p_6k, int32_t n_poses, double* sums_44k) {
+  if (!debug_cloud_ok(target_3n, nt) || !debug_cloud_ok(source_3n, ns) || !(resolution > 0.0f) || !p_6k ||
+      n_poses <= 0 || !sums_44k || search_method < SM_NDT_KDTREE || search_method > SM_NDT_DIRECT1)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  DevBuf tgt, src;
+  NdtStage st;
+  NdtGrid g;
+  SMB_RC(debug_ndt_build(target_3n, nt, ns, resolution, tgt, st, &g));
+  SMB_RC(debug_upload_f32(source_3n, ns, src));
+  ndt::Options o;
+  o.outlier_ratio = outlier_ratio;
+  o.resolution = resolution;
+  for (int k = 0; k < n_poses; ++k)
+    SMB_RC(st.eval((const float*)src.p, (int)ns, ndt::eval_params(o, false, p_6k + 6 * k), search_method,
+                   sums_44k + 44 * (int64_t)k, nullptr));
+  return SM_OK;
+}
+
+// test hook: the direct searches' cell walk and leaf test (ndt.cu for_each_direct_cell, the code the derivative
+// kernel runs) compiled for the host, over a caller's grid box and leaves — no GPU involved
+int sm_debug_ndt_direct_neighbors(int32_t search_method, const float* points_3n, int64_t n, float resolution,
+                                  const int32_t* min_b_3, const int32_t* div_b_3, const int32_t* leaf_key,
+                                  const int32_t* leaf_nr_points, int64_t n_leaves, int32_t* counts_n,
+                                  int32_t* keys_26n) {
+  if (search_method < SM_NDT_DIRECT26 || search_method > SM_NDT_DIRECT1 || !points_3n || n < 0 || !min_b_3 ||
+      !div_b_3 || n_leaves < 0 || (n_leaves > 0 && (!leaf_key || !leaf_nr_points)) || !counts_n || !keys_26n)
+    return SM_ERR_BAD_ARGUMENT;
+  NdtGrid g;
+  memset(&g, 0, sizeof(g));
+  for (int d = 0; d < 3; ++d) { g.min_b[d] = min_b_3[d]; g.div_b[d] = div_b_3[d]; }
+  g.mul[0] = 1; g.mul[1] = g.div_b[0]; g.mul[2] = g.div_b[0] * g.div_b[1];
+  std::map<int, int> nr;   // leaf index -> nr_points
+  for (int64_t l = 0; l < n_leaves; ++l) nr[leaf_key[l]] = leaf_nr_points[l];
+  for (int64_t i = 0; i < n; ++i) {
+    int cells[26];
+    const int m = ndt_debug_direct_cells_host(search_method, points_3n + 3 * i, resolution, g, cells);
+    int k = 0;
+    for (int j = 0; j < m; ++j) {
+      const auto it = nr.find(cells[j]);
+      if (it != nr.end() && ndt_debug_direct_leaf_accepted_host(it->second)) keys_26n[26 * i + k++] = cells[j];
+    }
+    counts_n[i] = k;
   }
   return SM_OK;
 }

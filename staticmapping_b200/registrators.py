@@ -41,6 +41,14 @@ class CheckFailure(RuntimeError):
     """Raised where the reference would glog CHECK-fail (abort)."""
 
 
+class NeighborSearchMethod(enum.IntEnum):
+    """pclomp::NeighborSearchMethod (registrators/pclomp/ndt_omp.h:52-57), for Ndt.SetNeighborhoodSearchMethod."""
+    KDTREE = 0
+    DIRECT26 = 1
+    DIRECT7 = 2
+    DIRECT1 = 3
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
@@ -253,6 +261,13 @@ class Ndt(Interface):
         transformation_epsilon, max_iterations); not reachable from the reference's XML."""
         for k, v in kw.items():
             self._check(self._lib.sm_set_option(self._h, k.encode(), str(v).encode()), "option")
+
+    def SetNeighborhoodSearchMethod(self, method):
+        """pclomp setNeighborhoodSearchMethod (ndt_omp.h:184): a NeighborSearchMethod; applies from the next
+        Align on.  KDTREE (the reference's choice, ndt.cc:33) is the default; see sm_set_ndt_search_method in
+        include/sm_b200.h for what the direct searches visit.  NdtWithGicp raises CheckFailure: its NDT stage is
+        stock PCL's, which has no such setter."""
+        self._check(self._lib.sm_set_ndt_search_method(self._h, int(method)), "SetNeighborhoodSearchMethod")
 
     def SetInputSource(self, cloud: InnerCloud):
         # Interface::SetInputSource (interface.cc:38-48): null resets, empty only warns
