@@ -261,6 +261,52 @@ inline void VoxelGridFilterB200(const data::InnerCloudType& input, float voxel_s
   output->points.resize(m);
 }
 
+// pre_processers::filter::Factory on the GPU (pre_processors/filter_factory.cc:63-106): one chain per Factory.  The
+// body of Factory::InitFromXmlNode becomes one Add per <filter> and one SetParam per <param>, and the body of
+// Factory::Filter (the call in DataCollector::CloudPreProcessing, builder/data/data_collector.cc:137-141)
+//   this->FilterPrepare(cloud); chain_.Filter(*this->inner_cloud_, cloud.get(), &this->inliers_);
+// RandomSampler is a deterministic stand-in for the reference's mt19937 draw (include/sm_b200.h).
+class FilterChainB200 {
+ public:
+  explicit FilterChainB200(int device = 0) { CHECK_EQ(sm_filter_chain_create(device, &chain_), 0); }
+  ~FilterChainB200() { sm_filter_chain_destroy(chain_); }
+  FilterChainB200(const FilterChainB200&) = delete;
+  FilterChainB200& operator=(const FilterChainB200&) = delete;
+
+  // index of the new filter, or -1 for a name the reference skips too ("not supported yet.")
+  int Add(const std::string& filter_name) {
+    const int index = sm_filter_chain_add(chain_, filter_name.c_str());
+    if (index == SM_ERR_UNKNOWN_OPTION) return -1;
+    CHECK_GE(index, 0) << sm_filter_chain_last_error(chain_);
+    return index;
+  }
+  // type: the <param>'s type attribute, -1 when it has none (the reference CHECK-fails, filter_interface.cc:57)
+  void SetParam(int filter, const std::string& name, int type, const std::string& text) {
+    CHECK_EQ(sm_filter_chain_set_param(chain_, filter, name.c_str(), type, text.c_str()), 0)
+        << sm_filter_chain_last_error(chain_);
+  }
+  bool ConfigsValid(int filter) { return sm_filter_chain_validate(chain_, filter) == 1; }
+
+  void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,
+              std::vector<int>* const inliers = nullptr) {
+    CHECK(output);
+    const int64_t n = static_cast<int64_t>(input.points.size());
+    output->points.resize(input.points.size());
+    std::vector<int32_t> index(input.points.size());
+    int64_t m = 0;
+    if (n > 0) {
+      const int rc = sm_filter_chain_run(chain_, &input.points[0].x, n, sizeof(data::InnerPointType),
+                                         &output->points[0].x, &m, index.data());
+      CHECK_EQ(rc, 0) << "sm_filter_chain_run failed (" << rc << "): " << sm_filter_chain_last_error(chain_);
+    }
+    output->points.resize(m);
+    if (inliers) inliers->assign(index.begin(), index.begin() + m);
+  }
+
+ private:
+  sm_filter_chain* chain_ = nullptr;
+};
+
 // descriptor::M2dp::setInputCloud + getFinalDescriptor on the GPU (descriptor/m2dp.cc:129-153): the body of
 // setInputCloud becomes   return registrator::M2dpB200(*source, r_, max_distance_, t_, p_, q_, &descriptor_);
 inline bool M2dpB200(const data::InnerCloudType& source, double r, double max_distance, int32_t t, int32_t p,

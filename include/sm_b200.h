@@ -44,6 +44,7 @@ enum sm_error {
   SM_ERR_NO_FINITE_MATCH = -2,   /* CHECK(!values.empty())            icp_fast.cc:81  */
   SM_ERR_NOTHING_TO_MINIMIZE = -3, /* CHECK_GT(points_count, 0)        icp_fast.cc:114 */
   SM_ERR_MISSING_INPUT = -4,     /* CHECK(cloud) / missing normals    icp_fast.cc:422-430 */
+  SM_ERR_CHECK_FAILED = -5,      /* a CHECK of the filter chain: bounding_box.cc:114, filter_ground_removal2.cc:403 */
   SM_ERR_UNKNOWN_OPTION = -10,   /* "Init an unknown option"          interface.cc:66-67 */
   SM_ERR_UNSUPPORTED_TYPE = -11, /* CreateMatcher default branch      interface.cc:158-160 */
   SM_ERR_NO_DEVICE = -20,        /* no CUDA device: the engine has no CPU fallback */
@@ -299,6 +300,68 @@ int64_t sm_m2dp_descriptor_length(double r, double max_distance, int32_t t, int3
 int sm_m2dp(int device, const float* points, int64_t n, int64_t stride_bytes, double r, double max_distance,
             int32_t t, int32_t p, int32_t q, float* descriptor, int64_t capacity, int32_t* A_out);
 double sm_m2dp_match(const float* P, const float* Q, int64_t n);
+
+/* ---- pre_processers::filter::Factory: the scan pre-processing chain --------------------------------------------
+ * Every scan the reference matches has gone through filter::Factory::Filter (builder/data/data_collector.cc:137-141;
+ * the chain is built from the <filters> node, pre_processors/filter_factory.cc:63-106).  A chain applies its filters
+ * in the order they were added; every filter emits its inliers in ascending input index, whole
+ * data::InnerPointType records (x, y, z, intensity, factor) copied.  One chain is used by one thread at a time.
+ * Built here, under the reference's names and parameter names (type 0 int, 1 float):
+ *   Range               filter_range.cc:45-88        min_range (0), max_range (FLT_MAX): sqrtf(x^2+y^2+z^2) in [min, max]
+ *   AxisRange           filter_axis_range.cc:41-102  min, max (-/+FLT_MAX), axis_index (2).  A NaN coordinate is kept,
+ *                                                    as in the reference (it is neither < min nor > max).
+ *   BoundingBoxRemoval  filter_bounding_box.cc:49-83 min_x .. max_z (-/+FLT_MAX): REMOVES the points inside the closed
+ *                                                    box; the default box removes every finite point.
+ *   RandomSampler       filter_random_sample.cc:35-77 sampling_rate (1); a rate > 0.999 passes everything.  The
+ *                       reference draws from std::mt19937 seeded by std::random_device: its result is not a function of
+ *                       its inputs.  DETERMINISTIC STAND-IN: point i is kept iff
+ *                       murmur3_fmix32(i * 0x9E3779B9 + sample_seed) <= sampling_rate * 2^32, i = the point's index in
+ *                       the scan handed to the chain (not in the filter's own input), sample_seed a chain option.
+ *   RangeImage          filter_range_image.cc:66-141 (Filter only) top_angle (30), btm_angle (-15), offset_x/y/z (0),
+ *                       vertical_line_num (40), horizontal_line_num (1800): the first point in input order per pixel.
+ *   GroundRemoval2      filter_ground_removal2.cc:127-414  r_max (100), r_min (1), bin_num (200), segment_num (180),
+ *                       start_ground_height (-0.25), long_line_threshold (1), max_long_line_height (0.1),
+ *                       max_start_height (0.2), max_error (0.05), max_slope (tan 15 deg), max_b (0.1, unused),
+ *                       max_dist_to_line (0.05), search_angle (10), thread_num (4, unused).
+ * atan2f is CUDA's here and glibc's in the reference: a point within a few float ulps of a RangeImage row / column
+ * border or a GroundRemoval2 segment border can land in the neighbouring pixel / segment.  A float -> int conversion
+ * outside int's range (undefined in C++) gives INT_MIN, as the reference's x86 build does. */
+typedef struct sm_filter_chain sm_filter_chain;
+/* filter::Factory::Factory (filter_factory.h).  Needs no device; the first run binds CUDA ordinal `device`. */
+int sm_filter_chain_create(int device, sm_filter_chain** out);
+int sm_filter_chain_destroy(sm_filter_chain* chain);
+/* One <filter name=...> of Factory::InitFromXmlNode (filter_factory.cc:64-80): appends the filter at its constructor's
+ * defaults and returns its index.  GroundRemoval, StatisticRemoval (an empty body in the reference,
+ * filter_statistic_removal.cc:44-59) and VoxelGrid (see sm_voxel_grid_filter) are not built into the chain:
+ * SM_ERR_UNSUPPORTED_TYPE.  A name the reference does not register either (it skips it, :68-71):
+ * SM_ERR_UNKNOWN_OPTION; the chain is unchanged. */
+int sm_filter_chain_add(sm_filter_chain* chain, const char* filter_name);
+/* One <param type=... name=...>text</param> of Interface::InitFromXmlNode (filter_interface.cc:38-58): `text` is read
+ * as pugixml's as_int (type 0) or as_float (type 1), then cast to the parameter's declared type
+ * (XmlInterface::SetValue, xml_interface.h:55-75).  Where the reference CHECK-fails (:57): SM_ERR_UNKNOWN_OPTION for a
+ * name the filter does not register, SM_ERR_BAD_ARGUMENT for a type other than 0 / 1 (a <param> without `type`). */
+int sm_filter_chain_set_param(sm_filter_chain* chain, int filter, const char* name, int type, const char* text);
+/* Interface::ConfigsValid of the filter (filter_interface.cc:59; AxisRange filter_axis_range.cc:41-43,
+ * BoundingBoxRemoval filter_bounding_box.cc:49-51, RandomSampler filter_random_sample.cc:35-37): 1 / 0.  As in the
+ * reference's Factory (filter_factory.cc:77), an invalid filter still runs. */
+int sm_filter_chain_validate(sm_filter_chain* chain, int filter);
+/* Chain options, no reference counterpart: sample_seed (unsigned, 1), the seed of RandomSampler's stand-in. */
+int sm_filter_chain_set_option(sm_filter_chain* chain, const char* name, const char* text);
+/* Factory::SetInputCloud + Factory::Filter (filter_factory.cc:83-106).  `points`: n records `stride_bytes` (>= 20)
+ * apart; `out`: capacity n packed 5-float records; *m_out = the number of inliers; inlier_index (optional, capacity
+ * n): their indices in `points`, ascending.  An empty chain copies the input (:90-93).  SM_ERR_BAD_ARGUMENT: a
+ * RangeImage with vertical_line_num <= 0 or horizontal_line_num <= 0 (its SetInputCloud keeps the previous cloud,
+ * filter_range_image.cc:72-74) or a grid of more than 2^24 pixels / cells.  SM_ERR_CHECK_FAILED: an inverted
+ * BoundingBoxRemoval box (CHECK in common/bounding_box.cc:114) or a fitted ground line that does not run outward
+ * (CHECK(line.start[0] < line.end[0]), filter_ground_removal2.cc:403).
+ * The _device form takes device pointers (in and out may not overlap), runs on `cuda_stream` (a cudaStream_t, NULL =
+ * default stream) and returns after the stream has finished; its output feeds sm_motion_compensation_device and
+ * sm_set_input_source_f32_device (stride 20) without a host copy. */
+int sm_filter_chain_run(sm_filter_chain* chain, const float* points, int64_t n, int64_t stride_bytes, float* out,
+                        int64_t* m_out, int32_t* inlier_index_or_null);
+int sm_filter_chain_run_device(sm_filter_chain* chain, const float* dev_points, int64_t n, int64_t stride_bytes,
+                               float* dev_out, int64_t* m_out, int32_t* dev_inlier_index_or_null, void* cuda_stream);
+const char* sm_filter_chain_last_error(const sm_filter_chain* chain);
 
 int sm_device_count(void);
 const char* sm_version(void);

@@ -20,6 +20,8 @@
  *     sm_debug_motion_host     InterpolateTransform(Identity, delta, factor) applied to a point
  *     sm_debug_normals_leaf    the leaf plane fit of CalculateNormals (cloud_types.cc:73-103)
  *     sm_debug_ndt_direct_neighbors  the NDT derivative kernel's DIRECT26 / DIRECT7 / DIRECT1 neighbour searches
+ *     sm_debug_filter_host     the filter chain's per-point functions: predicate, RangeImage pixel, GroundRemoval2 cell
+ *     sm_debug_filter_fit_host, sm_debug_filter_distance_host  GroundRemoval2's line fit and VerticalDistanceToSegment
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -36,6 +38,7 @@
  *     sm_debug_radix_sort      radix_sort_pairs_u64 as the tree build, the voxel filters and the NDT grid call it
  *     sm_debug_kd_tree         every array a k-d tree owner (KdCompactTree, NormalsPipeline, FloatTree) fills, after
  *                              an optional earlier build into the same owner
+ *     sm_debug_filter_ground_removal2  every intermediate of FilterChain's GroundRemoval2 stage
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
  *   each stage of M2DP meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
@@ -261,6 +264,32 @@ int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* fi
                      int64_t n_first, const void* cloud_3n, const double* normals_3n, int64_t n, int32_t levels,
                      void* nodes, uint32_t* order, double* cut, uint8_t* dim, double* node_2l, double* pb, double* pn,
                      int32_t* pid, void* bpts);
+
+/* The per-point functions of the filter chain (csrc/filters.cu) compiled for the host, for filter `filter` of `chain`
+ * over n packed 5-float records (record i is given scan index i):
+ *   op 0  the predicate of Range / AxisRange / BoundingBoxRemoval / RandomSampler: iout[i] = 1 kept, 0 removed
+ *   op 1  RangeImage's pixel (filter_range_image.cc:102-126): iout[2i] = row, iout[2i+1] = col, -1 -1 for an outlier
+ *   op 2  GroundRemoval2's cell (filter_ground_removal2.cc:163-191): iout[2i] = segment, iout[2i+1] = bin, fout[i] = range */
+struct sm_filter_chain;
+int sm_debug_filter_host(const struct sm_filter_chain* chain, int32_t filter, int32_t op, const float* records, int64_t n,
+                         int32_t* iout, float* fout);
+/* FitLocalLine (filter_ground_removal2.cc:29-44) over n >= 2 points (d, z): m_b = {m, b}. */
+int sm_debug_filter_fit_host(const float* d, const float* z, int32_t n, float* m_b);
+/* VerticalDistanceToSegment (filter_ground_removal2.cc:398-414) of point (d, z) to a segment's lines, each
+ * {start d, start z, end d, end z}; SM_ERR_CHECK_FAILED where the reference's CHECK(line.start[0] < line.end[0]) fails. */
+int sm_debug_filter_distance_host(const float* lines_4l, int32_t n_lines, float d, float z, float* distance);
+/* FilterChain's GroundRemoval2 stage with the parameters of filter `filter` of `chain`, over n host records:
+ *   cell[n]            segment * bin_num + bin of each point       member[n]  1 if the point joined its cell (:204-209)
+ *   cell_members[c]    members per cell                            cell_min_2c  min_z_point (d, z) per cell (valid
+ *                                                                               where the cell has a member)
+ *   lines_4, n_lines   [segment_num][max_lines] lines {d0, z0, d1, z1} and their number per segment;
+ *                      max_lines must be bin_num / 2 + 1
+ *   keep[n]            1 for the points that are not ground
+ * Returns SM_OK, or SM_ERR_CHECK_FAILED with the arrays filled when a line does not run outward. */
+int sm_debug_filter_ground_removal2(int device, const struct sm_filter_chain* chain, int32_t filter, const float* points,
+                                    int64_t n, int64_t stride_bytes, int32_t max_lines, uint32_t* cell, uint8_t* member,
+                                    uint32_t* cell_members, float* cell_min_2c, float* lines_4, int32_t* n_lines,
+                                    uint8_t* keep);
 
 #ifdef __cplusplus
 }

@@ -71,6 +71,15 @@ SIGNATURES = {
     "sm_m2dp": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32,
                           _VP, C.c_int64, _VP]),
     "sm_m2dp_match": (C.c_double, [_VP, _VP, C.c_int64]),
+    "sm_filter_chain_create": (C.c_int, [C.c_int, C.POINTER(_VP)]),
+    "sm_filter_chain_destroy": (C.c_int, [_VP]),
+    "sm_filter_chain_add": (C.c_int, [_VP, C.c_char_p]),
+    "sm_filter_chain_set_param": (C.c_int, [_VP, C.c_int, C.c_char_p, C.c_int, C.c_char_p]),
+    "sm_filter_chain_validate": (C.c_int, [_VP, C.c_int]),
+    "sm_filter_chain_set_option": (C.c_int, [_VP, C.c_char_p, C.c_char_p]),
+    "sm_filter_chain_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
+    "sm_filter_chain_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
+    "sm_filter_chain_last_error": (C.c_char_p, [_VP]),
     # include/sm_b200_debug.h (test hooks)
     "sm_debug_solve6": (C.c_int, [C.c_int, _VP, _VP, _VP, _VP]),
     "sm_debug_solve6_host": (C.c_int, [_VP, _VP, _VP, _VP]),
@@ -107,6 +116,11 @@ SIGNATURES = {
     "sm_debug_radix_sort": (C.c_int, [C.c_int, _VP, _VP, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _VP, _VP]),
     "sm_debug_kd_tree": (C.c_int, [C.c_int, C.c_int32, C.c_int32, _VP, _VP, C.c_int64, _VP, _VP, C.c_int64, C.c_int32,
                                    _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "sm_debug_filter_host": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, C.c_int64, _VP, _VP]),
+    "sm_debug_filter_fit_host": (C.c_int, [_VP, _VP, C.c_int32, _VP]),
+    "sm_debug_filter_distance_host": (C.c_int, [_VP, C.c_int32, C.c_float, C.c_float, _VP]),
+    "sm_debug_filter_ground_removal2": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, _VP,
+                                                  _VP, _VP, _VP, _VP, _VP]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

@@ -10,6 +10,8 @@
 
 #include "common.cuh"
 
+struct sm_filter_chain;
+
 namespace smb {
 
 // One device allocation, freed with its owner.  reserve() only grows, with 1/8 + 4 KB slack so
@@ -354,6 +356,74 @@ struct M2dpStage {
 void m2dp_axes(const float* cov6, float* E9);
 // [u1; v1] (rows + cols floats) from A and G = A A^T; zero when A is
 void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* out);
+
+// ---- filters.cu --------------------------------------------------------------------------
+// pre_processers::filter::Factory (pre_processors/filter_factory.cc:63-106) over the six filters built here
+enum FilterKind : int {
+  kFilterRange = 0, kFilterAxisRange, kFilterBoundingBoxRemoval, kFilterRandomSampler, kFilterRangeImage,
+  kFilterGroundRemoval2
+};
+// One filter of the chain: the members of the reference class of its kind under their XML names, at the
+// constructors' defaults (filter_range.cc:31-38, filter_axis_range.h:56-57, filter_bounding_box.h,
+// filter_random_sample.cc:29, filter_range_image.cc:29-37, filter_ground_removal2.cc:74-89).  Passed to the kernels
+// by value.
+struct FilterParams {
+  int kind;
+  float min_range, max_range;                                       // Range
+  float min, max; int axis_index;                                   // AxisRange
+  float min_x, min_y, min_z, max_x, max_y, max_z;                   // BoundingBoxRemoval
+  float sampling_rate;                                              // RandomSampler
+  float top_angle, btm_angle, offset_x, offset_y, offset_z;         // RangeImage
+  int vertical_line_num, horizontal_line_num;
+  float r_max, r_min, start_ground_height, long_line_threshold,     // GroundRemoval2
+      max_long_line_height, max_start_height, max_error, max_slope, max_b, max_dist_to_line, search_angle;
+  int bin_num, segment_num, thread_num;
+};
+FilterParams filter_defaults(int kind);
+// the reference's name for `kind`'s parameter -> its address and type (0 int32, 1 float), or false
+bool filter_param(FilterParams& f, const char* name, void** target, int* type);
+bool filter_configs_valid(const FilterParams& f);                   // ConfigsValid of the kind
+// constants the reference derives per Filter call, in its mix of float and double
+struct RangeImageConsts { float hres, vres; double btm; };         // filter_range_image.cc:89-93, :112
+struct Gr2Consts { float two_pi, delta_alpha, delta_bin; int search_steps; };   // filter_ground_removal2.cc:144-146, :340-341
+RangeImageConsts range_image_consts(const FilterParams& f);
+Gr2Consts gr2_consts(const FilterParams& f);
+struct Gr2Line { float d0, z0, d1, z1; };                           // GroundRemoval2::Line: start (d, z), end (d, z)
+// host builds of the per-point functions of filters.cu (test hook sm_debug_filter_host)
+bool filter_debug_keep_host(const FilterParams& f, const float* rec, uint32_t index, uint32_t seed);
+bool filter_debug_pixel_host(const FilterParams& f, const float* rec, int* row, int* col);
+void filter_debug_cell_host(const FilterParams& f, const float* rec, float* range, int* s, int* b);
+void filter_debug_fit_host(const float* d, const float* z, int n, float* m, float* b);
+float filter_debug_distance_host(const Gr2Line* lines, int n_lines, float d, float z, int* bad);
+struct FilterChain;
+const FilterChain* filter_chain_of(const ::sm_filter_chain* c);   // the chain behind the C handle, null for null
+
+// The device buffers and the stages of one filter chain.  reserve() sizes the buffers for n records and the chain's
+// RangeImage / GroundRemoval2 grids; they only grow.  run() applies the filters in order to n records of `stride`
+// bytes in device memory and leaves the inliers, packed, in `out` (capacity n records) with their indices in the
+// input scan in `out_index` (optional); it returns after the stream has finished, with the count in *m.
+struct FilterChain {
+  std::vector<FilterParams> filters;
+  uint32_t sample_seed = 1;
+  DevBuf rec[2], idx[2], flag, block_cnt, count, pixel, owner, sort, cell_of, pt, member, cells, occ, work, lines;
+  // the intermediates of the last GroundRemoval2 stage (test hook sm_debug_filter_ground_removal2)
+  struct Gr2View {
+    const uint32_t* cell_of; const uint8_t* member; const uint32_t* cell_cnt; const float2* cell_min;
+    const Gr2Line* lines; const int* n_lines; const uint8_t* keep; int max_lines; int status;
+  } gr2 = {};
+  int reserve(int64_t n);
+  int run(const char* in, int64_t n, int64_t stride, float* out, int32_t* out_index, int64_t* m, cudaStream_t stream);
+
+ private:
+  // each stage reads n records (index_in: their scan indices, null = identity) and compacts the inliers
+  int predicate_stage(int first, int count, const char* in, const uint32_t* index_in, int n, int64_t stride,
+                      float* out, uint32_t* index_out, cudaStream_t s);
+  int range_image_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,
+                        float* out, uint32_t* index_out, cudaStream_t s);
+  int ground_removal2_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,
+                            float* out, uint32_t* index_out, cudaStream_t s);
+  int stage_end(int first) const;   // one past the last filter of the stage that starts at `first`
+};
 
 }  // namespace smb
 

@@ -637,4 +637,70 @@ int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* fi
   return SM_OK;
 }
 
+// ---- test hooks of the filter chain (filters.cu) ---------------------------------------------------------------------
+int sm_debug_filter_host(const sm_filter_chain* chain, int32_t filter, int32_t op, const float* records, int64_t n,
+                         int32_t* iout, float* fout) {
+  const FilterChain* fc = filter_chain_of(chain);
+  if (!fc || filter < 0 || filter >= (int)fc->filters.size() || !records || !iout || n < 0) return SM_ERR_BAD_ARGUMENT;
+  const FilterParams& f = fc->filters[filter];
+  for (int64_t i = 0; i < n; ++i) {
+    const float* p = records + 5 * i;
+    switch (op) {
+      case 0: iout[i] = filter_debug_keep_host(f, p, (uint32_t)i, fc->sample_seed) ? 1 : 0; break;
+      case 1: if (!filter_debug_pixel_host(f, p, &iout[2 * i], &iout[2 * i + 1])) iout[2 * i] = iout[2 * i + 1] = -1; break;
+      case 2:
+        if (!fout) return SM_ERR_BAD_ARGUMENT;
+        filter_debug_cell_host(f, p, &fout[i], &iout[2 * i], &iout[2 * i + 1]);
+        break;
+      default: return SM_ERR_BAD_ARGUMENT;
+    }
+  }
+  return SM_OK;
+}
+
+int sm_debug_filter_fit_host(const float* d, const float* z, int32_t n, float* m_b) {
+  if (!d || !z || !m_b || n < 2) return SM_ERR_BAD_ARGUMENT;
+  filter_debug_fit_host(d, z, n, &m_b[0], &m_b[1]);
+  return SM_OK;
+}
+
+int sm_debug_filter_distance_host(const float* lines_4l, int32_t n_lines, float d, float z, float* distance) {
+  if ((n_lines > 0 && !lines_4l) || n_lines < 0 || !distance) return SM_ERR_BAD_ARGUMENT;
+  int bad = 0;
+  *distance = filter_debug_distance_host((const Gr2Line*)lines_4l, n_lines, d, z, &bad);
+  return bad ? SM_ERR_CHECK_FAILED : SM_OK;
+}
+
+int sm_debug_filter_ground_removal2(int device, const sm_filter_chain* chain, int32_t filter, const float* points,
+                                    int64_t n, int64_t stride_bytes, int32_t max_lines, uint32_t* cell, uint8_t* member,
+                                    uint32_t* cell_members, float* cell_min_2c, float* lines_4, int32_t* n_lines,
+                                    uint8_t* keep) {
+  const FilterChain* fc = filter_chain_of(chain);
+  if (!fc || filter < 0 || filter >= (int)fc->filters.size() || fc->filters[filter].kind != kFilterGroundRemoval2 ||
+      !points || n <= 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 || !cell || !member ||
+      !cell_members || !cell_min_2c || !lines_4 || !n_lines || !keep)
+    return SM_ERR_BAD_ARGUMENT;
+  const FilterParams& f = fc->filters[filter];
+  if (f.bin_num <= 0 || max_lines != f.bin_num / 2 + 1) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(debug_set_device(device));
+  FilterChain one;
+  one.filters.push_back(f);
+  DevBuf in, out;
+  SMB_RC(in.reserve((size_t)n * (size_t)stride_bytes));
+  SMB_RC(out.reserve((size_t)n * 20));
+  SMB_CUDA_OK(cudaMemcpy(in.p, points, (size_t)n * (size_t)stride_bytes, cudaMemcpyHostToDevice));
+  int64_t m = 0;
+  const int rc = one.run((const char*)in.p, n, stride_bytes, (float*)out.p, nullptr, &m, nullptr);
+  if (rc < 0 && rc != SM_ERR_CHECK_FAILED) return rc;
+  const size_t cells = (size_t)f.bin_num * (size_t)f.segment_num;
+  SMB_CUDA_OK(cudaMemcpy(cell, one.gr2.cell_of, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(member, one.gr2.member, (size_t)n, cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(cell_members, one.gr2.cell_cnt, cells * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(cell_min_2c, one.gr2.cell_min, cells * sizeof(float2), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(lines_4, one.gr2.lines, (size_t)f.segment_num * max_lines * sizeof(Gr2Line), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(n_lines, one.gr2.n_lines, (size_t)f.segment_num * sizeof(int), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(keep, one.gr2.keep, (size_t)n, cudaMemcpyDeviceToHost));
+  return rc;
+}
+
 }  // extern "C"

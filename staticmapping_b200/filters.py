@@ -1,0 +1,105 @@
+"""pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
+chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
+deterministic stand-in, see the header), RangeImage and GroundRemoval2.  There is no CPU fallback."""
+from __future__ import annotations
+
+import ctypes as C
+import xml.etree.ElementTree as ET
+
+import numpy as np
+
+from . import _lib
+from .registrators import CheckFailure, InnerCloud
+
+
+class Factory:
+    """filter::Factory.  InitFromXmlText / InitFromXmlNode take the <filters> node; SetInputCloud + Filter run the
+    chain on the GPU.  `Filter` returns the inlier InnerCloud; Inliers() / Outliers() are indices into the input."""
+
+    def __init__(self, device: int = 0):
+        self._lib = _lib.lib()
+        self._h = C.c_void_p()
+        if self._lib.sm_filter_chain_create(device, C.byref(self._h)) != 0:
+            raise RuntimeError("sm_filter_chain_create failed")
+        self._cloud = None
+        self._inliers = np.zeros(0, np.int32)
+        self._outliers = np.zeros(0, np.int32)
+        self.filter_names = []
+        self.messages = []
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._lib.sm_filter_chain_destroy(self._h)
+            self._h = None
+
+    def _error(self):
+        return (self._lib.sm_filter_chain_last_error(self._h) or b"").decode()
+
+    def InitFromXmlText(self, text):
+        self.InitFromXmlNode(ET.fromstring(text))
+
+    def InitFromXmlNode(self, filters_node):
+        """filter_factory.cc:63-81.  A name the reference does not register is skipped with a message; a <param> with
+        an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57), and so does a filter
+        the reference has but this chain does not build (GroundRemoval, StatisticRemoval, VoxelGrid)."""
+        if isinstance(filters_node, (str, bytes)):
+            filters_node = ET.fromstring(filters_node)
+        for node in filters_node.findall("filter"):
+            name = node.attrib.get("name", "")
+            index = self._lib.sm_filter_chain_add(self._h, name.encode())
+            if index == -10:
+                self.messages.append(f"{name} not supported yet.")
+                continue
+            if index < 0:
+                raise CheckFailure(self._error())
+            self.filter_names.append(name)
+            for param in node.findall("param"):
+                try:
+                    ptype = int(param.attrib["type"])
+                except (KeyError, ValueError):
+                    ptype = -1
+                rc = self._lib.sm_filter_chain_set_param(self._h, index, param.attrib.get("name", "").encode(), ptype,
+                                                         (param.text or "").strip().encode())
+                if rc != 0:
+                    raise CheckFailure(self._error())
+
+    def ConfigsValid(self, index):
+        return self._lib.sm_filter_chain_validate(self._h, index) == 1
+
+    def SetSampleSeed(self, seed):
+        self._lib.sm_filter_chain_set_option(self._h, b"sample_seed", str(int(seed)).encode())
+
+    def SetInputCloud(self, cloud):
+        pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
+        if pts.ndim != 2 or pts.shape[1] != 5:
+            raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
+        self._cloud = pts
+
+    def Filter(self):
+        if self._cloud is None:
+            return None
+        pts = self._cloud
+        n = pts.shape[0]
+        out = np.empty_like(pts)
+        index = np.empty(n, np.int32)
+        m = C.c_int64(0)
+        rc = self._lib.sm_filter_chain_run(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m), index.ctypes.data)
+        if rc == -20:
+            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
+        if rc == -5:
+            raise CheckFailure(self._error())
+        if rc == -1:       # e.g. a RangeImage size of 0, where the reference keeps its previous cloud without a CHECK
+            raise ValueError(self._error())
+        if rc != 0:
+            raise RuntimeError(f"sm_filter_chain_run failed with {rc}: {self._error()}")
+        self._inliers = index[:m.value].copy()
+        mask = np.ones(n, bool)
+        mask[self._inliers] = False
+        self._outliers = np.nonzero(mask)[0].astype(np.int32)
+        return InnerCloud(out[:m.value].copy())
+
+    def Inliers(self):
+        return self._inliers
+
+    def Outliers(self):
+        return self._outliers
