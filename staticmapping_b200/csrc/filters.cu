@@ -4,8 +4,7 @@
 //
 // Every filter emits its inliers in ascending input index, whole records (x, y, z, intensity, factor) copied.
 //   Range / AxisRange / BoundingBoxRemoval / RandomSampler are per-point predicates: consecutive ones run as ONE
-//     flag kernel, then an ordered compaction (per-tile counts, one exclusive scan of them, then each tile
-//     scatters).  RandomSampler is a deterministic stand-in, see filter_keep.
+//     flag kernel, then an ordered compaction (compact.cuh).  RandomSampler is a deterministic stand-in, see filter_keep.
 //   RangeImage (filter_range_image.cc:82-141): the first point in input order to reach an empty pixel is the inlier.
 //     atomicMin of the point index on a pixel-owner image gives exactly that, whatever the thread order.
 //   GroundRemoval2 (filter_ground_removal2.cc:127-414): polar cell per point -> stable radix sort by cell (members of
@@ -22,12 +21,12 @@
 
 #include "../../include/sm_b200.h"
 #include "common.cuh"
+#include "compact.cuh"
 #include "kernels.h"
 
 namespace smb {
 namespace {
 
-constexpr int kT = 256, kItems = 8, kTile = kT * kItems;
 constexpr int kMaxRun = 8;              // predicates of one flag kernel; a longer run is split
 constexpr int kMaxCells = 1 << 24;      // RangeImage pixels / GroundRemoval2 cells
 
@@ -214,25 +213,14 @@ __host__ __device__ inline float gr2_vertical_distance(const Gr2Line* lines, int
   return distance;
 }
 
-// ---- ordered compaction ---------------------------------------------------------------------------------------
-// thread t of tile b owns records b * kTile + t * kItems .. + kItems - 1; returns the tile's count to thread 0
-__device__ __forceinline__ uint32_t tile_count(uint32_t c) {
-  __shared__ uint32_t ws[kT / 32];
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
-  __syncthreads();
-  uint32_t t = 0;
-  if (threadIdx.x == 0) for (int w = 0; w < kT / 32; ++w) t += ws[w];
-  return t;
-}
-
-__global__ void __launch_bounds__(kT)
+// ---- predicates and the scatter every stage ends in ---------------------------------------------------------------
+__global__ void __launch_bounds__(kCompactThreads)
 filter_predicate_kernel(const char* __restrict__ pts, int64_t stride, const uint32_t* __restrict__ index_in, int n,
                         const __grid_constant__ PredicateRun run, uint8_t* __restrict__ flag,
                         uint32_t* __restrict__ block_cnt) {
-  const int base = blockIdx.x * kTile + threadIdx.x * kItems;
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
   uint32_t c = 0;
-  for (int r = 0; r < kItems; ++r) {
+  for (int r = 0; r < kCompactItems; ++r) {
     const int i = base + r;
     if (i >= n) break;
     const float* p = reinterpret_cast<const float*>(pts + (int64_t)i * stride);
@@ -242,27 +230,19 @@ filter_predicate_kernel(const char* __restrict__ pts, int64_t stride, const uint
     flag[i] = keep ? 1 : 0;
     c += keep ? 1u : 0u;
   }
-  const uint32_t t = tile_count(c);
-  if (threadIdx.x == 0) { block_cnt[blockIdx.x] = t; if (blockIdx.x == 0) block_cnt[gridDim.x] = 0; }
+  tile_count_store(c, block_cnt);
 }
 
 // out / index_out: the flagged records in input order; *m = their number.  tile_off: records kept before each tile
-__global__ void __launch_bounds__(kT)
+__global__ void __launch_bounds__(kCompactThreads)
 filter_scatter_kernel(const char* __restrict__ pts, int64_t stride, const uint32_t* __restrict__ index_in, int n,
                       const uint8_t* __restrict__ flag, const uint32_t* __restrict__ tile_off,
                       float* __restrict__ out, uint32_t* __restrict__ index_out, uint32_t* __restrict__ m) {
-  __shared__ uint32_t ws[kT / 32];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int base = blockIdx.x * kTile + threadIdx.x * kItems;
-  uint32_t f[kItems], c = 0;
-  for (int r = 0; r < kItems; ++r) { f[r] = (base + r < n) ? flag[base + r] : 0u; c += f[r]; }
-  uint32_t incl = c;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) ws[w] = incl;
-  __syncthreads();
-  uint32_t pos = tile_off[blockIdx.x] + incl - c;
-  for (int ww = 0; ww < w; ++ww) pos += ws[ww];
-  for (int r = 0; r < kItems; ++r) {
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  uint32_t f[kCompactItems], c = 0;
+  for (int r = 0; r < kCompactItems; ++r) { f[r] = (base + r < n) ? flag[base + r] : 0u; c += f[r]; }
+  uint32_t pos = tile_exclusive(c, tile_off);
+  for (int r = 0; r < kCompactItems; ++r) {
     if (!f[r]) continue;
     const int i = base + r;
     const float* p = reinterpret_cast<const float*>(pts + (int64_t)i * stride);
@@ -271,7 +251,7 @@ filter_scatter_kernel(const char* __restrict__ pts, int64_t stride, const uint32
     index_out[pos] = index_in ? index_in[i] : (uint32_t)i;
     ++pos;
   }
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == kT - 1) *m = pos;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *m = tile_off[gridDim.x];
 }
 
 // ---- RangeImage -----------------------------------------------------------------------------------------------
@@ -289,12 +269,12 @@ range_image_owner_kernel(const char* __restrict__ pts, int64_t stride, int n, co
   pixel[i] = px;
 }
 
-__global__ void __launch_bounds__(kT)
+__global__ void __launch_bounds__(kCompactThreads)
 range_image_flag_kernel(const uint32_t* __restrict__ pixel, const uint32_t* __restrict__ owner, int n,
                         uint8_t* __restrict__ flag, uint32_t* __restrict__ block_cnt) {
-  const int base = blockIdx.x * kTile + threadIdx.x * kItems;
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
   uint32_t c = 0;
-  for (int r = 0; r < kItems; ++r) {
+  for (int r = 0; r < kCompactItems; ++r) {
     const int i = base + r;
     if (i >= n) break;
     const uint32_t px = pixel[i];
@@ -302,8 +282,7 @@ range_image_flag_kernel(const uint32_t* __restrict__ pixel, const uint32_t* __re
     flag[i] = keep ? 1 : 0;
     c += keep ? 1u : 0u;
   }
-  const uint32_t t = tile_count(c);
-  if (threadIdx.x == 0) { block_cnt[blockIdx.x] = t; if (blockIdx.x == 0) block_cnt[gridDim.x] = 0; }
+  tile_count_store(c, block_cnt);
 }
 
 // ---- GroundRemoval2 -------------------------------------------------------------------------------------------
@@ -428,14 +407,14 @@ gr2_fit_kernel(const FilterParams f, const uint32_t* __restrict__ cell_cnt, cons
 // ClusterGround (filter_ground_removal2.cc:337-396) per member point: own segment first; on a distance < 0 the
 // neighbours +k, -k, ..., +1, -1, breaking on a distance > 0; ground iff 0 < distance <= max_dist_to_line.
 // flag = 1 for the points that stay (not ground).
-__global__ void __launch_bounds__(kT)
+__global__ void __launch_bounds__(kCompactThreads)
 gr2_ground_kernel(const FilterParams f, const Gr2Consts c, int n, const uint32_t* __restrict__ cell_of,
                   const float2* __restrict__ pt, const uint8_t* __restrict__ member,
                   const Gr2Line* __restrict__ lines, int max_lines, const int* __restrict__ n_lines,
                   uint8_t* __restrict__ flag, uint32_t* __restrict__ block_cnt, int* __restrict__ status) {
-  const int base = blockIdx.x * kTile + threadIdx.x * kItems;
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
   uint32_t cnt = 0;
-  for (int r = 0; r < kItems; ++r) {
+  for (int r = 0; r < kCompactItems; ++r) {
     const int i = base + r;
     if (i >= n) break;
     bool ground = false;
@@ -461,8 +440,7 @@ gr2_ground_kernel(const FilterParams f, const Gr2Consts c, int n, const uint32_t
     flag[i] = ground ? 0 : 1;
     cnt += ground ? 0u : 1u;
   }
-  const uint32_t t = tile_count(cnt);
-  if (threadIdx.x == 0) { block_cnt[blockIdx.x] = t; if (blockIdx.x == 0) block_cnt[gridDim.x] = 0; }
+  tile_count_store(cnt, block_cnt);
 }
 
 int sort_passes(int n_cells) { return n_cells <= (1 << 16) ? 2 : 4; }   // even: the sorted pairs end in the first buffers
@@ -571,13 +549,12 @@ int FilterChain::stage_end(int first) const {
 }
 
 int FilterChain::reserve(int64_t n) {
-  const size_t tiles = (size_t)ceil_div(n, kTile) + 1;
   for (int k = 0; k < 2; ++k) {
     SMB_RC(rec[k].reserve((size_t)n * 20));
     SMB_RC(idx[k].reserve((size_t)n * sizeof(uint32_t)));
   }
   SMB_RC(flag.reserve((size_t)n));
-  SMB_RC(block_cnt.reserve(tiles * sizeof(uint32_t)));
+  SMB_RC(block_cnt.reserve(compact_count_bytes(n)));
   SMB_RC(count.reserve(2 * sizeof(uint32_t)));
   for (const FilterParams& f : filters) {
     if (f.kind == kFilterRangeImage) {
@@ -605,11 +582,13 @@ int FilterChain::predicate_stage(int first, int cnt, const char* in, const uint3
   PredicateRun run;
   run.count = cnt; run.seed = sample_seed;
   for (int k = 0; k < cnt; ++k) run.f[k] = filters[first + k];
-  const int tiles = ceil_div(n, kTile);
-  filter_predicate_kernel<<<tiles, kT, 0, s>>>(in, stride, index_in, n, run, (uint8_t*)flag.p, (uint32_t*)block_cnt.p);
-  radix_scan_kernel_launch((uint32_t*)block_cnt.p, tiles + 1, 1, s);   // tile counts -> tile offsets
-  filter_scatter_kernel<<<tiles, kT, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
-                                             (const uint32_t*)block_cnt.p, out, index_out, (uint32_t*)count.p);
+  const int tiles = compact_tiles(n);
+  filter_predicate_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, run, (uint8_t*)flag.p,
+                                                            (uint32_t*)block_cnt.p);
+  compact_scan((uint32_t*)block_cnt.p, tiles, s);
+  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
+                                                          (const uint32_t*)block_cnt.p, out, index_out,
+                                                          (uint32_t*)count.p);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -618,14 +597,15 @@ int FilterChain::range_image_stage(const FilterParams& f, const char* in, const 
                                    int64_t stride, float* out, uint32_t* index_out, cudaStream_t s) {
   const RangeImageConsts c = range_image_consts(f);
   const size_t pixels = (size_t)f.vertical_line_num * (size_t)f.horizontal_line_num;
-  const int tiles = ceil_div(n, kTile);
+  const int tiles = compact_tiles(n);
   SMB_CUDA_OK(cudaMemsetAsync(owner.p, 0xff, pixels * sizeof(uint32_t), s));
   range_image_owner_kernel<<<ceil_div(n, 256), 256, 0, s>>>(in, stride, n, f, c, (uint32_t*)pixel.p, (uint32_t*)owner.p);
-  range_image_flag_kernel<<<tiles, kT, 0, s>>>((const uint32_t*)pixel.p, (const uint32_t*)owner.p, n, (uint8_t*)flag.p,
-                                               (uint32_t*)block_cnt.p);
-  radix_scan_kernel_launch((uint32_t*)block_cnt.p, tiles + 1, 1, s);   // tile counts -> tile offsets
-  filter_scatter_kernel<<<tiles, kT, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
-                                             (const uint32_t*)block_cnt.p, out, index_out, (uint32_t*)count.p);
+  range_image_flag_kernel<<<tiles, kCompactThreads, 0, s>>>((const uint32_t*)pixel.p, (const uint32_t*)owner.p, n,
+                                                            (uint8_t*)flag.p, (uint32_t*)block_cnt.p);
+  compact_scan((uint32_t*)block_cnt.p, tiles, s);
+  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
+                                                          (const uint32_t*)block_cnt.p, out, index_out,
+                                                          (uint32_t*)count.p);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -634,7 +614,7 @@ int FilterChain::ground_removal2_stage(const FilterParams& f, const char* in, co
                                        int64_t stride, float* out, uint32_t* index_out, cudaStream_t s) {
   const Gr2Consts c = gr2_consts(f);
   const int n_cells = f.bin_num * f.segment_num;
-  const int tiles = ceil_div(n, kTile);
+  const int tiles = compact_tiles(n);
   const int64_t st = ((int64_t)n + 63) & ~(int64_t)63;
   RadixPairs rp;
   rp.carve(sort.p, st);
@@ -656,12 +636,13 @@ int FilterChain::ground_removal2_stage(const FilterParams& f, const char* in, co
                                                          (uint8_t*)member.p, cell_cnt, cell_min);
   gr2_fit_kernel<<<ceil_div(f.segment_num, 64), 64, 0, s>>>(f, cell_cnt, cell_min, (float*)occ.p, (double*)work.p, ln,
                                                             max_lines, n_lines, status);
-  gr2_ground_kernel<<<tiles, kT, 0, s>>>(f, c, n, (const uint32_t*)cell_of.p, (const float2*)pt.p,
-                                         (const uint8_t*)member.p, ln, max_lines, n_lines, (uint8_t*)flag.p,
-                                         (uint32_t*)block_cnt.p, status);
-  radix_scan_kernel_launch((uint32_t*)block_cnt.p, tiles + 1, 1, s);   // tile counts -> tile offsets
-  filter_scatter_kernel<<<tiles, kT, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
-                                             (const uint32_t*)block_cnt.p, out, index_out, (uint32_t*)count.p);
+  gr2_ground_kernel<<<tiles, kCompactThreads, 0, s>>>(f, c, n, (const uint32_t*)cell_of.p, (const float2*)pt.p,
+                                                      (const uint8_t*)member.p, ln, max_lines, n_lines,
+                                                      (uint8_t*)flag.p, (uint32_t*)block_cnt.p, status);
+  compact_scan((uint32_t*)block_cnt.p, tiles, s);
+  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
+                                                          (const uint32_t*)block_cnt.p, out, index_out,
+                                                          (uint32_t*)count.p);
   SMB_CUDA_OK(cudaGetLastError());
   gr2 = {(const uint32_t*)cell_of.p, (const uint8_t*)member.p, cell_cnt, cell_min, ln, n_lines, (const uint8_t*)flag.p,
          max_lines, 0};

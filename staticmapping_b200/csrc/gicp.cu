@@ -16,6 +16,7 @@
 //                       the 3x3 matrix R that computeRDerivative contracts; 13 double sums.
 // Compiled with -fmad=false (same operation order as oracle/gicp_oracle.cc).
 #include "common.cuh"
+#include "compact.cuh"
 #include "gicp_host.h"
 #include "icp_dev.cuh"
 #include "kernels.h"
@@ -53,41 +54,30 @@ __device__ __forceinline__ uint32_t run_head(const float* pts, const uint32_t* o
   return (ax != bx || ay != by || az != bz) ? 1u : 0u;
 }
 
-constexpr int kRT = 256, kRI = 8, kRTile = kRT * kRI;
-
-__global__ void __launch_bounds__(kRT)
+__global__ void __launch_bounds__(kCompactThreads)
 approx_heads_count_kernel(const float* __restrict__ pts, const uint32_t* __restrict__ order,
-                          const uint64_t* __restrict__ keys, int n, float inv, uint32_t* __restrict__ block_sum) {
-  __shared__ uint32_t ws[kRT / 32];
+                          const uint64_t* __restrict__ keys, int n, float inv, uint32_t* __restrict__ tile_cnt) {
   uint32_t c = 0;
-  const int base = blockIdx.x * kRTile + threadIdx.x * kRI;
-  for (int r = 0; r < kRI; ++r) if (base + r < n) c += run_head(pts, order, keys, inv, base + r);
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < kRT / 32; ++w) t += ws[w]; block_sum[blockIdx.x] = t; }
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  for (int r = 0; r < kCompactItems; ++r) if (base + r < n) c += run_head(pts, order, keys, inv, base + r);
+  tile_count_store(c, tile_cnt);
 }
 
-__global__ void __launch_bounds__(kRT)
+__global__ void __launch_bounds__(kCompactThreads)
 approx_heads_scatter_kernel(const float* __restrict__ pts, const uint32_t* __restrict__ order,
                             const uint64_t* __restrict__ keys, int n, float inv,
-                            const uint32_t* __restrict__ block_off, int nblk, uint32_t* __restrict__ run_start,
+                            const uint32_t* __restrict__ tile_off, uint32_t* __restrict__ run_start,
                             uint32_t* __restrict__ n_runs) {
-  __shared__ uint32_t ws[kRT / 32];
-  const int base = blockIdx.x * kRTile + threadIdx.x * kRI;
-  uint32_t f[kRI], c = 0;
-  for (int r = 0; r < kRI; ++r) { f[r] = (base + r < n) ? run_head(pts, order, keys, inv, base + r) : 0u; c += f[r]; }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = c;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) ws[w] = incl;
-  __syncthreads();
-  uint32_t wb = 0, tot = 0;
-  for (int ww = 0; ww < kRT / 32; ++ww) { const uint32_t v = ws[ww]; if (ww < w) wb += v; tot += v; }
-  uint32_t pos = block_off[blockIdx.x] + wb + incl - c;
-  for (int r = 0; r < kRI; ++r) if (f[r]) run_start[pos++] = (uint32_t)(base + r);
-  if (blockIdx.x == nblk - 1 && threadIdx.x == 0) {
-    const uint32_t v = block_off[blockIdx.x] + tot;
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  uint32_t f[kCompactItems], c = 0;
+  for (int r = 0; r < kCompactItems; ++r) {
+    f[r] = (base + r < n) ? run_head(pts, order, keys, inv, base + r) : 0u;
+    c += f[r];
+  }
+  uint32_t pos = tile_exclusive(c, tile_off);
+  for (int r = 0; r < kCompactItems; ++r) if (f[r]) run_start[pos++] = (uint32_t)(base + r);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const uint32_t v = tile_off[gridDim.x];
     *n_runs = v;
     run_start[v] = (uint32_t)n;
   }
@@ -446,10 +436,10 @@ int ApproxVoxelGrid::filter(const float* pts, int n, float leaf, DevBuf& out, in
   const float inv = 1.0f / leaf;
   approx_key_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(pts, n, inv, keys0, ord0);
   SMB_RC(radix_sort_pairs_u64(keys0, ord0, keys1, ord1, n, 1, st, scratch, stream, 2));
-  const int nblk = ceil_div(n, kRTile);
-  approx_heads_count_kernel<<<nblk, kRT, 0, stream>>>(pts, ord0, keys0, n, inv, scratch);
-  radix_scan_kernel_launch(scratch, nblk, 1, stream);
-  approx_heads_scatter_kernel<<<nblk, kRT, 0, stream>>>(pts, ord0, keys0, n, inv, scratch, nblk, run_start, n_out_dev);
+  const int tiles = compact_tiles(n);
+  approx_heads_count_kernel<<<tiles, kCompactThreads, 0, stream>>>(pts, ord0, keys0, n, inv, scratch);
+  compact_scan(scratch, tiles, stream);
+  approx_heads_scatter_kernel<<<tiles, kCompactThreads, 0, stream>>>(pts, ord0, keys0, n, inv, scratch, run_start, n_out_dev);
   approx_run_kernel<<<ceil_div(n, 128), 128, 0, stream>>>(pts, ord0, keys0, run_start, n_out_dev, n, centroid, ekey0, eval0);
   SMB_CUDA_OK(cudaGetLastError());
   uint32_t m = 0;

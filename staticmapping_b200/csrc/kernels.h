@@ -330,6 +330,21 @@ struct NormalsPipeline {
   const double* normals() const { return (const double*)out_nrm.p; }
 };
 
+// ---- icp_pm.cu -------------------------------------------------------------------------
+// The reading filter and the score pass of the IcpUsingPointMatcher stand-in (icp_pointmatcher.cc:131-148, :173),
+// with their buffers, sized by reserve() for a reading cloud of n_source points.
+struct PmStage {
+  DevBuf cnt, sampled, score;   // tile counts; the kept reading points; pose, output and sort of the score pass
+  int reserve(int n_source);
+  // hash-subsample of the packed float cloud src into points(); waits for and returns the number kept
+  int sample(const float* src, int n, float prob, uint32_t seed, cudaStream_t s, uint32_t* kept);
+  const double* points() const { return (const double*)sampled.p; }   // AoS 3xM doubles
+  // the unfiltered reading moved by T (16 doubles, pinned host memory) against the target's float tree, trimmed at
+  // `ratio`; waits for out3_host = mean kept distance, kept, valid
+  int score_pass(const float* src, int n, const double* T_host_pinned, const FloatTree& target, double max_error2,
+                 float ratio, double* out3_host, cudaStream_t s);
+};
+
 // ---- m2dp.cu -----------------------------------------------------------------------------
 struct M2dpView { float xa[3], ya[3]; };   // x_axis, y_axis of one view (m2dp.cc:73-83), not normalised
 static_assert(sizeof(M2dpView) == 6 * sizeof(float), "the test hook copies views as 6 floats each");

@@ -21,6 +21,7 @@
 #include <limits>
 
 #include "common.cuh"
+#include "compact.cuh"
 #include "icp_dev.cuh"
 #include "kernels.h"
 #include "linalg_dev.cuh"
@@ -115,45 +116,31 @@ __global__ void ndt_key_kernel(const float* __restrict__ pts, int n, const NdtGr
   vals[i] = (uint32_t)i;
 }
 
-// ---- voxel segments (head flags -> compaction) --------------------------------------------
-constexpr int kSegT = 256, kSegI = 8, kSegTile = kSegT * kSegI;
-
+// ---- voxel segments ------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t is_head(const uint64_t* keys, int i) {
   return (i == 0 || keys[i] != keys[i - 1]) ? 1u : 0u;
 }
 
-__global__ void __launch_bounds__(kSegT)
-ndt_heads_count_kernel(const uint64_t* __restrict__ keys, int n, uint32_t* __restrict__ block_sum) {
-  __shared__ uint32_t ws[kSegT / 32];
+__global__ void __launch_bounds__(kCompactThreads)
+ndt_heads_count_kernel(const uint64_t* __restrict__ keys, int n, uint32_t* __restrict__ tile_cnt) {
   uint32_t c = 0;
-  const int base = blockIdx.x * kSegTile + threadIdx.x * kSegI;
-  for (int r = 0; r < kSegI; ++r) if (base + r < n) c += is_head(keys, base + r);
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < kSegT / 32; ++w) t += ws[w]; block_sum[blockIdx.x] = t; }
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  for (int r = 0; r < kCompactItems; ++r) if (base + r < n) c += is_head(keys, base + r);
+  tile_count_store(c, tile_cnt);
 }
 
-__global__ void __launch_bounds__(kSegT)
-ndt_heads_scatter_kernel(const uint64_t* __restrict__ keys, int n, const uint32_t* __restrict__ block_off,
-                         int nblk, uint32_t* __restrict__ voxel_start, int* __restrict__ voxel_key,
+__global__ void __launch_bounds__(kCompactThreads)
+ndt_heads_scatter_kernel(const uint64_t* __restrict__ keys, int n, const uint32_t* __restrict__ tile_off,
+                         uint32_t* __restrict__ voxel_start, int* __restrict__ voxel_key,
                          NdtGrid* __restrict__ grid) {
-  __shared__ uint32_t ws[kSegT / 32];
-  const int base = blockIdx.x * kSegTile + threadIdx.x * kSegI;
-  uint32_t f[kSegI], c = 0;
-  for (int r = 0; r < kSegI; ++r) { f[r] = (base + r < n) ? is_head(keys, base + r) : 0u; c += f[r]; }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = c;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) ws[w] = incl;
-  __syncthreads();
-  uint32_t wb = 0, tot = 0;
-  for (int ww = 0; ww < kSegT / 32; ++ww) { const uint32_t v = ws[ww]; if (ww < w) wb += v; tot += v; }
-  uint32_t pos = block_off[blockIdx.x] + wb + incl - c;
-  for (int r = 0; r < kSegI; ++r)
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  uint32_t f[kCompactItems], c = 0;
+  for (int r = 0; r < kCompactItems; ++r) { f[r] = (base + r < n) ? is_head(keys, base + r) : 0u; c += f[r]; }
+  uint32_t pos = tile_exclusive(c, tile_off);
+  for (int r = 0; r < kCompactItems; ++r)
     if (f[r]) { voxel_start[pos] = (uint32_t)(base + r); voxel_key[pos] = (int)keys[base + r]; ++pos; }
-  if (blockIdx.x == nblk - 1 && threadIdx.x == 0) {
-    const uint32_t v = block_off[blockIdx.x] + tot;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const uint32_t v = tile_off[gridDim.x];
     grid->n_voxels = (int)v;
     voxel_start[v] = (uint32_t)n;   // sentinel
   }
@@ -784,11 +771,11 @@ int NdtStage::build_grid(const float* tgt, int nt, float resolution, cudaStream_
   int rc = radix_sort_pairs_u64(ws.keys[0], ws.order[0], ws.keys[1], ws.order[1], nt, 1, ws.stride,
                                 ws.scratch, stream, 4);
   if (rc) return rc;
-  const int nblk = ceil_div(nt, kSegTile);
-  ndt_heads_count_kernel<<<nblk, kSegT, 0, stream>>>(ws.keys[0], nt, ws.scratch);
-  radix_scan_kernel_launch(ws.scratch, nblk, 1, stream);
-  ndt_heads_scatter_kernel<<<nblk, kSegT, 0, stream>>>(ws.keys[0], nt, ws.scratch, nblk, ws.voxel_start,
-                                                      ws.voxel_key, ws.grid);
+  const int tiles = compact_tiles(nt);
+  ndt_heads_count_kernel<<<tiles, kCompactThreads, 0, stream>>>(ws.keys[0], nt, ws.scratch);
+  compact_scan(ws.scratch, tiles, stream);
+  ndt_heads_scatter_kernel<<<tiles, kCompactThreads, 0, stream>>>(ws.keys[0], nt, ws.scratch, ws.voxel_start,
+                                                                 ws.voxel_key, ws.grid);
   // one warp per voxel; the voxel count is only known on the device, so launch for nt warps
   ndt_gather_kernel<<<ceil_div(nt, 256), 256, 0, stream>>>(tgt, ws.order[0], nt, ws.sorted_pts);
   ndt_leaf_kernel<<<ceil_div((int64_t)nt * 32, 256), 256, 0, stream>>>(ws.sorted_pts, ws.order[0], ws.voxel_start,

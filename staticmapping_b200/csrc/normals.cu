@@ -9,6 +9,7 @@
 // compaction of the surviving leaf representatives.  Compiled with -fmad=false: with
 // the same operation order as the oracle the output is bit-identical to it.
 #include "common.cuh"
+#include "compact.cuh"
 #include "kernels.h"
 #include "linalg_dev.cuh"
 
@@ -81,45 +82,24 @@ __global__ void normals_leaf_kernel(const double* __restrict__ coord, int64_t cs
   }
 }
 
-constexpr int kCT = 256, kCI = 8, kCTile = kCT * kCI;
-
-__global__ void __launch_bounds__(kCT)
-compact_count_kernel(const uint32_t* __restrict__ keep, int n, uint32_t* __restrict__ block_sum) {
-  __shared__ uint32_t ws[kCT / 32];
+__global__ void __launch_bounds__(kCompactThreads)
+compact_count_kernel(const uint32_t* __restrict__ keep, int n, uint32_t* __restrict__ tile_cnt) {
   uint32_t c = 0;
-  const int base = blockIdx.x * kCTile + threadIdx.x * kCI;
-  for (int r = 0; r < kCI; ++r) if (base + r < n) c += keep[base + r];
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t t = 0;
-    for (int w = 0; w < kCT / 32; ++w) t += ws[w];
-    block_sum[blockIdx.x] = t;
-  }
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  for (int r = 0; r < kCompactItems; ++r) if (base + r < n) c += keep[base + r];
+  tile_count_store(c, tile_cnt);
 }
 
-__global__ void __launch_bounds__(kCT)
-compact_scatter_kernel(const uint32_t* __restrict__ keep, int n, const uint32_t* __restrict__ block_off,
+__global__ void __launch_bounds__(kCompactThreads)
+compact_scatter_kernel(const uint32_t* __restrict__ keep, int n, const uint32_t* __restrict__ tile_off,
                        const double* __restrict__ pts, const double* __restrict__ nrm,
                        double* __restrict__ out_pts, double* __restrict__ out_nrm,
-                       uint32_t* __restrict__ total_out, int nblk) {
-  __shared__ uint32_t ws[kCT / 32];
-  const int base = blockIdx.x * kCTile + threadIdx.x * kCI;
-  uint32_t f[kCI], c = 0;
-  for (int r = 0; r < kCI; ++r) { f[r] = (base + r < n) ? keep[base + r] : 0u; c += f[r]; }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = c;
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += t;
-  }
-  if (lane == 31) ws[w] = incl;
-  __syncthreads();
-  uint32_t wb = 0, tot = 0;
-  for (int ww = 0; ww < kCT / 32; ++ww) { const uint32_t v = ws[ww]; if (ww < w) wb += v; tot += v; }
-  uint32_t pos = block_off[blockIdx.x] + wb + incl - c;
-  for (int r = 0; r < kCI; ++r) {
+                       uint32_t* __restrict__ total_out) {
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  uint32_t f[kCompactItems], c = 0;
+  for (int r = 0; r < kCompactItems; ++r) { f[r] = (base + r < n) ? keep[base + r] : 0u; c += f[r]; }
+  uint32_t pos = tile_exclusive(c, tile_off);
+  for (int r = 0; r < kCompactItems; ++r) {
     if (f[r]) {
       const int64_t i = base + r;
       for (int k = 0; k < 3; ++k) {
@@ -129,7 +109,7 @@ compact_scatter_kernel(const uint32_t* __restrict__ keep, int n, const uint32_t*
       ++pos;
     }
   }
-  if (blockIdx.x == nblk - 1 && threadIdx.x == 0) *total_out = block_off[blockIdx.x] + tot;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *total_out = tile_off[gridDim.x];
 }
 
 }  // namespace
@@ -151,14 +131,14 @@ int NormalsPipeline::reserve(int n) {
   SMB_RC(order.reserve((size_t)n * sizeof(uint32_t)));
   SMB_RC(tmp_pts.reserve(aos)); SMB_RC(tmp_nrm.reserve(aos));
   SMB_RC(keep.reserve((size_t)n * sizeof(uint32_t)));
-  SMB_RC(bsum.reserve((size_t)(ceil_div(n, kCTile) + 1) * sizeof(uint32_t)));
+  SMB_RC(bsum.reserve(compact_count_bytes(n)));
   SMB_RC(out_pts.reserve(aos)); SMB_RC(out_nrm.reserve(aos));
   return count.reserve(sizeof(uint32_t));
 }
 
 int NormalsPipeline::run(int n, cudaStream_t stream, uint32_t* m) {
   const int levels = kd_num_levels(n, 7);
-  uint32_t* block_sums = (uint32_t*)bsum.p;
+  uint32_t* tile_cnt = (uint32_t*)bsum.p;
   KdWorkspace ws;
   SMB_RC(ws.carve(kdws, n, 7));
   SMB_RC(kd_build(input(), stride, n, 7, ws, (KdNode*)nodes.p, (uint32_t*)order.p, stream));
@@ -167,12 +147,12 @@ int NormalsPipeline::run(int n, cudaStream_t stream, uint32_t* m) {
   normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(input(), stride, (const KdNode*)nodes.p,
                                                                (const uint32_t*)order.p, n, levels, (double*)tmp_pts.p,
                                                                (double*)tmp_nrm.p, (uint32_t*)keep.p);
-  const int nblk = ceil_div(n, kCTile);
-  compact_count_kernel<<<nblk, kCT, 0, stream>>>((const uint32_t*)keep.p, n, block_sums);
-  radix_scan_kernel_launch(block_sums, nblk, 1, stream);
-  compact_scatter_kernel<<<nblk, kCT, 0, stream>>>((const uint32_t*)keep.p, n, block_sums, (const double*)tmp_pts.p,
-                                                   (const double*)tmp_nrm.p, (double*)out_pts.p, (double*)out_nrm.p,
-                                                   (uint32_t*)count.p, nblk);
+  const int tiles = compact_tiles(n);
+  compact_count_kernel<<<tiles, kCompactThreads, 0, stream>>>((const uint32_t*)keep.p, n, tile_cnt);
+  compact_scan(tile_cnt, tiles, stream);
+  compact_scatter_kernel<<<tiles, kCompactThreads, 0, stream>>>(
+      (const uint32_t*)keep.p, n, tile_cnt, (const double*)tmp_pts.p, (const double*)tmp_nrm.p, (double*)out_pts.p,
+      (double*)out_nrm.p, (uint32_t*)count.p);
   SMB_CUDA_OK(cudaGetLastError());
   SMB_CUDA_OK(cudaMemcpyAsync(m, count.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
   SMB_CUDA_OK(cudaStreamSynchronize(stream));

@@ -16,7 +16,6 @@
 #include <nvtx3/nvToolsExt.h>
 
 #include "common.cuh"
-#include "icp_dev.cuh"
 #include "kernels.h"
 #include "gicp_host.h"
 #include "ndt_host.h"
@@ -64,101 +63,6 @@ int upload_soa(const double* pts, int64_t n, bool on_device, DevBuf& stage, doub
   deinterleave3_kernel<<<ceil_div(n, 256), 256, 0, s>>>(aos, soa, stride, (int)n);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
-}
-
-// ---- reading filter of the IcpUsingPointMatcher stand-in (see pm_align) ----------------------
-__device__ __forceinline__ bool pm_keep(uint32_t i, uint32_t seed, uint32_t thresh, bool all) {
-  uint32_t x = i * 0x9E3779B9u + seed;
-  x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
-  return all || x < thresh;
-}
-
-__global__ void __launch_bounds__(256)
-pm_sample_count_kernel(int n, uint32_t seed, uint32_t thresh, int all, uint32_t* __restrict__ block_cnt) {
-  __shared__ uint32_t wc[8];
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  const bool k = i < n && pm_keep((uint32_t)i, seed, thresh, all != 0);
-  const uint32_t m = __ballot_sync(0xffffffffu, k);
-  if ((threadIdx.x & 31) == 0) wc[threadIdx.x >> 5] = __popc(m);
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < 8; ++w) t += wc[w]; block_cnt[blockIdx.x] = t; }
-}
-
-// kept points, original order, as 3xN column-major doubles (EigenPointCloud::FromPointCloud)
-__global__ void __launch_bounds__(256)
-pm_sample_scatter_kernel(const float* __restrict__ pts, int n, uint32_t seed, uint32_t thresh, int all,
-                         const uint32_t* __restrict__ block_off, double* __restrict__ out) {
-  __shared__ uint32_t wc[8];
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const bool k = i < n && pm_keep((uint32_t)i, seed, thresh, all != 0);
-  const uint32_t m = __ballot_sync(0xffffffffu, k);
-  if (lane == 0) wc[w] = __popc(m);
-  __syncthreads();
-  uint32_t off = block_off[blockIdx.x];
-  for (int ww = 0; ww < w; ++ww) off += wc[ww];
-  if (k) {
-    const int64_t d = off + __popc(m & ((1u << lane) - 1u));
-    out[3 * d] = (double)pts[3 * (int64_t)i];
-    out[3 * d + 1] = (double)pts[3 * (int64_t)i + 1];
-    out[3 * d + 2] = (double)pts[3 * (int64_t)i + 2];
-  }
-}
-
-// ---- score of the IcpUsingPointMatcher stand-in (icp_pointmatcher.cc:131-148): the UNFILTERED
-// reading cloud moved by the result is matched against the UNFILTERED reference (same k-d tree
-// matcher, eps 3.16), trimmed at the 0.7 quantile, and the mean kept distance goes into exp(-x)
-__global__ void __launch_bounds__(256)
-pm_score_knn_kernel(const float* __restrict__ src, int n, const double* __restrict__ T, const KdNode* __restrict__ nodes,
-                    const BucketPoint* __restrict__ bpts, double max_error2, uint64_t* __restrict__ keys,
-                    uint32_t* __restrict__ vals) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const double x = (double)src[3 * (int64_t)i], y = (double)src[3 * (int64_t)i + 1], z = (double)src[3 * (int64_t)i + 2];
-  double px, py, pz;
-  dev::transform_point(T, x, y, z, px, py, pz);
-  int slot; double d2;
-  dev::knn1(nodes, bpts, px, py, pz, max_error2, slot, d2);
-  keys[i] = (uint64_t)__double_as_longlong(d2);     // non-negative doubles sort like their bit patterns; +inf = no match
-  vals[i] = (uint32_t)i;
-}
-
-// keys sorted ascending; out[0] = mean of sqrt(d2) over the kept matches, out[1] = kept, out[2] = valid
-__global__ void __launch_bounds__(1024)
-pm_score_reduce_kernel(const uint64_t* __restrict__ keys, int n, float ratio, double* __restrict__ out) {
-  __shared__ double red[32];
-  __shared__ int s_kept, s_valid;
-  const uint64_t inf_bits = 0x7ff0000000000000ull;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = n;                                // first index with key >= +inf
-    while (lo < hi) { const int mid = (lo + hi) >> 1; if (keys[mid] < inf_bits) lo = mid + 1; else hi = mid; }
-    const int valid = lo;
-    int kept = 0;
-    if (valid > 0) {
-      const double q = (double)ratio;                  // GetDistsQuantile, as icp_fast.cc:82-89
-      int qi = (q == 1.0) ? valid - 1 : (int)((double)valid * q);
-      if (qi > valid - 1) qi = valid - 1;
-      const uint64_t limit = keys[qi];
-      lo = qi; hi = valid;                             // first index with key > limit
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (keys[mid] <= limit) lo = mid + 1; else hi = mid; }
-      kept = lo;
-    }
-    s_kept = kept; s_valid = valid;
-  }
-  __syncthreads();
-  const int kept = s_kept;
-  double v = 0.0;
-  for (int i = threadIdx.x; i < kept; i += 1024) v += sqrt(__longlong_as_double((long long)keys[i]));
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < 32; ++w) t += red[w];
-    out[0] = kept > 0 ? t / (double)kept : 0.0;
-    out[1] = (double)kept;
-    out[2] = (double)s_valid;
-  }
 }
 
 enum OptKind { kOptInt, kOptFloat, kOptDouble, kOptBool };
@@ -273,7 +177,7 @@ struct sm_handle {
     int64_t n_src = 0, n_tgt = 0;
     bool src_dirty = false, tgt_dirty = false, score_tree_dirty = true;
     NormalsPipeline normals;
-    DevBuf cnt, src, score_buf;       // sampling counts, the sampled source, the score's sort and I/O
+    PmStage stage;
   } pm;
 
   ~sm_handle() {
@@ -583,7 +487,7 @@ int icp_align(sm_handle* h, const double* guess, double* result) {
 
 // ---- IcpUsingPointMatcher stand-in (type 1) ------------------------------------------------
 // registrators/icp_pointmatcher.cc:125-247 drives libpointmatcher 1.3.1 (external, float) with
-//   reading filter    RandomSampling prob 0.9                      -> pm_sample_* below (a counter
+//   reading filter    RandomSampling prob 0.9                      -> PmStage::sample (a counter
 //                     hash instead of std::rand, so the kept set is reproducible)
 //   reference filter  SamplingSurfaceNormal knn 7, one point per box -> CalculateNormals, the
 //                     reference author's own restatement of that filter (cloud_types.cc:73-144)
@@ -610,26 +514,14 @@ int pm_align(sm_handle* h, const double* guess, double* result) {
     H_RC(set_target(h, np.points(), np.normals(), (int64_t)m, true));
     h->pm.tgt_dirty = false;
   }
+  PmStage& st = h->pm.stage;
+  H_RC(st.reserve((int)h->pm.n_src));
   if (h->pm.src_dirty) {
-    const int64_t n = h->pm.n_src;
-    const int nb = ceil_div(n, 256);
-    H_RC(h->pm.cnt.reserve(((size_t)nb + 8) * sizeof(uint32_t)));
-    H_RC(h->pm.src.reserve((size_t)3 * (size_t)n * sizeof(double)));
-    const double prob = (double)h->icp.reading_sample_prob;
-    const int all = prob >= 1.0 ? 1 : 0;
-    const uint32_t thresh = prob <= 0.0 ? 0u : (all ? 0xffffffffu : (uint32_t)(prob * 4294967296.0));
-    uint32_t* cnt = (uint32_t*)h->pm.cnt.p;
-    H_CUDA(cudaMemsetAsync(cnt + nb, 0, sizeof(uint32_t), s));
-    pm_sample_count_kernel<<<nb, 256, 0, s>>>((int)n, (uint32_t)h->icp.sample_seed, thresh, all, cnt);
-    radix_scan_kernel_launch(cnt, nb + 1, 1, s);            // exclusive: cnt[nb] = number kept
-    pm_sample_scatter_kernel<<<nb, 256, 0, s>>>((const float*)h->f32.src.p, (int)n, (uint32_t)h->icp.sample_seed, thresh,
-                                              all, cnt, (double*)h->pm.src.p);
-    H_CUDA(cudaGetLastError());
     uint32_t kept = 0;
-    H_CUDA(cudaMemcpyAsync(&kept, cnt + nb, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    H_CUDA(cudaStreamSynchronize(s));
+    H_RC(st.sample((const float*)h->f32.src.p, (int)h->pm.n_src, h->icp.reading_sample_prob,
+                   (uint32_t)h->icp.sample_seed, s, &kept));
     if (kept == 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: the reading filter kept no point");
-    H_RC(set_source(h, (const double*)h->pm.src.p, (int64_t)kept, true));
+    H_RC(set_source(h, st.points(), (int64_t)kept, true));
     h->pm.src_dirty = false;
   }
   const int rc = icp_align(h, guess, result);
@@ -644,23 +536,10 @@ int pm_align(sm_handle* h, const double* guess, double* result) {
       H_RC(build_tree_f32(h, (const float*)h->f32.tgt.p, nt, h->f32.target_tree));
       h->pm.score_tree_dirty = false;
     }
-    const int64_t st = pad64(ns);
-    H_RC(h->pm.score_buf.reserve(256 + RadixPairs::bytes(st, ns)));
-    double* Tdev = (double*)h->pm.score_buf.p;      // 16 doubles of pose, 8 of output, then the sort
-    double* outdev = Tdev + 16;
-    RadixPairs sp;
-    sp.carve((char*)h->pm.score_buf.p + 256, st);
     for (int i = 0; i < 16; ++i) h->host_guess[i] = result[i];      // pinned staging
-    H_CUDA(cudaMemcpyAsync(Tdev, h->host_guess, 16 * sizeof(double), cudaMemcpyHostToDevice, s));
     const double eps = (double)h->icp.knn_epsilon;
-    pm_score_knn_kernel<<<ceil_div(ns, 256), 256, 0, s>>>((const float*)h->f32.src.p, ns, Tdev, (const KdNode*)h->f32.target_tree.nodes.p,
-                                                       (const BucketPoint*)h->f32.target_tree.bpts.p, (1.0 + eps) * (1.0 + eps),
-                                                       sp.keys[0], sp.vals[0]);
-    H_RC(radix_sort_pairs_u64(sp.keys[0], sp.vals[0], sp.keys[1], sp.vals[1], ns, 1, st, sp.scratch, s, 8));
-    pm_score_reduce_kernel<<<1, 1024, 0, s>>>(sp.keys[0], ns, h->icp.dist_outlier_ratio, outdev);
-    H_CUDA(cudaGetLastError());
-    H_CUDA(cudaMemcpyAsync(h->host->pm_score, outdev, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-    H_CUDA(cudaStreamSynchronize(s));
+    H_RC(st.score_pass((const float*)h->f32.src.p, ns, h->host_guess, h->f32.target_tree, (1.0 + eps) * (1.0 + eps),
+                       h->icp.dist_outlier_ratio, h->host->pm_score, s));
     if (!(h->host->pm_score[1] > 0.0)) return fail(h, SM_ERR_NOTHING_TO_MINIMIZE, "Align: no matched point for the score");
     h->final_score = exp(-h->host->pm_score[0]);
     h->info.aux[1] = h->host->pm_score[1];     // matches kept by the trim in the score pass

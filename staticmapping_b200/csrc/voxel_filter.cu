@@ -17,13 +17,13 @@
 
 #include "../../include/sm_b200.h"
 #include "common.cuh"
+#include "compact.cuh"
 #include "kernels.h"
 
 namespace smb {
 namespace {
 
 constexpr long long kSpan = 1ll << 21;   // voxel indices of one axis must span < 2^21 (3 x 21-bit key)
-constexpr int kT = 256, kItems = 8, kTile = kT * kItems;
 
 // meta[0..2]: per-axis minimum voxel index over the finite points; meta[3]: dropped (non-finite) points;
 // meta[4]: 1 if an axis spans 2^21 voxels or more
@@ -77,36 +77,24 @@ __device__ __forceinline__ uint32_t vf_is_head(const uint64_t* keys, int i) {
   return (keys[i] != ~0ull && (i == 0 || keys[i] != keys[i - 1])) ? 1u : 0u;
 }
 
-__global__ void __launch_bounds__(kT)
-vf_heads_count_kernel(const uint64_t* __restrict__ keys, int n, uint32_t* __restrict__ block_sum) {
-  __shared__ uint32_t ws[kT / 32];
+__global__ void __launch_bounds__(kCompactThreads)
+vf_heads_count_kernel(const uint64_t* __restrict__ keys, int n, uint32_t* __restrict__ tile_cnt) {
   uint32_t c = 0;
-  const int base = blockIdx.x * kTile + threadIdx.x * kItems;
-  for (int r = 0; r < kItems; ++r) if (base + r < n) c += vf_is_head(keys, base + r);
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) ws[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < kT / 32; ++w) t += ws[w]; block_sum[blockIdx.x] = t; }
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  for (int r = 0; r < kCompactItems; ++r) if (base + r < n) c += vf_is_head(keys, base + r);
+  tile_count_store(c, tile_cnt);
 }
 
 // voxel_start[v] = first sorted position of voxel v; voxel_start[n_voxels] = n
-__global__ void __launch_bounds__(kT)
-vf_heads_scatter_kernel(const uint64_t* __restrict__ keys, int n, const uint32_t* __restrict__ block_off,
+__global__ void __launch_bounds__(kCompactThreads)
+vf_heads_scatter_kernel(const uint64_t* __restrict__ keys, int n, const uint32_t* __restrict__ tile_off,
                         uint32_t* __restrict__ voxel_start, const long long* __restrict__ meta) {
-  __shared__ uint32_t ws[kT / 32];
-  const int base = blockIdx.x * kTile + threadIdx.x * kItems;
-  uint32_t f[kItems], c = 0;
-  for (int r = 0; r < kItems; ++r) { f[r] = (base + r < n) ? vf_is_head(keys, base + r) : 0u; c += f[r]; }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = c;
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) ws[w] = incl;
-  __syncthreads();
-  uint32_t wb = 0;
-  for (int ww = 0; ww < w; ++ww) wb += ws[ww];
-  uint32_t pos = block_off[blockIdx.x] + wb + incl - c;
-  for (int r = 0; r < kItems; ++r) if (f[r]) voxel_start[pos++] = (uint32_t)(base + r);
-  if (blockIdx.x == 0 && threadIdx.x == 0) voxel_start[block_off[gridDim.x]] = (uint32_t)(n - (int)meta[3]);   // sentinel: first dropped point
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  uint32_t f[kCompactItems], c = 0;
+  for (int r = 0; r < kCompactItems; ++r) { f[r] = (base + r < n) ? vf_is_head(keys, base + r) : 0u; c += f[r]; }
+  uint32_t pos = tile_exclusive(c, tile_off);
+  for (int r = 0; r < kCompactItems; ++r) if (f[r]) voxel_start[pos++] = (uint32_t)(base + r);
+  if (blockIdx.x == 0 && threadIdx.x == 0) voxel_start[tile_off[gridDim.x]] = (uint32_t)(n - (int)meta[3]);   // sentinel: first dropped point
 }
 
 __global__ void __launch_bounds__(256)
@@ -172,13 +160,13 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   *m_out = 0;
   if (n == 0) return SM_OK;
   const int ni = (int)n;
-  const int nblk = ceil_div(n, kTile);
+  const int tiles = compact_tiles(n);
   const int64_t st = (n + 63) & ~(int64_t)63;
   const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
   size_t bytes = in_bytes + 256;
   bytes += 2 * st * sizeof(uint64_t) + 2 * st * sizeof(uint32_t);            // keys, order (ping-pong)
   bytes += radix_sort_scratch_bytes(ni, 1) + 256;
-  bytes += ((size_t)nblk + 8) * sizeof(uint32_t) + ((size_t)n + 8) * sizeof(uint32_t);   // block sums, voxel_start
+  bytes += compact_count_bytes(n) + ((size_t)n + 8) * sizeof(uint32_t);                 // tile counts, voxel_start
   bytes += (size_t)n * sizeof(float4) + (size_t)n * 5 * sizeof(float) + 1024;
   DevBuf buf;
   SMB_RC(buf.reserve(bytes));
@@ -190,7 +178,7 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   uint32_t* ord0 = (uint32_t*)take(st * sizeof(uint32_t));
   uint32_t* ord1 = (uint32_t*)take(st * sizeof(uint32_t));
   uint32_t* scratch = (uint32_t*)take(radix_sort_scratch_bytes(ni, 1));
-  uint32_t* block_sum = (uint32_t*)take(((size_t)nblk + 8) * sizeof(uint32_t));
+  uint32_t* tile_cnt = (uint32_t*)take(compact_count_bytes(n));
   uint32_t* voxel_start = (uint32_t*)take(((size_t)n + 8) * sizeof(uint32_t));
   float4* sorted = (float4*)take((size_t)n * sizeof(float4));
   float* d_out = (float*)take((size_t)n * 5 * sizeof(float));
@@ -202,16 +190,15 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   vf_min_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ni, voxel_size, meta);
   vf_key_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ni, voxel_size, keys0, ord0, meta);
   SMB_RC(radix_sort_pairs_u64(keys0, ord0, keys1, ord1, ni, 1, st, scratch, s, 8));   // 8 passes: result back in [0]
-  vf_heads_count_kernel<<<nblk, kT, 0, s>>>(keys0, ni, block_sum);
-  cudaMemsetAsync(block_sum + nblk, 0, sizeof(uint32_t), s);
-  radix_scan_kernel_launch(block_sum, nblk + 1, 1, s);                                // block_sum[nblk] = number of voxels
-  vf_heads_scatter_kernel<<<nblk, kT, 0, s>>>(keys0, ni, block_sum, voxel_start, meta);
+  vf_heads_count_kernel<<<tiles, kCompactThreads, 0, s>>>(keys0, ni, tile_cnt);
+  compact_scan(tile_cnt, tiles, s);                                                   // tile_cnt[tiles] = number of voxels
+  vf_heads_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(keys0, ni, tile_cnt, voxel_start, meta);
   vf_gather_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ord0, ni, sorted);
-  vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sorted, voxel_start, block_sum + nblk, d_out);
+  vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sorted, voxel_start, tile_cnt + tiles, d_out);
   uint32_t m = 0;
   long long host_meta[8] = {0};
   SMB_CUDA_OK(cudaGetLastError());
-  SMB_CUDA_OK(cudaMemcpyAsync(&m, block_sum + nblk, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(&m, tile_cnt + tiles, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   SMB_CUDA_OK(cudaMemcpyAsync(host_meta, meta, sizeof(host_meta), cudaMemcpyDeviceToHost, s));
   SMB_CUDA_OK(cudaStreamSynchronize(s));
   if (host_meta[4]) return SM_ERR_BAD_ARGUMENT;   // the finite points span 2^21 voxels or more along an axis

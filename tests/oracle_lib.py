@@ -306,7 +306,7 @@ def average_transforms(transforms):
 # ---- IcpUsingPointMatcher stand-in (type 1): composition of the pieces above ---------------------
 def pm_keep_mask(n, prob=0.9, seed=1):
     """The engine's reading filter: counter hash of the point index (murmur3 finaliser) below
-    prob * 2^32 (staticmapping_b200/csrc/sm_api.cu pm_keep)."""
+    prob * 2^32 (staticmapping_b200/csrc/icp_pm.cu pm_keep)."""
     p = float(np.float32(prob))
     if p >= 1.0:
         return np.ones(n, dtype=bool)
