@@ -85,6 +85,11 @@ struct __align__(32) BucketPoint {
 struct __align__(32) BucketNormal {
   double x, y, z, pad;
 };
+// padded bucket entry of a normals tree as ICP phase B reads it: the point and its normal in one 64-byte line
+// (three LDG.128 from two sectors), pad = 0
+struct __align__(64) BucketMatch {
+  double x, y, z, nx, ny, nz, pad[2];
+};
 
 }  // namespace smb
 

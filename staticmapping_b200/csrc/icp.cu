@@ -209,6 +209,15 @@ icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __res
 // -------------------------------------------------------------------------------- phase B
 // kComp: inner compensation (icp_fast.cc:284-289): the points are the iteration's de-skewed ones and every
 // match's Jacobian column is scaled by the point's factor, both for the sums and for the parked candidates
+// SMB_ACC_SECTIONS (diagnostic builds, profiles/accum_sections.py): every block adds the clock64 cycles thread 0
+// spent in each section below to state->stamps[0..5] and 1 to stamps[6], over all iterations and alignments
+#ifdef SMB_ACC_SECTIONS
+constexpr bool kAccSections = true;
+#else
+constexpr bool kAccSections = false;
+#endif
+enum AccSection { kSecLoads, kSecSelectBin, kSecGather, kSecTerms, kSecCompaction, kSecReduction, kAccSectionCount };
+
 template <bool kComp>
 __global__ void __launch_bounds__(kAccThreads)
 icp_accum_kernel(IcpBuffers b, IcpParams p, const double* __restrict__ deskewed) {
@@ -219,90 +228,118 @@ icp_accum_kernel(IcpBuffers b, IcpParams p, const double* __restrict__ deskewed)
   __shared__ uint32_t cand_warp[kAccItems][kAccThreads / 32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int tile0 = blockIdx.x * kAccTile;
+  [[maybe_unused]] long long sec[kAccSectionCount] = {}, sec_t = 0;
+  const auto mark = [&](int s) {
+    if constexpr (kAccSections) { const long long now = clock64(); sec[s] += now - sec_t; sec_t = now; }
+  };
+  if constexpr (kAccSections) sec_t = clock64();
+  // Item r of a thread is point tile0 + r * kAccThreads + threadIdx.x; the items run in passes of kAccPass,
+  // so the registers held per thread do not grow with the tile.
   // (1) everything that does not depend on the quantile bin is requested up front, for all the
-  //     points of the thread at once (these reads overlap the histogram read of select_bin)
+  //     points of the pass at once (the first pass's reads overlap the histogram read of select_bin)
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
-  double d2[kAccItems], sx[kAccItems], sy[kAccItems], sz[kAccItems];
-  [[maybe_unused]] double fac[kAccItems];
-  int slot[kAccItems];
+  const double* src = kComp ? deskewed : b.src0;
+  double d2[kAccPass], sx[kAccPass], sy[kAccPass], sz[kAccPass];
+  [[maybe_unused]] double fac[kAccPass];
+  int slot[kAccPass];
+  const auto load_pass = [&](int r0) {
 #pragma unroll
-  for (int r = 0; r < kAccItems; ++r) {
-    const int i = tile0 + r * kAccThreads + threadIdx.x;
-    const bool in = i < p.n_source;
-    d2[r] = in ? b.d2[i] : inf;
-    slot[r] = in ? b.slot[i] : -1;
-    const double* src = kComp ? deskewed : b.src0;
-    sx[r] = in ? src[i] : 0.0;
-    sy[r] = in ? src[b.sstride + i] : 0.0;
-    sz[r] = in ? src[2 * b.sstride + i] : 0.0;
-    if constexpr (kComp) fac[r] = in ? source_factor(b.src_sort.vals[0][i], p.n_source) : 0.0;
-  }
+    for (int r = 0; r < kAccPass; ++r) {
+      const int i = tile0 + (r0 + r) * kAccThreads + threadIdx.x;
+      const bool in = i < p.n_source;
+      d2[r] = in ? b.d2[i] : inf;
+      slot[r] = in ? b.slot[i] : -1;
+      sx[r] = in ? src[i] : 0.0;
+      sy[r] = in ? src[b.sstride + i] : 0.0;
+      sz[r] = in ? src[2 * b.sstride + i] : 0.0;
+      if constexpr (kComp) fac[r] = in ? source_factor(b.src_sort.vals[0][i], p.n_source) : 0.0;
+    }
+  };
+  load_pass(0);
   if (b.state->done) return;
   if (threadIdx.x < 16) T[threadIdx.x] = b.state->T_iter[threadIdx.x];
+  mark(kSecLoads);
   const BinSel sel = select_bin(b.hist, p.dist_outlier_ratio, warp_tot, &sel_sm);
-  // (2) the matched target point and normal of every point at or below the quantile bin; the
-  //     other lanes read entry 0 and are masked out, so the gathers of all items go out together
-  bool use[kAccItems], is_cand[kAccItems];
-  int bin[kAccItems];
-  double2 qxy[kAccItems], nxy[kAccItems];
-  double qz[kAccItems], nz[kAccItems];
-#pragma unroll
-  for (int r = 0; r < kAccItems; ++r) {
-    bin[r] = finite_d2(d2[r]) ? dist_bin(d2[r]) : kHistBins;
-    use[r] = sel.bin >= 0 && slot[r] >= 0 && bin[r] <= sel.bin;
-    const int s = use[r] ? slot[r] : 0;
-    const double* pq = b.kc.pb + (int64_t)(s >> 3) * 24 + (s & 7);     // padded bucket: x[8] y[8] z[8]
-    qxy[r] = make_double2(__ldg(pq), __ldg(pq + 8));
-    qz[r] = __ldg(pq + 16);
-    nxy[r] = __ldg(reinterpret_cast<const double2*>(b.kc.pn + s));
-    nz[r] = __ldg(reinterpret_cast<const double*>(b.kc.pn + s) + 2);
-  }
+  mark(kSecSelectBin);
   double acc[kNumSums];
 #pragma unroll
   for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0;
-  double F[kAccItems][6], dot[kAccItems], sq[kAccItems];
-#pragma unroll
-  for (int r = 0; r < kAccItems; ++r) {
-    BucketPoint q; BucketNormal n;
-    q.x = qxy[r].x; q.y = qxy[r].y; q.z = qz[r];
-    n.x = nxy[r].x; n.y = nxy[r].y; n.z = nz[r];
-    if constexpr (kComp) {
-      compensated_match_terms(sx[r], sy[r], sz[r], q, n, fac[r], F[r], dot[r]);
-    } else {
-      double px, py, pz;
-      transform_point(T, sx[r], sy[r], sz[r], px, py, pz);
-      match_terms(px, py, pz, q, n, F[r], dot[r]);
-    }
-    sq[r] = sqrt(use[r] ? d2[r] : 0.0);
-    add_terms_if(acc, F[r], dot[r], sq[r], use[r] && bin[r] < sel.bin);
-    is_cand[r] = use[r] && bin[r] == sel.bin;
-    if (is_cand[r]) atomicAdd(&b.hist2[sub_bin(d2[r])], 1u);
-  }
-  // (3) ordered compaction of the quantile-bin members: (item, warp, lane) == ascending point index
-  uint32_t m[kAccItems];
-#pragma unroll
-  for (int r = 0; r < kAccItems; ++r) {
-    m[r] = __ballot_sync(0xffffffffu, is_cand[r]);
-    if (lane == 0) cand_warp[r][w] = __popc(m[r]);
-  }
-  __syncthreads();
   uint32_t base = 0;
+#pragma unroll 1
+  for (int r0 = 0; r0 < kAccItems; r0 += kAccPass) {
+    if (r0 > 0) { load_pass(r0); mark(kSecLoads); }
+    // (2) the matched target point and normal of every point at or below the quantile bin: one 64-byte
+    //     record, three 16-byte loads; the other lanes read entry 0 and are masked out, so the gathers of
+    //     all items of the pass go out together
+    bool use[kAccPass], is_cand[kAccPass];
+    int bin[kAccPass];
+    double2 r01[kAccPass], r23[kAccPass], r45[kAccPass];    // {x, y}, {z, nx}, {ny, nz}
 #pragma unroll
-  for (int r = 0; r < kAccItems; ++r) {
-    uint32_t off = base, tot = 0;
-#pragma unroll
-    for (int ww = 0; ww < kAccThreads / 32; ++ww) { const uint32_t c = cand_warp[r][ww]; if (ww < w) off += c; tot += c; }
-    if (is_cand[r]) {
-      const int64_t dst = tile0 + off + __popc(m[r] & ((1u << lane) - 1u));
-      b.cand_key[dst] = (unsigned long long)__double_as_longlong(d2[r]);
-      double2* o = reinterpret_cast<double2*>(b.cand_terms + 8 * dst);
-      o[0] = make_double2(F[r][0], F[r][1]); o[1] = make_double2(F[r][2], F[r][3]);
-      o[2] = make_double2(F[r][4], F[r][5]); o[3] = make_double2(dot[r], sq[r]);
+    for (int r = 0; r < kAccPass; ++r) {
+      bin[r] = finite_d2(d2[r]) ? dist_bin(d2[r]) : kHistBins;
+      use[r] = sel.bin >= 0 && slot[r] >= 0 && bin[r] <= sel.bin;
+      const double2* rec = reinterpret_cast<const double2*>(b.kc.pm + (use[r] ? slot[r] : 0));
+      r01[r] = __ldg(rec); r23[r] = __ldg(rec + 1); r45[r] = __ldg(rec + 2);
     }
-    base += tot;
+    mark(kSecGather);
+    double F[kAccPass][6], dot[kAccPass], sq[kAccPass];
+#pragma unroll
+    for (int r = 0; r < kAccPass; ++r) {
+      BucketPoint q; BucketNormal n;
+      q.x = r01[r].x; q.y = r01[r].y; q.z = r23[r].x;
+      n.x = r23[r].y; n.y = r45[r].x; n.z = r45[r].y;
+      if constexpr (kComp) {
+        compensated_match_terms(sx[r], sy[r], sz[r], q, n, fac[r], F[r], dot[r]);
+      } else {
+        double px, py, pz;
+        transform_point(T, sx[r], sy[r], sz[r], px, py, pz);
+        match_terms(px, py, pz, q, n, F[r], dot[r]);
+      }
+      sq[r] = sqrt(use[r] ? d2[r] : 0.0);
+      add_terms_if(acc, F[r], dot[r], sq[r], use[r] && bin[r] < sel.bin);
+      is_cand[r] = use[r] && bin[r] == sel.bin;
+      if (is_cand[r]) atomicAdd(&b.hist2[sub_bin(d2[r])], 1u);
+    }
+    mark(kSecTerms);
+    // (3) ordered compaction of the quantile-bin members: (item, warp, lane) == ascending point index; the
+    //     passes append in item order behind `base`
+    uint32_t m[kAccPass];
+#pragma unroll
+    for (int r = 0; r < kAccPass; ++r) {
+      m[r] = __ballot_sync(0xffffffffu, is_cand[r]);
+      if (lane == 0) cand_warp[r0 + r][w] = __popc(m[r]);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < kAccPass; ++r) {
+      uint32_t off = base, tot = 0;
+#pragma unroll
+      for (int ww = 0; ww < kAccThreads / 32; ++ww) {
+        const uint32_t c = cand_warp[r0 + r][ww];
+        if (ww < w) off += c;
+        tot += c;
+      }
+      if (is_cand[r]) {
+        const int64_t dst = tile0 + off + __popc(m[r] & ((1u << lane) - 1u));
+        b.cand_key[dst] = (unsigned long long)__double_as_longlong(d2[r]);
+        double2* o = reinterpret_cast<double2*>(b.cand_terms + 8 * dst);
+        o[0] = make_double2(F[r][0], F[r][1]); o[1] = make_double2(F[r][2], F[r][3]);
+        o[2] = make_double2(F[r][4], F[r][5]); o[3] = make_double2(dot[r], sq[r]);
+      }
+      base += tot;
+    }
+    mark(kSecCompaction);
   }
   if (threadIdx.x == 0) b.cand_cnt[blockIdx.x] = base;
   block_reduce_sums<kAccThreads>(acc, red, b.partials + (int64_t)blockIdx.x * 32);
+  if constexpr (kAccSections) {
+    mark(kSecReduction);
+    if (threadIdx.x == 0) {
+      unsigned long long* st = reinterpret_cast<unsigned long long*>(b.state->stamps);
+      for (int s = 0; s < kAccSectionCount; ++s) atomicAdd(st + s, (unsigned long long)sec[s]);
+      atomicAdd(st + kAccSectionCount, 1ull);
+    }
+  }
 }
 
 template <bool kAllSmem>

@@ -14,7 +14,18 @@ namespace dev {
 #endif
 constexpr int kKnnThreads = SMB_KNN_THREADS;
 constexpr int kAccThreads = 256;
-constexpr int kAccItems = 2;
+// points per thread of a phase-B block (icp_accum_kernel): a block pays the quantile-bin search, the compaction
+// barriers and the 29-sum reduction once per tile, so a wider tile pays them less often per point
+#ifndef SMB_ACC_ITEMS
+#define SMB_ACC_ITEMS 2
+#endif
+#ifndef SMB_ACC_PASS
+#define SMB_ACC_PASS 4
+#endif
+constexpr int kAccItems = SMB_ACC_ITEMS;
+// items of a thread whose loads are in flight together (at most 4: registers grow with it)
+constexpr int kAccPass = kAccItems < SMB_ACC_PASS ? kAccItems : SMB_ACC_PASS;
+static_assert(kAccItems >= 1 && kAccItems % kAccPass == 0, "phase-B items come in whole passes");
 constexpr int kAccTile = kAccThreads * kAccItems;  // points per accumulate block
 constexpr int kNumSums = 29;                        // 21 (A upper) + 6 (b) + sum sqrt + count
 constexpr int kFinThreads = 1024;
@@ -314,15 +325,19 @@ __device__ __forceinline__ void add_terms_if(double* acc, const double* Fin, dou
 // Sum 32 per-lane values across the warp: on return lane L holds the warp total of v[L].
 // 31 exchanges instead of the 160 of 32 separate butterflies; the pairing is the butterfly's
 // (offsets 16, 8, 4, 2, 1), so each total is bit-identical to the xor-shuffle reduction.
+// The inner loop has a constant trip count: bounded by h, it can be unrolled before h is known, only partly, and
+// v then lives in local memory (phase B's 256-byte stack frame).
 __device__ __forceinline__ double warp_transpose_reduce32(double (&v)[32], int lane) {
 #pragma unroll
   for (int h = 16; h >= 1; h >>= 1) {
     const bool up = (lane & h) != 0;
 #pragma unroll
-    for (int i = 0; i < h; ++i) {
-      const double send = up ? v[i] : v[i + h];
-      const double keep = up ? v[i + h] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, h);
+    for (int i = 0; i < 16; ++i) {
+      if (i < h) {
+        const double send = up ? v[i] : v[i + h];
+        const double keep = up ? v[i + h] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, h);
+      }
     }
   }
   return v[0];

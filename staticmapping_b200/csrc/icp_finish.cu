@@ -520,8 +520,14 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
   }
 #endif
   __syncwarp();
+#ifdef SMB_ACC_SECTIONS
+  // the stamps hold phase B's section sums in this build (icp.cu) and stay as phase B left them
+  constexpr int kCopyWords = (int)(offsetof(IcpState, stamps) / 8);
+#else
+  constexpr int kCopyWords = kStateWords;
+#endif
 #pragma unroll 1
-  for (int i = lane; i < kStateWords; i += 32) gstate[i] = sstate[i];
+  for (int i = lane; i < kCopyWords; i += 32) gstate[i] = sstate[i];
 }
 
 }  // namespace

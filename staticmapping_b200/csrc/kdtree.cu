@@ -422,11 +422,12 @@ __global__ void kd_leaf_kernel(const uint32_t* __restrict__ list0, int n, int bu
 // level `levels`, or (index << 1) of a leaf one level higher (its odd twin stays empty).
 // Coordinates are stored per bucket as x[8] y[8] z[8]; empty entries hold +inf, so their
 // squared distance is +inf (or NaN) and the strict '<' of the search never takes them.
+// pm (normals trees): the same point beside its normal, one 64-byte record per entry (zero normal when empty).
 __global__ void kd_compact_buckets_kernel(const double* __restrict__ coord, int64_t cstride,
                                           const double* __restrict__ nrm, int64_t nstride,
                                           const uint32_t* __restrict__ leaf_order, int n, int bucket,
                                           int levels, double* __restrict__ pb,
-                                          BucketNormal* __restrict__ pn, int32_t* __restrict__ pid) {
+                                          BucketMatch* __restrict__ pm, int32_t* __restrict__ pid) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= ((int64_t)8 << levels)) return;
   const int jL = (int)(e >> 3), k = (int)(e & 7);
@@ -440,16 +441,20 @@ __global__ void kd_compact_buckets_kernel(const double* __restrict__ coord, int6
   const bool valid = owner && k < count;
   const double inf = __longlong_as_double(0x7ff0000000000000ll);
   double x = inf, y = inf, z = inf;
-  BucketNormal q; q.x = 0.0; q.y = 0.0; q.z = 0.0; q.pad = 0.0;
+  double nx = 0.0, ny = 0.0, nz = 0.0;
   int32_t id = -1;
   if (valid) {
     id = (int32_t)leaf_order[first + k];
     x = coord[id]; y = coord[cstride + id]; z = coord[2 * cstride + id];
-    if (nrm) { q.x = nrm[id]; q.y = nrm[nstride + id]; q.z = nrm[2 * nstride + id]; }
+    if (nrm) { nx = nrm[id]; ny = nrm[nstride + id]; nz = nrm[2 * nstride + id]; }
   }
   double* o = pb + (int64_t)jL * 24 + k;
   o[0] = x; o[8] = y; o[16] = z;
-  if (pn) pn[e] = q;
+  if (pm) {
+    double2* r = reinterpret_cast<double2*>(pm + e);
+    r[0] = make_double2(x, y); r[1] = make_double2(z, nx);
+    r[2] = make_double2(ny, nz); r[3] = make_double2(0.0, 0.0);
+  }
   if (pid) pid[e] = id;
 }
 
@@ -604,7 +609,7 @@ int KdCompactTree::reserve(int n, int bucket, Payload payload) {
   SMB_RC(cut.reserve(slots * (sizeof(double) + sizeof(double2))));
   SMB_RC(dim.reserve(slots));
   SMB_RC(pb.reserve(entries * 3 * sizeof(double)));
-  return payload == kNormals ? pn.reserve(entries * sizeof(BucketNormal)) : pid.reserve(entries * sizeof(int32_t));
+  return payload == kNormals ? pm.reserve(entries * sizeof(BucketMatch)) : pid.reserve(entries * sizeof(int32_t));
 }
 
 int KdCompactTree::build(const double* coord, const double* nrm, int64_t cstride, int n, int bucket,
@@ -614,14 +619,14 @@ int KdCompactTree::build(const double* coord, const double* nrm, int64_t cstride
   const int64_t total = (int64_t)8 << levels;
   kd_compact_buckets_kernel<<<ceil_div(total, 256), 256, 0, stream>>>(
       coord, cstride, nrm, cstride, (const uint32_t*)leaf_order.p, n, bucket, levels, (double*)pb.p,
-      (BucketNormal*)pn.p, (int32_t*)pid.p);
+      (BucketMatch*)pm.p, (int32_t*)pid.p);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
 KdCompact KdCompactTree::view() const {
   return {(const double*)cut.p, (const uint8_t*)dim.p, compact_node_array(*this), (const double*)pb.p,
-          (const BucketNormal*)pn.p, (const int32_t*)pid.p, levels, 0};
+          (const BucketMatch*)pm.p, (const int32_t*)pid.p, levels, 0};
 }
 
 int FloatTree::build(const float* pts, int n, DevBuf& kdws, cudaStream_t stream) {

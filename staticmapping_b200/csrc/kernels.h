@@ -72,24 +72,25 @@ struct KdWorkspace {
 //   pb              padded buckets, x[8] y[8] z[8] doubles per leaf slot of the deepest level
 //                   (+inf padding), so a leaf's bucket address is pure index arithmetic and a
 //                   bucket scan is 12 aligned 16-byte loads;
-//   pn, pid         normals / original ids per padded entry (entry = bucket * 8 + k).
+//   pm, pid         per padded entry (entry = bucket * 8 + k): the point and its normal in one 64-byte record
+//                   (what ICP phase B gathers per match; the search reads pb only) / the original id.
 struct KdCompact {
   const double* cut;
   const uint8_t* dim;
   const double2* node;    // {cut, dim as a 64-bit integer} of heap node h at slot h + 1, 2^levels slots: the
                           // search reads the levels below the shared-memory ones with one 16-byte load per node
   const double* pb;
-  const BucketNormal* pn;
+  const BucketMatch* pm;
   const int32_t* pid;
   int levels;
   int pad;                // set too: IcpBuffers embeds this struct, and its bytes are a graph key
 };
 // The device buffers of one tree in the compact layout, with its blocked node array and leaf order.  reserve()
-// sizes them for (n, bucket) with one payload per padded entry, the normals (pn) or the original ids (pid);
-// they only grow, so a tree of the same size keeps its pointers.  build() fills them.
+// sizes them for (n, bucket) with one payload per padded entry, the point + normal records (pm) or the original
+// ids (pid); they only grow, so a tree of the same size keeps its pointers.  build() fills them.
 struct KdCompactTree {
   enum Payload { kNormals, kIds };
-  DevBuf nodes, leaf_order, cut, dim, pb, pn, pid;   // cut: cut[] then node[]
+  DevBuf nodes, leaf_order, cut, dim, pb, pm, pid;   // cut: cut[] then node[]
   int levels = 0;
   int reserve(int n, int bucket, Payload payload);
   // coord / nrm: SoA [3][cstride]; nrm only with the kNormals payload
@@ -164,7 +165,7 @@ struct IcpBuffers {
   RadixPairs src_sort;    // Morton keys and the permutation
   int64_t sstride;
   // per-iteration
-  int32_t* slot;          // [n_source] padded bucket entry of the match (kc.pb / kc.pn index)
+  int32_t* slot;          // [n_source] padded bucket entry of the match (kc.pb / kc.pm index)
   int4* knn_items;        // [knn_items_bytes(n_source)] parked searches of the k-NN kernel's second phase (16 B each)
   double* d2;             // [n_source]
   uint32_t* hist;         // [kHistBins] first-level histogram of dist^2 (phase A)

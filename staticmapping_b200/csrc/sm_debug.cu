@@ -629,7 +629,10 @@ int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* fi
     SMB_CUDA_OK(cudaMemcpy(dim, kc.dim, inner, cudaMemcpyDeviceToHost));
     SMB_CUDA_OK(cudaMemcpy(node_2l, kc.node, (inner + 1) * sizeof(double2), cudaMemcpyDeviceToHost));
     SMB_CUDA_OK(cudaMemcpy(pb, kc.pb, entries * 3 * sizeof(double), cudaMemcpyDeviceToHost));
-    if (variant == 0) SMB_CUDA_OK(cudaMemcpy(pn, kc.pn, entries * sizeof(BucketNormal), cudaMemcpyDeviceToHost));
+    // pn[e] = {nx, ny, nz, 0}: the normal half of the 64-byte record, pad included
+    if (variant == 0)
+      SMB_CUDA_OK(cudaMemcpy2D(pn, sizeof(BucketNormal), (const char*)kc.pm + offsetof(BucketMatch, nx),
+                               sizeof(BucketMatch), sizeof(BucketNormal), entries, cudaMemcpyDeviceToHost));
     else SMB_CUDA_OK(cudaMemcpy(pid, kc.pid, entries * sizeof(int32_t), cudaMemcpyDeviceToHost));
   } else if (variant == 3) {
     SMB_CUDA_OK(cudaMemcpy(bpts, o.ft.bpts.p, (size_t)n * sizeof(BucketPoint), cudaMemcpyDeviceToHost));
