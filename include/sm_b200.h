@@ -127,20 +127,23 @@ int sm_get_type(const sm_handle* h);
 /* IcpFast::SetInputSource / SetInputTarget (icp_fast.cc:421-431): deep copy into the
  * engine (host pointers are not retained).  The target must carry unit normals
  * (CHECK(HasNormals()), icp_fast.cc:430) — the caller computed them with
- * EigenPointCloud::CalculateNormals (map_builder.cc:286,389) or sm_calculate_normals. */
+ * EigenPointCloud::CalculateNormals (map_builder.cc:286,389) or sm_calculate_normals.
+ * SM_TYPE_FAST_ICP only: every other type returns SM_ERR_UNSUPPORTED_TYPE and keeps its clouds. */
 int sm_set_input_source(sm_handle* h, const double* points_3xn, int64_t n);
 int sm_set_input_target(sm_handle* h, const double* points_3xn, const double* normals_3xn,
                         int64_t n);
 /* Ndt / NdtWithGicp keep the caller's float cloud (Interface::SetInputSource/Target,
  * interface.cc:38-60, converted by ToPclPointCloud at Align, ndt.cc:48-51).  `xyz` points at
  * the first x; consecutive points are `stride_bytes` apart (sizeof(InnerPointType) == 20 for
- * the reference's std::vector<InnerPointType>, 12 for packed xyz). */
+ * the reference's std::vector<InnerPointType>, 12 for packed xyz).  Ndt, NdtWithGicp and SM_TYPE_ICP_PM only: an
+ * IcpFast handle returns SM_ERR_UNSUPPORTED_TYPE and keeps its clouds. */
 int sm_set_input_source_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride_bytes);
 int sm_set_input_target_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride_bytes);
 int sm_set_input_source_f32_device(sm_handle* h, const float* dev_xyz, int64_t n, int64_t stride_bytes);
 int sm_set_input_target_f32_device(sm_handle* h, const float* dev_xyz, int64_t n, int64_t stride_bytes);
 
-/* Same, for clouds already resident in this device's memory (same layout). */
+/* Same, for clouds already resident in this device's memory (same layout); SM_TYPE_FAST_ICP only, like the host
+ * variants. */
 int sm_set_input_source_device(sm_handle* h, const double* dev_points_3xn, int64_t n);
 int sm_set_input_target_device(sm_handle* h, const double* dev_points_3xn,
                                const double* dev_normals_3xn, int64_t n);
@@ -154,7 +157,7 @@ int sm_align(sm_handle* h, const double* guess_4x4, double* result_4x4);
  * distinct instances: map_builder.cc:655,706-708; loop_detector.cc:224-228):
  * sm_align_async enqueues everything and returns; sm_align_wait blocks for the result (and,
  * with the convergence test enabled, keeps enqueuing 8-iteration chunks until it fires).
- * IcpFast only; sm_align == async + wait. */
+ * IcpFast only: on any other type both return SM_ERR_UNSUPPORTED_TYPE.  sm_align == async + wait. */
 int sm_align_async(sm_handle* h, const double* guess_4x4);
 int sm_align_wait(sm_handle* h, double* result_4x4);
 /* Batched Align.  The reference fans independent Align calls out to a thread pool / TBB tasks

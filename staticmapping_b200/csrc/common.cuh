@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "../../include/sm_b200.h"
+
 namespace smb {
 
 // ---- error plumbing: every CUDA call inside the library goes through this ----------
@@ -26,6 +28,16 @@ namespace smb {
 
 void set_cuda_error(cudaError_t e, const char* expr, const char* file, int line);
 const char* last_cuda_error();
+
+// the preamble of every entry point given a device ordinal: SM_ERR_NO_DEVICE without a CUDA device,
+// SM_ERR_BAD_ARGUMENT for an ordinal out of range, else cudaSetDevice
+inline int select_device(int device) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
+  if (device < 0 || device >= ndev) return SM_ERR_BAD_ARGUMENT;
+  SMB_CUDA_OK(cudaSetDevice(device));
+  return SM_OK;
+}
 
 constexpr int kNumSMs = 132;  // H100 SXM; grids are sized in multiples
 

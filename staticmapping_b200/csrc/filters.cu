@@ -720,11 +720,12 @@ int chain_fail(sm_filter_chain* c, int rc, const char* fmt, const char* arg) {
   return rc;
 }
 int chain_device(sm_filter_chain* c) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    return chain_fail(c, SM_ERR_NO_DEVICE, "no CUDA device: the filter chain has no CPU fallback%s", "");
-  SMB_CUDA_OK(cudaSetDevice(c->device));
-  return 0;
+  const int rc = select_device(c->device);
+  if (rc == SM_ERR_NO_DEVICE)
+    return chain_fail(c, rc, "no CUDA device: the filter chain has no CPU fallback%s", "");
+  if (rc == SM_ERR_BAD_ARGUMENT)
+    snprintf(c->error, sizeof(c->error), "device %d is out of range: the filter chain has no CPU fallback", c->device);
+  return rc;
 }
 }  // namespace
 

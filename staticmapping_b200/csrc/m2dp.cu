@@ -340,9 +340,7 @@ extern "C" int sm_m2dp(int device, const float* points, int64_t n, int64_t strid
   const int64_t len = sm_m2dp_descriptor_length(r, max_distance, t, p, q);
   if (len < 0 || capacity < len) return SM_ERR_BAD_ARGUMENT;        // "r is too small" (m2dp.cc:64-67)
   if (n == 0) return 0;                                             // "source is empty": setInputCloud returns false
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   M2dpStage st;
   SMB_RC(st.run(points, n, stride_bytes, r, max_distance, t, p, q, nullptr));
   if (A_out) memcpy(A_out, st.A.data(), st.A.size() * sizeof(int));

@@ -88,9 +88,7 @@ int sm_motion_compensation_device(int device, const float* dev_points, int64_t n
                                   const double* delta_4x4, float* dev_out, void* cuda_stream) {
   if (!dev_points || !dev_out || !delta_4x4 || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4)
     return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   if (n == 0) return SM_OK;
   cudaStream_t s = (cudaStream_t)cuda_stream;
   DevBuf bad;
@@ -139,9 +137,7 @@ int sm_motion_compensation(int device, const float* points, int64_t n, int64_t s
                            const double* delta_4x4, float* out) {
   if (!points || !out || !delta_4x4 || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4)
     return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   if (n == 0) return SM_OK;
   const size_t bytes = (size_t)n * (size_t)stride_bytes;
   DevBuf din, dout;

@@ -11,6 +11,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <variant>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>
@@ -110,13 +111,61 @@ struct GraphCache {
   void reset() { if (exec) cudaGraphExecDestroy(exec); exec = nullptr; key.clear(); }
 };
 
+// One state object per matcher type; a handle holds the one of its type.  A cloud count of 0 means "not set".
+// IcpFast, and the ICP chain type 1 runs on its filtered clouds: the uploaded SoA double clouds, the iteration
+// buffers, the tree's build workspace and the in-flight Align (sm_align_async .. sm_align_wait)
+struct IcpFastMatcher {
+  IcpOptions opt;
+  bool inner_compensation = false;  // Interface::EnableInnerCompensation; set on IcpFast handles only
+  DevBuf kdws;                      // k-d build workspace of the target tree (and of type 1's score tree)
+  DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, nrm, src_raw;
+  IcpFastBuffers bufs;
+  int64_t n_source = 0, n_target = 0, sstride = 0, tstride = 0;
+  bool up_src = false, up_tgt = false;
+  IcpState* host_state = nullptr;  // pinned, allocated by sm_create
+  GraphCache g_prologue, g_iterations;
+  struct {
+    IcpBuffers b; IcpParams p; KdWorkspace ws; std::string key;
+    double* deskewed = nullptr;
+    bool graphs = false, active = false;
+    int enqueued = 0, launches = 0, max_it = 0;
+  } run;
+  ~IcpFastMatcher() { if (host_state) cudaFreeHost(host_state); }
+};
+
+// the packed float clouds (12 bytes per point) of the _f32 setters
+struct F32Clouds { DevBuf src, tgt; int64_t n_src = 0, n_tgt = 0; };
+
+// Ndt and NdtWithGicp: the float clouds, the NDT stage, the target's tree (fitness score, GICP correspondences) and
+// the build workspace of their trees
+struct NdtBase { F32Clouds in; NdtStage ndt; FloatTree target_tree; DevBuf kdws; };
+struct NdtMatcher : NdtBase { ndt::Options opt; };
+struct NdtGicpMatcher : NdtBase {
+  NdtGicpOptions opt;
+  DevBuf src_filt, tgt_filt;
+  ApproxVoxelGrid approx;
+  gicp::Stage gicp;
+};
+
+// IcpUsingPointMatcher stand-in (type 1): raw float clouds -> filtered double clouds -> the IcpFast chain it
+// composes.  The normals pipeline has its own k-d workspace: icp.kdws.p is part of the IcpFast graph keys.
+struct PmMatcher {
+  IcpFastMatcher icp;
+  F32Clouds in;
+  bool src_dirty = false, tgt_dirty = false, score_tree_dirty = true;
+  NormalsPipeline normals;
+  PmStage stage;
+  FloatTree score_tree;
+  PmMatcher() { icp.opt.max_iteration = 150; }   // CounterTransformationChecker, icp_pointmatcher.cc:214
+};
+
 }  // namespace
 }  // namespace smb
 
 using namespace smb;
 
-// Everything a handle owns is released by its destructor; each group of device buffers is used
-// by one matcher type only, so a handle allocates one group (plus the shared kdws).
+// What every matcher type uses, and the state object of the handle's type (created by sm_create).  Everything a
+// handle owns is released by its destructor.
 struct sm_handle {
   int type = 0;
   int device = 0;
@@ -130,61 +179,17 @@ struct sm_handle {
   HostBlock* host_dev = nullptr;   // its device view
   std::string error;
   double final_score = 0.0;
-  sm_align_info info;
-  int64_t n_source = 0, n_target = 0;
-  bool has_source = false, has_target = false;
-  IcpOptions icp;
-  bool inner_compensation = false;  // Interface::EnableInnerCompensation; only IcpFast reads it
-  ndt::Options ndt;
-  NdtGicpOptions ng;
-  DevBuf kdws;                     // k-d tree build workspace of every tree below
+  sm_align_info info = {};
+  std::variant<std::monostate, IcpFastMatcher, NdtMatcher, NdtGicpMatcher, PmMatcher> m;
 
-  // IcpFast, and the ICP chain of type 1: the uploaded SoA double clouds, the iteration buffers and the tree
-  struct {
-    DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, nrm, src_raw;
-    IcpFastBuffers bufs;
-    int64_t sstride = 0, tstride = 0;
-    bool up_src = false, up_tgt = false;
-    IcpState* host_state = nullptr;  // pinned
-    GraphCache g_prologue, g_iterations;
-    // in-flight Align (sm_align_async .. sm_align_wait)
-    struct {
-      IcpBuffers b; IcpParams p; KdWorkspace ws; std::string key;
-      double* deskewed = nullptr;
-      bool graphs = false, active = false;
-      int enqueued = 0, launches = 0, max_it = 0;
-    } run;
-  } fast;
-
-  // Ndt, NdtWithGicp and type 1: packed float clouds (12 bytes per point), the NDT stage and the
-  // target's tree (fitness scores, GICP correspondences, the type-1 score)
-  struct {
-    DevBuf src, tgt;
-    NdtStage ndt;
-    FloatTree target_tree;
-  } f32;
-
-  // NdtWithGicp
-  struct {
-    DevBuf src_filt, tgt_filt;
-    ApproxVoxelGrid approx;
-    gicp::Stage gicp;
-  } ndt_gicp;
-
-  // IcpUsingPointMatcher stand-in (type 1): raw float clouds -> filtered double clouds.  The normals
-  // pipeline has its own k-d workspace: h->kdws.p is part of the IcpFast graph keys.
-  struct {
-    int64_t n_src = 0, n_tgt = 0;
-    bool src_dirty = false, tgt_dirty = false, score_tree_dirty = true;
-    NormalsPipeline normals;
-    PmStage stage;
-  } pm;
+  template <class T> T* as() { return std::get_if<T>(&m); }   // the state object if it is a T, else null
+  // the ICP chain: IcpFast's own, or the one type 1 composes
+  IcpFastMatcher* icp_chain() { return as<PmMatcher>() ? &as<PmMatcher>()->icp : as<IcpFastMatcher>(); }
 
   ~sm_handle() {
     for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ev_up) if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : prof_events) cudaEventDestroy(e);
-    if (fast.host_state) cudaFreeHost(fast.host_state);
     if (host) cudaFreeHost(host);
     if (host_guess) cudaFreeHost(host_guess);
     if (own_stream) cudaStreamDestroy(own_stream);
@@ -224,12 +229,11 @@ const OptionDef kNdtGicpOptions[] = {   // ndt_gicp.cc:31-36
 // the option table of the handle's type and the struct its offsets point into
 struct OptionTable { const OptionDef* begin; const OptionDef* end; char* base; };
 OptionTable options_of(sm_handle* h) {
-  switch (h->type) {
-    case SM_TYPE_NDT: return {std::begin(kNdtOptions), std::end(kNdtOptions), reinterpret_cast<char*>(&h->ndt)};
-    case SM_TYPE_NDT_WITH_GICP:
-      return {std::begin(kNdtGicpOptions), std::end(kNdtGicpOptions), reinterpret_cast<char*>(&h->ng)};
-    default: return {std::begin(kIcpOptions), std::end(kIcpOptions), reinterpret_cast<char*>(&h->icp)};  // IcpFast, type 1
-  }
+  if (NdtMatcher* m = h->as<NdtMatcher>())
+    return {std::begin(kNdtOptions), std::end(kNdtOptions), reinterpret_cast<char*>(&m->opt)};
+  if (NdtGicpMatcher* m = h->as<NdtGicpMatcher>())
+    return {std::begin(kNdtGicpOptions), std::end(kNdtGicpOptions), reinterpret_cast<char*>(&m->opt)};
+  return {std::begin(kIcpOptions), std::end(kIcpOptions), reinterpret_cast<char*>(&h->icp_chain()->opt)};  // and type 1
 }
 
 // pugixml as_bool: first non-blank character in "1tTyY" -> true
@@ -291,67 +295,55 @@ void key_append(std::string& k, const T& v) { k.append(reinterpret_cast<const ch
 // has consumed it (stream order), the copy stays asynchronous and the caller's host array must
 // stay valid until the stream reaches it (sm_align_pairs); with the shared staging buffer the call
 // returns after the copy, which is the deep-copy contract of SetInputSource / SetInputTarget.
-int load_cloud(sm_handle* h, const double* pts, int64_t n, bool on_device, DevBuf& soa,
-               int64_t stride, DevBuf* own_stage = nullptr) {
+int load_cloud(sm_handle* h, const double* pts, int64_t n, bool on_device, DevBuf& soa, int64_t stride,
+               DevBuf& stage, bool own_stage) {
   H_RC(soa.reserve((size_t)(3 * stride) * sizeof(double)));
-  H_RC(upload_soa(pts, n, on_device, own_stage ? *own_stage : h->fast.stage, (double*)soa.p, stride, h->stream));
+  H_RC(upload_soa(pts, n, on_device, stage, (double*)soa.p, stride, h->stream));
   if (!on_device && !own_stage) H_CUDA(cudaStreamSynchronize(h->stream));  // the shared stage buffer is reused
   return 0;
 }
 
-int set_source(sm_handle* h, const double* pts, int64_t n, bool on_device, bool async = false) {
-  if (!h) return SM_ERR_BAD_ARGUMENT;
+int icp_set_source(sm_handle* h, IcpFastMatcher& f, const double* pts, int64_t n, bool on_device, bool async = false) {
   if (!pts || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInputSource: empty cloud");
   if (n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInputSource: too many points");
-  H_CUDA(cudaSetDevice(h->device));
   H_CUDA(cudaEventRecord(h->ev_up[0], h->stream));
-  auto& f = h->fast;
   f.sstride = pad64(n);
-  H_RC(load_cloud(h, pts, n, on_device, f.src_raw, f.sstride, async ? &f.stage_src : nullptr));
+  H_RC(load_cloud(h, pts, n, on_device, f.src_raw, f.sstride, async ? f.stage_src : f.stage, async));
   H_CUDA(cudaEventRecord(h->ev_up[1], h->stream));
   f.up_src = true;
-  h->n_source = n;
-  h->has_source = true;
+  f.n_source = n;
   return 0;
 }
 
-int set_target(sm_handle* h, const double* pts, const double* nrm, int64_t n, bool on_device, bool async = false) {
-  if (!h) return SM_ERR_BAD_ARGUMENT;
+int icp_set_target(sm_handle* h, IcpFastMatcher& f, const double* pts, const double* nrm, int64_t n, bool on_device,
+                   bool async = false) {
   if (!pts || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: empty cloud");
-  if (h->type == SM_TYPE_FAST_ICP && !nrm)
-    return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: IcpFast target needs normals");
+  if (!nrm) return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: IcpFast target needs normals");
   if (n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInputTarget: too many points");
-  H_CUDA(cudaSetDevice(h->device));
   H_CUDA(cudaEventRecord(h->ev_up[2], h->stream));
-  auto& f = h->fast;
   f.tstride = pad64(n);
-  H_RC(load_cloud(h, pts, n, on_device, f.tgt_raw, f.tstride, async ? &f.stage_tgt : nullptr));
-  if (nrm) H_RC(load_cloud(h, nrm, n, on_device, f.nrm, f.tstride, async ? &f.stage_nrm : nullptr));
+  H_RC(load_cloud(h, pts, n, on_device, f.tgt_raw, f.tstride, async ? f.stage_tgt : f.stage, async));
+  H_RC(load_cloud(h, nrm, n, on_device, f.nrm, f.tstride, async ? f.stage_nrm : f.stage, async));
   H_CUDA(cudaEventRecord(h->ev_up[3], h->stream));
   f.up_tgt = true;
-  h->n_target = n;
-  h->has_target = true;
+  f.n_target = n;
   return 0;
 }
 
-int ndt_align(sm_handle* h, const double* guess, double* result);
-int ndt_gicp_align(sm_handle* h, const double* guess, double* result);
-int pm_align(sm_handle* h, const double* guess, double* result);
-int build_tree_f32(sm_handle* h, const float* pts, int n, FloatTree& t) {
+int build_tree_f32(sm_handle* h, DevBuf& kdws, const float* pts, int n, FloatTree& t) {
   if (kd_num_levels(n, 8) > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "cloud too large");
-  H_RC(t.build(pts, n, h->kdws, h->stream));
+  H_RC(t.build(pts, n, kdws, h->stream));
   return 0;
 }
 
 // one chunk of iterations + the asynchronous read-back of the state record
-int icp_enqueue_chunk(sm_handle* h) {
-  auto& f = h->fast;
+int icp_enqueue_chunk(sm_handle* h, IcpFastMatcher& f) {
   auto& r = f.run;
   const IcpParams& p = r.p;
   const int chunk = p.disable_convergence ? (r.max_it - r.enqueued)
                                           : ((r.max_it - r.enqueued) < 8 ? (r.max_it - r.enqueued) : 8);
   cudaEvent_t* evs = nullptr;
-  if (h->icp.profile_kernels) {
+  if (f.opt.profile_kernels) {
     while ((int)h->prof_events.size() < 4 * (r.enqueued + chunk)) {
       cudaEvent_t e; H_CUDA(cudaEventCreate(&e)); h->prof_events.push_back(e);
     }
@@ -374,48 +366,45 @@ int icp_enqueue_chunk(sm_handle* h) {
 }
 
 // IcpFast::Align, first half: everything is enqueued, nothing is waited for
-int icp_begin(sm_handle* h, const double* guess) {
-  auto& f = h->fast;
+int icp_begin(sm_handle* h, IcpFastMatcher& f, const double* guess) {
   auto& r = f.run;
   r.active = false;
-  if (!h->has_source || !h->has_target)
-    return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
+  if (f.n_source <= 0 || f.n_target <= 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
   {   // CHECK(quantile >= 0 && quantile <= 1), icp_fast.cc:68
-    const float q = h->icp.dist_outlier_ratio;
+    const float q = f.opt.dist_outlier_ratio;
     if (!(q >= 0.0f && q <= 1.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: dist_outlier_ratio outside [0, 1] (icp_fast.cc:68)");
-    if (!(h->icp.knn_epsilon >= 0.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: knn_epsilon must be >= 0");
+    if (!(f.opt.knn_epsilon >= 0.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: knn_epsilon must be >= 0");
   }
   NvtxRange nvtx_align("IcpFast::Align");
-  const int ns = (int)h->n_source, nt = (int)h->n_target;
+  const int ns = (int)f.n_source, nt = (int)f.n_target;
   const int levels = kd_num_levels(nt, 8);
   // EnableInnerCompensation: IcpFast::Align reads it (icp_fast.cc:487, :509); type 1 runs the IcpFast chain but,
-  // like IcpUsingPointMatcher, ignores it
-  const bool comp = h->type == SM_TYPE_FAST_ICP && h->inner_compensation;
-  H_RC(f.bufs.reserve(ns, nt, f.sstride, f.tstride, comp));
+  // like IcpUsingPointMatcher, ignores it: its flag stays false
+  H_RC(f.bufs.reserve(ns, nt, f.sstride, f.tstride, f.inner_compensation));
   KdWorkspace& ws = r.ws;
-  H_RC(ws.carve(h->kdws, nt, 8));
+  H_RC(ws.carve(f.kdws, nt, 8));
 
   IcpBuffers& b = r.b;
   f.bufs.fill(b, (const double*)f.tgt_raw.p, (const double*)f.nrm.p, (const double*)f.src_raw.p);
   IcpParams& p = r.p;
   p.n_source = ns; p.n_target = nt;
-  p.max_iteration = h->icp.max_iteration;
-  p.dist_outlier_ratio = h->icp.dist_outlier_ratio;
-  const double eps = (double)h->icp.knn_epsilon;
+  p.max_iteration = f.opt.max_iteration;
+  p.dist_outlier_ratio = f.opt.dist_outlier_ratio;
+  const double eps = (double)f.opt.knn_epsilon;
   p.max_error2 = (1.0 + eps) * (1.0 + eps);
-  p.disable_convergence = h->icp.disable_convergence_check ? 1 : 0;
-  p.knn_queries_per_cta = h->icp.knn_queries_per_cta;
+  p.disable_convergence = f.opt.disable_convergence_check ? 1 : 0;
+  p.knn_queries_per_cta = f.opt.knn_queries_per_cta;
   p.tree_levels = levels;
-  p.inner_compensation = comp ? 1 : 0;
-  r.deskewed = comp ? (double*)f.bufs.deskewed.p : nullptr;
+  p.inner_compensation = f.inner_compensation ? 1 : 0;
+  r.deskewed = f.inner_compensation ? (double*)f.bufs.deskewed.p : nullptr;
   if (levels > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "target too large (tree deeper than 24 levels)");
 
   memcpy(h->host_guess, guess, 16 * sizeof(double));   // pinned: the caller's array may go away
   H_CUDA(cudaMemcpyAsync(f.bufs.guess.p, h->host_guess, 16 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   H_CUDA(cudaEventRecord(h->ev[0], h->stream));
-  r.graphs = h->icp.use_graphs && !h->icp.profile_kernels;
+  r.graphs = f.opt.use_graphs && !f.opt.profile_kernels;
   r.key.clear();
-  key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.bufs.guess.p); key_append(r.key, h->kdws.p);
+  key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.bufs.guess.p); key_append(r.key, f.kdws.p);
   key_append(r.key, r.deskewed);   // p.inner_compensation is part of p
   if (r.graphs) {
     H_RC(run_graphed(h, f.g_prologue, r.key, [&]() {
@@ -428,21 +417,20 @@ int icp_begin(sm_handle* h, const double* guess) {
   r.launches = icp_prologue_launches(levels);
   r.enqueued = 0;
   r.max_it = p.max_iteration > 0 ? p.max_iteration : 1;
-  H_RC(icp_enqueue_chunk(h));
+  H_RC(icp_enqueue_chunk(h, f));
   r.active = true;
   return 0;
 }
 
 // second half: wait, continue in chunks while the convergence test has not fired, report
-int icp_end(sm_handle* h, double* result) {
-  auto& f = h->fast;
+int icp_end(sm_handle* h, IcpFastMatcher& f, double* result) {
   auto& r = f.run;
   if (!r.active) return fail(h, SM_ERR_BAD_ARGUMENT, "sm_align_wait without sm_align_async");
   r.active = false;
   while (true) {
     H_CUDA(cudaStreamSynchronize(h->stream));
     if (f.host_state->done || r.enqueued >= r.max_it) break;
-    H_RC(icp_enqueue_chunk(h));
+    H_RC(icp_enqueue_chunk(h, f));
   }
   H_CUDA(cudaEventRecord(h->ev[2], h->stream));
   H_CUDA(cudaEventSynchronize(h->ev[2]));
@@ -462,7 +450,7 @@ int icp_end(sm_handle* h, double* result) {
   h->info.kernel_launches = r.launches;
   h->info.ms_knn = h->info.ms_accum = h->info.ms_finish = 0.f;
   h->info.profiled_iterations = 0;
-  if (h->icp.profile_kernels) {
+  if (f.opt.profile_kernels) {
     for (int it = 0; it < st.iteration && 4 * it + 3 < (int)h->prof_events.size(); ++it) {
       float a = 0.f, bb = 0.f, c = 0.f;
       cudaEventElapsedTime(&a, h->prof_events[4 * it], h->prof_events[4 * it + 1]);
@@ -480,9 +468,9 @@ int icp_end(sm_handle* h, double* result) {
   return 1;  // IcpFast::Align always returns true (icp_fast.cc:528)
 }
 
-int icp_align(sm_handle* h, const double* guess, double* result) {
-  H_RC(icp_begin(h, guess));
-  return icp_end(h, result);
+int icp_align(sm_handle* h, IcpFastMatcher& f, const double* guess, double* result) {
+  H_RC(icp_begin(h, f, guess));
+  return icp_end(h, f, result);
 }
 
 // ---- IcpUsingPointMatcher stand-in (type 1) ------------------------------------------------
@@ -499,71 +487,73 @@ int icp_align(sm_handle* h, const double* guess, double* result) {
 //                     trim 0.7, exp(-mean kept distance); Align() false below 0.6 (:145)
 // It is a deterministic equivalent, not a bit-level restatement: libpointmatcher's float
 // arithmetic and its rand() stream cannot be pinned from this tree.
-int pm_align(sm_handle* h, const double* guess, double* result) {
-  if (!h->has_source || !h->has_target || h->pm.n_src <= 0 || h->pm.n_tgt <= 0)
-    return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
+int pm_align(sm_handle* h, PmMatcher& pm, const double* guess, double* result) {
+  if (pm.in.n_src <= 0 || pm.in.n_tgt <= 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
   cudaStream_t s = h->stream;
-  if (h->pm.tgt_dirty) {
-    const int n = (int)h->pm.n_tgt;
-    NormalsPipeline& np = h->pm.normals;
+  if (pm.tgt_dirty) {
+    const int n = (int)pm.in.n_tgt;
+    NormalsPipeline& np = pm.normals;
     H_RC(np.reserve(n));
-    H_RC(ndt_float_to_soa((const float*)h->f32.tgt.p, n, np.input(), np.stride, s));
+    H_RC(ndt_float_to_soa((const float*)pm.in.tgt.p, n, np.input(), np.stride, s));
     uint32_t m = 0;
     H_RC(np.run(n, s, &m));
     if (m == 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: no target point survived the surface-normal filter");
-    H_RC(set_target(h, np.points(), np.normals(), (int64_t)m, true));
-    h->pm.tgt_dirty = false;
+    H_RC(icp_set_target(h, pm.icp, np.points(), np.normals(), (int64_t)m, true));
+    pm.tgt_dirty = false;
   }
-  PmStage& st = h->pm.stage;
-  H_RC(st.reserve((int)h->pm.n_src));
-  if (h->pm.src_dirty) {
+  PmStage& st = pm.stage;
+  H_RC(st.reserve((int)pm.in.n_src));
+  if (pm.src_dirty) {
     uint32_t kept = 0;
-    H_RC(st.sample((const float*)h->f32.src.p, (int)h->pm.n_src, h->icp.reading_sample_prob,
-                   (uint32_t)h->icp.sample_seed, s, &kept));
+    H_RC(st.sample((const float*)pm.in.src.p, (int)pm.in.n_src, pm.icp.opt.reading_sample_prob,
+                   (uint32_t)pm.icp.opt.sample_seed, s, &kept));
     if (kept == 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: the reading filter kept no point");
-    H_RC(set_source(h, st.points(), (int64_t)kept, true));
-    h->pm.src_dirty = false;
+    H_RC(icp_set_source(h, pm.icp, st.points(), (int64_t)kept, true));
+    pm.src_dirty = false;
   }
-  const int rc = icp_align(h, guess, result);
-  h->info.aux[2] = (double)h->n_source;   // reading points after the filter
-  h->info.aux[3] = (double)h->n_target;   // reference points after the filter
+  const int rc = icp_align(h, pm.icp, guess, result);
+  h->info.aux[2] = (double)pm.icp.n_source;   // reading points after the filter
+  h->info.aux[3] = (double)pm.icp.n_target;   // reference points after the filter
   if (rc < 0) return rc;
   h->info.aux[0] = h->final_score;        // IcpFast's own score (last iteration, filtered clouds)
   // ---- "compute the final score" (icp_pointmatcher.cc:131-148) -------------------------------
   {
-    const int ns = (int)h->pm.n_src, nt = (int)h->pm.n_tgt;
-    if (h->pm.score_tree_dirty) {
-      H_RC(build_tree_f32(h, (const float*)h->f32.tgt.p, nt, h->f32.target_tree));
-      h->pm.score_tree_dirty = false;
+    const int ns = (int)pm.in.n_src, nt = (int)pm.in.n_tgt;
+    if (pm.score_tree_dirty) {
+      H_RC(build_tree_f32(h, pm.icp.kdws, (const float*)pm.in.tgt.p, nt, pm.score_tree));
+      pm.score_tree_dirty = false;
     }
     for (int i = 0; i < 16; ++i) h->host_guess[i] = result[i];      // pinned staging
-    const double eps = (double)h->icp.knn_epsilon;
-    H_RC(st.score_pass((const float*)h->f32.src.p, ns, h->host_guess, h->f32.target_tree, (1.0 + eps) * (1.0 + eps),
-                       h->icp.dist_outlier_ratio, h->host->pm_score, s));
+    const double eps = (double)pm.icp.opt.knn_epsilon;
+    H_RC(st.score_pass((const float*)pm.in.src.p, ns, h->host_guess, pm.score_tree, (1.0 + eps) * (1.0 + eps),
+                       pm.icp.opt.dist_outlier_ratio, h->host->pm_score, s));
     if (!(h->host->pm_score[1] > 0.0)) return fail(h, SM_ERR_NOTHING_TO_MINIMIZE, "Align: no matched point for the score");
     h->final_score = exp(-h->host->pm_score[0]);
     h->info.aux[1] = h->host->pm_score[1];     // matches kept by the trim in the score pass
   }
-  return h->final_score < (double)h->icp.accept_min_score ? 0 : 1;
+  return h->final_score < (double)pm.icp.opt.accept_min_score ? 0 : 1;
 }
 
 // ---- Ndt ---------------------------------------------------------------------------------
-// the packed float source or target cloud (Ndt, NdtWithGicp, type 1)
+// the packed float source or target cloud of Ndt, NdtWithGicp and type 1
 int set_input_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride, bool target, bool on_device) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
+  NdtMatcher* nm = h->as<NdtMatcher>();
+  NdtGicpMatcher* gm = h->as<NdtGicpMatcher>();
+  PmMatcher* pm = h->as<PmMatcher>();
+  F32Clouds* in = nm ? &nm->in : gm ? &gm->in : pm ? &pm->in : nullptr;
+  if (!in) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetInput (float): IcpFast takes sm_set_input_source / _target");
   if (!xyz || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInput: empty cloud");
   if (stride < 12 || n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInput: bad stride / size");
   H_CUDA(cudaSetDevice(h->device));
-  DevBuf& dst = target ? h->f32.tgt : h->f32.src;
+  DevBuf& dst = target ? in->tgt : in->src;
   H_RC(dst.reserve((size_t)n * 12 + 64));
   H_CUDA(cudaMemcpy2DAsync(dst.p, 12, xyz, (size_t)stride, 12, (size_t)n,
                            on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
   if (!on_device) H_CUDA(cudaStreamSynchronize(h->stream));
-  if (target) {
-    h->n_target = n; h->has_target = true; h->pm.n_tgt = n; h->pm.tgt_dirty = true; h->pm.score_tree_dirty = true;
-  } else {
-    h->n_source = n; h->has_source = true; h->pm.n_src = n; h->pm.src_dirty = true;
-  }
+  (target ? in->n_tgt : in->n_src) = n;
+  if (pm && target) pm->tgt_dirty = pm->score_tree_dirty = true;
+  if (pm && !target) pm->src_dirty = true;
   return 0;
 }
 
@@ -576,9 +566,9 @@ struct NdtRunOut {
 
 // pcl::Registration::align -> NormalDistributionsTransform::computeTransformation
 // (ndt_omp_impl.hpp:81-171) -> getFitnessScore, on device clouds src/tgt (packed float xyz).
-int ndt_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, const ndt::Options& o,
+int ndt_run(sm_handle* h, NdtBase& m, const float* src, int ns, const float* tgt, int nt, const ndt::Options& o,
             bool f64_math, const double* guess, NdtRunOut* out) {
-  NdtStage& st = h->f32.ndt;
+  NdtStage& st = m.ndt;
   H_RC(st.reserve(nt, ns));
   H_CUDA(cudaEventRecord(h->ev[0], h->stream));
   H_RC(st.build_grid(tgt, nt, o.resolution, h->stream));        // setInputTarget -> init()
@@ -609,8 +599,8 @@ int ndt_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, co
   H_CUDA(cudaEventRecord(h->ev[2], h->stream));
   // getFitnessScore (ndt.cc:60): exact 1-NN over the full target (PCL builds this search
   // tree in setInputTarget; the reference calls that on every Align)
-  H_RC(build_tree_f32(h, tgt, nt, h->f32.target_tree));
-  H_RC(st.fitness(src, ns, tgt, final_T, h->f32.target_tree, h->host->ndt_sums, h->stream, &out->fitness));
+  H_RC(build_tree_f32(h, m.kdws, tgt, nt, m.target_tree));
+  H_RC(st.fitness(src, ns, tgt, final_T, m.target_tree, h->host->ndt_sums, h->stream, &out->fitness));
   H_CUDA(cudaEventRecord(h->ev[3], h->stream));
   H_CUDA(cudaEventSynchronize(h->ev[3]));
   out->iterations = nw.iterations;
@@ -625,14 +615,14 @@ int ndt_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, co
 }
 
 // Ndt::Align (ndt.cc:38-64)
-int ndt_align(sm_handle* h, const double* guess, double* result) {
-  if (!h->has_source || !h->has_target) {       // ndt.cc:40-42: return false
+int ndt_align(sm_handle* h, NdtMatcher& m, const double* guess, double* result) {
+  if (m.in.n_src <= 0 || m.in.n_tgt <= 0) {    // ndt.cc:40-42: return false
     for (int i = 0; i < 16; ++i) result[i] = guess[i];
     return 0;
   }
   NdtRunOut r;
-  const int rc = ndt_run(h, (const float*)h->f32.src.p, (int)h->n_source, (const float*)h->f32.tgt.p,
-                         (int)h->n_target, h->ndt, false, guess, &r);
+  const int rc = ndt_run(h, m, (const float*)m.in.src.p, (int)m.in.n_src, (const float*)m.in.tgt.p, (int)m.in.n_tgt,
+                         m.opt, false, guess, &r);
   if (rc < 0) return rc;                        // with ndt_run's own message
   h->final_score = r.fitness;
   for (int i = 0; i < 16; ++i) result[i] = (double)r.final_T[i];     // .cast<double>() (ndt.cc:61)
@@ -648,12 +638,12 @@ int ndt_align(sm_handle* h, const double* guess, double* result) {
 
 // ---- NdtWithGicp ---------------------------------------------------------------------------
 // GeneralizedIterativeClosestPoint::computeTransformation (gicp_omp_impl.hpp:381-514) with the
-// BFGS inner solver on the host; the target tree must be built in h->f32.target_tree.
-int gicp_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, const float* guess,
+// BFGS inner solver on the host; the target tree must be built in m.target_tree.
+int gicp_run(sm_handle* h, NdtGicpMatcher& m, const float* src, int ns, const float* tgt, int nt, const float* guess,
              const gicp::Options& o, float* final_T, int* iterations, int* bfgs_evals) {
-  gicp::Stage& g = h->ndt_gicp.gicp;
-  const FloatTree& tt = h->f32.target_tree;
-  H_RC(build_tree_f32(h, src, ns, g.source_tree));
+  gicp::Stage& g = m.gicp;
+  const FloatTree& tt = m.target_tree;
+  H_RC(build_tree_f32(h, m.kdws, src, ns, g.source_tree));
   H_RC(g.reserve(ns, nt, h->stream));
   volatile long long* seq_word = &h->host->gicp_seq;
   *seq_word = 0;
@@ -694,18 +684,17 @@ int gicp_run(sm_handle* h, const float* src, int ns, const float* tgt, int nt, c
 }
 
 // NdtWithGicp::Align (ndt_gicp.cc:55-112)
-int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
-  if (!h->has_source || !h->has_target)
+int ndt_gicp_align(sm_handle* h, NdtGicpMatcher& m, const double* guess, double* result) {
+  if (m.in.n_src <= 0 || m.in.n_tgt <= 0)
     return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");   // null deref in the reference
-  const float* src = (const float*)h->f32.src.p;
-  const float* tgt = (const float*)h->f32.tgt.p;
-  int ns = (int)h->n_source, nt = (int)h->n_target;
-  if (h->ng.using_voxel_filter) {
-    auto& g = h->ndt_gicp;    // pcl::ApproximateVoxelGrid::filter (ndt_gicp.cc:59-70)
-    H_RC(g.approx.filter(src, ns, h->ng.voxel_resolution, g.src_filt, &ns, h->stream));
-    H_RC(g.approx.filter(tgt, nt, h->ng.voxel_resolution, g.tgt_filt, &nt, h->stream));
-    src = (const float*)g.src_filt.p;
-    tgt = (const float*)g.tgt_filt.p;
+  const float* src = (const float*)m.in.src.p;
+  const float* tgt = (const float*)m.in.tgt.p;
+  int ns = (int)m.in.n_src, nt = (int)m.in.n_tgt;
+  if (m.opt.using_voxel_filter) {           // pcl::ApproximateVoxelGrid::filter (ndt_gicp.cc:59-70)
+    H_RC(m.approx.filter(src, ns, m.opt.voxel_resolution, m.src_filt, &ns, h->stream));
+    H_RC(m.approx.filter(tgt, nt, m.opt.voxel_resolution, m.tgt_filt, &nt, h->stream));
+    src = (const float*)m.src_filt.p;
+    tgt = (const float*)m.tgt_filt.p;
   }
   memset(&h->info, 0, sizeof(h->info));
   h->info.aux[2] = ns; h->info.aux[3] = nt;
@@ -713,18 +702,18 @@ int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
   float ndt_guess[16];
   for (int i = 0; i < 16; ++i) ndt_guess[i] = (float)guess[i];
   double ndt_score = 0.9;
-  if (h->ng.use_ndt) {                    // ndt_gicp.cc:82-88, configuration :44-47
+  if (m.opt.use_ndt) {                    // ndt_gicp.cc:82-88, configuration :44-47
     ndt::Options no;                      // stock pcl::NormalDistributionsTransform: KDTREE only
     no.transformation_epsilon = 0.01; no.step_size = 0.1; no.resolution = 1.0f; no.max_iterations = 35;
     NdtRunOut r;
-    const int rc = ndt_run(h, src, ns, tgt, nt, no, true, guess, &r);
+    const int rc = ndt_run(h, m, src, ns, tgt, nt, no, true, guess, &r);
     if (rc < 0) return rc;                      // with ndt_run's own message
     ndt_score = r.fitness;
     for (int i = 0; i < 16; ++i) ndt_guess[i] = r.final_T[i];
     h->info.evaluations = r.evaluations;
     h->info.ms_prologue = r.ms_grid + r.ms_iter + r.ms_fit;
   } else {
-    H_RC(build_tree_f32(h, tgt, nt, h->f32.target_tree));
+    H_RC(build_tree_f32(h, m.kdws, tgt, nt, m.target_tree));
   }
   h->info.aux[0] = ndt_score;
   double icp_score = 10.0;
@@ -732,10 +721,9 @@ int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
     float final_T[16];
     int it = 0, evals = 0;
     H_CUDA(cudaEventRecord(h->ev[0], h->stream));
-    H_RC(gicp_run(h, src, ns, tgt, nt, ndt_guess, gicp::Options(), final_T, &it, &evals));
-    NdtStage& st = h->f32.ndt;
-    H_RC(st.reserve(nt, ns));
-    H_RC(st.fitness(src, ns, tgt, final_T, h->f32.target_tree, h->host->ndt_sums, h->stream, &icp_score));
+    H_RC(gicp_run(h, m, src, ns, tgt, nt, ndt_guess, gicp::Options(), final_T, &it, &evals));
+    H_RC(m.ndt.reserve(nt, ns));
+    H_RC(m.ndt.fitness(src, ns, tgt, final_T, m.target_tree, h->host->ndt_sums, h->stream, &icp_score));
     H_CUDA(cudaEventRecord(h->ev[1], h->stream));
     H_CUDA(cudaEventSynchronize(h->ev[1]));
     cudaEventElapsedTime(&h->info.ms_iterations, h->ev[0], h->ev[1]);
@@ -749,6 +737,15 @@ int ndt_gicp_align(sm_handle* h, const double* guess, double* result) {
   for (int i = 0; i < 16; ++i) result[i] = guess[i];   // :104-108
   h->final_score = exp(-icp_score);
   return 0;
+}
+
+// the double source or target cloud: IcpFast's setters; the other types take float clouds through the _f32 setters
+int set_f64(sm_handle* h, bool target, bool on_device, const double* pts, int64_t n, const double* nrm = nullptr) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  IcpFastMatcher* f = h->as<IcpFastMatcher>();
+  if (!f) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "sm_set_input_source / _target (double clouds): IcpFast only");
+  H_CUDA(cudaSetDevice(h->device));
+  return target ? icp_set_target(h, *f, pts, nrm, n, on_device) : icp_set_source(h, *f, pts, n, on_device);
 }
 
 }  // namespace
@@ -766,19 +763,18 @@ const char* sm_version(void) { return "sm_b200 0.1 (sm_90a)"; }
 int sm_create(int type, int device, sm_handle** out) {
   if (!out) return SM_ERR_BAD_ARGUMENT;
   *out = nullptr;
-  if (type != SM_TYPE_FAST_ICP && type != SM_TYPE_NDT && type != SM_TYPE_NDT_WITH_GICP && type != SM_TYPE_ICP_PM)
-    return SM_ERR_UNSUPPORTED_TYPE;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  if (device < 0 || device >= ndev) return SM_ERR_BAD_ARGUMENT;
-  sm_handle* h = new sm_handle();
+  sm_handle* h = new sm_handle();   // its state objects allocate nothing until they are used
+  if (type == SM_TYPE_FAST_ICP) h->m.emplace<IcpFastMatcher>();
+  else if (type == SM_TYPE_NDT) h->m.emplace<NdtMatcher>();
+  else if (type == SM_TYPE_NDT_WITH_GICP) h->m.emplace<NdtGicpMatcher>();
+  else if (type == SM_TYPE_ICP_PM) h->m.emplace<PmMatcher>();
+  const int rc = h->m.index() == 0 ? SM_ERR_UNSUPPORTED_TYPE : select_device(device);
+  if (rc < 0) { delete h; return rc; }
   h->type = type;
   h->device = device;
-  if (type == SM_TYPE_ICP_PM) h->icp.max_iteration = 150;   // CounterTransformationChecker, icp_pointmatcher.cc:214
-  memset(&h->info, 0, sizeof(h->info));
-  if (cudaSetDevice(device) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaMallocHost((void**)&h->fast.host_state, sizeof(IcpState)) != cudaSuccess ||
+  IcpFastMatcher* f = h->icp_chain();
+  if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
+      (f && cudaMallocHost((void**)&f->host_state, sizeof(IcpState)) != cudaSuccess) ||
       cudaHostAlloc((void**)&h->host, sizeof(HostBlock), cudaHostAllocMapped) != cudaSuccess ||
       cudaHostGetDevicePointer((void**)&h->host_dev, h->host, 0) != cudaSuccess ||
       cudaMallocHost((void**)&h->host_guess, 16 * sizeof(double)) != cudaSuccess) {
@@ -828,17 +824,17 @@ int sm_set_option(sm_handle* h, const char* name, const char* text) {
 
 int sm_set_inner_compensation(sm_handle* h, int32_t enable) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
-  h->inner_compensation = enable != 0;
+  if (IcpFastMatcher* f = h->as<IcpFastMatcher>()) f->inner_compensation = enable != 0;   // the other types ignore it
   return SM_OK;
 }
 
 int sm_set_ndt_search_method(sm_handle* h, int32_t method) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
-  if (h->type != SM_TYPE_NDT)
-    return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetNeighborhoodSearchMethod: registrator::Ndt (type 5) only");
+  NdtMatcher* m = h->as<NdtMatcher>();
+  if (!m) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetNeighborhoodSearchMethod: registrator::Ndt (type 5) only");
   if (method < SM_NDT_KDTREE || method > SM_NDT_DIRECT1)
     return fail(h, SM_ERR_BAD_ARGUMENT, "SetNeighborhoodSearchMethod: method must be 0..3");
-  h->ndt.search = method;
+  m->opt.search = method;
   return SM_OK;
 }
 
@@ -862,13 +858,13 @@ int sm_print_options(sm_handle* h, char* buf, int64_t buf_len) {
   return (int)out.size();
 }
 
-int sm_set_input_source(sm_handle* h, const double* p, int64_t n) { return set_source(h, p, n, false); }
-int sm_set_input_source_device(sm_handle* h, const double* p, int64_t n) { return set_source(h, p, n, true); }
+int sm_set_input_source(sm_handle* h, const double* p, int64_t n) { return set_f64(h, false, false, p, n); }
+int sm_set_input_source_device(sm_handle* h, const double* p, int64_t n) { return set_f64(h, false, true, p, n); }
 int sm_set_input_target(sm_handle* h, const double* p, const double* nrm, int64_t n) {
-  return set_target(h, p, nrm, n, false);
+  return set_f64(h, true, false, p, n, nrm);
 }
 int sm_set_input_target_device(sm_handle* h, const double* p, const double* nrm, int64_t n) {
-  return set_target(h, p, nrm, n, true);
+  return set_f64(h, true, true, p, n, nrm);
 }
 
 int sm_set_input_source_f32(sm_handle* h, const float* xyz, int64_t n, int64_t stride) {
@@ -887,24 +883,27 @@ int sm_set_input_target_f32_device(sm_handle* h, const float* xyz, int64_t n, in
 int sm_align(sm_handle* h, const double* guess, double* result) {
   if (!h || !guess || !result) return SM_ERR_BAD_ARGUMENT;
   if (cudaSetDevice(h->device) != cudaSuccess) return fail(h, SM_ERR_CUDA, "cudaSetDevice failed");
-  if (h->type == SM_TYPE_FAST_ICP) return icp_align(h, guess, result);
-  if (h->type == SM_TYPE_NDT) return ndt_align(h, guess, result);
-  if (h->type == SM_TYPE_NDT_WITH_GICP) return ndt_gicp_align(h, guess, result);
-  if (h->type == SM_TYPE_ICP_PM) return pm_align(h, guess, result);
+  if (IcpFastMatcher* m = h->as<IcpFastMatcher>()) return icp_align(h, *m, guess, result);
+  if (NdtMatcher* m = h->as<NdtMatcher>()) return ndt_align(h, *m, guess, result);
+  if (NdtGicpMatcher* m = h->as<NdtGicpMatcher>()) return ndt_gicp_align(h, *m, guess, result);
+  if (PmMatcher* m = h->as<PmMatcher>()) return pm_align(h, *m, guess, result);
   return fail(h, SM_ERR_UNSUPPORTED_TYPE, "matcher type not supported");
 }
 
 int sm_align_async(sm_handle* h, const double* guess) {
   if (!h || !guess) return SM_ERR_BAD_ARGUMENT;
+  IcpFastMatcher* f = h->as<IcpFastMatcher>();
+  if (!f) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "sm_align_async: IcpFast only");
   if (cudaSetDevice(h->device) != cudaSuccess) return fail(h, SM_ERR_CUDA, "cudaSetDevice failed");
-  if (h->type != SM_TYPE_FAST_ICP) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "sm_align_async: IcpFast only");
-  return icp_begin(h, guess);
+  return icp_begin(h, *f, guess);
 }
 
 int sm_align_wait(sm_handle* h, double* result) {
   if (!h || !result) return SM_ERR_BAD_ARGUMENT;
+  IcpFastMatcher* f = h->as<IcpFastMatcher>();
+  if (!f) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "sm_align_wait: IcpFast only");
   if (cudaSetDevice(h->device) != cudaSuccess) return fail(h, SM_ERR_CUDA, "cudaSetDevice failed");
-  return icp_end(h, result);
+  return icp_end(h, *f, result);
 }
 
 int sm_align_batch(sm_handle* const* handles, int32_t n, const double* guesses_16n, double* results_16n,
@@ -917,9 +916,10 @@ int sm_align_batch(sm_handle* const* handles, int32_t n, const double* guesses_1
   for (int i = 0; i < n; ++i) {
     sm_handle* h = handles[i];
     rc_n[i] = 0;
-    if (h->type != SM_TYPE_FAST_ICP) { other.push_back(i); continue; }
+    IcpFastMatcher* f = h->as<IcpFastMatcher>();
+    if (!f) { other.push_back(i); continue; }
     if (cudaSetDevice(h->device) != cudaSuccess) { rc_n[i] = fail(h, SM_ERR_CUDA, "cudaSetDevice failed"); continue; }
-    rc_n[i] = icp_begin(h, guesses_16n + 16 * (size_t)i);
+    rc_n[i] = icp_begin(h, *f, guesses_16n + 16 * (size_t)i);
   }
   // the other matchers drive their optimiser from the host (Newton / BFGS steps with a read-back
   // each): one worker thread per instance, at most 16 at a time, like the reference's thread pool
@@ -937,9 +937,10 @@ int sm_align_batch(sm_handle* const* handles, int32_t n, const double* guesses_1
     });
   for (int i = 0; i < n; ++i) {
     sm_handle* h = handles[i];
-    if (h->type != SM_TYPE_FAST_ICP || rc_n[i] < 0) continue;
+    IcpFastMatcher* f = h->as<IcpFastMatcher>();
+    if (!f || rc_n[i] < 0) continue;
     if (cudaSetDevice(h->device) != cudaSuccess) { rc_n[i] = SM_ERR_CUDA; continue; }
-    rc_n[i] = icp_end(h, results_16n + 16 * (size_t)i);
+    rc_n[i] = icp_end(h, *f, results_16n + 16 * (size_t)i);
   }
   for (std::thread& t : workers) t.join();
   int worst = 0;
@@ -950,8 +951,9 @@ int sm_align_batch(sm_handle* const* handles, int32_t n, const double* guesses_1
 int sm_align_pairs(sm_handle* const* handles, int32_t n_handles, const sm_pair* pairs, int32_t n_pairs,
                    double* results_16n, double* scores_n, int32_t* rc_n) {
   if (!handles || n_handles <= 0 || !pairs || n_pairs < 0 || !results_16n || !rc_n) return SM_ERR_BAD_ARGUMENT;
-  for (int i = 0; i < n_handles; ++i)
-    if (!handles[i] || handles[i]->type != SM_TYPE_FAST_ICP) return SM_ERR_UNSUPPORTED_TYPE;
+  for (int i = 0; i < n_handles; ++i)   // fail() leaves a null handle alone
+    if (!handles[i] || !handles[i]->as<IcpFastMatcher>())
+      return fail(handles[i], SM_ERR_UNSUPPORTED_TYPE, "sm_align_pairs: IcpFast only");
   NvtxRange nvtx("sm_align_pairs");
   static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   std::vector<int> in_flight((size_t)n_handles, -1);     // pair index a pipeline is working on
@@ -960,22 +962,23 @@ int sm_align_pairs(sm_handle* const* handles, int32_t n_handles, const sm_pair* 
     if (k < 0) return;
     sm_handle* h = handles[hi];
     cudaSetDevice(h->device);
-    rc_n[k] = icp_end(h, results_16n + 16 * (size_t)k);
+    rc_n[k] = icp_end(h, *h->as<IcpFastMatcher>(), results_16n + 16 * (size_t)k);
     if (scores_n) scores_n[k] = h->final_score;
     in_flight[(size_t)hi] = -1;
   };
   for (int k = 0; k < n_pairs; ++k) {
     const int hi = k % n_handles;
     sm_handle* h = handles[hi];
+    IcpFastMatcher& f = *h->as<IcpFastMatcher>();
     collect(hi);                                          // the pipeline's previous pair
     const sm_pair& pr = pairs[k];
     rc_n[k] = 0;
     if (scores_n) scores_n[k] = 0.0;
     if (cudaSetDevice(h->device) != cudaSuccess) { rc_n[k] = fail(h, SM_ERR_CUDA, "cudaSetDevice failed"); continue; }
     const bool dev = pr.on_device != 0;
-    int rc = set_target(h, pr.target_3xn, pr.target_normals_3xn, pr.n_target, dev, !dev);
-    if (rc >= 0) rc = set_source(h, pr.source_3xn, pr.n_source, dev, !dev);
-    if (rc >= 0) rc = icp_begin(h, pr.guess_4x4 ? pr.guess_4x4 : kIdentity);
+    int rc = icp_set_target(h, f, pr.target_3xn, pr.target_normals_3xn, pr.n_target, dev, !dev);
+    if (rc >= 0) rc = icp_set_source(h, f, pr.source_3xn, pr.n_source, dev, !dev);
+    if (rc >= 0) rc = icp_begin(h, f, pr.guess_4x4 ? pr.guess_4x4 : kIdentity);
     if (rc < 0) { rc_n[k] = rc; continue; }
     in_flight[(size_t)hi] = k;
   }
@@ -999,8 +1002,9 @@ const char* sm_last_error(const sm_handle* h) { return h ? h->error.c_str() : "n
 // Diagnostics, not part of include/sm_b200.h: clock64 stamps of the sections of the last
 // icp_finish_kernel of the last IcpFast Align (profiles/finish_sections.py).
 int sm_debug_icp_stamps(const sm_handle* h, long long* out12) {
-  if (!h || !out12 || !h->fast.host_state) return SM_ERR_BAD_ARGUMENT;
-  for (int i = 0; i < 12; ++i) out12[i] = h->fast.host_state->stamps[i];
+  const IcpFastMatcher* f = h ? const_cast<sm_handle*>(h)->icp_chain() : nullptr;
+  if (!f || !out12 || !f->host_state) return SM_ERR_BAD_ARGUMENT;
+  for (int i = 0; i < 12; ++i) out12[i] = f->host_state->stamps[i];
   return SM_OK;
 }
 
@@ -1008,9 +1012,7 @@ int sm_calculate_normals(int device, const double* points, int64_t n, double* ou
                          double* out_normals, int64_t* m_out) {
   if (!points || !out_points || !out_normals || !m_out || n <= 0 || n > (1 << 30))
     return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   cudaStream_t s = nullptr;
   NormalsPipeline np;
   DevBuf stage;
@@ -1049,9 +1051,7 @@ static int knn1_impl(int device, const double* target, int64_t nt, const double*
   if (!target || !query || nt <= 0 || nt > (1 << 30) || nq < 0 || nq > (1 << 30) || bucket < 2 || bucket > 8 ||
       !(epsilon >= 0.0))
     return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   cudaStream_t s = nullptr;
   const int64_t ts = pad64(nt), qs = pad64(nq > 0 ? nq : 1);
   const int levels = kd_num_levels((int)nt, bucket);

@@ -32,9 +32,7 @@ extern "C" {
 
 int sm_debug_solve6(int device, const double* A, const double* b, double* x, int32_t* path) {
   if (!A || !b || !x || !path) return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   DevBuf buf;
   SMB_RC(buf.reserve(64 * sizeof(double)));
   double* d = (double*)buf.p;
@@ -276,13 +274,6 @@ int sm_debug_bfgs_minimize(sm_debug_fdf fn, void* user, double* x, double grad_t
 
 // ---- test hooks of the Ndt / NdtWithGicp device stages (include/sm_b200_debug.h) ------------------------------------
 // Each runs the product's own launch functions on buffers of its own, on the default stream, with no handle.
-static int debug_set_device(int device) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  if (device < 0 || device >= ndev) return SM_ERR_BAD_ARGUMENT;
-  SMB_CUDA_OK(cudaSetDevice(device));
-  return SM_OK;
-}
 
 // a packed float xyz cloud of n points copied into buf
 static int debug_upload_f32(const float* pts, int64_t n, DevBuf& buf) {
@@ -309,7 +300,7 @@ int sm_debug_ndt_grid(int device, const float* target_3n, int64_t n, float resol
   if (!debug_cloud_ok(target_3n, n) || !(resolution > 0.0f) || !n_voxels || !overflow || !key || !nr_points ||
       !searchable || !mean_3 || !icov_9 || !centroid_3)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DevBuf tgt;
   NdtStage st;
   NdtGrid g;
@@ -336,7 +327,7 @@ int sm_debug_ndt_derivatives(int device, const float* target_3n, int64_t nt, con
   if (!debug_cloud_ok(target_3n, nt) || !debug_cloud_ok(source_3n, ns) || !(resolution > 0.0f) || !p_6k ||
       n_poses <= 0 || !sums_44k)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DevBuf tgt, src;
   NdtStage st;
   NdtGrid g;
@@ -358,7 +349,7 @@ int sm_debug_ndt_derivatives_search(int device, const float* target_3n, int64_t 
   if (!debug_cloud_ok(target_3n, nt) || !debug_cloud_ok(source_3n, ns) || !(resolution > 0.0f) || !p_6k ||
       n_poses <= 0 || !sums_44k || search_method < SM_NDT_KDTREE || search_method > SM_NDT_DIRECT1)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DevBuf tgt, src;
   NdtStage st;
   NdtGrid g;
@@ -406,7 +397,7 @@ int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const 
   if (!debug_cloud_ok(cloud_3n, n) || !query_3m || nq <= 0 || nq > (1 << 24) || (k != 1 && k != 20) || !ids || !d2 ||
       kd_num_levels((int)n, 8) > 24)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DevBuf cloud, kdws, q, ids_d, d2_d;
   FloatTree t;
   SMB_RC(debug_upload_f32(cloud_3n, n, cloud));
@@ -424,7 +415,7 @@ int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const 
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,
                                int64_t* m_out) {
   if (!debug_cloud_ok(points_3n, n) || !(leaf > 0.0f) || !out_3n || !m_out) return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DevBuf pts, out;
   ApproxVoxelGrid filter;
   SMB_RC(debug_upload_f32(points_3n, n, pts));
@@ -437,7 +428,7 @@ int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, fl
 
 int sm_debug_gicp_covariances(int device, const float* cloud_3n, int64_t n, double* covs_9n) {
   if (!debug_cloud_ok(cloud_3n, n) || !covs_9n || kd_num_levels((int)n, 8) > 24) return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DevBuf cloud, kdws;
   gicp::Stage g;                       // the cloud as the stage's source
   SMB_RC(debug_upload_f32(cloud_3n, n, cloud));
@@ -455,7 +446,7 @@ int sm_debug_gicp_step(int device, const float* source_3n, int64_t ns, const flo
       !x_6k || n_states <= 0 || !match || !maha_9n || !count || !sums_13k || kd_num_levels((int)ns, 8) > 24 ||
       kd_num_levels((int)nt, 8) > 24)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   const gicp::Options o;
   DevBuf src, tgt, kdws;
   FloatTree tt;
@@ -512,7 +503,7 @@ int sm_debug_m2dp_stages(int device, const float* points, int64_t n, int64_t str
   if (!points || n <= 0 || n > (1ll << 30) || stride_bytes < 12 || stride_bytes % 4 || !mean_3 || !cov_sums_6 ||
       !cov_6 || !E_9 || !views_6r || !A || !gram || !descriptor || sm_m2dp_descriptor_length(r, max_distance, t, p, q) < 0)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   M2dpStage st;
   SMB_RC(st.run(points, n, stride_bytes, r, max_distance, t, p, q, nullptr));
   memcpy(mean_3, st.mean, sizeof(st.mean));
@@ -532,7 +523,7 @@ int sm_debug_radix_sort(int device, const uint64_t* keys, const uint32_t* vals, 
   if (!keys || !vals || !keys_out || !vals_out || n <= 0 || n > (1 << 30) || batch < 1 || batch > 16 || stride < n ||
       stride > (1 << 30) || passes < 1 || passes > 8)
     return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   const size_t words = (size_t)batch * (size_t)stride;
   DevBuf k, v, scratch;
   SMB_RC(k.reserve(2 * words * sizeof(uint64_t)));
@@ -613,7 +604,7 @@ int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* fi
   if ((variant == 2 && bucket != 7) || (variant == 3 && (bucket != 8 || !bpts))) return SM_ERR_BAD_ARGUMENT;
   const int lv = kd_num_levels((int)n, bucket);
   if (lv != levels || lv > 24 || (n_first > 0 && kd_num_levels((int)n_first, bucket) > 24)) return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   DebugKdOwners o;
   if (n_first > 0) SMB_RC(debug_kd_build(o, variant, bucket, first_3n, first_normals_3n, n_first));
   SMB_RC(debug_kd_build(o, variant, bucket, cloud_3n, normals_3n, n));
@@ -685,7 +676,7 @@ int sm_debug_filter_ground_removal2(int device, const sm_filter_chain* chain, in
     return SM_ERR_BAD_ARGUMENT;
   const FilterParams& f = fc->filters[filter];
   if (f.bin_num <= 0 || max_lines != f.bin_num / 2 + 1) return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(debug_set_device(device));
+  SMB_RC(select_device(device));
   FilterChain one;
   one.filters.push_back(f);
   DevBuf in, out;

@@ -154,9 +154,7 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   if (!points || !out || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 16 || stride_bytes % 4 ||
       !(voxel_size > 1.e-6f))       // ConfigsValid(), filter_voxel_grid.cc:35
     return SM_ERR_BAD_ARGUMENT;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) return SM_ERR_NO_DEVICE;
-  SMB_CUDA_OK(cudaSetDevice(device));
+  SMB_RC(select_device(device));
   *m_out = 0;
   if (n == 0) return SM_OK;
   const int ni = (int)n;
