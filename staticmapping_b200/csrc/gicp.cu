@@ -21,6 +21,7 @@
 #include "icp_dev.cuh"
 #include "kernels.h"
 #include "linalg_dev.cuh"
+#include "reduce.cuh"
 
 namespace smb {
 using namespace dev;
@@ -327,20 +328,8 @@ gicp_cost_kernel(const float* __restrict__ src, int ns, const float* __restrict_
       cost_terms(P.T, P.base, src + 3 * (int64_t)i, tgt + 3 * (int64_t)j, maha + 9 * (int64_t)i, acc);
     }
   }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kCostSums; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) red[w][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < kCostSums) {
-    double v = 0.0;
-    for (int ww = 0; ww < 8; ++ww) v += red[ww][threadIdx.x];
-    partials[(int64_t)blockIdx.x * kCostSums + threadIdx.x] = v;
-  }
+  const double v = block_sum<kCostSums, 256>(acc, red);
+  if (threadIdx.x < kCostSums) partials[(int64_t)blockIdx.x * kCostSums + threadIdx.x] = v;
   // The block that finishes last reduces the partial sums (fixed order: the same tree whichever block
   // it is) and hands the 13 results to the host through mapped pinned memory: one launch and no copy per
   // BFGS evaluation (31 per alignment) instead of two launches, a copy and a stream synchronisation.
@@ -350,13 +339,9 @@ gicp_cost_kernel(const float* __restrict__ src, int ns, const float* __restrict_
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  const int nblocks = (int)gridDim.x;
-  for (int k = w; k < kCostSums; k += 8) {
-    double v = 0.0;
-    for (int b = lane; b < nblocks; b += 32) v += *reinterpret_cast<volatile const double*>(partials + (int64_t)b * kCostSums + k);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) { sums[k] = v; if (host_sums) host_sums[k] = v; }
+  for (int k = threadIdx.x >> 5; k < kCostSums; k += 8) {
+    const double v = warp_sum_rows(reinterpret_cast<volatile const double*>(partials), (int)gridDim.x, kCostSums, k);
+    if ((threadIdx.x & 31) == 0) { sums[k] = v; if (host_sums) host_sums[k] = v; }
   }
   __syncthreads();
   if (threadIdx.x == 0) {

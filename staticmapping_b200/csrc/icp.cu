@@ -31,24 +31,15 @@ constexpr int kMeanChunk = 1024;   // target points per mean_partial_kernel bloc
 __global__ void __launch_bounds__(256)
 mean_partial_kernel(const double* __restrict__ raw, int64_t stride, int n,
                     double* __restrict__ partials) {
-  __shared__ double sm[3][8];
+  __shared__ double red[8][3];
   double s[3] = {0.0, 0.0, 0.0};
   const int base = blockIdx.x * kMeanChunk;
   for (int r = 0; r < 4; ++r) {
     const int i = base + r * 256 + threadIdx.x;
     if (i < n) { s[0] += raw[i]; s[1] += raw[stride + i]; s[2] += raw[2 * stride + i]; }
   }
-  for (int d = 0; d < 3; ++d) {
-    double v = s[d];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) sm[d][threadIdx.x >> 5] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 3) {
-    double v = 0.0;
-    for (int w = 0; w < 8; ++w) v += sm[threadIdx.x][w];
-    partials[blockIdx.x * 4 + threadIdx.x] = v;
-  }
+  const double v = block_sum<3, 256>(s, red);
+  if (threadIdx.x < 3) partials[blockIdx.x * 4 + threadIdx.x] = v;
 }
 
 __global__ void __launch_bounds__(256)

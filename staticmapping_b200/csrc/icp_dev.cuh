@@ -5,6 +5,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace smb {
 namespace dev {
@@ -235,25 +236,15 @@ struct BinSel { int bin; int below; int qi; int nvalid; };
 // every block locates the quantile bin from the global histogram (2048 bins, 8 per thread
 // on the first 256 threads; all threads of the block must call this)
 __device__ __forceinline__ BinSel select_bin(const uint32_t* __restrict__ ghist, float ratio,
-                                             uint32_t* warp_tot /*[8]*/, BinSel* out_sm) {
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+                                             uint32_t* warp_tot /*one per warp*/, BinSel* out_sm) {
+  const int t = threadIdx.x;
   const bool active = t < 256;
   uint32_t c[8], s = 0;
 #pragma unroll
   for (int k = 0; k < 8; ++k) { c[k] = active ? ghist[t * 8 + k] : 0u; s += c[k]; }
-  uint32_t incl = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += v;
-  }
-  if (active && lane == 31) warp_tot[w] = incl;
   if (t == 0) { out_sm->bin = -1; out_sm->below = 0; out_sm->qi = 0; out_sm->nvalid = 0; }   // never left unset
-  __syncthreads();
-  uint32_t base = 0, total = 0;
-#pragma unroll
-  for (int ww = 0; ww < 8; ++ww) { const uint32_t v = warp_tot[ww]; if (ww < w) base += v; total += v; }
-  const uint32_t excl = base + incl - s;
+  uint32_t total;
+  const uint32_t excl = block_scan_excl<8>(s, warp_tot, &total);
   // icp_fast.cc:82-89: quantile == 1.0 -> max element, else index int(size * quantile)
   const double q = (double)ratio;
   int qi = (q == 1.0) ? (int)total - 1 : (int)((double)total * q);

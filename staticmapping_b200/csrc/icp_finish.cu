@@ -60,9 +60,7 @@ __device__ __forceinline__ int solve_warp(SolveSmem& sm, int lane) {
   const int lj = l20 - tri(li, 0);
   // S holds the upper triangle row-major: A(i,j) with i >= j is entry (j, i)
   double a = sm.S[lj * 6 - (lj * (lj - 1)) / 2 + (li - lj)];
-  double trace = (li == lj && lane < 21) ? a : 0.0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) trace += __shfl_xor_sync(0xffffffffu, trace, o);
+  const double trace = warp_sum((li == lj && lane < 21) ? a : 0.0);
   // The dependent chain of the whole solve is its square roots and divisions (a double-precision
   // sqrt or divide is a ~20-instruction dependent sequence), so each pivot costs ONE such
   // sequence: r = 1/sqrt(d) gives l_kk = d*r and every later division by l_kk is a multiplication
@@ -220,30 +218,6 @@ __device__ __forceinline__ void update_pose(IcpState* st, const IcpParams& p, So
   }
 }
 
-// block-wide exclusive scan of one value per thread (the <= 32 warp totals are themselves
-// scanned by one shuffle pass in every warp)
-__device__ __forceinline__ uint32_t block_scan_excl(uint32_t v, uint32_t* warp_tot, uint32_t& total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += u;
-  }
-  __syncthreads();              // previous users of warp_tot are done
-  if (lane == 31) warp_tot[w] = incl;
-  __syncthreads();
-  const uint32_t x = lane < kSelWarps ? warp_tot[lane] : 0u;
-  uint32_t xi = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t u = __shfl_up_sync(0xffffffffu, xi, o);
-    if (lane >= o) xi += u;
-  }
-  total = __shfl_sync(0xffffffffu, xi, 31);
-  return __shfl_sync(0xffffffffu, xi - x, w) + incl - v;
-}
-
 // exclusive scan of the candidate counts of blocks [base, base + kSelThreads) into
 // blk_off[0..kSelThreads] (the last entry = number of candidates in the chunk)
 __device__ __forceinline__ void scan_chunk(const uint32_t* __restrict__ cand_cnt, int base, int nblocks,
@@ -253,8 +227,8 @@ __device__ __forceinline__ void scan_chunk(const uint32_t* __restrict__ cand_cnt
   const int blk = base + t;
   const uint32_t c = (have_cnt0 && base == 0) ? cnt0 : (blk < nblocks ? cand_cnt[blk] : 0);
   uint32_t tot;
-  const uint32_t excl = block_scan_excl(c, warp_tot, tot);   // syncs before touching warp_tot
-  blk_off[t] = excl;
+  __syncthreads();              // previous users of warp_tot are done
+  blk_off[t] = block_scan_excl<kSelWarps>(c, warp_tot, &tot);
   if (t == 0) blk_off[kSelThreads] = tot;
   __syncthreads();
 }
@@ -339,8 +313,8 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
     static_assert(kSelThreads * 4 == kHistBins, "4 second-level bins per thread");
     const uint32_t c[4] = {cq.x, cq.y, cq.z, cq.w};
     const uint32_t s = c[0] + c[1] + c[2] + c[3];
-    uint32_t tot2;
-    uint32_t run = block_scan_excl(s, warp_tot, tot2);
+    __syncthreads();            // previous users of warp_tot are done
+    uint32_t run = block_scan_excl<kSelWarps>(s, warp_tot);
     if ((uint32_t)r >= run && (uint32_t)r < run + s) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
@@ -434,13 +408,7 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
         uint32_t c[8], s = 0;
 #pragma unroll
         for (int k = 0; k < 8; ++k) { c[k] = sh_hist[lane * 8 + k]; s += c[k]; }
-        uint32_t incl = s;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
-          if (lane >= o) incl += v;
-        }
-        const uint32_t excl = incl - s;
+        const uint32_t excl = warp_inclusive_scan(s) - s;
         const uint32_t rk = (uint32_t)sh_rank;
         __syncwarp();
         if (rk >= excl && rk < excl + s) {

@@ -66,7 +66,7 @@ pm_score_knn_kernel(const float* __restrict__ src, int n, const double* __restri
 // keys sorted ascending; out[0] = mean of sqrt(d2) over the kept matches, out[1] = kept, out[2] = valid
 __global__ void __launch_bounds__(1024)
 pm_score_reduce_kernel(const uint64_t* __restrict__ keys, int n, float ratio, double* __restrict__ out) {
-  __shared__ double red[32];
+  __shared__ double red[32][1];
   __shared__ int s_kept, s_valid;
   const uint64_t inf_bits = 0x7ff0000000000000ull;
   if (threadIdx.x == 0) {
@@ -89,12 +89,8 @@ pm_score_reduce_kernel(const uint64_t* __restrict__ keys, int n, float ratio, do
   const int kept = s_kept;
   double v = 0.0;
   for (int i = threadIdx.x; i < kept; i += 1024) v += sqrt(__longlong_as_double((long long)keys[i]));
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
+  const double t = block_sum<1, 1024>(&v, red);
   if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < 32; ++w) t += red[w];
     out[0] = kept > 0 ? t / (double)kept : 0.0;
     out[1] = (double)kept;
     out[2] = (double)s_valid;

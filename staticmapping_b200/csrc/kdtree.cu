@@ -13,6 +13,7 @@
 //   * ties are broken by the total order (coordinate, original index).
 #include "common.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace smb {
 namespace {
@@ -154,23 +155,8 @@ kd_part_count_kernel(const uint32_t* __restrict__ lists, int64_t lstride, int n,
     isleft[r] = f;
     cnt += f;
   }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = cnt;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += t;
-  }
-  if (lane == 31) warp_sums[w] = incl;
-  __syncthreads();
-  uint32_t wbase = 0, total = 0;
-#pragma unroll
-  for (int ww = 0; ww < kPartThreads / 32; ++ww) {
-    const uint32_t v = warp_sums[ww];
-    if (ww < w) wbase += v;
-    total += v;
-  }
-  uint32_t run = wbase + incl - cnt;
+  uint32_t total;
+  uint32_t run = block_scan_excl<kPartThreads / 32>(cnt, warp_sums, &total);
 #pragma unroll
   for (int r = 0; r < kPartItems; ++r) {
     const int i = base + r;
@@ -192,16 +178,8 @@ kd_part_scatter_kernel(const uint32_t* __restrict__ lists, uint32_t* __restrict_
   __shared__ uint32_t s_warp[kPartThreads / 32];
   const int d = blockIdx.y;
   if (FUSED_SCAN) {
-    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-    const uint32_t c = t < nblk ? block_off[d * nblk + t] : 0u;
-    uint32_t incl = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-    if (lane == 31) s_warp[w] = incl;
-    __syncthreads();
-    uint32_t wb = 0;
-    for (int ww = 0; ww < w; ++ww) wb += s_warp[ww];
-    s_off[t] = wb + incl - c;
+    const int t = threadIdx.x;
+    s_off[t] = block_scan_excl<kPartThreads / 32>(t < nblk ? block_off[d * nblk + t] : 0u, s_warp);
     __syncthreads();
   }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -363,9 +341,7 @@ kd_subtree_kernel(const double* __restrict__ coord, int64_t cstride, uint32_t* _
         isleft[r] = (i < count0 && it_inner[r]) ? (flag[pid[r]] == 0 ? 1u : 0u) : 1u;
         cnt += isleft[r];
       }
-      uint32_t incl = cnt;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+      const uint32_t incl = warp_inclusive_scan(cnt);
       if (lane == 31) s_warp[w] = incl;
       __syncthreads();
       uint32_t wb = 0;

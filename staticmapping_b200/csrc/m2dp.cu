@@ -37,6 +37,7 @@
 #include "../../include/sm_b200.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace smb {
 namespace {
@@ -55,30 +56,21 @@ struct M2dpParams {
 
 __global__ void __launch_bounds__(256)
 m2dp_mean_kernel(const char* __restrict__ pts, int64_t stride, int64_t n, double* __restrict__ sums) {
-  __shared__ double sm[3][8];
+  __shared__ double red[8][3];
   double s[3] = {0.0, 0.0, 0.0};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float* p = reinterpret_cast<const float*>(pts + i * stride);
     s[0] += (double)p[0]; s[1] += (double)p[1]; s[2] += (double)p[2];
   }
-  for (int d = 0; d < 3; ++d) {
-    double v = s[d];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) sm[d][threadIdx.x >> 5] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 3) {
-    double v = 0.0;
-    for (int w = 0; w < 8; ++w) v += sm[threadIdx.x][w];
-    atomicAdd(&sums[threadIdx.x], v);
-  }
+  const double v = block_sum<3, 256>(s, red);
+  if (threadIdx.x < 3) atomicAdd(&sums[threadIdx.x], v);
 }
 
 // covariance sums of the float-demeaned cloud (pcl::demeanPointCloud works in float)
 __global__ void __launch_bounds__(256)
 m2dp_cov_kernel(const char* __restrict__ pts, int64_t stride, int64_t n, float cx, float cy, float cz,
                 double* __restrict__ sums) {
-  __shared__ double sm[6][8];
+  __shared__ double red[8][6];
   double s[6] = {0, 0, 0, 0, 0, 0};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float* p = reinterpret_cast<const float*>(pts + i * stride);
@@ -86,17 +78,8 @@ m2dp_cov_kernel(const char* __restrict__ pts, int64_t stride, int64_t n, float c
     s[0] += (double)(x * x); s[1] += (double)(x * y); s[2] += (double)(x * z);
     s[3] += (double)(y * y); s[4] += (double)(y * z); s[5] += (double)(z * z);
   }
-  for (int d = 0; d < 6; ++d) {
-    double v = s[d];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) sm[d][threadIdx.x >> 5] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 6) {
-    double v = 0.0;
-    for (int w = 0; w < 8; ++w) v += sm[threadIdx.x][w];
-    atomicAdd(&sums[threadIdx.x], v);
-  }
+  const double v = block_sum<6, 256>(s, red);
+  if (threadIdx.x < 6) atomicAdd(&sums[threadIdx.x], v);
 }
 
 // grid: (point chunks, view groups of P.views_per_cta).  Dynamic shared memory: views_per_cta * cols ints.
@@ -153,17 +136,13 @@ int hist_views_per_cta(int cols, int* vpc) {
 // G = A A^T (rows x rows) in double; one block per (a, b-tile)
 __global__ void __launch_bounds__(256)
 m2dp_gram_kernel(const int* __restrict__ A, int rows, int cols, double* __restrict__ G) {
-  __shared__ double red[8];
+  __shared__ double red[8][1];
   const int a = blockIdx.x, b = blockIdx.y;
   if (b < a) return;
   double s = 0.0;
   for (int k = threadIdx.x; k < cols; k += 256) s += (double)A[(int64_t)a * cols + k] * (double)A[(int64_t)b * cols + k];
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
+  const double t = block_sum<1, 256>(&s, red);   // integer-valued partial sums < 2^53: exact in any order
   if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int w = 0; w < 8; ++w) t += red[w];        // integer-valued partial sums < 2^53: exact in any order
     G[(int64_t)a * rows + b] = t; G[(int64_t)b * rows + a] = t;
   }
 }

@@ -25,6 +25,7 @@
 #include "icp_dev.cuh"
 #include "kernels.h"
 #include "linalg_dev.cuh"
+#include "reduce.cuh"
 
 namespace smb {
 using namespace dev;
@@ -54,45 +55,29 @@ __host__ __device__ __forceinline__ int grid_too_large(const float* mn, const fl
 
 __global__ void __launch_bounds__(256)
 ndt_minmax_partial_kernel(const float* __restrict__ pts, int n, float* __restrict__ partial) {
-  __shared__ float smn[3][8], smx[3][8];
   float mn[3] = {3.402823466e38f, 3.402823466e38f, 3.402823466e38f};
   float mx[3] = {-3.402823466e38f, -3.402823466e38f, -3.402823466e38f};
   for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256)
     for (int d = 0; d < 3; ++d) { const float v = pts[3 * (int64_t)i + d]; mn[d] = fminf(mn[d], v); mx[d] = fmaxf(mx[d], v); }
-  for (int d = 0; d < 3; ++d) {
-    for (int o = 16; o > 0; o >>= 1) {
-      mn[d] = fminf(mn[d], __shfl_xor_sync(0xffffffffu, mn[d], o));
-      mx[d] = fmaxf(mx[d], __shfl_xor_sync(0xffffffffu, mx[d], o));
-    }
-    if ((threadIdx.x & 31) == 0) { smn[d][threadIdx.x >> 5] = mn[d]; smx[d][threadIdx.x >> 5] = mx[d]; }
-  }
-  __syncthreads();
+  const float2 r = block_minmax3<256>(mn, mx);
   if (threadIdx.x < 3) {
-    float a = smn[threadIdx.x][0], b = smx[threadIdx.x][0];
-    for (int w = 1; w < 8; ++w) { a = fminf(a, smn[threadIdx.x][w]); b = fmaxf(b, smx[threadIdx.x][w]); }
-    partial[blockIdx.x * 6 + threadIdx.x] = a;
-    partial[blockIdx.x * 6 + 3 + threadIdx.x] = b;
+    partial[blockIdx.x * 6 + threadIdx.x] = r.x;
+    partial[blockIdx.x * 6 + 3 + threadIdx.x] = r.y;
   }
 }
 
 __global__ void __launch_bounds__(256)
 ndt_grid_params_kernel(const float* __restrict__ partial, int nparts, float resolution, NdtGrid* __restrict__ grid) {
-  __shared__ float smn[3][8], smx[3][8];
   float mn[3] = {3.402823466e38f, 3.402823466e38f, 3.402823466e38f};
   float mx[3] = {-3.402823466e38f, -3.402823466e38f, -3.402823466e38f};
   for (int b = threadIdx.x; b < nparts; b += 256)
     for (int d = 0; d < 3; ++d) { mn[d] = fminf(mn[d], partial[b * 6 + d]); mx[d] = fmaxf(mx[d], partial[b * 6 + 3 + d]); }
-  for (int d = 0; d < 3; ++d) {
-    for (int o = 16; o > 0; o >>= 1) {
-      mn[d] = fminf(mn[d], __shfl_xor_sync(0xffffffffu, mn[d], o));
-      mx[d] = fmaxf(mx[d], __shfl_xor_sync(0xffffffffu, mx[d], o));
-    }
-    if ((threadIdx.x & 31) == 0) { smn[d][threadIdx.x >> 5] = mn[d]; smx[d][threadIdx.x >> 5] = mx[d]; }
-  }
+  __shared__ float2 box[3];
+  const float2 r = block_minmax3<256>(mn, mx);
+  if (threadIdx.x < 3) box[threadIdx.x] = r;
   __syncthreads();
   if (threadIdx.x != 0) return;
-  for (int d = 0; d < 3; ++d)
-    for (int w = 0; w < 8; ++w) { mn[d] = fminf(mn[d], smn[d][w]); mx[d] = fmaxf(mx[d], smx[d][w]); }
+  for (int d = 0; d < 3; ++d) { mn[d] = box[d].x; mx[d] = box[d].y; }
   const float inv = 1.0f / resolution;
   grid->inv_leaf = inv;
   grid->overflow = grid_too_large(mn, mx, inv);
@@ -597,31 +582,15 @@ ndt_derivatives_kernel(const float* __restrict__ src, int n, NdtEvalParams P,
     for (int q = 0; q < 36; ++q) acc[7 + q] = hess_pt[q];
     acc[43] = (double)nc;
   }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < kNdtSums; ++k) {
-    double v = acc[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) red[w][k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < kNdtSums) {
-    double v = 0.0;
-    for (int ww = 0; ww < kNdtThreads / 32; ++ww) v += red[ww][threadIdx.x];
-    partials[(int64_t)blockIdx.x * kNdtSums + threadIdx.x] = v;
-  }
+  const double v = block_sum<kNdtSums, kNdtThreads>(acc, red);
+  if (threadIdx.x < kNdtSums) partials[(int64_t)blockIdx.x * kNdtSums + threadIdx.x] = v;
 }
 
 __global__ void __launch_bounds__(1024)
 ndt_reduce_kernel(const double* __restrict__ partials, int nblocks, int width, double* __restrict__ out) {
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int k = w; k < width; k += 32) {
-    double v = 0.0;
-    for (int b = lane; b < nblocks; b += 32) v += partials[(int64_t)b * width + k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) out[k] = v;
+  for (int k = threadIdx.x >> 5; k < width; k += 32) {
+    const double v = warp_sum_rows(partials, nblocks, width, k);
+    if ((threadIdx.x & 31) == 0) out[k] = v;
   }
 }
 
@@ -641,7 +610,7 @@ ndt_fitness_kernel(const float* __restrict__ src, int n, NdtEvalParams P, const 
                    double* __restrict__ partials) {
   __shared__ double red[8][2];
   const int i = blockIdx.x * 256 + threadIdx.x;
-  double s = 0.0, c = 0.0;
+  double sc[2] = {0.0, 0.0};   // squared distance, match count
   if (i < n) {
     const float xo[3] = {src[3 * (int64_t)i], src[3 * (int64_t)i + 1], src[3 * (int64_t)i + 2]};
     float xt[3];
@@ -651,19 +620,12 @@ ndt_fitness_kernel(const float* __restrict__ src, int n, NdtEvalParams P, const 
     knn1(nodes, bpts, (double)xt[0], (double)xt[1], (double)xt[2], 1.0, slot, d2);
     if (slot >= 0) {
       const long long id = bpts[slot].id;
-      s = (double)dist2f(xt[0], xt[1], xt[2], tgt + 3 * id);
-      c = 1.0;
+      sc[0] = (double)dist2f(xt[0], xt[1], xt[2], tgt + 3 * id);
+      sc[1] = 1.0;
     }
   }
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
-  if (lane == 0) { red[w][0] = s; red[w][1] = c; }
-  __syncthreads();
-  if (threadIdx.x < 2) {
-    double v = 0.0;
-    for (int ww = 0; ww < 8; ++ww) v += red[ww][threadIdx.x];
-    partials[(int64_t)blockIdx.x * 2 + threadIdx.x] = v;
-  }
+  const double v = block_sum<2, 256>(sc, red);
+  if (threadIdx.x < 2) partials[(int64_t)blockIdx.x * 2 + threadIdx.x] = v;
 }
 
 }  // namespace

@@ -8,6 +8,7 @@
 // that (tile, warp, row, lane) order == input order, which is what makes it stable.
 #include "common.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace smb {
 namespace {
@@ -45,27 +46,7 @@ radix_scan_kernel(uint32_t* __restrict__ data, int count) {
   const int lo = min(count, (int)threadIdx.x * per), hi = min(count, lo + per);
   uint32_t s = 0;
   for (int i = lo; i < hi; ++i) s += d[i];
-  // block exclusive scan of s
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  uint32_t incl = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += t;
-  }
-  if (lane == 31) warp_sums[w] = incl;
-  __syncthreads();
-  if (w == 0) {
-    uint32_t v = warp_sums[lane], iv = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, iv, o);
-      if (lane >= o) iv += t;
-    }
-    warp_sums[lane] = iv - v;
-  }
-  __syncthreads();
-  uint32_t run = warp_sums[w] + incl - s;
+  uint32_t run = block_scan_excl<32>(s, warp_sums);
   for (int i = lo; i < hi; ++i) {
     const uint32_t v = d[i];
     d[i] = run;
@@ -92,21 +73,9 @@ radix_scan_chunks_kernel(uint32_t* __restrict__ data, int count, int nchunks, ui
   uint32_t v[4], s = 0;
 #pragma unroll
   for (int r = 0; r < 4; ++r) { v[r] = (i0 + r < count) ? d[i0 + r] : 0u; s += v[r]; }
-  uint32_t incl = s;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  if (lane == 31) warp_sums[w] = incl;
-  __syncthreads();
-  if (w == 0) {
-    const uint32_t x = warp_sums[lane];
-    uint32_t xi = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, xi, o); if (lane >= o) xi += t; }
-    warp_sums[lane] = xi - x;
-    if (lane == 31) chunk_tot[b * nchunks + c] = xi;
-  }
-  __syncthreads();
-  uint32_t run = warp_sums[w] + incl - s;
+  uint32_t total;
+  uint32_t run = block_scan_excl<32>(s, warp_sums, &total);
+  if (threadIdx.x == 0) chunk_tot[b * nchunks + c] = total;
 #pragma unroll
   for (int r = 0; r < 4; ++r) { if (i0 + r < count) d[i0 + r] = run; run += v[r]; }
   // ---- last block: chunk totals -> exclusive chunk offsets, per batch --------------------------
@@ -123,9 +92,7 @@ radix_scan_chunks_kernel(uint32_t* __restrict__ data, int count, int nchunks, ui
     for (int base = 0; base < nchunks; base += 32) {
       const int k = base + lane;
       const uint32_t x = k < nchunks ? *reinterpret_cast<volatile uint32_t*>(chunk_tot + bb * nchunks + k) : 0u;
-      uint32_t xi = x;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, xi, o); if (lane >= o) xi += t; }
+      const uint32_t xi = warp_inclusive_scan(x);
       if (k < nchunks) chunk_tot[bb * nchunks + k] = carry + xi - x;
       carry += __shfl_sync(0xffffffffu, xi, 31);
     }
@@ -175,14 +142,7 @@ radix_scatter_kernel(const uint64_t* __restrict__ keys_in, const uint32_t* __res
       const uint32_t* row = block_offs + ((int64_t)b * 256 + d) * nblk;
       uint32_t before = 0, total = 0;
       for (int t = 0; t < nblk; ++t) { const uint32_t c = row[t]; if (t < (int)blockIdx.x) before += c; total += c; }
-      uint32_t incl = total;                       // exclusive scan of the digit totals over the block
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-      if (lane == 31) digit_base[w] = incl;
-      __syncthreads();
-      uint32_t wb = 0;
-      for (int ww = 0; ww < w; ++ww) wb += digit_base[ww];
-      run = wb + incl - total + before;
+      run = block_scan_excl<kWarps>(total, digit_base) + before;   // exclusive scan of the digit totals
     } else {
       const int64_t e = (int64_t)d * nblk + blockIdx.x;          // entry inside this batch
       run = block_offs[(int64_t)b * 256 * nblk + e];

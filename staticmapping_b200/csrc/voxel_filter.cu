@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "compact.cuh"
 #include "kernels.h"
+#include "reduce.cuh"
 
 namespace smb {
 namespace {
@@ -43,11 +44,7 @@ vf_min_kernel(const char* __restrict__ pts, int64_t stride, int n, float voxel, 
     long long a, b, c;
     if (vf_index(reinterpret_cast<const float*>(pts + (int64_t)i * stride), voxel, &a, &b, &c)) { ix = a; iy = b; iz = c; }
   }
-  for (int o = 16; o > 0; o >>= 1) {
-    ix = min(ix, __shfl_xor_sync(0xffffffffu, ix, o));
-    iy = min(iy, __shfl_xor_sync(0xffffffffu, iy, o));
-    iz = min(iz, __shfl_xor_sync(0xffffffffu, iz, o));
-  }
+  ix = warp_min(ix); iy = warp_min(iy); iz = warp_min(iz);
   if ((threadIdx.x & 31) == 0) { atomicMin(&meta[0], ix); atomicMin(&meta[1], iy); atomicMin(&meta[2], iz); }
 }
 
