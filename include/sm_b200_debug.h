@@ -31,6 +31,8 @@
  *     sm_debug_ndt_derivatives the 44 sums of NdtStage::eval (computeDerivatives) at given pose vectors, both forms
  *     sm_debug_ndt_derivatives_search  the same with each of pclomp's four neighbour searches
  *     sm_debug_float_tree_knn  the float tree's exact searches: knn1 (eps = 0) and the 20-NN of the covariances
+ *     sm_debug_pm_stages       the IcpUsingPointMatcher stand-in's reading filter and score pass: kept points, sorted
+ *                              squared distances of the approximate search, trim counts and mean
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
  *     sm_debug_gicp_step       correspondences, Mahalanobis matrices and cost sums of one GICP outer iteration
@@ -203,6 +205,15 @@ int sm_debug_ndt_direct_neighbors(int32_t search_method, const float* points_3n,
  * -1 / +inf.  ids / d2 hold nq * k entries; ids are indices into the cloud. */
 int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const double* query_3m, int64_t nq,
                             int32_t k, int32_t* ids, double* d2);
+
+/* The IcpUsingPointMatcher stand-in's device stages (csrc/icp_pm.cu PmStage) as pm_align runs them, on packed float
+ * clouds: PmStage::sample of the n reading points with prob and seed -> *kept and sampled_3n (3 * kept doubles in input
+ * order; capacity 3 * n); FloatTree::build of the nt target points, then PmStage::score_pass of the UNFILTERED reading
+ * moved by T_4x4 (column-major) with the bound (1 + knn_epsilon)^2 and the trim ratio -> keys_n (the n squared
+ * distances in ascending order, +inf where no match was found) and out_3 = {mean kept distance, kept, valid}. */
+int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const float* target_3n, int64_t nt, float prob,
+                       uint32_t seed, const double* T_4x4, float knn_epsilon, float ratio, int64_t* kept,
+                       double* sampled_3n, double* keys_n, double* out_3);
 
 /* ApproxVoxelGrid::filter (pcl::ApproximateVoxelGrid): *m_out points into out_3n (capacity n). */
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,

@@ -106,6 +106,8 @@ SIGNATURES = {
     "sm_debug_ndt_direct_neighbors": (C.c_int, [C.c_int32, _VP, C.c_int64, C.c_float, _VP, _VP, _VP, _VP, C.c_int64,
                                                 _VP, _VP]),
     "sm_debug_float_tree_knn": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, _VP, _VP]),
+    "sm_debug_pm_stages": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_float, C.c_uint32, _VP, C.c_float,
+                                     C.c_float, _VP, _VP, _VP, _VP]),
     "sm_debug_approx_voxel_grid": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_float, _VP, _VP]),
     "sm_debug_gicp_covariances": (C.c_int, [C.c_int, _VP, C.c_int64, _VP]),
     "sm_debug_gicp_step": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, _VP, _VP, _VP, C.c_int32, _VP, _VP, _VP,

@@ -141,4 +141,7 @@ int PmStage::score_pass(const float* src, int n, const double* T_host_pinned, co
   return 0;
 }
 
+// an even number of passes leaves the sort's result in keys[0], the first array carved behind the head
+const uint64_t* PmStage::sorted_keys() const { return (const uint64_t*)((const char*)score.p + kScoreHead); }
+
 }  // namespace smb

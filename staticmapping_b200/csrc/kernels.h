@@ -344,6 +344,8 @@ struct PmStage {
   // `ratio`; waits for out3_host = mean kept distance, kept, valid
   int score_pass(const float* src, int n, const double* T_host_pinned, const FloatTree& target, double max_error2,
                  float ratio, double* out3_host, cudaStream_t s);
+  // the last score pass's n squared distances in ascending order, as sorted bit patterns (+inf = no match)
+  const uint64_t* sorted_keys() const;
 };
 
 // ---- m2dp.cu -----------------------------------------------------------------------------

@@ -817,6 +817,9 @@ int sm_set_option(sm_handle* h, const char* name, const char* text) {
       case kOptDouble: *reinterpret_cast<double*>(v) = strtod(text, nullptr); break;
       case kOptBool: *reinterpret_cast<bool*>(v) = as_bool(text); break;
     }
+    // type 1 keeps the filtered reading cloud until the source changes; a new filter option must filter it anew
+    PmMatcher* pm = h->as<PmMatcher>();
+    if (pm && (strcmp(name, "reading_sample_prob") == 0 || strcmp(name, "sample_seed") == 0)) pm->src_dirty = true;
     return SM_OK;
   }
   return fail(h, SM_ERR_UNKNOWN_OPTION, std::string("Init an unknown option of this matcher! ") + name);

@@ -412,6 +412,37 @@ int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const 
   return SM_OK;
 }
 
+int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const float* target_3n, int64_t nt, float prob,
+                       uint32_t seed, const double* T_4x4, float knn_epsilon, float ratio, int64_t* kept,
+                       double* sampled_3n, double* keys_n, double* out_3) {
+  if (!debug_cloud_ok(reading_3n, n) || !debug_cloud_ok(target_3n, nt) || !T_4x4 || !kept || !sampled_3n || !keys_n ||
+      !out_3 || kd_num_levels((int)nt, 8) > 24)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  DevBuf src, tgt, kdws;
+  PmStage st;
+  FloatTree tree;
+  SMB_RC(debug_upload_f32(reading_3n, n, src));
+  SMB_RC(debug_upload_f32(target_3n, nt, tgt));
+  SMB_RC(st.reserve((int)n));
+  uint32_t m = 0;
+  SMB_RC(st.sample((const float*)src.p, (int)n, prob, seed, nullptr, &m));
+  SMB_CUDA_OK(cudaMemcpy(sampled_3n, st.points(), (size_t)m * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  *kept = (int64_t)m;
+  SMB_RC(tree.build((const float*)tgt.p, (int)nt, kdws, nullptr));
+  double* pinned = nullptr;   // the pose, as score_pass expects it, and the three outputs
+  SMB_CUDA_OK(cudaMallocHost((void**)&pinned, 19 * sizeof(double)));
+  memcpy(pinned, T_4x4, 16 * sizeof(double));
+  const double eps = (double)knn_epsilon;   // as pm_align derives the search's bound from the option
+  const int rc = st.score_pass((const float*)src.p, (int)n, pinned, tree, (1.0 + eps) * (1.0 + eps), ratio,
+                               pinned + 16, nullptr);
+  if (rc == 0) memcpy(out_3, pinned + 16, 3 * sizeof(double));
+  cudaFreeHost(pinned);
+  SMB_RC(rc);
+  SMB_CUDA_OK(cudaMemcpy(keys_n, st.sorted_keys(), (size_t)n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,
                                int64_t* m_out) {
   if (!debug_cloud_ok(points_3n, n) || !(leaf > 0.0f) || !out_3n || !m_out) return SM_ERR_BAD_ARGUMENT;

@@ -336,21 +336,56 @@ def icp_pm_equivalent(source_f32, target_f32, guess=None, prob=0.9, seed=1, max_
     o["n_target"] = int(tp.shape[0])
     # "compute the final score" (icp_pointmatcher.cc:131-148): UNFILTERED reading moved by the result,
     # matched against the UNFILTERED reference (same matcher, eps 3.16), trimmed at 0.7
-    R = o["result"]
-    s64 = src.astype(np.float64)
-    moved = np.empty_like(s64)
-    for r in range(3):   # the engine's (and cloud_types.cc:288-296) accumulation order
-        moved[:, r] = ((R[r, 0] * s64[:, 0] + R[r, 1] * s64[:, 1]) + R[r, 2] * s64[:, 2]) + R[r, 3]
-    _, d2 = knn1(tgt.astype(np.float64), moved, epsilon=3.16)
-    v = np.sort(d2[np.isfinite(d2)])
-    if v.size:
-        q = float(np.float32(0.7))
-        qi = v.size - 1 if q == 1.0 else min(int(v.size * q), v.size - 1)
-        kept = v[v <= v[qi]]
-        o["score"] = float(np.exp(-(np.sqrt(kept).sum() / kept.size)))
-        o["score_kept"] = int(kept.size)
+    _, d2 = knn1(tgt.astype(np.float64), pm_moved(src, o["result"]), epsilon=3.16)
+    v, _, kept = pm_score_trim(d2)
+    if kept:
+        o["score"] = float(np.exp(-(np.sqrt(v[:kept]).sum() / kept)))
+        o["score_kept"] = kept
     o["ok"] = o["score"] >= float(np.float32(accept_min_score))
     return o
+
+
+def pm_moved(source_f32, R):
+    """The reading cloud (float) moved by the 4x4 R in double, in the engine's (and cloud_types.cc:288-296)
+    accumulation order: ((R00 x + R01 y) + R02 z) + R03 per row."""
+    s64 = np.asarray(source_f32, dtype=np.float32).astype(np.float64)
+    moved = np.empty_like(s64)
+    for r in range(3):
+        moved[:, r] = ((R[r, 0] * s64[:, 0] + R[r, 1] * s64[:, 1]) + R[r, 2] * s64[:, 2]) + R[r, 3]
+    return moved
+
+
+def pm_score_trim(d2, ratio=0.7):
+    """The score pass's trim (GetDistsQuantile, icp_fast.cc:82-89): over the finite squared distances, the limit is
+    element int(valid * ratio) of the sorted values, or the last one when ratio is 1 or that index is past the end,
+    and every value <= limit is kept.  Returns (sorted finite values, valid, kept); kept values are the first `kept`."""
+    v = np.sort(np.asarray(d2, dtype=np.float64)[np.isfinite(d2)])
+    if not v.size:
+        return v, 0, 0
+    q = float(np.float32(ratio))
+    qi = v.size - 1 if q == 1.0 else min(int(v.size * q), v.size - 1)
+    return v, int(v.size), int(np.count_nonzero(v <= v[qi]))
+
+
+def pm_score_block_sum(values, threads=1024):
+    """The sum of `values` in the order the score pass adds them (one block of `threads` threads, reduce.cuh
+    block_sum): thread t adds values[i] for i = t (mod threads) in ascending i from 0.0, each warp of 32 adds with an
+    xor butterfly (offsets 16, 8, 4, 2, 1), and the warp totals are added in warp order from 0.0."""
+    v = np.asarray(values, dtype=np.float64)
+    rows = -(-v.size // threads)
+    grid = np.zeros(rows * threads)
+    grid[:v.size] = v
+    acc = np.zeros(threads)
+    for row in grid.reshape(rows, threads):   # adding the zero padding leaves every partial sum unchanged
+        acc = acc + row
+    lanes = acc.reshape(threads // 32, 32)
+    idx = np.arange(32)
+    for off in (16, 8, 4, 2, 1):
+        lanes = lanes + lanes[:, idx ^ off]
+    total = 0.0
+    for w in lanes[:, 0]:
+        total += float(w)
+    return total
 
 
 def voxel_grid_filter(points5, voxel_size, order_mode=0):

@@ -2,6 +2,8 @@
 restated on the CPU (tests/gpu_quantile_model.py), returns the value std::nth_element returns and keeps the set the
 reference keeps (registrators/icp_fast.cc:65-90, :497-498) — on ordinary distance distributions and on the ones that
 force the fallback paths."""
+import math
+
 import numpy as np
 import pytest
 
@@ -57,3 +59,42 @@ def test_quantile_index_is_the_reference_expression():
     assert O.quantile_index(120_000, 0.7) == 83_999
     d2 = np.arange(120_000, dtype=np.float64) + 1.0
     assert select(d2)["limit"] == 84_000.0 and int(select(d2)["kept"].sum()) == 84_000
+
+
+# ---- the type-1 score pass (staticmapping_b200/csrc/icp_pm.cu pm_score_reduce_kernel) --------------------------------
+def _block_sum_literal(values, threads):
+    """oracle_lib.pm_score_block_sum's order written out one addition at a time"""
+    part = [0.0] * threads
+    for i, x in enumerate(values):
+        part[i % threads] += float(x)
+    for off in (16, 8, 4, 2, 1):
+        part = [part[t] + part[t ^ off] for t in range(threads)]
+    total = 0.0
+    for w in range(threads // 32):
+        total += part[32 * w]
+    return total
+
+
+def test_score_pass_sum_restatement_has_teeth():
+    # the GPU test holds the score pass's mean to this restatement bit for bit; it must tell the device's order
+    # from numpy's pairwise sum and from the same shape over 512 threads
+    rng = np.random.default_rng(3)
+    roots = np.sqrt(rng.uniform(0.0, 4.0, 262_145))
+    s1024 = O.pm_score_block_sum(roots)
+    assert s1024 != float(np.sum(roots))
+    assert s1024 != O.pm_score_block_sum(roots, threads=512)
+    assert abs(s1024 - math.fsum(roots)) <= 1e-13 * math.fsum(roots)
+    for n in (1, 31, 1025, 5000):
+        x = roots[:n]
+        assert O.pm_score_block_sum(x) == _block_sum_literal(x, 1024)
+        assert O.pm_score_block_sum(x, threads=512) == _block_sum_literal(x, 512)
+
+
+def test_score_trim_rule_edges():
+    d2 = np.array([0.5, np.inf, 0.25, 0.5, np.nan, 0.5, 1.0, 0.25])
+    v, valid, kept = O.pm_score_trim(d2, 0.0)
+    assert list(v) == [0.25, 0.25, 0.5, 0.5, 0.5, 1.0] and (valid, kept) == (6, 2)     # ties at the limit are kept
+    assert O.pm_score_trim(d2, 0.7)[1:] == (6, 5)              # qi = int(6 * 0.7f) = 4: the 0.5 run
+    assert O.pm_score_trim(d2, 1.0)[1:] == (6, 6)
+    assert O.pm_score_trim(d2, 1.5)[1:] == (6, 6)              # qi clamped to the last value
+    assert O.pm_score_trim(np.array([np.inf, np.nan]), 0.7)[1:] == (0, 0)
