@@ -303,6 +303,30 @@ class FilterChainB200 {
     if (inliers) inliers->assign(index.begin(), index.begin() + m);
   }
 
+  // RangeImage::DepthCluster (pre_processors/filter_range_image.cc:143-173) of the chain's RangeImage `filter` over
+  // `input`, that filter's own input cloud: appends {x, y, z, label} records (pcl::PointXYZL, or any cloud whose
+  // value_type has those members and that has push_back) in ascending label, each cluster in the reference's order.
+  // An empty input CHECK-fails as in the reference (CHECK(inner_cloud_ != nullptr)).
+  template <typename LabeledCloud>
+  void DepthCluster(int filter, const data::InnerCloudType& input, LabeledCloud* const cloud) {
+    const int64_t n = static_cast<int64_t>(input.points.size());
+    std::vector<float> xyz(3 * input.points.size());
+    std::vector<uint32_t> label(input.points.size());
+    std::vector<int32_t> index(input.points.size());
+    int64_t m = 0;
+    const int rc = sm_filter_chain_depth_cluster(chain_, filter, n ? &input.points[0].x : nullptr, n,
+                                                 sizeof(data::InnerPointType), xyz.data(), label.data(), index.data(),
+                                                 &m, nullptr);
+    CHECK_EQ(rc, 0) << "sm_filter_chain_depth_cluster failed (" << rc << "): " << sm_filter_chain_last_error(chain_);
+    if (!cloud) return;
+    for (int64_t j = 0; j < m; ++j) {
+      typename LabeledCloud::value_type point;
+      point.x = xyz[3 * j]; point.y = xyz[3 * j + 1]; point.z = xyz[3 * j + 2];
+      point.label = label[j];
+      cloud->push_back(point);
+    }
+  }
+
  private:
   sm_filter_chain* chain_ = nullptr;
 };

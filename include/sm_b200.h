@@ -364,6 +364,25 @@ int sm_filter_chain_run(sm_filter_chain* chain, const float* points, int64_t n, 
                         int64_t* m_out, int32_t* inlier_index_or_null);
 int sm_filter_chain_run_device(sm_filter_chain* chain, const float* dev_points, int64_t n, int64_t stride_bytes,
                                float* dev_out, int64_t* m_out, int32_t* dev_inlier_index_or_null, void* cuda_stream);
+/* RangeImage::DepthCluster (filter_range_image.cc:143-173, :245-309) after SetInputCloud + Filter of `points` by the
+ * chain's filter `filter`, which must be a RangeImage (its parameters are used; the rest of the chain is not run).
+ * The range image is Filter's: the first point in input order per pixel, its range sqrtf(x^2+y^2+z^2) of the offset
+ * point.  Components of the image under the steps (0,+-1), (0,+-2) (columns wrap) and (+-1,0), an edge where
+ * beta = atan2f(d2 sinf(alpha), d1 - d2 cosf(alpha)) > float(10 deg) (d1 / d2 the larger / smaller range, alpha the
+ * horizontal resolution for the column steps and the vertical one for the row steps).  Labels 1, 2, ... in row-major
+ * order of each component's first pixel, every component counted; the components of >= 20 pixels are emitted in
+ * ascending label, each in the reference's breadth-first (std::queue) order.
+ * Outputs, capacity n each: out_xyz (3 floats per point: the un-offset input point), out_label, out_index (the
+ * point's index in `points`); *m_out = their number.  point_label_or_null (capacity n): the label of every input point
+ * that owns its pixel, components under 20 points included, 0 for every other point.
+ * SM_ERR_BAD_ARGUMENT: `filter` is not a RangeImage, vertical_line_num <= 0, horizontal_line_num < 2 (the reference
+ * steps outside its image there) or more than 2^24 pixels.  SM_ERR_CHECK_FAILED: n == 0 (CHECK(inner_cloud_ !=
+ * nullptr), :144).
+ * sinf and cosf are taken on the host; atan2f is CUDA's here and glibc's in the reference, so besides the pixel
+ * borders above, an edge whose beta lies within a few float ulps of the threshold can differ. */
+int sm_filter_chain_depth_cluster(sm_filter_chain* chain, int filter, const float* points, int64_t n,
+                                  int64_t stride_bytes, float* out_xyz, uint32_t* out_label, int32_t* out_index,
+                                  int64_t* m_out, uint32_t* point_label_or_null);
 const char* sm_filter_chain_last_error(const sm_filter_chain* chain);
 
 int sm_device_count(void);

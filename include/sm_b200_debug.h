@@ -22,6 +22,7 @@
  *     sm_debug_ndt_direct_neighbors  the NDT derivative kernel's DIRECT26 / DIRECT7 / DIRECT1 neighbour searches
  *     sm_debug_filter_host     the filter chain's per-point functions: predicate, RangeImage pixel, GroundRemoval2 cell
  *     sm_debug_filter_fit_host, sm_debug_filter_distance_host  GroundRemoval2's line fit and VerticalDistanceToSegment
+ *     sm_debug_depth_edge_host RangeImage::DepthCluster's edge predicate
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -41,6 +42,7 @@
  *     sm_debug_kd_tree         every array a k-d tree owner (KdCompactTree, NormalsPipeline, FloatTree) fills, after
  *                              an optional earlier build into the same owner
  *     sm_debug_filter_ground_removal2  every intermediate of FilterChain's GroundRemoval2 stage
+ *     sm_debug_depth_cluster   DepthCluster's range image, edge mask, labels and BFS level / position per pixel
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
  *   each stage of M2DP meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
@@ -301,6 +303,20 @@ int sm_debug_filter_ground_removal2(int device, const struct sm_filter_chain* ch
                                     int64_t n, int64_t stride_bytes, int32_t max_lines, uint32_t* cell, uint8_t* member,
                                     uint32_t* cell_members, float* cell_min_2c, float* lines_4, int32_t* n_lines,
                                     uint8_t* keep);
+/* RangeImage::DepthCluster's edge predicate (csrc/depth_cluster.cu, filter_range_image.cc:288-301) compiled for the
+ * host, with the resolutions of filter `filter` (a RangeImage) of `chain`: for pair i of ranges a[i], b[i] and
+ * neighbour step step[i] (0..3 the column steps, 4..5 the row steps) edge[i] = 1 / 0 and beta[i].
+ * sin_cos4 (optional): sinf / cosf of the horizontal, then of the vertical resolution. */
+int sm_debug_depth_edge_host(const struct sm_filter_chain* chain, int32_t filter, const float* a, const float* b,
+                             const int32_t* step, int64_t n, uint8_t* edge, float* beta, float* sin_cos4);
+/* sm_filter_chain_depth_cluster's device stages for filter `filter` of `chain` over n host records, per pixel
+ * (row-major, vertical_line_num x horizontal_line_num): image (the owner's range, 0 when empty), owner (input index,
+ * -1), mask (bit k: an edge along neighbour step k), label (0 when empty), level (BFS level in its cluster, -1 outside
+ * the kept clusters) and seq (position in its cluster's output order, -1 likewise); *components = every component,
+ * dropped ones included.  Return codes as sm_filter_chain_depth_cluster. */
+int sm_debug_depth_cluster(int device, const struct sm_filter_chain* chain, int32_t filter, const float* points,
+                           int64_t n, int64_t stride_bytes, float* image, int32_t* owner, uint8_t* mask, uint32_t* label,
+                           int32_t* level, int32_t* seq, int32_t* components);
 
 #ifdef __cplusplus
 }

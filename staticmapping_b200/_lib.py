@@ -79,6 +79,8 @@ SIGNATURES = {
     "sm_filter_chain_set_option": (C.c_int, [_VP, C.c_char_p, C.c_char_p]),
     "sm_filter_chain_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
     "sm_filter_chain_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
+    "sm_filter_chain_depth_cluster": (C.c_int, [_VP, C.c_int, _VP, C.c_int64, C.c_int64, _VP, _VP, _VP,
+                                                C.POINTER(C.c_int64), _VP]),
     "sm_filter_chain_last_error": (C.c_char_p, [_VP]),
     # include/sm_b200_debug.h (test hooks)
     "sm_debug_solve6": (C.c_int, [C.c_int, _VP, _VP, _VP, _VP]),
@@ -123,6 +125,9 @@ SIGNATURES = {
     "sm_debug_filter_distance_host": (C.c_int, [_VP, C.c_int32, C.c_float, C.c_float, _VP]),
     "sm_debug_filter_ground_removal2": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, _VP,
                                                   _VP, _VP, _VP, _VP, _VP]),
+    "sm_debug_depth_edge_host": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, C.c_int64, _VP, _VP, _VP]),
+    "sm_debug_depth_cluster": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, _VP, _VP, _VP, _VP, _VP,
+                                         _VP, _VP]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

@@ -540,6 +540,20 @@ float filter_debug_distance_host(const Gr2Line* lines, int n_lines, float d, flo
   return gr2_vertical_distance(lines, n_lines, d, z, bad);
 }
 
+int range_image_owner(const FilterParams& f, const char* pts, int n, int64_t stride, uint32_t* pixel, uint32_t* owner,
+                      cudaStream_t s) {
+  const size_t pixels = (size_t)f.vertical_line_num * (size_t)f.horizontal_line_num;
+  SMB_CUDA_OK(cudaMemsetAsync(owner, 0xff, pixels * sizeof(uint32_t), s));
+  range_image_owner_kernel<<<ceil_div(n, 256), 256, 0, s>>>(pts, stride, n, f, range_image_consts(f), pixel, owner);
+  return 0;
+}
+
+// horizontal_line_num < 2: a (0, +-2) step wraps once and still leaves the image in the reference (:277-281)
+bool depth_cluster_grid_ok(const FilterParams& f) {
+  return f.vertical_line_num > 0 && f.horizontal_line_num >= 2 &&
+         (int64_t)f.vertical_line_num * f.horizontal_line_num <= kMaxCells;
+}
+
 // ---- FilterChain ------------------------------------------------------------------------------------------------
 int FilterChain::stage_end(int first) const {
   if (filters[first].kind > kFilterRandomSampler) return first + 1;
@@ -595,11 +609,8 @@ int FilterChain::predicate_stage(int first, int cnt, const char* in, const uint3
 
 int FilterChain::range_image_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n,
                                    int64_t stride, float* out, uint32_t* index_out, cudaStream_t s) {
-  const RangeImageConsts c = range_image_consts(f);
-  const size_t pixels = (size_t)f.vertical_line_num * (size_t)f.horizontal_line_num;
   const int tiles = compact_tiles(n);
-  SMB_CUDA_OK(cudaMemsetAsync(owner.p, 0xff, pixels * sizeof(uint32_t), s));
-  range_image_owner_kernel<<<ceil_div(n, 256), 256, 0, s>>>(in, stride, n, f, c, (uint32_t*)pixel.p, (uint32_t*)owner.p);
+  SMB_RC(range_image_owner(f, in, n, stride, (uint32_t*)pixel.p, (uint32_t*)owner.p, s));
   range_image_flag_kernel<<<tiles, kCompactThreads, 0, s>>>((const uint32_t*)pixel.p, (const uint32_t*)owner.p, n,
                                                             (uint8_t*)flag.p, (uint32_t*)block_cnt.p);
   compact_scan((uint32_t*)block_cnt.p, tiles, s);
@@ -705,6 +716,7 @@ using namespace smb;
 struct sm_filter_chain {
   int device = 0;
   FilterChain chain;
+  DepthCluster depth;
   cudaStream_t stream = nullptr;
   DevBuf host_in, host_out, host_idx;
   char error[256] = {0};
@@ -826,6 +838,46 @@ int sm_filter_chain_run(sm_filter_chain* c, const float* points, int64_t n, int6
                                   c->stream));
     SMB_CUDA_OK(cudaStreamSynchronize(c->stream));
   }
+  return SM_OK;
+}
+
+int sm_filter_chain_depth_cluster(sm_filter_chain* c, int filter, const float* points, int64_t n, int64_t stride_bytes,
+                                  float* out_xyz, uint32_t* out_label, int32_t* out_index, int64_t* m_out,
+                                  uint32_t* point_label) {
+  if (!c || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 ||
+      (n > 0 && (!points || !out_xyz || !out_label || !out_index)))
+    return SM_ERR_BAD_ARGUMENT;
+  *m_out = 0;
+  if (filter < 0 || filter >= (int)c->chain.filters.size() || c->chain.filters[filter].kind != kFilterRangeImage)
+    return chain_fail(c, SM_ERR_BAD_ARGUMENT, "DepthCluster needs a RangeImage of the chain%s", "");
+  // SetInputCloud drops an empty cloud (filter_range_image.cc:67-71), then CHECK(this->inner_cloud_ != nullptr) (:144)
+  if (n == 0) return chain_fail(c, SM_ERR_CHECK_FAILED, "Check failed: this->inner_cloud_ != nullptr%s", "");
+  const FilterParams& f = c->chain.filters[filter];
+  if (!depth_cluster_grid_ok(f))
+    return chain_fail(c, SM_ERR_BAD_ARGUMENT, "%s", "a RangeImage grid DepthCluster cannot run");
+  SMB_RC(chain_device(c));
+  if (!c->stream) SMB_CUDA_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+  const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
+  SMB_RC(c->host_in.reserve(in_bytes));
+  SMB_RC(c->host_out.reserve((size_t)n * 24));    // xyz, label, index, point label
+  float* d_xyz = (float*)c->host_out.p;
+  uint32_t* d_label = (uint32_t*)(d_xyz + 3 * n);
+  int32_t* d_index = (int32_t*)(d_label + n);
+  uint32_t* d_point = (uint32_t*)(d_index + n);
+  SMB_CUDA_OK(cudaMemcpyAsync(c->host_in.p, points, in_bytes, cudaMemcpyHostToDevice, c->stream));
+  const int rc = c->depth.run(f, (const char*)c->host_in.p, (int)n, stride_bytes, d_xyz, d_label, d_index,
+                              point_label ? d_point : nullptr, m_out, c->stream);
+  if (rc == SM_ERR_CUDA) return chain_fail(c, rc, "%s", last_cuda_error());
+  SMB_RC(rc);
+  const size_t m = (size_t)*m_out;
+  if (m > 0) {
+    SMB_CUDA_OK(cudaMemcpyAsync(out_xyz, d_xyz, m * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    SMB_CUDA_OK(cudaMemcpyAsync(out_label, d_label, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    SMB_CUDA_OK(cudaMemcpyAsync(out_index, d_index, m * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  }
+  if (point_label)
+    SMB_CUDA_OK(cudaMemcpyAsync(point_label, d_point, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+  SMB_CUDA_OK(cudaStreamSynchronize(c->stream));
   return SM_OK;
 }
 

@@ -413,8 +413,32 @@ bool filter_debug_pixel_host(const FilterParams& f, const float* rec, int* row, 
 void filter_debug_cell_host(const FilterParams& f, const float* rec, float* range, int* s, int* b);
 void filter_debug_fit_host(const float* d, const float* z, int n, float* m, float* b);
 float filter_debug_distance_host(const Gr2Line* lines, int n_lines, float d, float z, int* bad);
+// the RangeImage stage's pixel of every point (0xffffffff: outlier) and the first point per pixel (0xffffffff: empty)
+int range_image_owner(const FilterParams& f, const char* pts, int n, int64_t stride, uint32_t* pixel, uint32_t* owner,
+                      cudaStream_t s);
 struct FilterChain;
 const FilterChain* filter_chain_of(const ::sm_filter_chain* c);   // the chain behind the C handle, null for null
+
+// ---- depth_cluster.cu --------------------------------------------------------------------------
+// sinf / cosf of RangeImage::LabelOneComponent's horizontal and vertical resolution (filter_range_image.cc:255-259)
+struct DepthConsts { float sin_h, cos_h, sin_v, cos_v; };
+bool depth_cluster_grid_ok(const FilterParams& f);   // a RangeImage grid DepthCluster can run (filters.cu)
+DepthConsts depth_consts(const FilterParams& f);
+// the edge predicate compiled for the host (test hook sm_debug_depth_edge_host): step k of the neighbour list
+bool depth_debug_edge_host(const DepthConsts& c, float a, float b, int k, float* beta);
+// RangeImage::DepthCluster (filter_range_image.cc:143-173) over n records in device memory, for a RangeImage `f`
+// with vertical_line_num >= 1, horizontal_line_num >= 2 and at most 2^24 pixels.  Writes the clustered points
+// (capacity: the occupied pixels, at most n) and, if point_label is not null, the label of every input point that
+// owns its pixel (0 elsewhere); returns after the stream has finished, with the count in *m.  The per-pixel arrays
+// stay valid until the next run (test hook sm_debug_depth_cluster).
+struct DepthCluster {
+  DevBuf pixel, owner, image, mask, parent, label, size, kept, kept_off, claim, level, seq, order, roots, block_cnt,
+      count;
+  int components = 0;                // of the last run, dropped ones included
+  int reserve(int64_t n, int64_t pixels);
+  int run(const FilterParams& f, const char* pts, int n, int64_t stride, float* out_xyz, uint32_t* out_label,
+          int32_t* out_index, uint32_t* point_label, int64_t* m, cudaStream_t s);
+};
 
 // The device buffers and the stages of one filter chain.  reserve() sizes the buffers for n records and the chain's
 // RangeImage / GroundRemoval2 grids; they only grow.  run() applies the filters in order to n records of `stride`

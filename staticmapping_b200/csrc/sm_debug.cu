@@ -728,4 +728,51 @@ int sm_debug_filter_ground_removal2(int device, const sm_filter_chain* chain, in
   return rc;
 }
 
+// ---- test hooks of DepthCluster (depth_cluster.cu) -------------------------------------------------------------------
+int sm_debug_depth_edge_host(const sm_filter_chain* chain, int32_t filter, const float* a, const float* b,
+                             const int32_t* step, int64_t n, uint8_t* edge, float* beta, float* sin_cos4) {
+  const FilterChain* fc = filter_chain_of(chain);
+  if (!fc || filter < 0 || filter >= (int)fc->filters.size() || fc->filters[filter].kind != kFilterRangeImage ||
+      n < 0 || (n > 0 && (!a || !b || !step || !edge || !beta)))
+    return SM_ERR_BAD_ARGUMENT;
+  const DepthConsts c = depth_consts(fc->filters[filter]);
+  for (int64_t i = 0; i < n; ++i) {
+    if (step[i] < 0 || step[i] > 5) return SM_ERR_BAD_ARGUMENT;
+    edge[i] = depth_debug_edge_host(c, a[i], b[i], step[i], &beta[i]) ? 1 : 0;
+  }
+  if (sin_cos4) { sin_cos4[0] = c.sin_h; sin_cos4[1] = c.cos_h; sin_cos4[2] = c.sin_v; sin_cos4[3] = c.cos_v; }
+  return SM_OK;
+}
+
+int sm_debug_depth_cluster(int device, const sm_filter_chain* chain, int32_t filter, const float* points, int64_t n,
+                           int64_t stride_bytes, float* image, int32_t* owner, uint8_t* mask, uint32_t* label,
+                           int32_t* level, int32_t* seq, int32_t* components) {
+  const FilterChain* fc = filter_chain_of(chain);
+  if (!fc || filter < 0 || filter >= (int)fc->filters.size() || fc->filters[filter].kind != kFilterRangeImage ||
+      n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 || !image || !owner || !mask || !label ||
+      !level || !seq || !components)
+    return SM_ERR_BAD_ARGUMENT;
+  if (n == 0) return SM_ERR_CHECK_FAILED;   // before the points: an empty cloud may come without them
+  if (!points) return SM_ERR_BAD_ARGUMENT;
+  const FilterParams& f = fc->filters[filter];
+  if (!depth_cluster_grid_ok(f)) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  DepthCluster dc;
+  DevBuf in;
+  SMB_RC(in.reserve((size_t)n * (size_t)stride_bytes));
+  SMB_CUDA_OK(cudaMemcpy(in.p, points, (size_t)n * (size_t)stride_bytes, cudaMemcpyHostToDevice));
+  int64_t m = 0;
+  SMB_RC(dc.run(f, (const char*)in.p, (int)n, stride_bytes, nullptr, nullptr, nullptr, nullptr, &m, nullptr));
+  const size_t P = (size_t)f.vertical_line_num * (size_t)f.horizontal_line_num;
+  SMB_CUDA_OK(cudaMemcpy(image, dc.image.p, P * sizeof(float), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(owner, dc.owner.p, P * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(mask, dc.mask.p, P, cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(label, dc.label.p, P * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(level, dc.level.p, P * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(seq, dc.seq.p, P * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  for (size_t p = 0; p < P; ++p) if (level[p] < 0) seq[p] = -1;   // seq is written for the visited pixels only
+  *components = dc.components;
+  return SM_OK;
+}
+
 }  // extern "C"

@@ -1,15 +1,25 @@
 """pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
 chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
-deterministic stand-in, see the header), RangeImage and GroundRemoval2.  There is no CPU fallback."""
+deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster.  There is no CPU
+fallback."""
 from __future__ import annotations
 
 import ctypes as C
 import xml.etree.ElementTree as ET
+from typing import NamedTuple
 
 import numpy as np
 
 from . import _lib
 from .registrators import CheckFailure, InnerCloud
+
+
+class DepthClusters(NamedTuple):
+    """RangeImage::DepthCluster's labelled cloud: clusters in ascending label, each in the reference's visiting order."""
+    xyz: np.ndarray            # (m, 3) float32, the input points
+    label: np.ndarray          # (m,) uint32
+    index: np.ndarray          # (m,) int32, the points' indices in the input cloud
+    point_label: np.ndarray    # (n,) uint32, the label of every pixel owner of the input (small clusters too), else 0
 
 
 class Factory:
@@ -103,3 +113,31 @@ class Factory:
 
     def Outliers(self):
         return self._outliers
+
+    def DepthCluster(self, filter_index, cloud):
+        """RangeImage::DepthCluster (filter_range_image.cc:143-173) after SetInputCloud(cloud) + Filter on the chain's
+        filter `filter_index`, which must be a RangeImage; `cloud` is that filter's own input, (N,5) records.  An empty
+        cloud raises CheckFailure (CHECK(inner_cloud_ != nullptr)); a filter that is not a RangeImage or a grid with
+        horizontal_line_num < 2 raises ValueError."""
+        pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
+        if pts.ndim != 2 or pts.shape[1] != 5:
+            raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
+        n = pts.shape[0]
+        xyz = np.empty((max(n, 1), 3), np.float32)
+        label = np.empty(max(n, 1), np.uint32)
+        index = np.empty(max(n, 1), np.int32)
+        point_label = np.zeros(max(n, 1), np.uint32)
+        m = C.c_int64(0)
+        rc = self._lib.sm_filter_chain_depth_cluster(self._h, int(filter_index), pts.ctypes.data, n, 20, xyz.ctypes.data,
+                                                     label.ctypes.data, index.ctypes.data, C.byref(m),
+                                                     point_label.ctypes.data)
+        if rc == -20:
+            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
+        if rc == -5:
+            raise CheckFailure(self._error())
+        if rc == -1:
+            raise ValueError(self._error())
+        if rc != 0:
+            raise RuntimeError(f"sm_filter_chain_depth_cluster failed with {rc}: {self._error()}")
+        k = m.value
+        return DepthClusters(xyz[:k].copy(), label[:k].copy(), index[:k].copy(), point_label[:n].copy())
