@@ -32,6 +32,9 @@
  *     sm_debug_ndt_derivatives the 44 sums of NdtStage::eval (computeDerivatives) at given pose vectors, both forms
  *     sm_debug_ndt_derivatives_search  the same with each of pclomp's four neighbour searches
  *     sm_debug_float_tree_knn  the float tree's exact searches: knn1 (eps = 0) and the 20-NN of the covariances
+ *     sm_debug_icp_iteration   one IcpFast iteration phase by phase: the prologue's mean, G0 and Morton order; phase A's
+ *                              matches, distances and histogram; phase B's candidates and per-block partial sums;
+ *                              phase C's 29 reduced sums, limit, kept count and pose update
  *     sm_debug_pm_stages       the IcpUsingPointMatcher stand-in's reading filter and score pass: kept points, sorted
  *                              squared distances of the approximate search, trim counts and mean
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
@@ -44,7 +47,7 @@
  *     sm_debug_filter_ground_removal2  every intermediate of FilterChain's GroundRemoval2 stage
  *     sm_debug_depth_cluster   DepthCluster's range image, edge mask, labels and BFS level / position per pixel
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
- *   each stage of M2DP meets a float64 model fed with the device's previous stage */
+ *   each stage of M2DP and of IcpFast's iteration meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
 #define SM_B200_DEBUG_H_
 
@@ -216,6 +219,27 @@ int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const 
 int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const float* target_3n, int64_t nt, float prob,
                        uint32_t seed, const double* T_4x4, float knn_epsilon, float ratio, int64_t* kept,
                        double* sampled_3n, double* keys_n, double* out_3);
+
+/* One IcpFast iteration as sm_align runs it (IcpFastBuffers, KdWorkspace, no graphs; csrc/icp.cu): icp_prologue and
+ * iterations 1 .. iteration-1, then iteration `iteration` one phase at a time with a synchronise and a copy after
+ * each.  Double clouds are n x 3 in caller order; guess_4x4 is column-major; max_iteration = iteration and the
+ * convergence test is off, so the iteration computes the final score.  geometry_2 = {nb, tile}: the phase-B blocks
+ * for ns and the Morton positions per block; with source_3n NULL only geometry_2 is written.  Every other output
+ * may be NULL and is sized by the caller:
+ *   prologue_35   target mean[3], G0[16], T_iter entering the iteration[16]       perm_n  Morton position -> caller index
+ *   phase A (per source point, caller order)   match_n  target index (caller order) or -1, d2_n, pm_6n the {point,
+ *                 normal} record phase B gathers (zero without a match); hist_2048
+ *   phase B       hist2_2048, cand_cnt[nb], cand_key[nb * tile] and cand_terms_8[nb * tile * 8] (block j's candidates
+ *                 start at j * tile: the d2 bits; F[6], residual, sqrt(d2)), partials_29[nb * 29]
+ *   phase C       sums_29 (all-ones bit patterns unless phase C reached its reduction), final_18 = {limit, final_score,
+ *                 T_iter[16]}, final_5 = {kept, status, solve_path, iteration, done}, hist_after_4096 (hist, hist2). */
+int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, const double* target_3n,
+                           const double* normals_3n, int64_t nt, const double* guess_4x4, float dist_outlier_ratio,
+                           float knn_epsilon, int32_t knn_queries_per_cta, int32_t inner_compensation, int32_t iteration,
+                           int32_t* geometry_2, double* prologue_35, uint32_t* perm_n, int32_t* match_n, double* d2_n,
+                           double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048, uint32_t* cand_cnt, uint64_t* cand_key,
+                           double* cand_terms_8, double* partials_29, double* sums_29, double* final_18, int64_t* final_5,
+                           uint32_t* hist_after_4096);
 
 /* ApproxVoxelGrid::filter (pcl::ApproximateVoxelGrid): *m_out points into out_3n (capacity n). */
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,

@@ -110,6 +110,8 @@ SIGNATURES = {
     "sm_debug_float_tree_knn": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, _VP, _VP]),
     "sm_debug_pm_stages": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_float, C.c_uint32, _VP, C.c_float,
                                      C.c_float, _VP, _VP, _VP, _VP]),
+    "sm_debug_icp_iteration": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP, C.c_float, C.c_float,
+                                         C.c_int32, C.c_int32, C.c_int32] + [_VP] * 16),
     "sm_debug_approx_voxel_grid": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_float, _VP, _VP]),
     "sm_debug_gicp_covariances": (C.c_int, [C.c_int, _VP, C.c_int64, _VP]),
     "sm_debug_gicp_step": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, _VP, _VP, _VP, C.c_int32, _VP, _VP, _VP,

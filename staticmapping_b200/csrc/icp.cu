@@ -373,7 +373,7 @@ knn_query_batch_kernel(KdCompact kc, const double* __restrict__ query, int64_t q
 
 }  // namespace
 
-static int icp_accum_blocks(int n_source) { return ceil_div(n_source, kAccTile); }
+int icp_accum_blocks(int n_source) { return ceil_div(n_source, kAccTile); }
 
 // a warp's item list may extend past the last query of the last batch
 size_t knn_items_bytes(int nq) { return ((size_t)nq + 4096) * sizeof(int4); }
@@ -503,14 +503,25 @@ void icp_enqueue_search(const IcpBuffers& b, const IcpParams& p, int grid, int p
   }
 }
 
+void icp_search_launch(const IcpBuffers& b, const IcpParams& p, const double* deskewed, cudaStream_t stream) {
+  int grid, per;
+  knn_geometry(p.n_source, p.knn_queries_per_cta, &grid, &per);
+  const size_t smem = knn_smem_bytes(p.tree_levels);
+  if (p.inner_compensation) icp_enqueue_search<true>(b, p, grid, per, smem, stream, deskewed);
+  else icp_enqueue_search<false>(b, p, grid, per, smem, stream, nullptr);
+}
+
+void icp_accum_launch(const IcpBuffers& b, const IcpParams& p, const double* deskewed, cudaStream_t stream) {
+  const int nb = icp_accum_blocks(p.n_source);
+  if (p.inner_compensation) icp_accum_kernel<true><<<nb, kAccThreads, 0, stream>>>(b, p, deskewed);
+  else icp_accum_kernel<false><<<nb, kAccThreads, 0, stream>>>(b, p, nullptr);
+}
+
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
                            cudaStream_t stream, cudaEvent_t* events, double* deskewed) {
   const bool comp = p.inner_compensation != 0;
   if (comp && !deskewed) return -1;
   const int nb = icp_accum_blocks(p.n_source);
-  int grid, per;
-  knn_geometry(p.n_source, p.knn_queries_per_cta, &grid, &per);
-  const size_t smem = knn_smem_bytes(p.tree_levels);
   for (int it = 0; it < count; ++it) {
     nvtxRangePushA("Iteration");                 // REGISTER_BLOCK("Iteration"), icp_fast.cc:484
     if (events) cudaEventRecord(events[4 * it + 0], stream);
@@ -520,13 +531,11 @@ int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_it
       nvtxRangePop();
     }
     nvtxRangePushA("FindClosests");              // icp_fast.cc:169-180
-    if (comp) icp_enqueue_search<true>(b, p, grid, per, smem, stream, deskewed);
-    else icp_enqueue_search<false>(b, p, grid, per, smem, stream, nullptr);
+    icp_search_launch(b, p, deskewed, stream);
     nvtxRangePop();
     if (events) cudaEventRecord(events[4 * it + 1], stream);
     nvtxRangePushA("ErrorElements");             // icp_fast.cc:92-167 (+ the sums of ComputePointToPlane)
-    if (comp) icp_accum_kernel<true><<<nb, kAccThreads, 0, stream>>>(b, p, deskewed);
-    else icp_accum_kernel<false><<<nb, kAccThreads, 0, stream>>>(b, p, nullptr);
+    icp_accum_launch(b, p, deskewed, stream);
     nvtxRangePop();
     if (events) cudaEventRecord(events[4 * it + 2], stream);
     nvtxRangePushA("ComputePointToPlane");       // icp_fast.cc:256-323

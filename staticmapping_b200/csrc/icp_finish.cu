@@ -463,7 +463,7 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
     double v = lane < kSelWarps ? red[lane][k] : 0.0;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if (lane == 0) solve.S[k] = v;
+    if (lane == 0) { solve.S[k] = v; b.sums[k] = v; }
   }
   __syncthreads();
   if (w != 0) return;

@@ -170,7 +170,8 @@ struct IcpBuffers {
   double* d2;             // [n_source]
   uint32_t* hist;         // [kHistBins] first-level histogram of dist^2 (phase A)
   uint32_t* hist2;        // [kHistBins] second-level histogram inside the quantile bin (phase B)
-  double* sums;           // [32] reduced normal-equation sums of the iteration (phase C1 -> C2)
+  double* sums;           // [32] the iteration's 29 reduced normal-equation sums, written by phase C before it tests
+                          // the kept count (a record for tests; nothing reads it back)
   double* cand_terms;     // [blocks*tile][8] per-block compacted candidates (members of the quantile bin):
                           // the 6 Jacobian terms, the residual and sqrt(d2) of the match (phase B -> C)
   unsigned long long* cand_key;  // [blocks*tile] bit pattern of the candidate's dist^2
@@ -204,7 +205,12 @@ int icp_prologue_launches(int tree_levels);
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
                            cudaStream_t stream, cudaEvent_t* events, double* deskewed = nullptr);
 int icp_iteration_launches(bool inner_compensation);
+// The phases of one iteration, in the order icp_enqueue_iterations runs them (the stage test hook runs them one at a
+// time): icp_deskew_launch with inner compensation, then A, B and C.  nblocks_b = icp_accum_blocks(p.n_source).
+void icp_search_launch(const IcpBuffers& b, const IcpParams& p, const double* deskewed, cudaStream_t stream);
+void icp_accum_launch(const IcpBuffers& b, const IcpParams& p, const double* deskewed, cudaStream_t stream);
 void icp_finish_launch(const IcpBuffers& b, const IcpParams& p, int nblocks_b, cudaStream_t stream);
+int icp_accum_blocks(int n_source);
 // stand-alone k-NN over an already built tree (compact layout incl. pid): ids = original indices
 int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, double max_error2,
               int32_t* ids, double* d2, cudaStream_t stream, int queries_per_cta = 0, int4* items = nullptr);

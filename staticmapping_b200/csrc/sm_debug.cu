@@ -662,6 +662,137 @@ int sm_debug_kd_tree(int device, int32_t variant, int32_t bucket, const void* fi
   return SM_OK;
 }
 
+// ---- test hook of IcpFast's iteration (icp.cu, icp_finish.cu) -------------------------------------------------------
+// caller index of the target point in padded bucket entry e of a bucket-8 normals tree (kd_compact_buckets_kernel's
+// walk from the root to the leaf that owns the entry)
+static int32_t debug_entry_target(const std::vector<uint32_t>& leaf_order, int n, int levels, int64_t e) {
+  const int jL = (int)(e >> 3), k = (int)(e & 7);
+  int first = 0, count = n, l = 0;
+  while (l < levels && count > 8) {
+    const int right = count >> 1, left = count - right;
+    if ((jL >> (levels - 1 - l)) & 1) { first += left; count = right; } else { count = left; }
+    ++l;
+  }
+  return k < count ? (int32_t)leaf_order[first + k] : -1;
+}
+
+static int debug_copy_out(void* dst, const void* src, size_t bytes) {
+  if (dst) SMB_CUDA_OK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
+int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, const double* target_3n,
+                           const double* normals_3n, int64_t nt, const double* guess_4x4, float dist_outlier_ratio,
+                           float knn_epsilon, int32_t knn_queries_per_cta, int32_t inner_compensation, int32_t iteration,
+                           int32_t* geometry_2, double* prologue_35, uint32_t* perm_n, int32_t* match_n, double* d2_n,
+                           double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048, uint32_t* cand_cnt, uint64_t* cand_key,
+                           double* cand_terms_8, double* partials_29, double* sums_29, double* final_18, int64_t* final_5,
+                           uint32_t* hist_after_4096) {
+  if (!geometry_2 || ns <= 0 || ns > (1 << 30)) return SM_ERR_BAD_ARGUMENT;
+  const int nb = icp_accum_blocks((int)ns);
+  geometry_2[0] = nb; geometry_2[1] = dev::kAccTile;
+  if (!source_3n) return SM_OK;
+  if (!target_3n || !normals_3n || nt <= 0 || nt > (1 << 30) || kd_num_levels((int)nt, 8) > 24 || !guess_4x4 ||
+      iteration < 1 || !(dist_outlier_ratio >= 0.0f && dist_outlier_ratio <= 1.0f) || !(knn_epsilon >= 0.0f) ||
+      knn_queries_per_cta < 0)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  // the owners and the parameters of icp_begin, without graphs
+  const int64_t sstride = (ns + 63) & ~(int64_t)63, tstride = (nt + 63) & ~(int64_t)63;
+  const bool comp = inner_compensation != 0;
+  IcpFastBuffers f;
+  DevBuf src_raw, tgt_raw, nrm, kdws;
+  SMB_RC(f.reserve((int)ns, (int)nt, sstride, tstride, comp));
+  SMB_RC(src_raw.reserve((size_t)(3 * sstride) * sizeof(double)));
+  SMB_RC(tgt_raw.reserve((size_t)(3 * tstride) * sizeof(double)));
+  SMB_RC(nrm.reserve((size_t)(3 * tstride) * sizeof(double)));
+  SMB_RC(debug_soa(source_3n, ns, sstride, (double*)src_raw.p));
+  SMB_RC(debug_soa(target_3n, nt, tstride, (double*)tgt_raw.p));
+  SMB_RC(debug_soa(normals_3n, nt, tstride, (double*)nrm.p));
+  KdWorkspace ws;
+  SMB_RC(ws.carve(kdws, (int)nt, 8));
+  IcpBuffers b;
+  f.fill(b, (const double*)tgt_raw.p, (const double*)nrm.p, (const double*)src_raw.p);
+  IcpParams p = {};
+  p.n_source = (int)ns; p.n_target = (int)nt;
+  p.max_iteration = iteration;
+  p.dist_outlier_ratio = dist_outlier_ratio;
+  p.max_error2 = (1.0 + (double)knn_epsilon) * (1.0 + (double)knn_epsilon);
+  p.disable_convergence = 1;
+  p.knn_queries_per_cta = knn_queries_per_cta;
+  p.tree_levels = kd_num_levels((int)nt, 8);
+  p.inner_compensation = comp ? 1 : 0;
+  double* deskewed = comp ? (double*)f.deskewed.p : nullptr;
+  SMB_CUDA_OK(cudaMemcpy(f.guess.p, guess_4x4, 16 * sizeof(double), cudaMemcpyHostToDevice));
+  SMB_CUDA_OK(cudaMemset(b.sums, 0xff, dev::kNumSums * sizeof(double)));   // all-ones until phase C writes it
+  SMB_RC(icp_prologue(b, p, (const double*)f.guess.p, ws, f.tree, nullptr));
+  if (iteration > 1) SMB_RC(icp_enqueue_iterations(b, p, 0, iteration - 1, nullptr, nullptr, deskewed));
+  SMB_CUDA_OK(cudaDeviceSynchronize());
+  IcpState st;
+  SMB_CUDA_OK(cudaMemcpy(&st, b.state, sizeof(IcpState), cudaMemcpyDeviceToHost));
+  std::vector<uint32_t> perm((size_t)ns);
+  SMB_CUDA_OK(cudaMemcpy(perm.data(), b.src_sort.vals[0], (size_t)ns * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  if (prologue_35) {
+    memcpy(prologue_35, st.mean, 3 * sizeof(double));
+    memcpy(prologue_35 + 3, st.G0, 16 * sizeof(double));
+    memcpy(prologue_35 + 19, st.T_iter, 16 * sizeof(double));
+  }
+  if (perm_n) memcpy(perm_n, perm.data(), (size_t)ns * sizeof(uint32_t));
+  // phase A, per source point in caller order
+  if (comp) icp_deskew_launch(b, p, deskewed, nullptr);
+  icp_search_launch(b, p, deskewed, nullptr);
+  SMB_CUDA_OK(cudaDeviceSynchronize());
+  {
+    std::vector<int32_t> slot((size_t)ns);
+    std::vector<double> d2((size_t)ns);
+    std::vector<uint32_t> leaf_order((size_t)nt);
+    const int64_t entries = (int64_t)8 << f.tree.levels;
+    std::vector<BucketMatch> pm((size_t)entries);
+    SMB_CUDA_OK(cudaMemcpy(slot.data(), b.slot, (size_t)ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    SMB_CUDA_OK(cudaMemcpy(d2.data(), b.d2, (size_t)ns * sizeof(double), cudaMemcpyDeviceToHost));
+    SMB_CUDA_OK(cudaMemcpy(leaf_order.data(), f.tree.leaf_order.p, (size_t)nt * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    SMB_CUDA_OK(cudaMemcpy(pm.data(), b.kc.pm, (size_t)entries * sizeof(BucketMatch), cudaMemcpyDeviceToHost));
+    for (int64_t i = 0; i < ns; ++i) {
+      const uint32_t c = perm[(size_t)i];
+      const int32_t s = slot[(size_t)i];
+      const bool ok = s >= 0 && s < entries;
+      if (match_n) match_n[c] = ok ? debug_entry_target(leaf_order, (int)nt, f.tree.levels, s) : -1;
+      if (d2_n) d2_n[c] = d2[(size_t)i];
+      if (pm_6n) {
+        const BucketMatch r = ok ? pm[(size_t)s] : BucketMatch{};
+        const double v[6] = {r.x, r.y, r.z, r.nx, r.ny, r.nz};
+        memcpy(pm_6n + 6 * c, v, sizeof(v));
+      }
+    }
+  }
+  SMB_RC(debug_copy_out(hist_2048, b.hist, kHistBins * sizeof(uint32_t)));
+  // phase B, per block of Morton positions
+  icp_accum_launch(b, p, deskewed, nullptr);
+  SMB_CUDA_OK(cudaDeviceSynchronize());
+  SMB_RC(debug_copy_out(hist2_2048, b.hist2, kHistBins * sizeof(uint32_t)));
+  SMB_RC(debug_copy_out(cand_cnt, b.cand_cnt, (size_t)nb * sizeof(uint32_t)));
+  SMB_RC(debug_copy_out(cand_key, b.cand_key, (size_t)nb * dev::kAccTile * sizeof(uint64_t)));
+  SMB_RC(debug_copy_out(cand_terms_8, b.cand_terms, (size_t)nb * dev::kAccTile * 8 * sizeof(double)));
+  if (partials_29)
+    SMB_CUDA_OK(cudaMemcpy2D(partials_29, dev::kNumSums * sizeof(double), b.partials, 32 * sizeof(double),
+                             dev::kNumSums * sizeof(double), nb, cudaMemcpyDeviceToHost));
+  // phase C
+  icp_finish_launch(b, p, nb, nullptr);
+  SMB_CUDA_OK(cudaDeviceSynchronize());
+  SMB_RC(debug_copy_out(sums_29, b.sums, dev::kNumSums * sizeof(double)));
+  SMB_RC(debug_copy_out(hist_after_4096, b.hist, 2 * kHistBins * sizeof(uint32_t)));
+  SMB_CUDA_OK(cudaMemcpy(&st, b.state, sizeof(IcpState), cudaMemcpyDeviceToHost));
+  if (final_18) {
+    final_18[0] = st.limit; final_18[1] = st.final_score;
+    memcpy(final_18 + 2, st.T_iter, 16 * sizeof(double));
+  }
+  if (final_5) {
+    final_5[0] = st.kept; final_5[1] = st.status; final_5[2] = st.solve_path; final_5[3] = st.iteration;
+    final_5[4] = st.done;
+  }
+  return SM_OK;
+}
+
 // ---- test hooks of the filter chain (filters.cu) ---------------------------------------------------------------------
 int sm_debug_filter_host(const sm_filter_chain* chain, int32_t filter, int32_t op, const float* records, int64_t n,
                          int32_t* iout, float* fout) {
