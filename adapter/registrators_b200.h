@@ -83,6 +83,11 @@ class IcpFastB200 : public Interface {
     return rc == 1;
   }
 
+  // The ICP error minimizer (sm_icp_error_minimizer): SM_ICP_POINT_TO_PLANE, what IcpFast::Align calls
+  // (icp_fast.cc:506-510) and the default, or SM_ICP_POINT_TO_POINT, its ComputePointToPoint (:326-375).  Kept for
+  // every later Align and AlignBatch.  A value outside 0..1 CHECK-fails.
+  void SetErrorMinimizer(int minimizer) { Check(sm_set_icp_error_minimizer(handle_, minimizer)); }
+
   // hooks of AlignBatch (below)
   sm_handle* handle() const { return handle_; }
   // Enable/DisableInnerCompensation are not virtual (interface.h:89-91): the flag is read at every Align
@@ -189,6 +194,10 @@ class NdtWithGicpB200 : public FloatCloudMatcherB200<SM_TYPE_NDT_WITH_GICP> {
 class IcpUsingPointMatcherB200 : public FloatCloudMatcherB200<SM_TYPE_ICP_PM> {
  public:
   explicit IcpUsingPointMatcherB200(int device = 0) : FloatCloudMatcherB200<SM_TYPE_ICP_PM>(device) {}
+  // The error minimizer of the ICP chain (sm_icp_error_minimizer): the reference's loadDefaultConfig builds
+  // PointToPointErrorMinimizer (icp_pointmatcher.cc:202-204) and then installs point-to-plane (:239), the default
+  // here.  A value outside 0..1 CHECK-fails.
+  void SetErrorMinimizer(int minimizer) { CheckRc(sm_set_icp_error_minimizer(handle_, minimizer)); }
 };
 
 // MotionCompensation (builder/map_builder.cc:232-257) on the GPU: same signature as the static

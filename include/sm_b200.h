@@ -121,6 +121,32 @@ enum sm_ndt_search_method {
   SM_NDT_DIRECT1 = 3
 };
 int sm_set_ndt_search_method(sm_handle* h, int32_t method);
+/* The error minimizer of the ICP iteration.  POINT_TO_PLANE (the default) is what IcpFast::Align calls
+ * (registrators/icp_fast.cc:506-510).  POINT_TO_POINT is the reference's ComputePointToPoint (:326-375), a copy of
+ * libpointmatcher's PointToPointErrorMinimizer: over the matches the trim keeps, p the step cloud's point and q its
+ * matched target point (target-mean frame), M = sum (q - qbar)(p - pbar)^T = U S V^T, R = U V^T with the last row
+ * of V^T negated when det R < 0, t = qbar - R pbar, T_iter <- [R t; 0 1] T_iter.  Everything else (tree, search,
+ * trim, convergence test, score) is unchanged, and there is no NaN guard, as in the reference.
+ *   - Normals are still required: SetInputTarget CHECKs them whatever the minimizer (:430); they are not read.
+ *   - With inner compensation the step cloud is de-skewed as before (:487-491); the minimizer has no factor term,
+ *     so f_i is not used.
+ *   - Degenerate M: the 3x3 SVD is written out (csrc/linalg_dev.cuh kabsch_rotation, one-sided Jacobi).  One kept
+ *     match gives M = 0 and R = I.  Where R is not unique (rank-1 M, e.g. collinear matches) the result is the
+ *     rotation that completes U to a right-handed basis as documented there; it attains the optimal objective.
+ *     Every operation of the solve is rounded on its own (no FMA), so the device gives the same bits as the host
+ *     build of the same code.
+ *   - The sums are raw moments about the origin of the target-mean frame, centred in one sweep (DESIGN §4); the
+ *     reference centres the points in a second pass.  The two differ by rounding.
+ * sm_align_info.solve_path reports 3 (Kabsch) or 4 (Kabsch with the reflection fix).
+ * Applies from the next Align on (sm_align, sm_align_async / wait, sm_align_batch and sm_align_pairs alike).
+ * SM_TYPE_FAST_ICP sets it on the handle, SM_TYPE_ICP_PM on the IcpFast chain it composes; every other type returns
+ * SM_ERR_UNSUPPORTED_TYPE.  A value outside 0..1 returns SM_ERR_BAD_ARGUMENT and leaves the setting unchanged.
+ * Not an XML option: sm_print_options does not list it. */
+enum sm_icp_error_minimizer {
+  SM_ICP_POINT_TO_PLANE = 0,
+  SM_ICP_POINT_TO_POINT = 1
+};
+int sm_set_icp_error_minimizer(sm_handle* h, int32_t minimizer);
 /* Interface::GetType (interface.h:106). */
 int sm_get_type(const sm_handle* h);
 
@@ -196,7 +222,8 @@ double sm_get_fitness_score(const sm_handle* h);
 typedef struct sm_align_info {
   int32_t iterations;      /* ICP iterations executed */
   int32_t status;          /* 0 or sm_error */
-  int32_t solve_path;      /* last 6x6 solve: 0 Cholesky, 1 rank-reduced, 2 SVD */
+  int32_t solve_path;      /* last 6x6 solve: 0 Cholesky, 1 rank-reduced, 2 SVD; point-to-point: 3 Kabsch,
+                              4 Kabsch with the reflection fix */
   int32_t reserved;
   int64_t kept;            /* matches kept by the 70 % trim in the last iteration */
   double limit;            /* its squared-distance limit */

@@ -12,6 +12,8 @@
  *     sm_debug_m2dp_host       M2DP's two eigenproblems: PCA axes from the float covariance, [u1; v1] from A and A A^T
  *   device math of the product compiled for the host (the same __host__ __device__ source the kernels call)
  *     sm_debug_solve6_host     SolvePossiblyUnderdeterminedLinearSystem (csrc/linalg_dev.cuh, icp_fast.cc:204-254)
+ *     sm_debug_kabsch_host     the point-to-point minimizer: centring, 3x3 SVD, reflection fix (csrc/linalg_dev.cuh,
+ *                              icp_fast.cc:326-375)
  *     sm_debug_icp_host        per-match normal-equation terms, AngleAxis / quaternion / angularDistance helpers
  *     sm_debug_ndt_leaf        one leaf of the NDT target grid: covariance, eigenvalue inflation, inverse
  *     sm_debug_ndt_term        one (point, voxel) term of computeDerivatives, pclomp float and stock-PCL double forms
@@ -32,6 +34,7 @@
  *     sm_debug_ndt_derivatives the 44 sums of NdtStage::eval (computeDerivatives) at given pose vectors, both forms
  *     sm_debug_ndt_derivatives_search  the same with each of pclomp's four neighbour searches
  *     sm_debug_float_tree_knn  the float tree's exact searches: knn1 (eps = 0) and the 20-NN of the covariances
+ *     sm_debug_icp_iteration_minimizer  the same with the point-to-point minimizer's phases B and C
  *     sm_debug_icp_iteration   one IcpFast iteration phase by phase: the prologue's mean, G0 and Morton order; phase A's
  *                              matches, distances and histogram; phase B's candidates and per-block partial sums;
  *                              phase C's 29 reduced sums, limit, kept count and pose update
@@ -62,6 +65,11 @@ int sm_debug_solve6(int device, const double* A_36, const double* b_6, double* x
 
 /* the same routine compiled for the host (no GPU needed): the source both builds share is csrc/linalg_dev.cuh */
 int sm_debug_solve6_host(const double* A_36, const double* b_6, double* x_6, int32_t* path);
+
+/* The point-to-point minimizer's solve (la::kabsch_from_sums, as icp_finish_kernel<true> runs it) on the host.
+ * sums_32 in the layout phase B/C reduce: [0..2] sum p, [3..5] sum q, [6 + 3i + j] sum q_i p_j, [27] sum sqrt(d2),
+ * [28] count (> 0).  R_9 row-major, t_3; path: 3 Kabsch, 4 Kabsch with the reflection fix. */
+int sm_debug_kabsch_host(const double* sums_32, double* R_9, double* t_3, int32_t* path);
 
 /* f and/or g may be NULL (value-only / gradient-only evaluations of the line search); return < 0 to abort. */
 typedef int (*sm_debug_fdf)(const double* x_6, double* f, double* g_6, void* user);
@@ -240,6 +248,20 @@ int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, cons
                            double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048, uint32_t* cand_cnt, uint64_t* cand_key,
                            double* cand_terms_8, double* partials_29, double* sums_29, double* final_18, int64_t* final_5,
                            uint32_t* hist_after_4096);
+
+/* sm_debug_icp_iteration with the error minimizer of sm_set_icp_error_minimizer (SM_ICP_POINT_TO_PLANE gives
+ * sm_debug_icp_iteration itself; another value returns SM_ERR_BAD_ARGUMENT).  With SM_ICP_POINT_TO_POINT every
+ * iteration runs the point-to-point phases B and C: cand_terms_8 holds {p[3], q[3], 0, sqrt(d2)} per candidate,
+ * partials_29 and sums_29 the moments of la::kabsch_from_sums ([0..2] sum p, [3..5] sum q, [6 + 3i + j] sum q_i p_j,
+ * [27] sum sqrt(d2), [28] count, the rest 0), final_5[2] the solve path 3 / 4. */
+int sm_debug_icp_iteration_minimizer(int device, const double* source_3n, int64_t ns, const double* target_3n,
+                                     const double* normals_3n, int64_t nt, const double* guess_4x4,
+                                     float dist_outlier_ratio, float knn_epsilon, int32_t knn_queries_per_cta,
+                                     int32_t inner_compensation, int32_t error_minimizer, int32_t iteration,
+                                     int32_t* geometry_2, double* prologue_35, uint32_t* perm_n, int32_t* match_n,
+                                     double* d2_n, double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048,
+                                     uint32_t* cand_cnt, uint64_t* cand_key, double* cand_terms_8, double* partials_29,
+                                     double* sums_29, double* final_18, int64_t* final_5, uint32_t* hist_after_4096);
 
 /* ApproxVoxelGrid::filter (pcl::ApproximateVoxelGrid): *m_out points into out_3n (capacity n). */
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,

@@ -44,6 +44,7 @@ SIGNATURES = {
     "sm_print_options": (C.c_int, [_VP, C.c_char_p, C.c_int64]),
     "sm_set_inner_compensation": (C.c_int, [_VP, C.c_int32]),
     "sm_set_ndt_search_method": (C.c_int, [_VP, C.c_int32]),
+    "sm_set_icp_error_minimizer": (C.c_int, [_VP, C.c_int32]),
     "sm_get_type": (C.c_int, [_VP]),
     "sm_set_input_source": (C.c_int, [_VP, _VP, C.c_int64]),
     "sm_set_input_target": (C.c_int, [_VP, _VP, _VP, C.c_int64]),
@@ -85,6 +86,7 @@ SIGNATURES = {
     # include/sm_b200_debug.h (test hooks)
     "sm_debug_solve6": (C.c_int, [C.c_int, _VP, _VP, _VP, _VP]),
     "sm_debug_solve6_host": (C.c_int, [_VP, _VP, _VP, _VP]),
+    "sm_debug_kabsch_host": (C.c_int, [_VP, _VP, _VP, _VP]),
     "sm_debug_bfgs_minimize": (C.c_int, [_VP, _VP, _VP, C.c_double, C.c_int32, _VP, _VP, _VP]),
     "sm_debug_ndt_newton": (C.c_int, [_VP, _VP, _VP, C.c_int32, C.c_float, C.c_double, C.c_double, C.c_double, C.c_int32,
                                       _VP, _VP, _VP, _VP]),
@@ -112,6 +114,8 @@ SIGNATURES = {
                                      C.c_float, _VP, _VP, _VP, _VP]),
     "sm_debug_icp_iteration": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP, C.c_float, C.c_float,
                                          C.c_int32, C.c_int32, C.c_int32] + [_VP] * 16),
+    "sm_debug_icp_iteration_minimizer": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP, C.c_float,
+                                                   C.c_float, C.c_int32, C.c_int32, C.c_int32, C.c_int32] + [_VP] * 16),
     "sm_debug_approx_voxel_grid": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_float, _VP, _VP]),
     "sm_debug_gicp_covariances": (C.c_int, [C.c_int, _VP, C.c_int64, _VP]),
     "sm_debug_gicp_step": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, _VP, _VP, _VP, C.c_int32, _VP, _VP, _VP,

@@ -200,6 +200,8 @@ icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __res
 // -------------------------------------------------------------------------------- phase B
 // kComp: inner compensation (icp_fast.cc:284-289): the points are the iteration's de-skewed ones and every
 // match's Jacobian column is scaled by the point's factor, both for the sums and for the parked candidates
+// kP2P: the point-to-point minimizer (icp_fast.cc:326-375): a match contributes the raw moments of add_p2p_terms_if
+// (no normal is read, and with kComp the factor is not used); a parked candidate is {p, q, 0, sqrt(d2)}
 // SMB_ACC_SECTIONS (diagnostic builds, profiles/accum_sections.py): every block adds the clock64 cycles thread 0
 // spent in each section below to state->stamps[0..5] and 1 to stamps[6], over all iterations and alignments
 #ifdef SMB_ACC_SECTIONS
@@ -209,7 +211,7 @@ constexpr bool kAccSections = false;
 #endif
 enum AccSection { kSecLoads, kSecSelectBin, kSecGather, kSecTerms, kSecCompaction, kSecReduction, kAccSectionCount };
 
-template <bool kComp>
+template <bool kComp, bool kP2P>
 __global__ void __launch_bounds__(kAccThreads)
 icp_accum_kernel(IcpBuffers b, IcpParams p, const double* __restrict__ deskewed) {
   __shared__ uint32_t warp_tot[8];
@@ -243,7 +245,7 @@ icp_accum_kernel(IcpBuffers b, IcpParams p, const double* __restrict__ deskewed)
       sx[r] = in ? src[i] : 0.0;
       sy[r] = in ? src[b.sstride + i] : 0.0;
       sz[r] = in ? src[2 * b.sstride + i] : 0.0;
-      if constexpr (kComp) fac[r] = in ? source_factor(b.src_sort.vals[0][i], p.n_source) : 0.0;
+      if constexpr (kComp && !kP2P) fac[r] = in ? source_factor(b.src_sort.vals[0][i], p.n_source) : 0.0;
     }
   };
   load_pass(0);
@@ -270,14 +272,26 @@ icp_accum_kernel(IcpBuffers b, IcpParams p, const double* __restrict__ deskewed)
       bin[r] = finite_d2(d2[r]) ? dist_bin(d2[r]) : kHistBins;
       use[r] = sel.bin >= 0 && slot[r] >= 0 && bin[r] <= sel.bin;
       const double2* rec = reinterpret_cast<const double2*>(b.kc.pm + (use[r] ? slot[r] : 0));
-      r01[r] = __ldg(rec); r23[r] = __ldg(rec + 1); r45[r] = __ldg(rec + 2);
+      r01[r] = __ldg(rec); r23[r] = __ldg(rec + 1);
+      if constexpr (!kP2P) r45[r] = __ldg(rec + 2);
     }
     mark(kSecGather);
-    double F[kAccPass][6], dot[kAccPass], sq[kAccPass];
+    double F[kAccPass][6], dot[kAccPass], sq[kAccPass];   // kP2P: F = {p, q}, dot = 0
 #pragma unroll
     for (int r = 0; r < kAccPass; ++r) {
       BucketPoint q; BucketNormal n;
       q.x = r01[r].x; q.y = r01[r].y; q.z = r23[r].x;
+      if constexpr (kP2P) {
+        if constexpr (kComp) { F[r][0] = sx[r]; F[r][1] = sy[r]; F[r][2] = sz[r]; }
+        else transform_point(T, sx[r], sy[r], sz[r], F[r][0], F[r][1], F[r][2]);
+        F[r][3] = q.x; F[r][4] = q.y; F[r][5] = q.z;
+        dot[r] = 0.0;
+        sq[r] = sqrt(use[r] ? d2[r] : 0.0);
+        add_p2p_terms_if(acc, F[r], F[r] + 3, sq[r], use[r] && bin[r] < sel.bin);
+        is_cand[r] = use[r] && bin[r] == sel.bin;
+        if (is_cand[r]) atomicAdd(&b.hist2[sub_bin(d2[r])], 1u);
+        continue;
+      }
       n.x = r23[r].y; n.y = r45[r].x; n.z = r45[r].y;
       if constexpr (kComp) {
         compensated_match_terms(sx[r], sy[r], sz[r], q, n, fac[r], F[r], dot[r]);
@@ -513,8 +527,14 @@ void icp_search_launch(const IcpBuffers& b, const IcpParams& p, const double* de
 
 void icp_accum_launch(const IcpBuffers& b, const IcpParams& p, const double* deskewed, cudaStream_t stream) {
   const int nb = icp_accum_blocks(p.n_source);
-  if (p.inner_compensation) icp_accum_kernel<true><<<nb, kAccThreads, 0, stream>>>(b, p, deskewed);
-  else icp_accum_kernel<false><<<nb, kAccThreads, 0, stream>>>(b, p, nullptr);
+  if (p.error_minimizer == kIcpPointToPoint) {
+    if (p.inner_compensation) icp_accum_kernel<true, true><<<nb, kAccThreads, 0, stream>>>(b, p, deskewed);
+    else icp_accum_kernel<false, true><<<nb, kAccThreads, 0, stream>>>(b, p, nullptr);
+  } else if (p.inner_compensation) {
+    icp_accum_kernel<true, false><<<nb, kAccThreads, 0, stream>>>(b, p, deskewed);
+  } else {
+    icp_accum_kernel<false, false><<<nb, kAccThreads, 0, stream>>>(b, p, nullptr);
+  }
 }
 
 int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_iteration, int count,
@@ -538,7 +558,8 @@ int icp_enqueue_iterations(const IcpBuffers& b, const IcpParams& p, int start_it
     icp_accum_launch(b, p, deskewed, stream);
     nvtxRangePop();
     if (events) cudaEventRecord(events[4 * it + 2], stream);
-    nvtxRangePushA("ComputePointToPlane");       // icp_fast.cc:256-323
+    nvtxRangePushA(p.error_minimizer == kIcpPointToPoint ? "ComputePointToPoint"    // icp_fast.cc:326-375
+                                                         : "ComputePointToPlane");  // icp_fast.cc:256-323
     icp_finish_launch(b, p, nb, stream);
     nvtxRangePop();
     if (events) cudaEventRecord(events[4 * it + 3], stream);

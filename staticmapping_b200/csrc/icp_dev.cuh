@@ -313,6 +313,25 @@ __device__ __forceinline__ void add_terms_if(double* acc, const double* Fin, dou
   acc[28] += pred ? 1.0 : 0.0;
 }
 
+// Point-to-point (ComputePointToPoint, icp_fast.cc:326-375): the raw moments of one match about the origin of the
+// target-mean frame in the layout of la::kabsch_from_sums: acc[0..2] += p, acc[3..5] += q, acc[6 + 3i + j] += q_i p_j,
+// acc[27] += sqrt(d2), acc[28] += 1; acc += pred ? terms : 0 like add_terms_if.  p is the step cloud's point
+// (transformed, or de-skewed with inner compensation), q its matched target point.
+__device__ __forceinline__ void add_p2p_terms_if(double* acc, const double* pin, const double* qin, double sq,
+                                                 bool pred) {
+  double p[3], q[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) { p[r] = pred ? pin[r] : 0.0; q[r] = pred ? qin[r] : 0.0; }
+#pragma unroll
+  for (int r = 0; r < 3; ++r) { acc[r] += p[r]; acc[3 + r] += q[r]; }
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) acc[6 + 3 * i + j] += q[i] * p[j];
+  acc[27] += pred ? sq : 0.0;
+  acc[28] += pred ? 1.0 : 0.0;
+}
+
 // Sum 32 per-lane values across the warp: on return lane L holds the warp total of v[L].
 // 31 exchanges instead of the 160 of 32 separate butterflies; the pairing is the butterfly's
 // (offsets 16, 8, 4, 2, 1), so each total is bit-identical to the xor-shuffle reduction.

@@ -10,7 +10,8 @@
 //     the exact limit;
 //   * all partial sums are reduced in a fixed order (deterministic result);
 //   * warp 0: 6x6 solve, pose update, convergence test, score (icp_fast.cc:204-254,
-//     307-321, 377-405, 513-527).  The code is deliberately compact (rolled loops, shared
+//     307-321, 377-405, 513-527); with the point-to-point minimizer (kP2P) lane 0 centres the
+//     moments and runs the 3x3 SVD of la::kabsch_from_sums instead of the solve (:326-375).  The code is deliberately compact (rolled loops, shared
 //     memory): a single warp fetching kilobytes of straight-line code cold costs far more
 //     than the arithmetic.
 // The per-block candidate lists are never flattened: thread t handles the global candidate
@@ -142,10 +143,24 @@ __device__ __forceinline__ void mul4_warp(const double* A, const double* B, doub
 }
 
 // pose update + convergence + score on warp 0 (icp_fast.cc:307-321,377-405,513-527); `st` is
-// the shared-memory copy of the state
+// the shared-memory copy of the state.  kP2P: dT = [R t; 0 1] of la::kabsch_from_sums over the reduced moments
+// (icp_fast.cc:326-375, no NaN guard there), and its return value is the solve path.
+template <bool kP2P>
 __device__ __forceinline__ void update_pose(IcpState* st, const IcpParams& p, SolveSmem& sm, int path,
                                             int lane) {
-  if (lane == 0) {
+  if (kP2P && lane == 0) {
+    double R[9], t[3];
+    st->solve_path = la::kabsch_from_sums(sm.S, R, t);
+#pragma unroll 1
+    for (int i = 0; i < 16; ++i) sm.dT[i] = (i % 5 == 0) ? 1.0 : 0.0;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) sm.dT[r + 4 * c] = R[r * 3 + c];
+      sm.dT[12 + r] = t[r];
+    }
+  }
+  if (!kP2P && lane == 0) {
     const double* x = sm.x;
     st->solve_path = path;
     const double sq = x[0] * x[0] + x[1] * x[1] + x[2] * x[2];
@@ -268,11 +283,14 @@ __device__ __forceinline__ CandTerms load_candidate(const IcpBuffers& b, uint32_
   const double2* o = reinterpret_cast<const double2*>(b.cand_terms + 8 * (int64_t)slot);
   return CandTerms{o[0], o[1], o[2], o[3]};
 }
+template <bool kP2P>
 __device__ __forceinline__ void add_candidate(double* acc, const CandTerms& c, bool member) {
   const double F[6] = {c.a0.x, c.a0.y, c.a1.x, c.a1.y, c.a2.x, c.a2.y};
-  add_terms_if(acc, F, c.a3.x, c.a3.y, member);
+  if constexpr (kP2P) add_p2p_terms_if(acc, F, F + 3, c.a3.y, member);   // {p, q, 0, sqrt(d2)}
+  else add_terms_if(acc, F, c.a3.x, c.a3.y, member);
 }
 
+template <bool kP2P>
 __global__ void __launch_bounds__(kSelThreads)
 icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
   __shared__ IcpState sst;
@@ -355,7 +373,7 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
 #pragma unroll
         for (int q = 0; q < R; ++q) {
           const int sub = (int)((key[q] >> 36) & 2047ull);
-          add_candidate(acc, ct[q], valid[q] && sub < sb);
+          add_candidate<kP2P>(acc, ct[q], valid[q] && sub < sb);
           if (valid[q] && sub == sb) {
             const uint32_t j = atomicAdd(&nkeys, 1u);
             if (j < (uint32_t)kMaxExactKeys) { keys[j] = key[q]; kslot[j] = slot[q]; }
@@ -387,7 +405,7 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
     limit = __longlong_as_double((long long)limit_bits);
 #pragma unroll 1
     for (int i = t; i < nk; i += kSelThreads)   // non-negative doubles order like their bit patterns
-      if (skeys[i] <= limit_bits) add_candidate(acc, load_candidate(b, sslot[i]), true);
+      if (skeys[i] <= limit_bits) add_candidate<kP2P>(acc, load_candidate(b, sslot[i]), true);
   } else {
     // ---- general path (clamp bins, e.g. identical clouds: all d2 == 0): MSB radix select ---
     if (t == 0) { sh_rank = r; limit_bits = 0ull; }
@@ -429,7 +447,7 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
     // ---- members of the quantile bin with d2 <= limit (icp_fast.cc:497-498) ---------------
     for_each_candidate(b, nblocks_b, blk_off, warp_tot, have_scan, [&](uint32_t slot) {
       const double d2 = __longlong_as_double((long long)b.cand_key[slot]);
-      if (d2 <= limit) add_candidate(acc, load_candidate(b, slot), true);
+      if (d2 <= limit) add_candidate<kP2P>(acc, load_candidate(b, slot), true);
     });
   }
   if (t == 0) sst.stamps[4] = clock64();
@@ -477,9 +495,9 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
     }
     return;
   }
-  const int path = solve_warp(solve, lane);
+  const int path = kP2P ? 0 : solve_warp(solve, lane);
   if (lane == 0) sst.stamps[7] = clock64();
-  update_pose(&sst, p, solve, path, lane);
+  update_pose<kP2P>(&sst, p, solve, path, lane);
   if (lane == 0) sst.stamps[8] = clock64();
 #ifdef SMB_FINISH_EXPERIMENT
   {   // how long does the same solve take with its code already fetched?
@@ -501,7 +519,8 @@ icp_finish_kernel(IcpBuffers b, IcpParams p, int nblocks_b) {
 }  // namespace
 
 void icp_finish_launch(const IcpBuffers& b, const IcpParams& p, int nblocks_b, cudaStream_t stream) {
-  icp_finish_kernel<<<1, kSelThreads, 0, stream>>>(b, p, nblocks_b);
+  if (p.error_minimizer == kIcpPointToPoint) icp_finish_kernel<true><<<1, kSelThreads, 0, stream>>>(b, p, nblocks_b);
+  else icp_finish_kernel<false><<<1, kSelThreads, 0, stream>>>(b, p, nblocks_b);
 }
 
 }  // namespace smb

@@ -130,7 +130,7 @@ struct IcpState {
   int iteration;
   int done;               // 1 once converged or max_iteration reached
   int status;             // 0 ok, <0 error (-2 no finite distance, -3 nothing kept)
-  int solve_path;         // 0 LLT, 1 min-norm, 2 SVD (last iteration)
+  int solve_path;         // 0 LLT, 1 min-norm, 2 SVD; point-to-point: 3 Kabsch, 4 with the reflection fix (last iteration)
   int pad;
   long long stamps[12];   // clock64 at the section boundaries of the last finish kernel (diagnostics)
 };
@@ -144,9 +144,14 @@ struct IcpParams {
   int disable_convergence;
   int tree_levels;         // kd_num_levels(n_target, 8): depth of the root-to-leaf path
   int knn_queries_per_cta; // phase A: 0 = one query per thread, else queries per 256-thread CTA
-  int inner_compensation;  // 1: IcpFast::EnableInnerCompensation, the source is de-skewed in every iteration
+  // host-side selectors (no kernel reads them; they pick the instantiations and are part of the graph keys).  Both
+  // are 16 bits so that they share the 4 bytes inner_compensation had as an int: the struct stays 40 bytes with no
+  // padding, and no kernel argument moves.
+  int16_t inner_compensation;  // 1: IcpFast::EnableInnerCompensation, the source is de-skewed in every iteration
+  int16_t error_minimizer;     // kIcpPointToPlane or kIcpPointToPoint (phases B and C)
 };
-static_assert(sizeof(IcpParams) == 40, "inner_compensation takes the tail padding: kernel argument offsets stay put");
+static_assert(sizeof(IcpParams) == 40, "the two 16-bit selectors share inner_compensation's former 4 bytes: kernel argument offsets stay put");
+constexpr int kIcpPointToPlane = 0, kIcpPointToPoint = 1;   // sm_icp_error_minimizer
 
 struct IcpBuffers {
   // target (caller order, SoA, centred in place by the prologue)

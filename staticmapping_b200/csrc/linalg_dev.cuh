@@ -282,6 +282,151 @@ __host__ __device__ inline double quaternion_angular_distance(const double* a, c
   return 2.0 * atan2(sqrt(x * x + y * y + z * z), fabs(w));
 }
 
+// a * b, a + b and a - b rounded on their own: never contracted into an FMA, on the device or the host.  The point-to-
+// point solve below is written with them only (division and sqrt are correctly rounded on both), so the device build
+// inside icp_finish.o (which contracts elsewhere) and the host build give the same bits.
+__host__ __device__ __forceinline__ double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ double sub_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+// ((a0 b0 + a1 b1) + a2 b2), each operation rounded
+__host__ __device__ __forceinline__ double dot3_rn(double a0, double a1, double a2, double b0, double b1, double b2) {
+  return add_rn(add_rn(mul_rn(a0, b0), mul_rn(a1, b1)), mul_rn(a2, b2));
+}
+// a0 b0 - a1 b1, each operation rounded
+__host__ __device__ __forceinline__ double cross_rn(double a0, double b0, double a1, double b1) {
+  return sub_rn(mul_rn(a0, b0), mul_rn(a1, b1));
+}
+
+// The rotation of ComputePointToPoint (icp_fast.cc:353-367) for M = sum (q - qbar)(p - pbar)^T, row-major.
+// M = U S V^T by one-sided Jacobi (Hestenes) on the columns of M, accumulated into V, singular values sorted
+// descending (a stable sort: equal values keep their column order).  u_k = column k / s_k while
+// s_k > 8 eps s_0; the other columns of U complete a right-handed orthonormal basis: u3 = u1 x u2, and at rank 1
+// u2 = normalize(u1 x e_m) with e_m the axis u1 leans on least (the first of equals).  M = 0 gives U = V = I, so R = I.
+// R = U V^T; if det R < 0 the column of V of the smallest singular value is negated (the last row of V^T) and
+// R = U V^T again.  Returns 1 when that reflection fix ran.  Every array index is a constant once the loops are
+// unrolled, so the device keeps it all in registers; every operation is rounded on its own (see mul_rn).
+__host__ __device__ __forceinline__ int kabsch_rotation(const double* M, double* R) {
+  double A[9], V[9], U[9], s[3];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) { A[i] = M[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
+#pragma unroll 1
+  for (int sweep = 0; sweep < 32; ++sweep) {
+    bool rotated = false;
+#pragma unroll
+    for (int pq = 0; pq < 3; ++pq) {
+      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;     // (0,1), (0,2), (1,2)
+      const double alpha = dot3_rn(A[p], A[3 + p], A[6 + p], A[p], A[3 + p], A[6 + p]);
+      const double beta = dot3_rn(A[q], A[3 + q], A[6 + q], A[q], A[3 + q], A[6 + q]);
+      const double gamma = dot3_rn(A[p], A[3 + p], A[6 + p], A[q], A[3 + q], A[6 + q]);
+      if (!(fabs(gamma) > mul_rn(mul_rn(kEps, sqrt(alpha)), sqrt(beta)))) continue;   // orthogonal to working precision
+      rotated = true;
+      const double zeta = sub_rn(beta, alpha) / mul_rn(2.0, gamma);
+      const double t = (zeta >= 0.0 ? 1.0 : -1.0) / add_rn(fabs(zeta), sqrt(add_rn(1.0, mul_rn(zeta, zeta))));
+      const double c = 1.0 / sqrt(add_rn(1.0, mul_rn(t, t))), sn = mul_rn(c, t);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double ap = A[k * 3 + p], aq = A[k * 3 + q];
+        A[k * 3 + p] = cross_rn(c, ap, sn, aq); A[k * 3 + q] = add_rn(mul_rn(sn, ap), mul_rn(c, aq));
+        const double vp = V[k * 3 + p], vq = V[k * 3 + q];
+        V[k * 3 + p] = cross_rn(c, vp, sn, vq); V[k * 3 + q] = add_rn(mul_rn(sn, vp), mul_rn(c, vq));
+      }
+    }
+    if (!rotated) break;
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) s[k] = sqrt(dot3_rn(A[k], A[3 + k], A[6 + k], A[k], A[3 + k], A[6 + k]));
+#pragma unroll
+  for (int pq = 0; pq < 3; ++pq) {                        // bubble sort, descending: (0,1), (1,2), (0,1)
+    const int p = pq == 1 ? 1 : 0, q = p + 1;
+    if (s[p] < s[q]) {
+      const double ts = s[p]; s[p] = s[q]; s[q] = ts;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        double x = A[k * 3 + p]; A[k * 3 + p] = A[k * 3 + q]; A[k * 3 + q] = x;
+        x = V[k * 3 + p]; V[k * 3 + p] = V[k * 3 + q]; V[k * 3 + q] = x;
+      }
+    }
+  }
+  const double tol = mul_rn(8.0 * kEps, s[0]);
+  const int rank = (s[0] > 0.0 ? 1 : 0) + (s[1] > tol ? 1 : 0) + (s[2] > tol ? 1 : 0);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) U[i] = (i % 4 == 0) ? 1.0 : 0.0;
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    if (k < rank) {
+#pragma unroll
+      for (int r = 0; r < 3; ++r) U[r * 3 + k] = A[r * 3 + k] / s[k];
+    }
+  if (rank == 1) {
+    const double a0 = fabs(U[0]), a1 = fabs(U[3]), a2 = fabs(U[6]);
+    const int m = (a0 <= a1 && a0 <= a2) ? 0 : (a1 <= a2 ? 1 : 2);
+    const double e0 = m == 0 ? 1.0 : 0.0, e1 = m == 1 ? 1.0 : 0.0, e2 = m == 2 ? 1.0 : 0.0;
+    const double w0 = cross_rn(U[3], e2, U[6], e1), w1 = cross_rn(U[6], e0, U[0], e2),
+                 w2 = cross_rn(U[0], e1, U[3], e0);   // u1 x e_m
+    const double nw = sqrt(dot3_rn(w0, w1, w2, w0, w1, w2));
+    U[1] = w0 / nw; U[4] = w1 / nw; U[7] = w2 / nw;
+  }
+  if (rank == 1 || rank == 2) {
+    U[2] = cross_rn(U[3], U[7], U[6], U[4]);
+    U[5] = cross_rn(U[6], U[1], U[0], U[7]);
+    U[8] = cross_rn(U[0], U[4], U[3], U[1]);
+  }
+  int fix = 0;
+#pragma unroll 1
+  for (int pass = 0; pass < 2; ++pass) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) R[r * 3 + c] = dot3_rn(U[r * 3], U[r * 3 + 1], U[r * 3 + 2], V[c * 3], V[c * 3 + 1], V[c * 3 + 2]);
+    const double det = add_rn(sub_rn(mul_rn(R[0], cross_rn(R[4], R[8], R[5], R[7])),
+                                      mul_rn(R[1], cross_rn(R[3], R[8], R[5], R[6]))),
+                              mul_rn(R[2], cross_rn(R[3], R[7], R[4], R[6])));
+    if (pass == 1 || !(det < 0.0)) break;
+    fix = 1;
+    V[2] = -V[2]; V[5] = -V[5]; V[8] = -V[8];
+  }
+  return fix;
+}
+
+// Number of sums of one point-to-point match record.  S[0..2] = sum p, S[3..5] = sum q, S[6 + 3i + j] =
+// sum q_i p_j (all about the origin of the target-mean frame), S[27] = sum sqrt(d2), S[28] = count; the rest is 0.
+// The centring (icp_fast.cc:337-350) as one sweep: pbar = S[0..2] / n, qbar = S[3..5] / n,
+// M_ij = S[6+3i+j] - S[3+i] * pbar_j (one rounding each: one kept match gives M = 0 exactly), then
+// R = kabsch_rotation(M) and t = qbar - R pbar.  Returns the solve path: 3 Kabsch, 4 Kabsch with the reflection fix.
+// Every operation is rounded on its own, so the device and the host give the same bits.
+__host__ __device__ __forceinline__ int kabsch_from_sums(const double* S, double* R, double* t) {
+  const double inv_n = 1.0 / S[28];
+  double pm[3], qm[3], M[9];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) { pm[i] = mul_rn(S[i], inv_n); qm[i] = mul_rn(S[3 + i], inv_n); }
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) M[i * 3 + j] = sub_rn(S[6 + 3 * i + j], mul_rn(S[3 + i], pm[j]));
+  const int fix = kabsch_rotation(M, R);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) t[i] = sub_rn(qm[i], dot3_rn(R[i * 3], R[i * 3 + 1], R[i * 3 + 2], pm[0], pm[1], pm[2]));
+  return fix ? 4 : 3;
+}
+
 // column-major 4x4 product, k-order accumulation
 __host__ __device__ inline void mul4(const double* A, const double* B, double* C) {
   double out[16];

@@ -117,6 +117,7 @@ struct GraphCache {
 struct IcpFastMatcher {
   IcpOptions opt;
   bool inner_compensation = false;  // Interface::EnableInnerCompensation; set on IcpFast handles only
+  int error_minimizer = kIcpPointToPlane;   // sm_set_icp_error_minimizer
   DevBuf kdws;                      // k-d build workspace of the target tree (and of type 1's score tree)
   DevBuf stage, stage_src, stage_tgt, stage_nrm, tgt_raw, nrm, src_raw;
   IcpFastBuffers bufs;
@@ -396,6 +397,7 @@ int icp_begin(sm_handle* h, IcpFastMatcher& f, const double* guess) {
   p.knn_queries_per_cta = f.opt.knn_queries_per_cta;
   p.tree_levels = levels;
   p.inner_compensation = f.inner_compensation ? 1 : 0;
+  p.error_minimizer = (int16_t)f.error_minimizer;
   r.deskewed = f.inner_compensation ? (double*)f.bufs.deskewed.p : nullptr;
   if (levels > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "target too large (tree deeper than 24 levels)");
 
@@ -405,7 +407,7 @@ int icp_begin(sm_handle* h, IcpFastMatcher& f, const double* guess) {
   r.graphs = f.opt.use_graphs && !f.opt.profile_kernels;
   r.key.clear();
   key_append(r.key, b); key_append(r.key, p); key_append(r.key, f.bufs.guess.p); key_append(r.key, f.kdws.p);
-  key_append(r.key, r.deskewed);   // p.inner_compensation is part of p
+  key_append(r.key, r.deskewed);   // p.inner_compensation and p.error_minimizer are part of p
   if (r.graphs) {
     H_RC(run_graphed(h, f.g_prologue, r.key, [&]() {
       return icp_prologue(b, p, (const double*)f.bufs.guess.p, ws, f.bufs.tree, h->stream);
@@ -828,6 +830,16 @@ int sm_set_option(sm_handle* h, const char* name, const char* text) {
 int sm_set_inner_compensation(sm_handle* h, int32_t enable) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
   if (IcpFastMatcher* f = h->as<IcpFastMatcher>()) f->inner_compensation = enable != 0;   // the other types ignore it
+  return SM_OK;
+}
+
+int sm_set_icp_error_minimizer(sm_handle* h, int32_t minimizer) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  IcpFastMatcher* f = h->icp_chain();
+  if (!f) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetErrorMinimizer: IcpFast (type 6) and IcpUsingPointMatcher (type 1) only");
+  if (minimizer < SM_ICP_POINT_TO_PLANE || minimizer > SM_ICP_POINT_TO_POINT)
+    return fail(h, SM_ERR_BAD_ARGUMENT, "SetErrorMinimizer: minimizer must be 0..1");
+  f->error_minimizer = minimizer;
   return SM_OK;
 }
 

@@ -54,6 +54,14 @@ int sm_debug_solve6_host(const double* A, const double* b, double* x, int32_t* p
   return SM_OK;
 }
 
+// test hook: the point-to-point minimizer's centring, 3x3 SVD and reflection fix (csrc/linalg_dev.cuh
+// kabsch_from_sums, the code icp_finish_kernel<true> runs on lane 0) compiled for the HOST
+int sm_debug_kabsch_host(const double* sums, double* R, double* t, int32_t* path) {
+  if (!sums || !R || !t || !path) return SM_ERR_BAD_ARGUMENT;
+  *path = la::kabsch_from_sums(sums, R, t);
+  return SM_OK;
+}
+
 // test hook: the NDT Newton loop of the product (ndt_host.h newton_loop, the function ndt_run drives the device
 // with) over a caller-supplied evaluation — no GPU involved
 int sm_debug_ndt_newton(sm_debug_ndt_eval fn, void* user, const double* guess_4x4, int32_t n_source, float resolution,
@@ -681,14 +689,16 @@ static int debug_copy_out(void* dst, const void* src, size_t bytes) {
   return SM_OK;
 }
 
-int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, const double* target_3n,
-                           const double* normals_3n, int64_t nt, const double* guess_4x4, float dist_outlier_ratio,
-                           float knn_epsilon, int32_t knn_queries_per_cta, int32_t inner_compensation, int32_t iteration,
-                           int32_t* geometry_2, double* prologue_35, uint32_t* perm_n, int32_t* match_n, double* d2_n,
-                           double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048, uint32_t* cand_cnt, uint64_t* cand_key,
-                           double* cand_terms_8, double* partials_29, double* sums_29, double* final_18, int64_t* final_5,
-                           uint32_t* hist_after_4096) {
+int sm_debug_icp_iteration_minimizer(int device, const double* source_3n, int64_t ns, const double* target_3n,
+                                     const double* normals_3n, int64_t nt, const double* guess_4x4,
+                                     float dist_outlier_ratio, float knn_epsilon, int32_t knn_queries_per_cta,
+                                     int32_t inner_compensation, int32_t error_minimizer, int32_t iteration,
+                                     int32_t* geometry_2, double* prologue_35, uint32_t* perm_n, int32_t* match_n,
+                                     double* d2_n, double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048,
+                                     uint32_t* cand_cnt, uint64_t* cand_key, double* cand_terms_8, double* partials_29,
+                                     double* sums_29, double* final_18, int64_t* final_5, uint32_t* hist_after_4096) {
   if (!geometry_2 || ns <= 0 || ns > (1 << 30)) return SM_ERR_BAD_ARGUMENT;
+  if (error_minimizer < SM_ICP_POINT_TO_PLANE || error_minimizer > SM_ICP_POINT_TO_POINT) return SM_ERR_BAD_ARGUMENT;
   const int nb = icp_accum_blocks((int)ns);
   geometry_2[0] = nb; geometry_2[1] = dev::kAccTile;
   if (!source_3n) return SM_OK;
@@ -722,6 +732,7 @@ int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, cons
   p.knn_queries_per_cta = knn_queries_per_cta;
   p.tree_levels = kd_num_levels((int)nt, 8);
   p.inner_compensation = comp ? 1 : 0;
+  p.error_minimizer = (int16_t)error_minimizer;
   double* deskewed = comp ? (double*)f.deskewed.p : nullptr;
   SMB_CUDA_OK(cudaMemcpy(f.guess.p, guess_4x4, 16 * sizeof(double), cudaMemcpyHostToDevice));
   SMB_CUDA_OK(cudaMemset(b.sums, 0xff, dev::kNumSums * sizeof(double)));   // all-ones until phase C writes it
@@ -791,6 +802,20 @@ int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, cons
     final_5[4] = st.done;
   }
   return SM_OK;
+}
+
+int sm_debug_icp_iteration(int device, const double* source_3n, int64_t ns, const double* target_3n,
+                           const double* normals_3n, int64_t nt, const double* guess_4x4, float dist_outlier_ratio,
+                           float knn_epsilon, int32_t knn_queries_per_cta, int32_t inner_compensation, int32_t iteration,
+                           int32_t* geometry_2, double* prologue_35, uint32_t* perm_n, int32_t* match_n, double* d2_n,
+                           double* pm_6n, uint32_t* hist_2048, uint32_t* hist2_2048, uint32_t* cand_cnt, uint64_t* cand_key,
+                           double* cand_terms_8, double* partials_29, double* sums_29, double* final_18, int64_t* final_5,
+                           uint32_t* hist_after_4096) {
+  return sm_debug_icp_iteration_minimizer(device, source_3n, ns, target_3n, normals_3n, nt, guess_4x4,
+                                          dist_outlier_ratio, knn_epsilon, knn_queries_per_cta, inner_compensation,
+                                          SM_ICP_POINT_TO_PLANE, iteration, geometry_2, prologue_35, perm_n, match_n,
+                                          d2_n, pm_6n, hist_2048, hist2_2048, cand_cnt, cand_key, cand_terms_8,
+                                          partials_29, sums_29, final_18, final_5, hist_after_4096);
 }
 
 // ---- test hooks of the filter chain (filters.cu) ---------------------------------------------------------------------

@@ -49,6 +49,14 @@ class NeighborSearchMethod(enum.IntEnum):
     DIRECT1 = 3
 
 
+class ErrorMinimizer(enum.IntEnum):
+    """The ICP iteration's error minimizer, for IcpFast / IcpUsingPointMatcher.SetErrorMinimizer.
+    POINT_TO_PLANE (the default) is what the reference runs; POINT_TO_POINT is its ComputePointToPoint
+    (icp_fast.cc:326-375), libpointmatcher's PointToPointErrorMinimizer."""
+    POINT_TO_PLANE = 0
+    POINT_TO_POINT = 1
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
@@ -236,6 +244,11 @@ class IcpFast(Interface):
                                                   cloud.normals.ctypes.data,
                                                   cloud.points.shape[0]), "SetInputTarget")
 
+    def SetErrorMinimizer(self, minimizer):
+        """An ErrorMinimizer; applies from the next Align on.  Target normals are still required (icp_fast.cc:430)
+        but point-to-point does not read them.  See sm_set_icp_error_minimizer in include/sm_b200.h."""
+        self._check(self._lib.sm_set_icp_error_minimizer(self._h, int(minimizer)), "SetErrorMinimizer")
+
     # device-resident variants (pointers to 3xN column-major doubles in this GPU's memory)
     def SetInputSourceDevice(self, dev_ptr: int, n: int):
         self._check(self._lib.sm_set_input_source_device(self._h, dev_ptr, n), "SetInputSource")
@@ -333,6 +346,12 @@ class IcpUsingPointMatcher(Ndt):
         if ymal_file:
             raise CheckFailure("IcpUsingPointMatcher: YAML configs are not supported, only loadDefaultConfig()")
         super().__init__(device)
+
+    def SetErrorMinimizer(self, minimizer):
+        """An ErrorMinimizer for the ICP chain of the stand-in (the reference's loadDefaultConfig builds
+        PointToPointErrorMinimizer, icp_pointmatcher.cc:202-204, before it installs point-to-plane, :239);
+        applies from the next Align on."""
+        self._check(self._lib.sm_set_icp_error_minimizer(self._h, int(minimizer)), "SetErrorMinimizer")
 
     def Align(self, guess):
         if self._source is None or self._target is None:
