@@ -14,6 +14,7 @@
 #include <stdio.h>
 
 #include <algorithm>
+#include <limits>
 #include <memory>
 #include <string>
 #include <vector>
@@ -367,6 +368,41 @@ inline void CalculateNormalsB200(data::EigenPointCloud* cloud, int device = 0) {
   cloud->points = pts.leftCols(m);
   cloud->normals = nrm.leftCols(m);
 }
+
+// libnabo's Nabo::NearestNeighbourSearch<double> with KDTREE_LINEAR_HEAP, searched on the GPU: construct it where the
+// reference calls NNS::create(cloud, 3, KDTREE_LINEAR_HEAP, 0, {bucketSize}) and call knn() as NNS::knn.  Like libnabo
+// it keeps a reference to `cloud`, which must outlive it; the tree is built on the device at every knn() call.
+// indices (int32, e.g. Eigen::MatrixXi) and dists2 (double) must be sized k x query.cols(), as libnabo requires; k
+// 1..64.  Rows past the neighbours found are -1 / +inf (libnabo's InvalidIndex / InvalidValue).
+class KnnB200 {
+ public:
+  enum SearchOptionFlags { ALLOW_SELF_MATCH = SM_KNN_ALLOW_SELF_MATCH, SORT_RESULTS = SM_KNN_SORT_RESULTS };
+
+  explicit KnnB200(const Eigen::MatrixXd& cloud, unsigned bucket_size = 8, int device = 0)
+      : cloud_(cloud), bucket_size_(static_cast<int>(bucket_size)), device_(device) {
+    CHECK_EQ(cloud.rows(), 3);
+  }
+
+  template <class IndexMatrix, class DistMatrix>
+  void knn(const Eigen::MatrixXd& query, IndexMatrix& indices, DistMatrix& dists2, int k = 1, double epsilon = 0.0,
+           unsigned option_flags = 0, double max_radius = std::numeric_limits<double>::infinity()) const {
+    CHECK_EQ(query.rows(), 3);
+    CHECK_EQ(static_cast<long>(indices.rows()), static_cast<long>(k));
+    CHECK_EQ(static_cast<long>(indices.cols()), static_cast<long>(query.cols()));
+    CHECK_EQ(static_cast<long>(dists2.rows()), static_cast<long>(k));
+    CHECK_EQ(static_cast<long>(dists2.cols()), static_cast<long>(query.cols()));
+    static_assert(sizeof(*indices.data()) == sizeof(int32_t), "indices: 32-bit integers, as libnabo's IndexMatrix");
+    const int rc = sm_knn(device_, cloud_.data(), static_cast<int64_t>(cloud_.cols()), query.data(),
+                          static_cast<int64_t>(query.cols()), k, epsilon, max_radius, option_flags, bucket_size_,
+                          reinterpret_cast<int32_t*>(indices.data()), dists2.data());
+    CHECK_EQ(rc, 0) << "sm_knn failed (" << rc << ")";
+  }
+
+ private:
+  const Eigen::MatrixXd& cloud_;
+  int bucket_size_;
+  int device_;
+};
 
 }  // namespace registrator
 }  // namespace static_map

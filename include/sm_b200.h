@@ -266,6 +266,29 @@ const char* sm_last_error(const sm_handle* h);
 int sm_knn1(int device, const double* target_3xn, int64_t n_target, const double* query_3xn,
             int64_t n_query, double epsilon, int bucket_size, int32_t* ids, double* dists2);
 
+/* libnabo's k-nearest-neighbour search: NNS::create(target, 3, KDTREE_LINEAR_HEAP, 0, {bucketSize}) +
+ * knn(query, indices, dists2, k, epsilon, optionFlags, maxRadius), on the tree sm_knn1 builds.  It is what the
+ * reference's k > 1 and radius searches call (libpointmatcher's SamplingSurfaceNormalDataPointsFilter knn 7,
+ * KDTreeMatcher's maxDist, icp_pointmatcher.cc:178,186-189).  Rules (libnabo 1.0.7, restated in
+ * tests/cpp/knn_oracle.cc): a point enters the sorted k-list iff d2 <= max_radius^2, d2 < the k-th entry and, without
+ * SM_KNN_ALLOW_SELF_MATCH, d2 > DBL_EPSILON; it goes after every entry of equal distance (the earlier-visited one
+ * first).  A far side is visited iff rd <= max_radius^2 and rd * (1 + epsilon)^2 < the k-th entry.
+ * ids / dists2: k x n_query column-major (libnabo's MatrixXi(k, nQ)), i.e. row i of an n_query x k row-major array
+ * holds query i's neighbours, ascending.  SORT_RESULTS is accepted and changes nothing: the list is always sorted.
+ * When fewer than k points qualify (k > n_target, the radius, self-match exclusion) the rest of the row is
+ * -1 / +inf.  Whether libnabo itself accepts k > n_target, and how it fills such a row, is not verified here.
+ * SM_ERR_BAD_ARGUMENT: k outside 1..64, epsilon < 0 or NaN, max_radius < 0 or NaN, bucket_size outside 2..8, a flag
+ * bit other than the two below, n_target < 1.  The _device form takes device pointers (3xN clouds and the outputs),
+ * runs on `cuda_stream` (a cudaStream_t, NULL = default stream) and returns after that stream has finished. */
+#define SM_KNN_ALLOW_SELF_MATCH 1u   /* NNS::ALLOW_SELF_MATCH */
+#define SM_KNN_SORT_RESULTS 2u       /* NNS::SORT_RESULTS */
+int sm_knn(int device, const double* target_3xn, int64_t n_target, const double* query_3xn, int64_t n_query,
+           int32_t k, double epsilon, double max_radius, uint32_t flags, int bucket_size, int32_t* ids,
+           double* dists2);
+int sm_knn_device(int device, const double* target_3xn, int64_t n_target, const double* query_3xn, int64_t n_query,
+                  int32_t k, double epsilon, double max_radius, uint32_t flags, int bucket_size, int32_t* ids,
+                  double* dists2, void* cuda_stream);
+
 /* EigenPointCloud::CalculateNormals (builder/data/cloud_types.cc:347-368): median-split
  * the cloud into leaves of <= 7 points, fit n.p = 1 per leaf, keep one point (the leaf
  * mean) + unit normal per valid leaf, survivors in ascending order of the smallest

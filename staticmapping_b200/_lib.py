@@ -64,6 +64,10 @@ SIGNATURES = {
     "sm_set_stream": (C.c_int, [_VP, _VP]),
     "sm_last_error": (C.c_char_p, [_VP]),
     "sm_knn1": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_double, C.c_int, _VP, _VP]),
+    "sm_knn": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, C.c_double, C.c_double, C.c_uint32,
+                         C.c_int, _VP, _VP]),
+    "sm_knn_device": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, C.c_double, C.c_double,
+                                C.c_uint32, C.c_int, _VP, _VP, _VP]),
     "sm_calculate_normals": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.POINTER(C.c_int64)]),
     "sm_motion_compensation": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _DP, _VP]),
     "sm_motion_compensation_device": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _DP, _VP, _VP]),

@@ -220,6 +220,12 @@ int icp_accum_blocks(int n_source);
 int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, double max_error2,
               int32_t* ids, double* d2, cudaStream_t stream, int queries_per_cta = 0, int4* items = nullptr);
 
+// ---- knn.cu ------------------------------------------------------------------------------
+// libnabo's k-NN (KDTREE_LINEAR_HEAP) over an already built tree (compact layout incl. pid), k = 1..64: ids / d2 are
+// nq x k row-major, each row ascending, (-1, +inf) where fewer than k points qualify.  max_radius2 = maxRadius^2.
+int knn_k_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, int k, double max_error2,
+                double max_radius2, bool allow_self_match, int32_t* ids, double* d2, cudaStream_t stream);
+
 // ---- motion.cu ---------------------------------------------------------------------------
 // one iteration's de-skewed source of IcpFast with inner compensation: out = Interp(T_iter, f_i) (x) src0_i
 void icp_deskew_launch(const IcpBuffers& b, const IcpParams& p, double* out, cudaStream_t stream);

@@ -1096,4 +1096,61 @@ static int knn1_impl(int device, const double* target, int64_t nt, const double*
   return SM_OK;
 }
 
+// sm_knn / sm_knn_device: the tree of sm_knn1, then knn_k_query.  Host clouds go through a staging buffer on the
+// default stream; device clouds are read in place and the results written to the caller's buffers on its stream.
+static int knn_impl(int device, const double* target, int64_t nt, const double* query, int64_t nq, int32_t k,
+                    double epsilon, double max_radius, uint32_t flags, int bucket, int32_t* ids, double* d2,
+                    bool on_device, cudaStream_t s) {
+  if (!target || !query || !ids || !d2 || nt <= 0 || nt > (1 << 30) || nq < 0 || nq > (1 << 30) || k < 1 ||
+      k > 64 || !(epsilon >= 0.0) || !(max_radius >= 0.0) || bucket < 2 || bucket > 8 ||
+      (flags & ~(uint32_t)(SM_KNN_ALLOW_SELF_MATCH | SM_KNN_SORT_RESULTS)) != 0u)
+    return SM_ERR_BAD_ARGUMENT;
+  if (kd_num_levels((int)nt, bucket) > 24) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  const int64_t ts = pad64(nt), qs = pad64(nq > 0 ? nq : 1);
+  DevBuf stage, tgt, qry, kdws, ids_d, d2_d;
+  KdCompactTree tree;
+  if (!on_device) SMB_RC(stage.reserve((size_t)3 * (size_t)(nt > nq ? nt : nq) * sizeof(double)));
+  SMB_RC(tgt.reserve((size_t)3 * ts * sizeof(double)));
+  SMB_RC(qry.reserve((size_t)3 * qs * sizeof(double)));
+  SMB_RC(tree.reserve((int)nt, bucket, KdCompactTree::kIds));
+  KdWorkspace ws;
+  SMB_RC(ws.carve(kdws, (int)nt, bucket));
+  const size_t n_out = (size_t)(nq > 0 ? nq : 1) * (size_t)k;
+  if (!on_device) {
+    SMB_RC(ids_d.reserve(n_out * sizeof(int32_t)));
+    SMB_RC(d2_d.reserve(n_out * sizeof(double)));
+  }
+  SMB_RC(upload_soa(target, nt, on_device, stage, (double*)tgt.p, ts, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  SMB_RC(tree.build((const double*)tgt.p, nullptr, ts, (int)nt, bucket, ws, s));
+  if (nq > 0) {
+    SMB_RC(upload_soa(query, nq, on_device, stage, (double*)qry.p, qs, s));
+    int32_t* ids_out = on_device ? ids : (int32_t*)ids_d.p;
+    double* d2_out = on_device ? d2 : (double*)d2_d.p;
+    SMB_RC(knn_k_query(tree.view(), (const double*)qry.p, qs, (int)nq, k, (1.0 + epsilon) * (1.0 + epsilon),
+                       max_radius * max_radius, (flags & SM_KNN_ALLOW_SELF_MATCH) != 0u, ids_out, d2_out, s));
+    if (!on_device) {
+      SMB_CUDA_OK(cudaMemcpyAsync(ids, ids_d.p, (size_t)nq * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+      SMB_CUDA_OK(cudaMemcpyAsync(d2, d2_d.p, (size_t)nq * k * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+  }
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  return SM_OK;
+}
+
+int sm_knn(int device, const double* target_3xn, int64_t n_target, const double* query_3xn, int64_t n_query,
+           int32_t k, double epsilon, double max_radius, uint32_t flags, int bucket_size, int32_t* ids,
+           double* dists2) {
+  return knn_impl(device, target_3xn, n_target, query_3xn, n_query, k, epsilon, max_radius, flags, bucket_size, ids,
+                  dists2, false, nullptr);
+}
+
+int sm_knn_device(int device, const double* target_3xn, int64_t n_target, const double* query_3xn, int64_t n_query,
+                  int32_t k, double epsilon, double max_radius, uint32_t flags, int bucket_size, int32_t* ids,
+                  double* dists2, void* cuda_stream) {
+  return knn_impl(device, target_3xn, n_target, query_3xn, n_query, k, epsilon, max_radius, flags, bucket_size, ids,
+                  dists2, true, (cudaStream_t)cuda_stream);
+}
+
 }  // extern "C"

@@ -471,6 +471,33 @@ def knn1(target, query, epsilon=3.16, bucket_size=8, device=0, queries_per_cta=0
     return ids, d2
 
 
+def knn(target, query, k, epsilon=0.0, max_radius=float("inf"), allow_self_match=True, bucket_size=8, device=0):
+    """libnabo's k-nearest-neighbour search on the GPU: NNS::create(target, 3, KDTREE_LINEAR_HEAP) + knn(query, k,
+    epsilon, flags, max_radius), k = 1..64.  target / query: (n, 3) float64.  Returns (ids int32, d2 float64), each of
+    shape (n_query, k): row i holds query i's neighbours in ascending squared distance, (-1, +inf) where fewer than k
+    points lie within max_radius (or the target is smaller than k).  allow_self_match=False drops points at squared
+    distance <= DBL_EPSILON (libnabo's ALLOW_SELF_MATCH flag unset)."""
+    lib = _lib.lib()
+    t = np.ascontiguousarray(np.asarray(target, dtype=np.float64))
+    q = np.ascontiguousarray(np.asarray(query, dtype=np.float64))
+    if t.ndim != 2 or t.shape[1] != 3 or q.ndim != 2 or q.shape[1] != 3:
+        raise ValueError("knn needs (n, 3) target and query clouds")
+    kk = int(k)
+    ids = np.empty((q.shape[0], max(kk, 1)), dtype=np.int32)
+    d2 = np.empty((q.shape[0], max(kk, 1)), dtype=np.float64)
+    flags = 1 if allow_self_match else 0
+    rc = lib.sm_knn(device, t.ctypes.data, t.shape[0], q.ctypes.data, q.shape[0], kk, float(epsilon),
+                    float(max_radius), flags, int(bucket_size), ids.ctypes.data, d2.ctypes.data)
+    if rc == -20:
+        raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
+    if rc == -1:
+        raise ValueError(f"sm_knn rejected its arguments (k={k}, epsilon={epsilon}, max_radius={max_radius}, "
+                         f"bucket_size={bucket_size}, n_target={t.shape[0]})")
+    if rc != 0:
+        raise RuntimeError(f"sm_knn failed with {rc}")
+    return ids, d2
+
+
 def CalculateNormals(points, device=0) -> EigenCloud:
     """EigenPointCloud::CalculateNormals on the GPU (cloud_types.cc:347-368): returns the
     decimated cloud (one mean point + unit normal per valid <=7-point leaf)."""
