@@ -270,7 +270,7 @@ int sm_knn1(int device, const double* target_3xn, int64_t n_target, const double
  * knn(query, indices, dists2, k, epsilon, optionFlags, maxRadius), on the tree sm_knn1 builds.  It is what the
  * reference's k > 1 and radius searches call (libpointmatcher's SamplingSurfaceNormalDataPointsFilter knn 7,
  * KDTreeMatcher's maxDist, icp_pointmatcher.cc:178,186-189).  Rules (libnabo 1.0.7, restated in
- * tests/cpp/knn_oracle.cc): a point enters the sorted k-list iff d2 <= max_radius^2, d2 < the k-th entry and, without
+ * oracle/knn_oracle.cc): a point enters the sorted k-list iff d2 <= max_radius^2, d2 < the k-th entry and, without
  * SM_KNN_ALLOW_SELF_MATCH, d2 > DBL_EPSILON; it goes after every entry of equal distance (the earlier-visited one
  * first).  A far side is visited iff rd <= max_radius^2 and rd * (1 + epsilon)^2 < the k-th entry.
  * ids / dists2: k x n_query column-major (libnabo's MatrixXi(k, nQ)), i.e. row i of an n_query x k row-major array

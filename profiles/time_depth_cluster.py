@@ -7,7 +7,7 @@ column full height: the deepest BFS the grid allows with its +-2 column hops), R
   device_ms   per run, the summed duration of its kernels in a torch.profiler trace (CUDA activities) of PROF more runs
   kernels     per kernel name, the mean duration per run in that trace
   levels      BFS levels of the deepest cluster (test hook sm_debug_depth_cluster)
-  cpu_ms      the sequential C++ restatement (tests/cpp/depth_cluster_oracle.cc) on one host core, best of 3
+  cpu_ms      the sequential C++ restatement (oracle/depth_cluster_oracle.cc) on one host core, best of 3
 Prints the card's name, power limit and clocks with the numbers, and one JSON line at the end."""
 import ctypes as C
 import json

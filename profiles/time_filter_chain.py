@@ -7,7 +7,7 @@ runs each:
               read-back and its synchronise included), median of a round's runs
   host_ms     host clock around sm_filter_chain_run (upload, the same stages, download; it ends in a synchronise)
   kernels     per kernel name, summed duration in a torch.profiler trace (CUDA activities) of one more device run
-  cpu_ms      the sequential C++ restatement (tests/cpp/filters_oracle.cc) on one host core, best of 3
+  cpu_ms      the sequential C++ restatement (oracle/filters_oracle.cc) on one host core, best of 3
 Also: the population of the densest GroundRemoval2 cell of the scan (what one thread of gr2_cell_kernel walks) and the
 longest list of occupied cells in a segment (what one thread of gr2_fit_kernel walks), from the stage hook.
 Prints the card's name, power limit and clocks with the numbers, a markdown table, and one JSON line at the end."""

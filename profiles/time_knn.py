@@ -3,7 +3,7 @@
 (about 107 000 points), eps = 3.16 as IcpFast searches and eps = 0, k = 1 (with sm_knn1 beside it), 7, 8, 20 and 64.
   call_ms    median host time of one sm_knn_device call (device clouds, tree build included), REPS calls
   kernel_ms  device time of the search kernel alone (torch.profiler, a separate pass)
-  oracle_ms  one call of the CPU oracle (tests/cpp/knn_oracle.cc) on all host cores
+  oracle_ms  one call of the CPU oracle (oracle/knn_oracle.cc) on all host cores
 Prints the card name, power limit and SM clock with the numbers, and one JSON line at the end."""
 import ctypes as C
 import json, os, subprocess, sys, time

@@ -1,43 +1,20 @@
-"""ctypes binding of tests/cpp/icp_compensation_oracle.cc: IcpFast::Align with EnableInnerCompensation, restated
-on the CPU over libsm_oracle.so's pieces.  TEST INFRASTRUCTURE.  The library is compiled on first use into a
-per-user temporary directory (keyed by the source's hash), so a read-only tree works."""
+"""ctypes binding of oracle/icp_compensation_oracle.cc: IcpFast::Align with EnableInnerCompensation, restated
+on the CPU over libsm_oracle.so's pieces.  TEST INFRASTRUCTURE."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
 import oracle_lib as O
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_SRC = os.path.join(_ROOT, "tests", "cpp", "icp_compensation_oracle.cc")
-_ORACLE_DIR = os.path.join(_ROOT, "oracle")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        O.lib()                                          # builds libsm_oracle.so if needed; loaded first
-        with open(_SRC, "rb") as f:
-            tag = hashlib.sha256(f.read() + _ORACLE_DIR.encode()).hexdigest()[:16]   # the rpath is part of it
-        out_dir = os.path.join(tempfile.gettempdir(), f"sm_icp_comp_oracle_{os.getuid()}")
-        os.makedirs(out_dir, exist_ok=True)
-        so = os.path.join(out_dir, f"libsm_icp_comp_oracle_{tag}.so")
-        if not os.path.exists(so):
-            cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-            tmp = so + f".{os.getpid()}.tmp"
-            # the flags of oracle/Makefile: no FMA contraction, so the arithmetic is the written one
-            subprocess.check_call([cxx, "-O2", "-fopenmp", "-fPIC", "-std=c++17", "-ffp-contract=off", "-shared",
-                                   "-I", _ORACLE_DIR, _SRC, "-o", tmp, "-L", _ORACLE_DIR, "-l:libsm_oracle.so",
-                                   "-Wl,-rpath," + _ORACLE_DIR])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
+        _lib = O.lib()
         dp, ip = C.POINTER(C.c_double), C.POINTER(C.c_int32)
         _lib.sm_oracle_icp_fast_align_compensated.argtypes = [
             dp, C.c_int64, dp, dp, C.c_int64, dp, C.POINTER(O.IcpOptions), C.c_int32, dp, dp, ip,

@@ -1,21 +1,14 @@
-"""ctypes binding of tests/cpp/depth_cluster_oracle.cc: RangeImage::DepthCluster modelled on the CPU,
-sequential.  TEST INFRASTRUCTURE.  Compiled on first use into a per-user temporary directory (keyed by the source's
-hash), so a read-only tree works."""
+"""ctypes binding of oracle/depth_cluster_oracle.cc: RangeImage::DepthCluster modelled on the CPU,
+sequential.  TEST INFRASTRUCTURE."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
 import oracle_filters as OF
+import oracle_lib as O
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_SRC = os.path.join(_ROOT, "tests", "cpp", "depth_cluster_oracle.cc")
 _lib = None
 
 
@@ -26,17 +19,7 @@ class CheckFailed(RuntimeError):
 def lib():
     global _lib
     if _lib is None:
-        with open(_SRC, "rb") as f:
-            tag = hashlib.sha256(f.read()).hexdigest()[:16]
-        out_dir = os.path.join(tempfile.gettempdir(), f"sm_depth_cluster_oracle_{os.getuid()}")
-        os.makedirs(out_dir, exist_ok=True)
-        so = os.path.join(out_dir, f"libsm_depth_cluster_oracle_{tag}.so")
-        if not os.path.exists(so):
-            cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-            tmp = so + f".{os.getpid()}.tmp"
-            subprocess.check_call([cxx, "-O2", "-fPIC", "-std=c++17", "-ffp-contract=off", "-shared", _SRC, "-o", tmp])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
+        _lib = O.lib()
         vp, i64 = C.c_void_p, C.c_int64
         _lib.sm_oracle_depth_cluster.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp]
         _lib.sm_oracle_depth_cluster.restype = i64

@@ -1,19 +1,13 @@
-"""ctypes binding of tests/cpp/filters_oracle.cc: the reference's scan pre-processing filters restated on the CPU,
-sequential and in the reference's order.  TEST INFRASTRUCTURE.  The library is compiled on first use into a per-user
-temporary directory (keyed by the source's hash), so a read-only tree works."""
+"""ctypes binding of oracle/filters_oracle.cc: the reference's scan pre-processing filters restated on the CPU,
+sequential and in the reference's order.  TEST INFRASTRUCTURE."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_SRC = os.path.join(_ROOT, "tests", "cpp", "filters_oracle.cc")
+import oracle_lib as O
+
 _lib = None
 
 KINDS = ("Range", "AxisRange", "BoundingBoxRemoval", "RandomSampler", "RangeImage", "GroundRemoval2")
@@ -42,19 +36,7 @@ class CheckFailed(RuntimeError):
 def lib():
     global _lib
     if _lib is None:
-        with open(_SRC, "rb") as f:
-            tag = hashlib.sha256(f.read()).hexdigest()[:16]
-        out_dir = os.path.join(tempfile.gettempdir(), f"sm_filters_oracle_{os.getuid()}")
-        os.makedirs(out_dir, exist_ok=True)
-        so = os.path.join(out_dir, f"libsm_filters_oracle_{tag}.so")
-        if not os.path.exists(so):
-            cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-            tmp = so + f".{os.getpid()}.tmp"
-            # the flags of oracle/Makefile: no FMA contraction, so the arithmetic is the written one
-            subprocess.check_call([cxx, "-O2", "-fopenmp", "-fPIC", "-std=c++17", "-ffp-contract=off", "-shared", _SRC,
-                                   "-o", tmp])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
+        _lib = O.lib()
         vp, i64, i32 = C.c_void_p, C.c_int64, C.c_int32
         _lib.sm_oracle_filter.argtypes = [C.c_int, vp, vp, C.c_uint32, vp, i64, vp, vp]
         _lib.sm_oracle_gr2_stages.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, vp]

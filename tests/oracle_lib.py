@@ -45,9 +45,6 @@ _lib = None
 
 
 def build():
-    srcs = [os.path.join(_DIR, f) for f in os.listdir(_DIR) if f.endswith((".cc", ".h"))]
-    if os.path.exists(_SO) and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in srcs):
-        return
     subprocess.check_call(["make", "-C", _DIR, "-s"])
 
 

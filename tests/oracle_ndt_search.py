@@ -1,15 +1,8 @@
-"""ctypes binding of tests/cpp/ndt_search_oracle.cc: registrator::Ndt with each of pclomp's neighbour searches
-(KDTREE, DIRECT26, DIRECT7, DIRECT1), restated on the CPU over libsm_oracle.so's pieces.  TEST INFRASTRUCTURE.  The
-library is compiled on first use into a per-user temporary directory (keyed by the source's hash), so a read-only
-tree works."""
+"""ctypes binding of oracle/ndt_search_oracle.cc: registrator::Ndt with each of pclomp's neighbour searches
+(KDTREE, DIRECT26, DIRECT7, DIRECT1), restated on the CPU over libsm_oracle.so's pieces.  TEST INFRASTRUCTURE."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
@@ -18,33 +11,13 @@ import oracle_lib as O
 KDTREE, DIRECT26, DIRECT7, DIRECT1 = 0, 1, 2, 3
 METHODS = (KDTREE, DIRECT26, DIRECT7, DIRECT1)
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_SRC = os.path.join(_ROOT, "tests", "cpp", "ndt_search_oracle.cc")
-_ORACLE_DIR = os.path.join(_ROOT, "oracle")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        O.lib()                                          # builds libsm_oracle.so if needed; loaded first
-        h = hashlib.sha256()
-        for path in (_SRC, os.path.join(_ORACLE_DIR, "ndt_math.h"), os.path.join(_ORACLE_DIR, "linalg.h")):
-            with open(path, "rb") as f:
-                h.update(f.read())
-        tag = hashlib.sha256(h.digest() + _ORACLE_DIR.encode()).hexdigest()[:16]   # the rpath is part of it
-        out_dir = os.path.join(tempfile.gettempdir(), f"sm_ndt_search_oracle_{os.getuid()}")
-        os.makedirs(out_dir, exist_ok=True)
-        so = os.path.join(out_dir, f"libsm_ndt_search_oracle_{tag}.so")
-        if not os.path.exists(so):
-            cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-            tmp = so + f".{os.getpid()}.tmp"
-            # the flags of oracle/Makefile: no FMA contraction, so the arithmetic is the written one
-            subprocess.check_call([cxx, "-O2", "-fopenmp", "-fPIC", "-std=c++17", "-ffp-contract=off", "-shared",
-                                   "-I", _ORACLE_DIR, _SRC, "-o", tmp, "-L", _ORACLE_DIR, "-l:libsm_oracle.so",
-                                   "-Wl,-rpath," + _ORACLE_DIR])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
+        _lib = O.lib()
         fp, dp, ip, i64 = C.POINTER(C.c_float), C.POINTER(C.c_double), C.POINTER(C.c_int32), C.c_int64
         _lib.sm_oracle_ndt_search_neighbors.argtypes = [fp, i64, C.c_float, C.c_int32, fp, i64, ip, ip]
         _lib.sm_oracle_ndt_search_derivatives.argtypes = [fp, i64, fp, i64, C.POINTER(O.NdtOptions), C.c_int32, dp,

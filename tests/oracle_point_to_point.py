@@ -1,24 +1,14 @@
-"""ctypes binding of tests/cpp/icp_point_to_point_oracle.cc: IcpFast::Align with the point-to-point minimizer
+"""ctypes binding of oracle/icp_point_to_point_oracle.cc: IcpFast::Align with the point-to-point minimizer
 (ComputePointToPoint, icp_fast.cc:326-375), restated on the CPU over libsm_oracle.so's pieces.  TEST
-INFRASTRUCTURE.  The library is compiled on first use into a per-user temporary directory (keyed by the sources'
-hash), so a read-only tree works."""
+INFRASTRUCTURE."""
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
 import oracle_lib as O
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_SRC = os.path.join(_ROOT, "tests", "cpp", "icp_point_to_point_oracle.cc")
-_SVD = os.path.join(_ROOT, "staticmapping_b200", "csrc", "linalg_dev.cuh")
-_ORACLE_DIR = os.path.join(_ROOT, "oracle")
 _lib = None
 
 
@@ -31,23 +21,7 @@ class P2PTrace(C.Structure):
 def lib():
     global _lib
     if _lib is None:
-        O.lib()                                          # builds libsm_oracle.so if needed; loaded first
-        h = hashlib.sha256(_ORACLE_DIR.encode())         # the rpath is part of it
-        for path in (_SRC, _SVD):
-            with open(path, "rb") as f:
-                h.update(f.read())
-        out_dir = os.path.join(tempfile.gettempdir(), f"sm_icp_p2p_oracle_{os.getuid()}")
-        os.makedirs(out_dir, exist_ok=True)
-        so = os.path.join(out_dir, f"libsm_icp_p2p_oracle_{h.hexdigest()[:16]}.so")
-        if not os.path.exists(so):
-            cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-            tmp = so + f".{os.getpid()}.tmp"
-            # the flags of oracle/Makefile: no FMA contraction, so the arithmetic is the written one
-            subprocess.check_call([cxx, "-O2", "-fopenmp", "-fPIC", "-std=c++17", "-ffp-contract=off",
-                                   "-Wno-unknown-pragmas", "-shared", "-I", _ORACLE_DIR, _SRC, "-o", tmp,
-                                   "-L", _ORACLE_DIR, "-l:libsm_oracle.so", "-Wl,-rpath," + _ORACLE_DIR])
-            os.replace(tmp, so)
-        _lib = C.CDLL(so)
+        _lib = O.lib()
         dp, ip = C.POINTER(C.c_double), C.POINTER(C.c_int32)
         _lib.sm_oracle_icp_fast_align_point_to_point.argtypes = [
             dp, C.c_int64, dp, C.c_int64, dp, C.POINTER(O.IcpOptions), C.c_int32, dp, dp, ip,

@@ -1,5 +1,5 @@
 """numpy restatement of RangeImage::DepthCluster (pre_processors/filter_range_image.cc:143-173, :245-309), written from
-the reference independently of tests/cpp/depth_cluster_oracle.cc.  TEST INFRASTRUCTURE.
+the reference independently of oracle/depth_cluster_oracle.cc.  TEST INFRASTRUCTURE.
 
 The image comes from pyref_filters.range_image_pixels (first point per pixel).  The edge mask is computed for the whole
 image at once in float32 (numpy, no contraction); sin, cos and atan2 are taken in float64 and rounded to float32.  The

@@ -1,5 +1,5 @@
 """numpy restatement of the reference's scan pre-processing filters (pre_processors/filter_*.cc), written from the
-reference sources independently of tests/cpp/filters_oracle.cc.  TEST INFRASTRUCTURE: a transcription error shared by
+reference sources independently of oracle/filters_oracle.cc.  TEST INFRASTRUCTURE: a transcription error shared by
 the GPU chain and the C++ restatement does not pass both.  float32 arithmetic is numpy's (IEEE, no contraction); the
 line fit is numpy.linalg.lstsq in float64, cast to float32 as FitLocalLine does; atan2 is taken in float64 and rounded
 to float32."""

@@ -1,6 +1,6 @@
 """Second, independent restatement of libnabo's k-NN search (KDTREE_LINEAR_HEAP) in pure Python, on the tree of
 tests/pyref.py's PyNabo.  TEST INFRASTRUCTURE ONLY: written from the published libnabo 1.0.7 algorithm, not from
-tests/cpp/knn_oracle.cc, and compared with it in tests/test_knn_oracle.py.  Python floats are IEEE doubles without
+oracle/knn_oracle.cc, and compared with it in tests/test_knn_oracle.py.  Python floats are IEEE doubles without
 contraction, so ids and squared distances are expected to agree bit for bit, order included.
 
   heap      IndexHeapBruteForceVector: k entries (-1, +inf), sorted ascending, the head is the last one; replaceHead

@@ -4,28 +4,13 @@ libsm_b200.so and driven by tests/cpp/adapter_run.cc.
 CPU: it builds, links, and — there being no CPU fallback — dies loudly in sm_create without a GPU.
 GPU: every result it prints matches the oracle."""
 import os
-import shutil
 import struct
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIBDIR = os.path.join(ROOT, "staticmapping_b200")
-
-
-def build(tmp_path):
-    cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-    if cxx is None:
-        pytest.skip("no g++")
-    exe = str(tmp_path / "adapter_run")
-    cmd = [cxx, "-std=c++14", "-O1", "-Wall", "-I", os.path.join(ROOT, "tests", "stubs"), "-I", os.path.join(ROOT, "include"),
-           "-I", os.path.join(ROOT, "adapter"), os.path.join(ROOT, "tests", "cpp", "adapter_run.cc"), "-o", exe,
-           "-L", LIBDIR, "-l:libsm_b200.so", "-Wl,-rpath," + LIBDIR]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
+from cxx import CC, LINK, LIBDIR, ROOT, adapter_exe
 
 
 def write_input(path, src, tgt, delta):
@@ -38,7 +23,7 @@ def write_input(path, src, tgt, delta):
 
 def test_builds_links_and_fails_loudly_without_a_gpu(tmp_path):
     import ctypes
-    exe = build(tmp_path)
+    exe = adapter_exe(tmp_path, "adapter_run")
     lib = ctypes.CDLL(os.path.join(LIBDIR, "libsm_b200.so"))
     if lib.sm_device_count() > 0:
         pytest.skip("a GPU is present: covered by the gpu test")
@@ -52,7 +37,7 @@ def test_builds_links_and_fails_loudly_without_a_gpu(tmp_path):
 def test_cpp_adapter_matches_oracle(tmp_path):
     import oracle_lib as O
     import scenes
-    exe = build(tmp_path)
+    exe = adapter_exe(tmp_path, "adapter_run")
     src, sub, P = scenes.lidar_pair(pair=2)
     s32, t32 = src.astype(np.float32), sub.astype(np.float32)
     delta = np.linalg.inv(P)
@@ -97,8 +82,7 @@ def test_cpp_adapter_matches_oracle(tmp_path):
 def test_header_is_plain_c_and_links_from_c(tmp_path):
     """include/sm_b200.h is a C ABI: a C99 translation unit includes it, calls through it and links
     against libsm_b200.so without any C++ runtime on its side."""
-    cc = "/usr/bin/gcc" if os.path.exists("/usr/bin/gcc") else shutil.which("gcc")
-    if cc is None:
+    if CC is None:
         pytest.skip("no gcc")
     src = tmp_path / "c_client.c"
     src.write_text(
@@ -112,8 +96,8 @@ def test_header_is_plain_c_and_links_from_c(tmp_path):
         "  return (n <= 0 && rc == SM_ERR_NO_DEVICE) ? 0 : 1;   /* no device: the documented loud error */\n"
         "}\n")
     exe = str(tmp_path / "c_client")
-    r = subprocess.run([cc, "-std=c99", "-Wall", "-Werror", "-pedantic", "-I", os.path.join(ROOT, "include"), str(src), "-o", exe,
-                        "-L", LIBDIR, "-l:libsm_b200.so", "-Wl,-rpath," + LIBDIR], capture_output=True, text=True)
+    r = subprocess.run([CC, "-std=c99", "-Wall", "-Werror", "-pedantic", "-I", os.path.join(ROOT, "include"), str(src), "-o", exe,
+                        *LINK], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 0, (r.stdout, r.stderr)

@@ -1,4 +1,4 @@
-"""RangeImage::DepthCluster without a GPU: the C++ restatement (tests/cpp/depth_cluster_oracle.cc) against the
+"""RangeImage::DepthCluster without a GPU: the C++ restatement (oracle/depth_cluster_oracle.cc) against the
 independent numpy one (tests/pyref_depth_cluster.py) on the 120 k scan and on clouds built for each case of the
 labelling and the order; the product's edge predicate compiled for the host against both; and the C ABI's argument
 checks, which answer before any device is touched."""

@@ -1,13 +1,11 @@
 """RangeImage::DepthCluster on the GPU, stage by stage, through the test hook sm_debug_depth_cluster and the C ABI:
-the range image against the C++ restatement (tests/cpp/depth_cluster_oracle.cc) up to the pixels a point within 4 float
+the range image against the C++ restatement (oracle/depth_cluster_oracle.cc) up to the pixels a point within 4 float
 ulps of a row / column border can reach (CUDA's atan2f against glibc's, as for the RangeImage stage); the edge mask
 against the numpy restatement evaluated on the GPU's image, up to edges whose beta lies within 2 ulps of the
 threshold; and, with the restatement fed the GPU's own image and edges, labels, point labels, levels, cluster set,
 output order and records bit for bit.  Then sizes around the compaction tile, two chains on two streams at once,
 repeated calls on one chain, and the Python and C++ mirrors."""
 import ctypes as C
-import os
-import shutil
 import struct
 import subprocess
 import threading
@@ -15,6 +13,7 @@ import threading
 import numpy as np
 import pytest
 
+from cxx import adapter_exe
 import depth_cluster_scenes as DS
 import filter_scenes as FS
 import oracle_depth_cluster as OD
@@ -24,7 +23,6 @@ import staticmapping_b200 as smb
 from test_gpu_filters import range_image_border_pixels
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TILE = 2048
 
 
@@ -228,13 +226,7 @@ def test_factory_mirror(scan):
 
 
 def test_cpp_adapter(tmp_path, scan):
-    cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-    exe = str(tmp_path / "depth_cluster_adapter_run")
-    libdir = os.path.join(ROOT, "staticmapping_b200")
-    subprocess.check_call([cxx, "-std=c++14", "-O1", "-Wall", "-I", os.path.join(ROOT, "tests", "stubs"), "-I",
-                           os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "adapter"),
-                           os.path.join(ROOT, "tests", "cpp", "depth_cluster_adapter_run.cc"), "-o", exe, "-L", libdir,
-                           "-l:libsm_b200.so", "-Wl,-rpath," + libdir])
+    exe = adapter_exe(tmp_path, "depth_cluster_adapter_run")
     with open(tmp_path / "in.bin", "wb") as fh:
         fh.write(struct.pack("<qiiff", len(scan), 60, 1800, 30.0, -20.0))
         fh.write(np.ascontiguousarray(scan, np.float32).tobytes())

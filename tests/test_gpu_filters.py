@@ -1,4 +1,4 @@
-"""The filter chain on the GPU against the C++ restatement (tests/cpp/filters_oracle.cc): every filter alone and the two
+"""The filter chain on the GPU against the C++ restatement (oracle/filters_oracle.cc): every filter alone and the two
 chains of the shipped configuration on a 120 k-point scan through the host and the device entry points, GroundRemoval2
 stage by stage, sizes around the compaction's tile, and chains on two streams.  atan2f is CUDA's on one side and glibc's
 on the other: the predicate filters must match exactly, RangeImage and GroundRemoval2 may differ on the few points that

@@ -1,11 +1,11 @@
 """IcpFast with inner compensation on the GPU (sm_set_inner_compensation) against the CPU restatement
-(tests/cpp/icp_compensation_oracle.cc), through every entry point."""
-import os
+(oracle/icp_compensation_oracle.cc), through every entry point."""
 import subprocess
 
 import numpy as np
 import pytest
 
+from cxx import adapter_exe
 import inner_compensation_scenes as ICS
 import oracle_compensation as OC
 import oracle_lib as O
@@ -155,16 +155,7 @@ def test_ndt_ignores_the_flag():
 
 
 def test_cpp_adapter_enable_inner_compensation(tmp_path):
-    import test_adapter_cpp as A
-    exe = str(tmp_path / "adapter_compensation_run")
-    root = A.ROOT
-    cmd = ["/usr/bin/g++", "-std=c++14", "-O1", "-Wall", "-I", os.path.join(root, "tests", "stubs_inner_compensation"),
-           "-I", os.path.join(root, "tests", "stubs"),
-           "-I", os.path.join(root, "include"), "-I", os.path.join(root, "adapter"),
-           os.path.join(root, "tests", "cpp", "adapter_compensation_run.cc"), "-o", exe,
-           "-L", A.LIBDIR, "-l:libsm_b200.so", "-Wl,-rpath," + A.LIBDIR]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
+    exe = adapter_exe(tmp_path, "adapter_compensation_run", overlay="stubs_inner_compensation")
     src, tp, tn = _corner()
     inp = tmp_path / "in.bin"
     with open(inp, "wb") as f:

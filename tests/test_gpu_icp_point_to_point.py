@@ -1,13 +1,13 @@
 """IcpFast and the IcpUsingPointMatcher stand-in with the point-to-point minimizer on the GPU
-(sm_set_icp_error_minimizer) against the CPU oracle (tests/cpp/icp_point_to_point_oracle.cc), through every entry
+(sm_set_icp_error_minimizer) against the CPU oracle (oracle/icp_point_to_point_oracle.cc), through every entry
 point, and the switch back to point-to-plane."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+from cxx import adapter_exe
 import inner_compensation_scenes as ICS
 import oracle_lib as O
 import oracle_point_to_point as OP
@@ -180,16 +180,7 @@ def test_rejections():
 
 
 def test_cpp_adapter(tmp_path):
-    import test_adapter_cpp as A
-    exe = str(tmp_path / "adapter_point_to_point_run")
-    root = A.ROOT
-    cmd = ["/usr/bin/g++", "-std=c++14", "-O1", "-Wall", "-I", os.path.join(root, "tests", "stubs_inner_compensation"),
-           "-I", os.path.join(root, "tests", "stubs"),
-           "-I", os.path.join(root, "include"), "-I", os.path.join(root, "adapter"),
-           os.path.join(root, "tests", "cpp", "adapter_point_to_point_run.cc"), "-o", exe,
-           "-L", A.LIBDIR, "-l:libsm_b200.so", "-Wl,-rpath," + A.LIBDIR]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
+    exe = adapter_exe(tmp_path, "adapter_point_to_point_run", overlay="stubs_inner_compensation")
     src, tp, tn, _, _ = S.corner()
     inp = tmp_path / "in.bin"
     with open(inp, "wb") as f:

@@ -1,6 +1,6 @@
 """IcpFast's point-to-point iteration on the GPU one phase at a time (sm_debug_icp_iteration_minimizer), every
 iteration of every point-to-point scene, each phase against a float64 model fed with the device's own previous phase
-and against the oracle's trace (tests/cpp/icp_point_to_point_oracle.cc):
+and against the oracle's trace (oracle/icp_point_to_point_oracle.cc):
   prologue  the target mean bit for bit, the Morton order of the source;
   A         matches and squared distances bit for bit (the oracle's k-NN), the gathered target points, the histogram;
   B         the sub-bin histogram, every block's candidates {p, q, 0, sqrt(d2)} bit for bit, its partial moments to the

@@ -1,5 +1,5 @@
 """sm_knn on an H100: libnabo's k-NN (k = 1..64, epsilon, maxRadius, self-match exclusion) bit for bit against the oracle
-(tests/cpp/knn_oracle.cc), on ids and squared distances, order included.  Also: k = 1 against sm_knn1, the device
+(oracle/knn_oracle.cc), on ids and squared distances, order included.  Also: k = 1 against sm_knn1, the device
 entry point against the host one, and two host threads on two streams against one."""
 import ctypes as C
 import threading

@@ -1,8 +1,6 @@
 """KnnB200 (adapter/registrators_b200.h), libnabo's NearestNeighbourSearch<double>::knn on the GPU, built the way
 tests/test_adapter_cpp.py builds the matcher adapter (stand-in headers of tests/stubs, linked to libsm_b200.so) and
 driven by tests/cpp/knn_adapter_run.cc: bit for bit against the oracle."""
-import os
-import shutil
 import struct
 import subprocess
 
@@ -10,23 +8,7 @@ import numpy as np
 import pytest
 
 import oracle_knn as OK
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIBDIR = os.path.join(ROOT, "staticmapping_b200")
-
-
-def _build(tmp_path):
-    cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else shutil.which("g++")
-    if cxx is None:
-        pytest.skip("no g++")
-    exe = str(tmp_path / "knn_adapter_run")
-    cmd = [cxx, "-std=c++14", "-O1", "-Wall", "-I", os.path.join(ROOT, "tests", "stubs"), "-I",
-           os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "adapter"),
-           os.path.join(ROOT, "tests", "cpp", "knn_adapter_run.cc"), "-o", exe, "-L", LIBDIR, "-l:libsm_b200.so",
-           "-Wl,-rpath," + LIBDIR]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    return exe
+from cxx import adapter_exe
 
 
 def _run(exe, tmp_path, T, Q, k, flags, eps, radius, bucket):
@@ -43,7 +25,7 @@ def test_adapter_builds_and_fails_loudly_without_a_gpu(tmp_path):
     from staticmapping_b200 import _lib
     if _lib.lib().sm_device_count() > 0:
         pytest.skip("GPU present")
-    exe = _build(tmp_path)
+    exe = adapter_exe(tmp_path, "knn_adapter_run")
     T = np.random.default_rng(0).normal(size=(50, 3))
     r, _ = _run(exe, tmp_path, T, T, 4, 1, 0.0, float("inf"), 8)
     assert r.returncode != 0 and "sm_knn failed" in r.stderr
@@ -51,7 +33,7 @@ def test_adapter_builds_and_fails_loudly_without_a_gpu(tmp_path):
 
 @pytest.mark.gpu
 def test_adapter_matches_oracle(tmp_path):
-    exe = _build(tmp_path)
+    exe = adapter_exe(tmp_path, "knn_adapter_run")
     rng = np.random.default_rng(1)
     T = rng.normal(size=(20_000, 3)) * 3.0
     Q = np.concatenate([T[::5] + rng.normal(size=(4000, 3)) * 0.1, rng.normal(size=(2000, 3)) * 4.0])

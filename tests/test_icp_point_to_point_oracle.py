@@ -1,4 +1,4 @@
-"""IcpFast's point-to-point minimizer without a GPU: the C++ oracle (tests/cpp/icp_point_to_point_oracle.cc) against
+"""IcpFast's point-to-point minimizer without a GPU: the C++ oracle (oracle/icp_point_to_point_oracle.cc) against
 the numpy restatement (tests/pyref_point_to_point.py) iteration by iteration, the product's Kabsch solve compiled
 for the host (sm_debug_kabsch_host) against numpy and the oracle, and the ABI's argument checks."""
 import ctypes as C

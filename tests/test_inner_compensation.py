@@ -1,4 +1,4 @@
-"""IcpFast with inner compensation on the CPU: the C++ restatement (tests/cpp/icp_compensation_oracle.cc) against
+"""IcpFast with inner compensation on the CPU: the C++ restatement (oracle/icp_compensation_oracle.cc) against
 the numpy one (tests/pyref_compensation.py), against a scene with a known answer, against the plain oracle with the flag clear, and the
 engine's host build of its per-point arithmetic against the oracle's pieces."""
 import ctypes as C

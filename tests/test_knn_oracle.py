@@ -1,4 +1,4 @@
-"""libnabo's k-NN (sm_knn) without a GPU: the oracle (tests/cpp/knn_oracle.cc) against an independent Python
+"""libnabo's k-NN (sm_knn) without a GPU: the oracle (oracle/knn_oracle.cc) against an independent Python
 restatement (tests/pyref_knn.py), against the oracle's own 1-NN, against scipy's cKDTree and brute force, the radius,
 self-match and tie rules, the kernel's search formulation (tests/gpu_knn_k_model.py), and the C ABI's argument checks."""
 import sys

@@ -1,6 +1,6 @@
 """pclomp's neighbour searches of Ndt (KDTREE, DIRECT26, DIRECT7, DIRECT1) without a GPU: the product's direct
 searches (csrc/ndt.cu for_each_direct_cell and its leaf test, compiled for the host through
-sm_debug_ndt_direct_neighbors), the oracle (tests/cpp/ndt_search_oracle.cc) and the numpy restatement
+sm_debug_ndt_direct_neighbors), the oracle (oracle/ndt_search_oracle.cc) and the numpy restatement
 (tests/pyref_ndt_search.py) on hand-built grids with known answers, on lidar scenes and on degenerate leaves."""
 import numpy as np
 import pytest
