@@ -199,6 +199,11 @@ class IcpUsingPointMatcherB200 : public FloatCloudMatcherB200<SM_TYPE_ICP_PM> {
   // PointToPointErrorMinimizer (icp_pointmatcher.cc:202-204) and then installs point-to-plane (:239), the default
   // here.  A value outside 0..1 CHECK-fails.
   void SetErrorMinimizer(int minimizer) { CheckRc(sm_set_icp_error_minimizer(handle_, minimizer)); }
+  // The leaf of the surface-normal reference filter (sm_pm_surface_normals): SM_PM_NORMALS_LEAST_SQUARES, the
+  // default, is CalculateNormals' plane fit (cloud_types.cc:73-103); SM_PM_NORMALS_EIGENVECTOR is libpointmatcher's
+  // own float box mean and smallest-eigenvector normal.  Applies from the next Align; a value outside 0..1
+  // CHECK-fails.
+  void SetSurfaceNormals(int mode) { CheckRc(sm_set_pm_surface_normals(handle_, mode)); }
 };
 
 // MotionCompensation (builder/map_builder.cc:232-257) on the GPU: same signature as the static

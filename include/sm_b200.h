@@ -76,6 +76,7 @@ int sm_destroy(sm_handle* h);
  * same module chain (DESIGN.md section 4e): bit-checked against a composition of this repository's oracle
  * pieces, and shown to lie within the literal chain's own call-to-call variation by a restatement of
  * libpointmatcher's filters (tests/pyref.py icp_pm_literal, tests/test_oracle_vs_python_restatement.py).
+ * sm_set_pm_surface_normals switches its reference filter to libpointmatcher's own eigenvector normals.
  * SM_TYPE_ICP_PM (stand-in for IcpUsingPointMatcher's default libpointmatcher chain,
  * icp_pointmatcher.cc:166-247; float clouds through the _f32 setters) registers no option in the
  * reference either; the engine accepts the IcpFast names (max_iteration defaults to 150, :214)
@@ -147,6 +148,28 @@ enum sm_icp_error_minimizer {
   SM_ICP_POINT_TO_POINT = 1
 };
 int sm_set_icp_error_minimizer(sm_handle* h, int32_t minimizer);
+/* The reference filter of SM_TYPE_ICP_PM, libpointmatcher's SamplingSurfaceNormalDataPointsFilter (knn 7,
+ * samplingMethod 1, icp_pointmatcher.cc:187-192).  Both modes split the reference cloud into the same boxes of at
+ * most 7 points (the median-split recursion of CalculateNormals, cloud_types.cc:105-144) and keep one point and
+ * one normal per box, in ascending order of the box's smallest point index.
+ *   LEAST_SQUARES (the default)  CalculateNormals' leaf (cloud_types.cc:73-103), the reference author's own port of
+ *             the filter: in double, the box mean and normalize(M^-1 b), M = sum d d^T, b = sum d.
+ *   EIGENVECTOR  the filter's own leaf in PointMatcher<float>: the float box mean (members summed in ascending
+ *             index order, divided by float(count)), C = sum (d - mean)(d - mean)^T in float, the box dropped if
+ *             rank(C) + 1 < 3 (FullPivHouseholderQR's rank with a float matrix's threshold, on C widened to
+ *             double), and the eigenvector of the smallest eigenvalue of C (symmetric Jacobi in double, normalised,
+ *             rounded to float) with its component of largest magnitude positive.  The kept point is the float mean.
+ *             The point-to-plane terms do not depend on the normal's sign; the sign only makes the output
+ *             deterministic.  libpointmatcher's own eigensolver is not reproduced (DESIGN.md section 4e).
+ * Applies from the next Align on (sm_align and sm_align_batch alike); a change of mode filters the reference cloud
+ * anew, setting the mode it already has does not.  SM_TYPE_ICP_PM only: every other type returns
+ * SM_ERR_UNSUPPORTED_TYPE and is left unchanged.  A mode outside 0..1 returns SM_ERR_BAD_ARGUMENT and leaves the
+ * setting unchanged.  Not an XML option: sm_print_options does not list it. */
+enum sm_pm_surface_normals {
+  SM_PM_NORMALS_LEAST_SQUARES = 0,
+  SM_PM_NORMALS_EIGENVECTOR = 1
+};
+int sm_set_pm_surface_normals(sm_handle* h, int32_t mode);
 /* Interface::GetType (interface.h:106). */
 int sm_get_type(const sm_handle* h);
 

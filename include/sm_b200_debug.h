@@ -21,6 +21,7 @@
  *     sm_debug_voxel_index     the voxel index of a point in the submap filter, the NDT grid and ApproximateVoxelGrid
  *     sm_debug_motion_host     InterpolateTransform(Identity, delta, factor) applied to a point
  *     sm_debug_normals_leaf    the leaf plane fit of CalculateNormals (cloud_types.cc:73-103)
+ *     sm_debug_pm_surface_normal_leaf_host  the eigenvector leaf of libpointmatcher's SamplingSurfaceNormal filter
  *     sm_debug_ndt_direct_neighbors  the NDT derivative kernel's DIRECT26 / DIRECT7 / DIRECT1 neighbour searches
  *     sm_debug_filter_host     the filter chain's per-point functions: predicate, RangeImage pixel, GroundRemoval2 cell
  *     sm_debug_filter_fit_host, sm_debug_filter_distance_host  GroundRemoval2's line fit and VerticalDistanceToSegment
@@ -40,6 +41,8 @@
  *                              phase C's 29 reduced sums, limit, kept count and pose update
  *     sm_debug_pm_stages       the IcpUsingPointMatcher stand-in's reading filter and score pass: kept points, sorted
  *                              squared distances of the approximate search, trim counts and mean
+ *     sm_debug_pm_surface_normals  the stand-in's reference filter (NormalsPipeline) in either leaf mode: kept means,
+ *                              normals and box indices, after an optional earlier build into the same owner
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
  *     sm_debug_gicp_step       correspondences, Mahalanobis matrices and cost sums of one GICP outer iteration
@@ -152,6 +155,13 @@ int sm_debug_gicp_host(int32_t op, const double* in, double* out);
  * when rank(covariance) + 1 < 3. */
 int sm_debug_normals_leaf(const double* members_3k, int32_t count, double* mean_3, double* normal_3, int32_t* kept);
 
+/* The leaf of libpointmatcher's SamplingSurfaceNormalDataPointsFilter as sm_set_pm_surface_normals(EIGENVECTOR) runs it
+ * (csrc/normals.cu leaf_eigen_normal compiled for the host): count (1..7) float members {x, y, z} in member order ->
+ * the float mean, the float covariance sum (row-major 3x3) and the unit normal; kept = 0 when rank(C) + 1 < 3 (mean and
+ * covariance are still written, the normal is not). */
+int sm_debug_pm_surface_normal_leaf_host(const float* members_3k, int32_t count, float* mean_3, float* cov_9,
+                                         float* normal_3, int32_t* kept);
+
 /* sm_motion_compensation's arithmetic on the host (csrc/motion_dev.cuh make_motion_params + motion_point): packed
  * {x, y, z, intensity, factor} float records in and out; SM_ERR_BAD_ARGUMENT if a factor is outside [0, 1]. */
 int sm_debug_motion_host(const float* points_5n, int64_t n, const double* delta_4x4, float* out_5n);
@@ -227,6 +237,13 @@ int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const 
 int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const float* target_3n, int64_t nt, float prob,
                        uint32_t seed, const double* T_4x4, float knn_epsilon, float ratio, int64_t* kept,
                        double* sampled_3n, double* keys_n, double* out_3);
+
+/* The IcpUsingPointMatcher stand-in's reference filter as pm_align runs it: the packed float cloud widened into a
+ * NormalsPipeline and run with `mode` (sm_pm_surface_normals).  With n_first > 0 the first cloud is run first, with
+ * the same mode, into the SAME owner.  Writes the m kept boxes in output order: points_3m and normals_3m (doubles,
+ * capacity 3 * n each), the smallest member index of each box index_m (capacity n), and *m. */
+int sm_debug_pm_surface_normals(int device, int32_t mode, const float* first_3n, int64_t n_first, const float* cloud_3n,
+                                int64_t n, double* points_3m, double* normals_3m, int64_t* index_m, int64_t* m);
 
 /* One IcpFast iteration as sm_align runs it (IcpFastBuffers, KdWorkspace, no graphs; csrc/icp.cu): icp_prologue and
  * iterations 1 .. iteration-1, then iteration `iteration` one phase at a time with a synchronise and a copy after

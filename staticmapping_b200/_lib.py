@@ -45,6 +45,7 @@ SIGNATURES = {
     "sm_set_inner_compensation": (C.c_int, [_VP, C.c_int32]),
     "sm_set_ndt_search_method": (C.c_int, [_VP, C.c_int32]),
     "sm_set_icp_error_minimizer": (C.c_int, [_VP, C.c_int32]),
+    "sm_set_pm_surface_normals": (C.c_int, [_VP, C.c_int32]),
     "sm_get_type": (C.c_int, [_VP]),
     "sm_set_input_source": (C.c_int, [_VP, _VP, C.c_int64]),
     "sm_set_input_target": (C.c_int, [_VP, _VP, _VP, C.c_int64]),
@@ -95,6 +96,7 @@ SIGNATURES = {
     "sm_debug_ndt_newton": (C.c_int, [_VP, _VP, _VP, C.c_int32, C.c_float, C.c_double, C.c_double, C.c_double, C.c_int32,
                                       _VP, _VP, _VP, _VP]),
     "sm_debug_normals_leaf": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP]),
+    "sm_debug_pm_surface_normal_leaf_host": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, _VP]),
     "sm_debug_voxel_index": (C.c_int, [C.c_int32, _VP, C.c_float, C.c_int32, _VP]),
     "sm_debug_gicp_point": (C.c_int, [C.c_int32, _VP, _VP]),
     "sm_debug_gicp_outer": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _VP, _VP]),
@@ -116,6 +118,7 @@ SIGNATURES = {
     "sm_debug_float_tree_knn": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, _VP, _VP]),
     "sm_debug_pm_stages": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_float, C.c_uint32, _VP, C.c_float,
                                      C.c_float, _VP, _VP, _VP, _VP]),
+    "sm_debug_pm_surface_normals": (C.c_int, [C.c_int, C.c_int32, _VP, C.c_int64, _VP, C.c_int64, _VP, _VP, _VP, _VP]),
     "sm_debug_icp_iteration": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP, C.c_float, C.c_float,
                                          C.c_int32, C.c_int32, C.c_int32] + [_VP] * 16),
     "sm_debug_icp_iteration_minimizer": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP, C.c_float,

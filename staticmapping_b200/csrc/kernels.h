@@ -265,6 +265,9 @@ int ndt_debug_direct_cells_host(int search, const float* x, float leaf, const Nd
 bool ndt_debug_direct_leaf_accepted_host(int nr_points);
 // host build of the leaf plane fit of normals.cu (test hook sm_debug_normals_leaf): 1 kept, 0 dropped, < 0 bad count
 int normals_debug_leaf_host(const double* members, int count, double* mean, double* unit);
+// host build of the eigenvector leaf of normals.cu (test hook sm_debug_pm_surface_normal_leaf_host), float members;
+// mean, row-major covariance and normal as the leaf computes them: 1 kept, 0 dropped, < 0 bad count
+int pm_normals_debug_leaf_host(const float* members, int count, float* mean, float* cov, float* unit);
 // host build of one target-grid leaf of ndt.cu (test hook sm_debug_ndt_leaf)
 void ndt_debug_leaf_host(const float* pts, int n, int min_points, double eig_mult, double* mean3, double* icov9,
                          float* centroid3, int* nr_points, int* searchable);
@@ -335,6 +338,9 @@ int float_tree_debug_knn(const FloatTree& t, const double* q, int nq, int k, int
                          cudaStream_t stream);
 
 // ---- normals.cu ------------------------------------------------------------------------
+// The leaf routine of the normals pipeline, same values as sm_pm_surface_normals: CalculateNormals' least-squares
+// plane (double) or libpointmatcher SamplingSurfaceNormal's smallest eigenvector of the box covariance (float)
+enum NormalsMode : int { kNormalsLeastSquares = 0, kNormalsEigenvector = 1 };
 // The device buffers of CalculateNormals over n points, sized by reserve(n): the input cloud, the bucket-7 tree
 // with its workspace, the per-leaf scratch, and the AoS 3xM outputs with their count M.
 struct NormalsPipeline {
@@ -342,8 +348,9 @@ struct NormalsPipeline {
   int64_t stride = 0;
   int reserve(int n);
   double* input() const { return (double*)coord.p; }   // SoA [3][stride], filled by the caller
-  // runs the pipeline on the first n points of input() and waits for M
-  int run(int n, cudaStream_t stream, uint32_t* m);
+  // runs the pipeline with the given leaf routine on the first n points of input() and waits for M; keep then holds
+  // 1 at the smallest member index of every kept box (the outputs' source positions, in order)
+  int run(int n, NormalsMode mode, cudaStream_t stream, uint32_t* m);
   const double* points() const { return (const double*)out_pts.p; }
   const double* normals() const { return (const double*)out_nrm.p; }
 };

@@ -150,6 +150,46 @@ __host__ __device__ inline void jacobi_eig_sym(const double* Ain, int n, double*
   for (int i = 0; i < n; ++i) w[i] = A[i * n + i];
 }
 
+// jacobi_eig_sym at n = 3 with every index a compile-time constant, so the device keeps A and V in registers: the
+// same rotations in the same order and the same operations, hence the same bits.
+__host__ __device__ __forceinline__ void jacobi_eig_sym3(const double* Ain, double* w, double* V) {
+  double A[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) { A[i] = Ain[i]; V[i] = (i % 4 == 0) ? 1.0 : 0.0; }
+#pragma unroll 1
+  for (int sweep = 0; sweep < 64; ++sweep) {
+    double off = 0.0;
+    off += A[1] * A[1]; off += A[2] * A[2]; off += A[5] * A[5];
+    if (off == 0.0) break;
+#pragma unroll
+    for (int pq = 0; pq < 3; ++pq) {
+      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;     // (0,1), (0,2), (1,2)
+      const double apq = A[p * 3 + q];
+      if (apq == 0.0) continue;
+      const double theta = (A[q * 3 + q] - A[p * 3 + p]) / (2.0 * apq);
+      const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+      const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double akp = A[k * 3 + p], akq = A[k * 3 + q];
+        A[k * 3 + p] = c * akp - s * akq; A[k * 3 + q] = s * akp + c * akq;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double apk = A[p * 3 + k], aqk = A[q * 3 + k];
+        A[p * 3 + k] = c * apk - s * aqk; A[q * 3 + k] = s * apk + c * aqk;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double vkp = V[k * 3 + p], vkq = V[k * 3 + q];
+        V[k * 3 + p] = c * vkp - s * vkq; V[k * 3 + q] = s * vkp + c * vkq;
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) w[i] = A[i * 3 + i];
+}
+
 __host__ __device__ inline void sym_svd_solve(const double* A, const double* b, double* x, int n) {
   double w[6], V[36];
   jacobi_eig_sym(A, n, w, V);

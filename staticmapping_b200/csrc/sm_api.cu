@@ -154,6 +154,7 @@ struct PmMatcher {
   IcpFastMatcher icp;
   F32Clouds in;
   bool src_dirty = false, tgt_dirty = false, score_tree_dirty = true;
+  int surface_normals = SM_PM_NORMALS_LEAST_SQUARES;   // sm_set_pm_surface_normals
   NormalsPipeline normals;
   PmStage stage;
   FloatTree score_tree;
@@ -479,15 +480,17 @@ int icp_align(sm_handle* h, IcpFastMatcher& f, const double* guess, double* resu
 // registrators/icp_pointmatcher.cc:125-247 drives libpointmatcher 1.3.1 (external, float) with
 //   reading filter    RandomSampling prob 0.9                      -> PmStage::sample (a counter
 //                     hash instead of std::rand, so the kept set is reproducible)
-//   reference filter  SamplingSurfaceNormal knn 7, one point per box -> CalculateNormals, the
-//                     reference author's own restatement of that filter (cloud_types.cc:73-144)
+//   reference filter  SamplingSurfaceNormal knn 7, one point per box -> NormalsPipeline: by default
+//                     CalculateNormals, the reference author's own restatement of that filter
+//                     (cloud_types.cc:73-144); with sm_set_pm_surface_normals(EIGENVECTOR) the filter's
+//                     own float box mean and smallest-eigenvector normal (normals.cu leaf_eigen_normal)
 //   matcher / outlier filter / minimiser / checkers                 -> the IcpFast chain, which
 //                     icp_fast.cc ported from exactly these modules (k-d tree eps 3.16, trim 0.7,
 //                     point-to-plane, 4-sample differential checker 0.001 rad / 0.01 m), here in
 //                     double, capped at 150 iterations
 //   score (:131-148)  unfiltered reading moved by the result vs unfiltered reference, same matcher,
 //                     trim 0.7, exp(-mean kept distance); Align() false below 0.6 (:145)
-// It is a deterministic equivalent, not a bit-level restatement: libpointmatcher's float
+// It is a deterministic equivalent, not a bit-level restatement: libpointmatcher's float ICP
 // arithmetic and its rand() stream cannot be pinned from this tree.
 int pm_align(sm_handle* h, PmMatcher& pm, const double* guess, double* result) {
   if (pm.in.n_src <= 0 || pm.in.n_tgt <= 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
@@ -498,7 +501,7 @@ int pm_align(sm_handle* h, PmMatcher& pm, const double* guess, double* result) {
     H_RC(np.reserve(n));
     H_RC(ndt_float_to_soa((const float*)pm.in.tgt.p, n, np.input(), np.stride, s));
     uint32_t m = 0;
-    H_RC(np.run(n, s, &m));
+    H_RC(np.run(n, (NormalsMode)pm.surface_normals, s, &m));
     if (m == 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: no target point survived the surface-normal filter");
     H_RC(icp_set_target(h, pm.icp, np.points(), np.normals(), (int64_t)m, true));
     pm.tgt_dirty = false;
@@ -843,6 +846,17 @@ int sm_set_icp_error_minimizer(sm_handle* h, int32_t minimizer) {
   return SM_OK;
 }
 
+int sm_set_pm_surface_normals(sm_handle* h, int32_t mode) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  PmMatcher* pm = h->as<PmMatcher>();
+  if (!pm) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetSurfaceNormals: IcpUsingPointMatcher (type 1) only");
+  if (mode < SM_PM_NORMALS_LEAST_SQUARES || mode > SM_PM_NORMALS_EIGENVECTOR)
+    return fail(h, SM_ERR_BAD_ARGUMENT, "SetSurfaceNormals: mode must be 0..1");
+  if (mode != pm->surface_normals) pm->tgt_dirty = true;   // the filtered reference cloud is built anew
+  pm->surface_normals = mode;
+  return SM_OK;
+}
+
 int sm_set_ndt_search_method(sm_handle* h, int32_t method) {
   if (!h) return SM_ERR_BAD_ARGUMENT;
   NdtMatcher* m = h->as<NdtMatcher>();
@@ -1034,7 +1048,7 @@ int sm_calculate_normals(int device, const double* points, int64_t n, double* ou
   SMB_RC(np.reserve((int)n));
   SMB_RC(upload_soa(points, n, false, stage, np.input(), np.stride, s));
   uint32_t m = 0;
-  SMB_RC(np.run((int)n, s, &m));
+  SMB_RC(np.run((int)n, kNormalsLeastSquares, s, &m));
   if (m > 0) {
     SMB_CUDA_OK(cudaMemcpyAsync(out_points, np.points(), (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));
     SMB_CUDA_OK(cudaMemcpyAsync(out_normals, np.normals(), (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));

@@ -126,6 +126,16 @@ int sm_debug_normals_leaf(const double* members_3k, int32_t count, double* mean3
   return SM_OK;
 }
 
+// test hook: the eigenvector leaf of SamplingSurfaceNormal (normals.cu leaf_eigen_normal) compiled for the host
+int sm_debug_pm_surface_normal_leaf_host(const float* members_3k, int32_t count, float* mean_3, float* cov_9,
+                                         float* normal_3, int32_t* kept) {
+  if (!members_3k || !mean_3 || !cov_9 || !normal_3 || !kept) return SM_ERR_BAD_ARGUMENT;
+  const int r = pm_normals_debug_leaf_host(members_3k, count, mean_3, cov_9, normal_3);
+  if (r < 0) return SM_ERR_BAD_ARGUMENT;
+  *kept = r;
+  return SM_OK;
+}
+
 // test hook: the voxel index of a point as the three voxelisations compute it, compiled for the host
 int sm_debug_voxel_index(int32_t op, const float* p3, float param, int32_t min_b, int64_t* out4) {
   if (!p3 || !out4) return SM_ERR_BAD_ARGUMENT;
@@ -451,6 +461,35 @@ int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const flo
   return SM_OK;
 }
 
+int sm_debug_pm_surface_normals(int device, int32_t mode, const float* first_3n, int64_t n_first, const float* cloud_3n,
+                                int64_t n, double* points_3m, double* normals_3m, int64_t* index_m, int64_t* m) {
+  if ((mode != kNormalsLeastSquares && mode != kNormalsEigenvector) || !debug_cloud_ok(cloud_3n, n) || n_first < 0 ||
+      (n_first > 0 && !debug_cloud_ok(first_3n, n_first)) || !points_3m || !normals_3m || !index_m || !m)
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  NormalsPipeline np;
+  DevBuf in;
+  uint32_t kept = 0;
+  for (int pass = n_first > 0 ? 0 : 1; pass < 2; ++pass) {   // as pm_align: widen the float cloud, then run
+    const float* c = pass == 0 ? first_3n : cloud_3n;
+    const int64_t k = pass == 0 ? n_first : n;
+    SMB_RC(np.reserve((int)k));
+    SMB_RC(debug_upload_f32(c, k, in));
+    SMB_RC(ndt_float_to_soa((const float*)in.p, (int)k, np.input(), np.stride, nullptr));
+    SMB_RC(np.run((int)k, (NormalsMode)mode, nullptr, &kept));
+  }
+  SMB_CUDA_OK(cudaMemcpy(points_3m, np.points(), (size_t)kept * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(normals_3m, np.normals(), (size_t)kept * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  std::vector<uint32_t> keep((size_t)n);
+  SMB_CUDA_OK(cudaMemcpy(keep.data(), np.keep.p, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  int64_t j = 0;
+  for (int64_t i = 0; i < n; ++i)
+    if (keep[(size_t)i]) { if (j < (int64_t)kept) index_m[j] = i; ++j; }
+  if (j != (int64_t)kept) return SM_ERR_CUDA;   // the compaction's count disagrees with its flags
+  *m = (int64_t)kept;
+  return SM_OK;
+}
+
 int sm_debug_approx_voxel_grid(int device, const float* points_3n, int64_t n, float leaf, float* out_3n,
                                int64_t* m_out) {
   if (!debug_cloud_ok(points_3n, n) || !(leaf > 0.0f) || !out_3n || !m_out) return SM_ERR_BAD_ARGUMENT;
@@ -621,7 +660,7 @@ static int debug_kd_build(DebugKdOwners& o, int variant, int bucket, const void*
     SMB_RC(o.np.reserve((int)n));
     SMB_RC(debug_soa((const double*)cloud, n, o.np.stride, o.np.input()));
     uint32_t m = 0;
-    SMB_RC(o.np.run((int)n, nullptr, &m));
+    SMB_RC(o.np.run((int)n, kNormalsLeastSquares, nullptr, &m));
   } else {
     SMB_RC(debug_upload_f32((const float*)cloud, n, o.coord));
     SMB_RC(o.ft.build((const float*)o.coord.p, (int)n, o.kdws, nullptr));

@@ -57,6 +57,15 @@ class ErrorMinimizer(enum.IntEnum):
     POINT_TO_POINT = 1
 
 
+class SurfaceNormals(enum.IntEnum):
+    """The reference filter of IcpUsingPointMatcher (libpointmatcher's SamplingSurfaceNormalDataPointsFilter, knn 7),
+    for IcpUsingPointMatcher.SetSurfaceNormals.  LEAST_SQUARES (the default) is CalculateNormals' plane fit
+    (cloud_types.cc:73-103), the reference author's port of the filter; EIGENVECTOR is the filter's own leaf: the
+    float box mean and the smallest eigenvector of the box covariance.  See sm_set_pm_surface_normals."""
+    LEAST_SQUARES = 0
+    EIGENVECTOR = 1
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
@@ -352,6 +361,11 @@ class IcpUsingPointMatcher(Ndt):
         PointToPointErrorMinimizer, icp_pointmatcher.cc:202-204, before it installs point-to-plane, :239);
         applies from the next Align on."""
         self._check(self._lib.sm_set_icp_error_minimizer(self._h, int(minimizer)), "SetErrorMinimizer")
+
+    def SetSurfaceNormals(self, mode):
+        """A SurfaceNormals mode for the reference filter; applies from the next Align on, which filters the
+        reference cloud anew when the mode changed.  See sm_set_pm_surface_normals in include/sm_b200.h."""
+        self._check(self._lib.sm_set_pm_surface_normals(self._h, int(mode)), "SetSurfaceNormals")
 
     def Align(self, guess):
         if self._source is None or self._target is None:
