@@ -346,6 +346,47 @@ class FilterChainB200 {
   sm_filter_chain* chain_ = nullptr;
 };
 
+// pre_processers::filter::StatisticRemoval as PCL's StatisticalOutlierRemoval (setMeanK(point_num_meank),
+// setStddevMulThresh(std_mul)), the call filter_statistic_removal.cc:44-59 leaves as a TODO, on the GPU: one per
+// StatisticRemoval.  The body of its InitFromXmlNode becomes one SetParam per <param>, and that of Filter
+//   this->FilterPrepare(cloud); filter_.Filter(*this->inner_cloud_, cloud.get(), &this->inliers_);
+// The two sums behind the threshold are correctly rounded instead of PCL's serial double sums (include/sm_b200.h).
+class StatisticRemovalB200 {
+ public:
+  explicit StatisticRemovalB200(int device = 0) { CHECK_EQ(sm_statistic_removal_create(device, &filter_), 0); }
+  ~StatisticRemovalB200() { sm_statistic_removal_destroy(filter_); }
+  StatisticRemovalB200(const StatisticRemovalB200&) = delete;
+  StatisticRemovalB200& operator=(const StatisticRemovalB200&) = delete;
+
+  // point_num_meank (type 0) or std_mul (type 1); type -1 when the <param> has none (the reference CHECK-fails,
+  // filter_interface.cc:57)
+  void SetParam(const std::string& name, int type, const std::string& text) {
+    CHECK_EQ(sm_statistic_removal_set_param(filter_, name.c_str(), type, text.c_str()), 0)
+        << sm_statistic_removal_last_error(filter_);
+  }
+
+  // CHECK-fails for 1..point_num_meank finite points (PCL reads past its k-list there) and for a point_num_meank
+  // outside 1..63
+  void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,
+              std::vector<int>* const inliers = nullptr) {
+    CHECK(output);
+    const int64_t n = static_cast<int64_t>(input.points.size());
+    output->points.resize(input.points.size());
+    std::vector<int32_t> index(input.points.size());
+    int64_t m = 0;
+    if (n > 0) {
+      const int rc = sm_statistic_removal_run(filter_, &input.points[0].x, n, sizeof(data::InnerPointType),
+                                              &output->points[0].x, &m, index.data());
+      CHECK_EQ(rc, 0) << "sm_statistic_removal_run failed (" << rc << "): " << sm_statistic_removal_last_error(filter_);
+    }
+    output->points.resize(m);
+    if (inliers) inliers->assign(index.begin(), index.begin() + m);
+  }
+
+ private:
+  sm_statistic_removal* filter_ = nullptr;
+};
+
 // descriptor::M2dp::setInputCloud + getFinalDescriptor on the GPU (descriptor/m2dp.cc:129-153): the body of
 // setInputCloud becomes   return registrator::M2dpB200(*source, r_, max_distance_, t_, p_, q_, &descriptor_);
 inline bool M2dpB200(const data::InnerCloudType& source, double r, double max_distance, int32_t t, int32_t p,

@@ -408,7 +408,8 @@ int sm_filter_chain_create(int device, sm_filter_chain** out);
 int sm_filter_chain_destroy(sm_filter_chain* chain);
 /* One <filter name=...> of Factory::InitFromXmlNode (filter_factory.cc:64-80): appends the filter at its constructor's
  * defaults and returns its index.  GroundRemoval, StatisticRemoval (an empty body in the reference,
- * filter_statistic_removal.cc:44-59) and VoxelGrid (see sm_voxel_grid_filter) are not built into the chain:
+ * filter_statistic_removal.cc:44-59; PCL's filter is sm_statistic_removal_*) and VoxelGrid (see sm_voxel_grid_filter)
+ * are not built into the chain:
  * SM_ERR_UNSUPPORTED_TYPE.  A name the reference does not register either (it skips it, :68-71):
  * SM_ERR_UNKNOWN_OPTION; the chain is unchanged. */
 int sm_filter_chain_add(sm_filter_chain* chain, const char* filter_name);
@@ -457,6 +458,54 @@ int sm_filter_chain_depth_cluster(sm_filter_chain* chain, int filter, const floa
                                   int64_t stride_bytes, float* out_xyz, uint32_t* out_label, int32_t* out_index,
                                   int64_t* m_out, uint32_t* point_label_or_null);
 const char* sm_filter_chain_last_error(const sm_filter_chain* chain);
+
+/* ---- pre_processers::filter::StatisticRemoval: PCL's statistical outlier removal ---------------------------------
+ * The reference registers StatisticRemoval (filter_factory.cc:44-52) with point_num_meank (int32, 30) and std_mul
+ * (float, 1.0), but its Filter body is a commented-out pcl::StatisticalOutlierRemoval call (setMeanK(point_num_meank),
+ * setStddevMulThresh(std_mul)) under a TODO (filter_statistic_removal.cc:44-59): there the filter does nothing.  This
+ * is that PCL filter (StatisticalOutlierRemoval::applyFilterIndices of PCL 1.8 / 1.10), restated from upstream PCL and
+ * FLANN; no PCL is compiled to check it.  It is not part of the chain (sm_filter_chain_add refuses it); it has its own
+ * handle, used by one thread at a time.  Its device buffers belong to the handle and only grow.
+ *   1. A point is finite when x, y and z are; only finite points are searched.  A non-finite point gets distance 0.
+ *   2. The K + 1 nearest finite points of each finite point, K = point_num_meank: exact search, self-match allowed, over
+ *      the coordinates widened to double, with libnabo's tie rules (sm_knn).  Entry 0 (d2 = 0) is dropped.
+ *   3. For entries 1..K, in list order: dx = qx - px in float, d2 = ((0 + dx*dx) + dy*dy) + dz*dz in float (FLANN's
+ *      L2_Simple<float>), dist_sum += sqrt((double)d2); distance = (float)(dist_sum / K).
+ *   4. valid = the number of finite points; sum = sum of distance and sq_sum = sum of (distance * distance, a float
+ *      product) over all points; mean = sum / valid, variance = (sq_sum - sum * sum / valid) / (valid - 1),
+ *      stddev = sqrt(variance), threshold = mean + (double)std_mul * stddev, all in double.
+ *   5. A point is kept iff !(distance > threshold): whole records (x, y, z, intensity, factor) in input order.
+ * DIFFERENCE from PCL: sum and sq_sum are the exact sums of their float terms rounded once to double, not PCL's serial
+ * double sums in index order, so mean, stddev and threshold depend on the set of inputs alone and are the same on
+ * every launch shape.  A point whose distance lies within the few ulps the two sums differ by of the threshold can be
+ * kept where PCL removes it, or the reverse (DESIGN.md section 4j).  A slightly negative variance gives a NaN threshold
+ * and keeps every point, as in PCL; with no finite point every point is kept.  PCL's setNegative and keep_organized are
+ * not used by the reference and are not built. */
+typedef struct sm_statistic_removal sm_statistic_removal;
+/* Needs no device; the first run binds CUDA ordinal `device`. */
+int sm_statistic_removal_create(int device, sm_statistic_removal** out);
+int sm_statistic_removal_destroy(sm_statistic_removal* filter);
+/* One <param type=... name=...>text</param> of the filter's XML node, parsed exactly as sm_filter_chain_set_param parses
+ * it: SM_ERR_UNKNOWN_OPTION for a name other than point_num_meank / std_mul, SM_ERR_BAD_ARGUMENT for a type other than
+ * 0 / 1.  Any value is stored; run refuses a point_num_meank outside 1..63. */
+int sm_statistic_removal_set_param(sm_statistic_removal* filter, const char* name, int type, const char* text);
+/* SetInputCloud + Filter.  `points`: n records `stride_bytes` (>= 20, a multiple of 4) apart, float x, y, z,
+ * intensity, factor first; `out`: capacity n packed 5-float records; *m_out = the number kept; inlier_index (optional,
+ * capacity n): their indices in `points`, ascending.  n = 0: *m_out = 0.  SM_ERR_BAD_ARGUMENT: point_num_meank outside
+ * 1..63 (K + 1 must stay within sm_knn's 64), a bad stride, null pointers with n > 0, more than 2^30 points or more
+ * finite points than a 24-level tree of 8-point buckets holds.  SM_ERR_CHECK_FAILED, outputs untouched: between 1 and
+ * point_num_meank finite points (PCL reads past its k-list there).
+ * The _device form takes device pointers (in and out may not overlap), runs on `cuda_stream` (a cudaStream_t, NULL =
+ * default stream) and returns after the stream has finished; it reads the stream's results back twice (the finite
+ * count, which sizes the tree, and the number kept).  Its output feeds sm_set_input_source_f32_device (stride 20). */
+int sm_statistic_removal_run(sm_statistic_removal* filter, const float* points, int64_t n, int64_t stride_bytes,
+                             float* out, int64_t* m_out, int32_t* inlier_index_or_null);
+int sm_statistic_removal_run_device(sm_statistic_removal* filter, const float* dev_points, int64_t n,
+                                    int64_t stride_bytes, float* dev_out, int64_t* m_out,
+                                    int32_t* dev_inlier_index_or_null, void* cuda_stream);
+/* The last successful run's mean, stddev, threshold and valid (step 4), as four doubles. */
+int sm_statistic_removal_stats(const sm_statistic_removal* filter, double* out4);
+const char* sm_statistic_removal_last_error(const sm_statistic_removal* filter);
 
 int sm_device_count(void);
 const char* sm_version(void);

@@ -26,6 +26,8 @@
  *     sm_debug_filter_host     the filter chain's per-point functions: predicate, RangeImage pixel, GroundRemoval2 cell
  *     sm_debug_filter_fit_host, sm_debug_filter_distance_host  GroundRemoval2's line fit and VerticalDistanceToSegment
  *     sm_debug_depth_edge_host RangeImage::DepthCluster's edge predicate
+ *     sm_debug_statistic_removal_exact_sum_host  StatisticRemoval's correctly rounded sum of non-negative floats
+ *     sm_debug_statistic_removal_distance_host   StatisticRemoval's per-point mean distance over a neighbour list
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -52,6 +54,7 @@
  *                              an optional earlier build into the same owner
  *     sm_debug_filter_ground_removal2  every intermediate of FilterChain's GroundRemoval2 stage
  *     sm_debug_depth_cluster   DepthCluster's range image, edge mask, labels and BFS level / position per pixel
+ *     sm_debug_statistic_removal_distances  the per-point distances of a StatisticRemoval handle's last run
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
  *   each stage of M2DP and of IcpFast's iteration meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
@@ -380,6 +383,18 @@ int sm_debug_depth_edge_host(const struct sm_filter_chain* chain, int32_t filter
 int sm_debug_depth_cluster(int device, const struct sm_filter_chain* chain, int32_t filter, const float* points,
                            int64_t n, int64_t stride_bytes, float* image, int32_t* owner, uint8_t* mask, uint32_t* label,
                            int32_t* level, int32_t* seq, int32_t* components);
+
+/* StatisticRemoval's correctly rounded sum (csrc/statistic_removal.cuh) compiled for the host: the double nearest the
+ * exact sum of n non-negative floats, +inf if one term is +inf.  SM_ERR_BAD_ARGUMENT for a negative or NaN term. */
+int sm_debug_statistic_removal_exact_sum_host(const float* terms, int64_t n, double* sum);
+/* StatisticRemoval's step 3 (csrc/statistic_removal.cuh) compiled for the host: the distance of query (x, y, z) over
+ * its neighbours 1..K, given as K (x, y, z) triples in list order (entry 0 excluded), K = 1..63. */
+int sm_debug_statistic_removal_distance_host(const float* query_3, const float* neighbours_3k, int32_t K,
+                                             float* distance);
+/* The per-point distances of `filter`'s last successful run, in input order (0 for a non-finite point): *n = that
+ * run's point count (0 before any run); SM_ERR_BAD_ARGUMENT when capacity < *n. */
+int sm_debug_statistic_removal_distances(const struct sm_statistic_removal* filter, float* out, int64_t capacity,
+                                         int64_t* n);
 
 #ifdef __cplusplus
 }

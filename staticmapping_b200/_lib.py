@@ -88,6 +88,14 @@ SIGNATURES = {
     "sm_filter_chain_depth_cluster": (C.c_int, [_VP, C.c_int, _VP, C.c_int64, C.c_int64, _VP, _VP, _VP,
                                                 C.POINTER(C.c_int64), _VP]),
     "sm_filter_chain_last_error": (C.c_char_p, [_VP]),
+    "sm_statistic_removal_create": (C.c_int, [C.c_int, C.POINTER(_VP)]),
+    "sm_statistic_removal_destroy": (C.c_int, [_VP]),
+    "sm_statistic_removal_set_param": (C.c_int, [_VP, C.c_char_p, C.c_int, C.c_char_p]),
+    "sm_statistic_removal_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
+    "sm_statistic_removal_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP,
+                                                  _VP]),
+    "sm_statistic_removal_stats": (C.c_int, [_VP, _DP]),
+    "sm_statistic_removal_last_error": (C.c_char_p, [_VP]),
     # include/sm_b200_debug.h (test hooks)
     "sm_debug_solve6": (C.c_int, [C.c_int, _VP, _VP, _VP, _VP]),
     "sm_debug_solve6_host": (C.c_int, [_VP, _VP, _VP, _VP]),
@@ -141,6 +149,9 @@ SIGNATURES = {
     "sm_debug_depth_edge_host": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, C.c_int64, _VP, _VP, _VP]),
     "sm_debug_depth_cluster": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, _VP, _VP, _VP, _VP, _VP,
                                          _VP, _VP]),
+    "sm_debug_statistic_removal_exact_sum_host": (C.c_int, [_VP, C.c_int64, _DP]),
+    "sm_debug_statistic_removal_distance_host": (C.c_int, [_VP, _VP, C.c_int32, _VP]),
+    "sm_debug_statistic_removal_distances": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

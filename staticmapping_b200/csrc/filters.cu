@@ -461,6 +461,7 @@ FilterParams filter_defaults(int kind) {
   f.start_ground_height = -0.25f; f.long_line_threshold = 1.0f; f.max_long_line_height = 0.1f;
   f.max_start_height = 0.2f; f.max_error = 0.05f; f.max_slope = (float)tan(M_PI / 12.); f.max_b = 0.1f;
   f.max_dist_to_line = 0.05f; f.search_angle = 10.f; f.thread_num = 4;
+  if (kind == kFilterStatisticRemoval) { f.point_num_meank = 30; f.std_mul = 1.f; }   // in Range's storage
   return f;
 }
 
@@ -490,10 +491,24 @@ bool filter_param(FilterParams& f, const char* name, void** target, int* type) {
       {kFilterGroundRemoval2, "search_angle", 1, &f.search_angle},
       {kFilterGroundRemoval2, "bin_num", 0, &f.bin_num}, {kFilterGroundRemoval2, "segment_num", 0, &f.segment_num},
       {kFilterGroundRemoval2, "thread_num", 0, &f.thread_num},
+      {kFilterStatisticRemoval, "point_num_meank", 0, &f.point_num_meank},
+      {kFilterStatisticRemoval, "std_mul", 1, &f.std_mul},
   };
   for (const Entry& e : table)
     if (e.kind == f.kind && strcmp(e.name, name) == 0) { *target = e.p; *type = e.type; return true; }
   return false;
+}
+
+int filter_set_param(FilterParams& f, const char* name, int type, const char* text) {
+  void* target = nullptr;
+  int declared = 0;
+  if (!filter_param(f, name, &target, &declared)) return SM_ERR_UNKNOWN_OPTION;
+  if (type != 0 && type != 1) return SM_ERR_BAD_ARGUMENT;
+  // pugixml's as_int / as_float by the XML type, then XmlInterface::SetValue's cast to the declared type
+  const double v = type == 0 ? (double)(int32_t)strtol(text, nullptr, 10) : (double)(float)strtod(text, nullptr);
+  if (declared == 0) *(int32_t*)target = type == 0 ? (int32_t)v : (int32_t)to_int(v);
+  else *(float*)target = (float)v;
+  return SM_OK;
 }
 
 bool filter_configs_valid(const FilterParams& f) {
@@ -538,6 +553,13 @@ void filter_debug_fit_host(const float* d, const float* z, int n, float* m, floa
 }
 float filter_debug_distance_host(const Gr2Line* lines, int n_lines, float d, float z, int* bad) {
   return gr2_vertical_distance(lines, n_lines, d, z, bad);
+}
+
+void filter_compact_records(const char* pts, int64_t stride, const uint32_t* index_in, int n, const uint8_t* flag,
+                            uint32_t* tile_cnt, float* out, uint32_t* index_out, uint32_t* m, cudaStream_t s) {
+  const int tiles = compact_tiles(n);
+  compact_scan(tile_cnt, tiles, s);
+  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, index_in, n, flag, tile_cnt, out, index_out, m);
 }
 
 int range_image_owner(const FilterParams& f, const char* pts, int n, int64_t stride, uint32_t* pixel, uint32_t* owner,
@@ -599,10 +621,8 @@ int FilterChain::predicate_stage(int first, int cnt, const char* in, const uint3
   const int tiles = compact_tiles(n);
   filter_predicate_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, run, (uint8_t*)flag.p,
                                                             (uint32_t*)block_cnt.p);
-  compact_scan((uint32_t*)block_cnt.p, tiles, s);
-  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
-                                                          (const uint32_t*)block_cnt.p, out, index_out,
-                                                          (uint32_t*)count.p);
+  filter_compact_records(in, stride, index_in, n, (const uint8_t*)flag.p, (uint32_t*)block_cnt.p, out, index_out,
+                         (uint32_t*)count.p, s);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -613,10 +633,8 @@ int FilterChain::range_image_stage(const FilterParams& f, const char* in, const 
   SMB_RC(range_image_owner(f, in, n, stride, (uint32_t*)pixel.p, (uint32_t*)owner.p, s));
   range_image_flag_kernel<<<tiles, kCompactThreads, 0, s>>>((const uint32_t*)pixel.p, (const uint32_t*)owner.p, n,
                                                             (uint8_t*)flag.p, (uint32_t*)block_cnt.p);
-  compact_scan((uint32_t*)block_cnt.p, tiles, s);
-  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
-                                                          (const uint32_t*)block_cnt.p, out, index_out,
-                                                          (uint32_t*)count.p);
+  filter_compact_records(in, stride, index_in, n, (const uint8_t*)flag.p, (uint32_t*)block_cnt.p, out, index_out,
+                         (uint32_t*)count.p, s);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -650,10 +668,8 @@ int FilterChain::ground_removal2_stage(const FilterParams& f, const char* in, co
   gr2_ground_kernel<<<tiles, kCompactThreads, 0, s>>>(f, c, n, (const uint32_t*)cell_of.p, (const float2*)pt.p,
                                                       (const uint8_t*)member.p, ln, max_lines, n_lines,
                                                       (uint8_t*)flag.p, (uint32_t*)block_cnt.p, status);
-  compact_scan((uint32_t*)block_cnt.p, tiles, s);
-  filter_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, (const uint8_t*)flag.p,
-                                                          (const uint32_t*)block_cnt.p, out, index_out,
-                                                          (uint32_t*)count.p);
+  filter_compact_records(in, stride, index_in, n, (const uint8_t*)flag.p, (uint32_t*)block_cnt.p, out, index_out,
+                         (uint32_t*)count.p, s);
   SMB_CUDA_OK(cudaGetLastError());
   gr2 = {(const uint32_t*)cell_of.p, (const uint8_t*)member.p, cell_cnt, cell_min, ln, n_lines, (const uint8_t*)flag.p,
          max_lines, 0};
@@ -774,17 +790,12 @@ int sm_filter_chain_add(sm_filter_chain* c, const char* filter_name) {
 
 int sm_filter_chain_set_param(sm_filter_chain* c, int filter, const char* name, int type, const char* text) {
   if (!c || !name || !text || filter < 0 || filter >= (int)c->chain.filters.size()) return SM_ERR_BAD_ARGUMENT;
-  void* target = nullptr;
-  int declared = 0;
-  if (!filter_param(c->chain.filters[filter], name, &target, &declared))
-    return chain_fail(c, SM_ERR_UNKNOWN_OPTION, "Check failed: all_right (unknown param %s)", name);
-  if (type != 0 && type != 1)
-    return chain_fail(c, SM_ERR_BAD_ARGUMENT, "Check failed: all_right (param %s without a type of 0 or 1)", name);
-  // pugixml's as_int / as_float by the XML type, then XmlInterface::SetValue's cast to the declared type
-  const double v = type == 0 ? (double)(int32_t)strtol(text, nullptr, 10) : (double)(float)strtod(text, nullptr);
-  if (declared == 0) *(int32_t*)target = type == 0 ? (int32_t)v : (int32_t)to_int(v);
-  else *(float*)target = (float)v;
-  return SM_OK;
+  const int rc = filter_set_param(c->chain.filters[filter], name, type, text);
+  if (rc == SM_ERR_UNKNOWN_OPTION)
+    return chain_fail(c, rc, "Check failed: all_right (unknown param %s)", name);
+  if (rc == SM_ERR_BAD_ARGUMENT)
+    return chain_fail(c, rc, "Check failed: all_right (param %s without a type of 0 or 1)", name);
+  return rc;
 }
 
 int sm_filter_chain_validate(sm_filter_chain* c, int filter) {

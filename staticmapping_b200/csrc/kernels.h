@@ -225,6 +225,11 @@ int knn_query(const KdCompact& kc, const double* query, int64_t qstride, int nq,
 // nq x k row-major, each row ascending, (-1, +inf) where fewer than k points qualify.  max_radius2 = maxRadius^2.
 int knn_k_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, int k, double max_error2,
                 double max_radius2, bool allow_self_match, int32_t* ids, double* d2, cudaStream_t stream);
+// StatisticalOutlierRemoval's mean distance over the same search: for each query i, its mean_k + 1 (<= 64) nearest
+// points (eps = 0, self-match allowed, no radius), entry 0 dropped, mean_k terms of statistic_removal.cuh; the float
+// lands at dist[qindex[i]].  The tree must hold more than mean_k points.
+int knn_mean_distance_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, int mean_k,
+                            const uint32_t* qindex, float* dist, cudaStream_t stream);
 
 // ---- motion.cu ---------------------------------------------------------------------------
 // one iteration's de-skewed source of IcpFast with inner compensation: out = Interp(T_iter, f_i) (x) src0_i
@@ -401,17 +406,23 @@ void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* o
 
 // ---- filters.cu --------------------------------------------------------------------------
 // pre_processers::filter::Factory (pre_processors/filter_factory.cc:63-106) over the six filters built here
+// kFilterStatisticRemoval is not a kind of the chain (sm_filter_chain_add refuses it): it runs behind its own handle,
+// sm_statistic_removal (statistic_removal.cu), and shares only the parameter parsing.
 enum FilterKind : int {
   kFilterRange = 0, kFilterAxisRange, kFilterBoundingBoxRemoval, kFilterRandomSampler, kFilterRangeImage,
-  kFilterGroundRemoval2
+  kFilterGroundRemoval2, kFilterStatisticRemoval
 };
 // One filter of the chain: the members of the reference class of its kind under their XML names, at the
 // constructors' defaults (filter_range.cc:31-38, filter_axis_range.h:56-57, filter_bounding_box.h,
-// filter_random_sample.cc:29, filter_range_image.cc:29-37, filter_ground_removal2.cc:74-89).  Passed to the kernels
-// by value.
+// filter_random_sample.cc:29, filter_range_image.cc:29-37, filter_ground_removal2.cc:74-89,
+// filter_statistic_removal.h).  Passed to the kernels by value.  StatisticRemoval's two members share Range's storage:
+// a FilterParams holds the parameters of one kind, and its size and layout are what the chain's kernels take.
 struct FilterParams {
   int kind;
-  float min_range, max_range;                                       // Range
+  union {
+    struct { float min_range, max_range; };                         // Range
+    struct { int32_t point_num_meank; float std_mul; };             // StatisticRemoval
+  };
   float min, max; int axis_index;                                   // AxisRange
   float min_x, min_y, min_z, max_x, max_y, max_z;                   // BoundingBoxRemoval
   float sampling_rate;                                              // RandomSampler
@@ -421,9 +432,14 @@ struct FilterParams {
       max_long_line_height, max_start_height, max_error, max_slope, max_b, max_dist_to_line, search_angle;
   int bin_num, segment_num, thread_num;
 };
+static_assert(sizeof(FilterParams) == 136, "the chain's kernels take FilterParams by value: its layout stays put");
 FilterParams filter_defaults(int kind);
 // the reference's name for `kind`'s parameter -> its address and type (0 int32, 1 float), or false
 bool filter_param(FilterParams& f, const char* name, void** target, int* type);
+// One <param type=... name=...>text</param> of Interface::InitFromXmlNode on `f`: pugixml's as_int / as_float by the
+// XML type, then XmlInterface::SetValue's cast to the declared type.  SM_OK, SM_ERR_UNKNOWN_OPTION for a name the kind
+// does not register, SM_ERR_BAD_ARGUMENT for a type other than 0 / 1; `f` is unchanged on an error.
+int filter_set_param(FilterParams& f, const char* name, int type, const char* text);
 bool filter_configs_valid(const FilterParams& f);                   // ConfigsValid of the kind
 // constants the reference derives per Filter call, in its mix of float and double
 struct RangeImageConsts { float hres, vres; double btm; };         // filter_range_image.cc:89-93, :112
@@ -442,6 +458,11 @@ int range_image_owner(const FilterParams& f, const char* pts, int n, int64_t str
                       cudaStream_t s);
 struct FilterChain;
 const FilterChain* filter_chain_of(const ::sm_filter_chain* c);   // the chain behind the C handle, null for null
+// The end of every filter stage: after a flag kernel has stored its tile counts (compact.cuh), copies the flagged
+// records of `pts` (5 floats each) to out in input order with their scan indices (index_in, null = identity) and
+// leaves their number in *m (device memory).  tile_cnt: compact_count_bytes(n), turned into offsets in place.
+void filter_compact_records(const char* pts, int64_t stride, const uint32_t* index_in, int n, const uint8_t* flag,
+                            uint32_t* tile_cnt, float* out, uint32_t* index_out, uint32_t* m, cudaStream_t s);
 
 // ---- depth_cluster.cu --------------------------------------------------------------------------
 // sinf / cosf of RangeImage::LabelOneComponent's horizontal and vertical resolution (filter_range_image.cc:255-259)

@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "knn_smem.cuh"
+#include "statistic_removal.cuh"
 
 namespace smb {
 using namespace dev;
@@ -192,6 +193,48 @@ knn_k_kernel(KdCompact kc, const double* __restrict__ query, int64_t qstride, in
   }
 }
 
+// StatisticalOutlierRemoval's per-point mean distance (statistic_removal.cuh): the same search as knn_k_kernel for
+// k = K + 1 (eps = 0, self-match allowed, no radius), but instead of the k-row it reads each list entry's point back
+// from the padded bucket the entry names and writes one float per query, at dist[qindex[i]].  Entry 0 (d2 = 0: the
+// query or a duplicate of it) is dropped.  The minimum of one CTA per SM leaves ptxas room for the shared-memory list
+// variant's epilogue without a spill (it holds two CTAs per SM at K = 30 by its shared memory anyway).
+template <int K, bool kAllSmem>
+__global__ void __launch_bounds__(kKnnCtaThreads, 1)
+knn_mean_distance_kernel(KdCompact kc, const double* __restrict__ query, int64_t qstride, int nq, KnnKParams p,
+                         const uint32_t* __restrict__ qindex, float* __restrict__ dist) {
+  extern __shared__ __align__(128) unsigned char knn_smem[];
+  uint64_t* bar; double* extra;
+  const SmemTree tree = stage_tree(kc, knn_smem, &bar, &extra);
+  const int i = blockIdx.x * kKnnCtaThreads + threadIdx.x;
+  const double qx = i < nq ? query[i] : 0.0, qy = i < nq ? query[qstride + i] : 0.0,
+               qz = i < nq ? query[2 * qstride + i] : 0.0;
+  mbar_wait(bar, 0);
+  if (i >= nq) return;
+  const float fx = (float)qx, fy = (float)qy, fz = (float)qz;     // exact: the coordinates are widened floats
+  double sum = 0.0;
+  auto add = [&](int en) {
+    if (en < 0) return;                                            // not reached: the tree holds more than K points
+    const double* b = kc.pb + (int64_t)(en >> 3) * 24 + (en & 7);
+    sum = sr_dadd(sum, sr_neighbour_term(fx, fy, fz, (float)__ldg(b), (float)__ldg(b + 8), (float)__ldg(b + 16)));
+  };
+  if constexpr (K > 0) {
+    RegList<K> list;
+    list.init(p.k);
+    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+      if (j > K - p.k) add(list.e[j]);
+  } else {
+    const size_t at = (knn_smem_bytes(kc.levels) + 15) & ~(size_t)15;
+    SmemList list{reinterpret_cast<double*>(knn_smem + at) + threadIdx.x,
+                  reinterpret_cast<int*>(knn_smem + at + (size_t)p.k * kKnnCtaThreads * sizeof(double)) + threadIdx.x};
+    list.init(p.k);
+    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
+    for (int j = 1; j < p.k; ++j) add(list.e[j * kKnnCtaThreads]);
+  }
+  dist[qindex[i]] = sr_mean_distance(sum, p.k - 1);
+}
+
 size_t knn_k_smem_bytes(int levels, int k) {
   const size_t tree = (knn_smem_bytes(levels) + 15) & ~(size_t)15;
   return k <= 8 ? knn_smem_bytes(levels) : tree + (size_t)k * kKnnCtaThreads * (sizeof(double) + sizeof(int));
@@ -204,6 +247,19 @@ int launch_k(const KdCompact& kc, const double* query, int64_t qstride, int nq, 
   if (smem > 48 * 1024)
     SMB_CUDA_OK(cudaFuncSetAttribute(knn_k_kernel<K, kAllSmem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   knn_k_kernel<K, kAllSmem><<<ceil_div(nq, kKnnCtaThreads), kKnnCtaThreads, smem, s>>>(kc, query, qstride, nq, p, ids, d2);
+  SMB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+template <int K, bool kAllSmem>
+int launch_mean_distance(const KdCompact& kc, const double* query, int64_t qstride, int nq, const KnnKParams& p,
+                         const uint32_t* qindex, float* dist, cudaStream_t s) {
+  const size_t smem = knn_k_smem_bytes(kc.levels, p.k);
+  if (smem > 48 * 1024)
+    SMB_CUDA_OK(cudaFuncSetAttribute(knn_mean_distance_kernel<K, kAllSmem>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+  knn_mean_distance_kernel<K, kAllSmem><<<ceil_div(nq, kKnnCtaThreads), kKnnCtaThreads, smem, s>>>(kc, query, qstride, nq,
+                                                                                                   p, qindex, dist);
   SMB_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -222,6 +278,20 @@ int knn_k_query(const KdCompact& kc, const double* query, int64_t qstride, int n
                          : launch_k<8, false>(kc, query, qstride, nq, p, ids, d2, stream);
   return all ? launch_k<0, true>(kc, query, qstride, nq, p, ids, d2, stream)
              : launch_k<0, false>(kc, query, qstride, nq, p, ids, d2, stream);
+}
+
+int knn_mean_distance_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, int mean_k,
+                            const uint32_t* qindex, float* dist, cudaStream_t stream) {
+  if (nq <= 0) return 0;
+  if (mean_k < 1 || mean_k >= kKnnMaxK) return -1;
+  const KnnKParams p{mean_k + 1, 1, 1.0, kInfD};
+  const bool all = kc.levels <= kKnnSmemLevels;
+  if (p.k <= 4) return all ? launch_mean_distance<4, true>(kc, query, qstride, nq, p, qindex, dist, stream)
+                           : launch_mean_distance<4, false>(kc, query, qstride, nq, p, qindex, dist, stream);
+  if (p.k <= 8) return all ? launch_mean_distance<8, true>(kc, query, qstride, nq, p, qindex, dist, stream)
+                           : launch_mean_distance<8, false>(kc, query, qstride, nq, p, qindex, dist, stream);
+  return all ? launch_mean_distance<0, true>(kc, query, qstride, nq, p, qindex, dist, stream)
+             : launch_mean_distance<0, false>(kc, query, qstride, nq, p, qindex, dist, stream);
 }
 
 }  // namespace smb

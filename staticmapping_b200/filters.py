@@ -1,7 +1,7 @@
 """pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
 chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
-deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster.  There is no CPU
-fallback."""
+deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster.  StatisticRemoval,
+PCL's statistical outlier removal, runs on its own handle (sm_statistic_removal_*).  There is no CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -141,3 +141,94 @@ class Factory:
             raise RuntimeError(f"sm_filter_chain_depth_cluster failed with {rc}: {self._error()}")
         k = m.value
         return DepthClusters(xyz[:k].copy(), label[:k].copy(), index[:k].copy(), point_label[:n].copy())
+
+
+class StatisticRemoval:
+    """pre_processers::filter::StatisticRemoval as PCL's StatisticalOutlierRemoval (setMeanK(point_num_meank),
+    setStddevMulThresh(std_mul)), the call the reference leaves as a TODO, on the GPU (sm_statistic_removal_*,
+    include/sm_b200.h).  InitFromXmlText / InitFromXmlNode take one <filter name="StatisticRemoval"> node and parse its
+    <param>s as Factory does; SetInputCloud + Filter run it.  `Filter` returns the kept InnerCloud; Inliers() /
+    Outliers() are indices into the input and Stats() is (mean, stddev, threshold, valid) of the last run."""
+
+    def __init__(self, device: int = 0):
+        self._lib = _lib.lib()
+        self._h = C.c_void_p()
+        if self._lib.sm_statistic_removal_create(device, C.byref(self._h)) != 0:
+            raise RuntimeError("sm_statistic_removal_create failed")
+        self._cloud = None
+        self._inliers = np.zeros(0, np.int32)
+        self._outliers = np.zeros(0, np.int32)
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._lib.sm_statistic_removal_destroy(self._h)
+            self._h = None
+
+    def _error(self):
+        return (self._lib.sm_statistic_removal_last_error(self._h) or b"").decode()
+
+    def InitFromXmlText(self, text):
+        self.InitFromXmlNode(ET.fromstring(text))
+
+    def InitFromXmlNode(self, filter_node):
+        """A <param> with an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57);
+        a node that is not <filter name="StatisticRemoval"> raises ValueError."""
+        if isinstance(filter_node, (str, bytes)):
+            filter_node = ET.fromstring(filter_node)
+        if filter_node.tag != "filter" or filter_node.attrib.get("name", "") != "StatisticRemoval":
+            raise ValueError('expected a <filter name="StatisticRemoval"> node')
+        for param in filter_node.findall("param"):
+            self.SetParam(param.attrib.get("name", ""), param.attrib.get("type"), (param.text or "").strip())
+
+    def SetParam(self, name, ptype, text):
+        try:
+            ptype = int(ptype)
+        except (TypeError, ValueError):
+            ptype = -1
+        rc = self._lib.sm_statistic_removal_set_param(self._h, str(name).encode(), ptype, str(text).encode())
+        if rc != 0:
+            raise CheckFailure(self._error())
+
+    def SetInputCloud(self, cloud):
+        pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
+        if pts.ndim != 2 or pts.shape[1] != 5:
+            raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
+        self._cloud = pts
+
+    def Filter(self):
+        """CheckFailure for 1..point_num_meank finite points; ValueError for a point_num_meank outside 1..63."""
+        if self._cloud is None:
+            return None
+        pts = self._cloud
+        n = pts.shape[0]
+        out = np.empty_like(pts)
+        index = np.empty(n, np.int32)
+        m = C.c_int64(0)
+        rc = self._lib.sm_statistic_removal_run(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m),
+                                                index.ctypes.data)
+        if rc == -20:
+            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
+        if rc == -5:
+            raise CheckFailure(self._error())
+        if rc == -1:
+            raise ValueError(self._error())
+        if rc != 0:
+            raise RuntimeError(f"sm_statistic_removal_run failed with {rc}: {self._error()}")
+        self._inliers = index[:m.value].copy()
+        mask = np.ones(n, bool)
+        mask[self._inliers] = False
+        self._outliers = np.nonzero(mask)[0].astype(np.int32)
+        return InnerCloud(out[:m.value].copy())
+
+    def Inliers(self):
+        return self._inliers
+
+    def Outliers(self):
+        return self._outliers
+
+    def Stats(self):
+        """(mean, stddev, threshold, valid) of the last run"""
+        s = (C.c_double * 4)()
+        self._lib.sm_statistic_removal_stats(self._h, s)
+        return tuple(s)
+
