@@ -276,6 +276,24 @@ inline void VoxelGridFilterB200(const data::InnerCloudType& input, float voxel_s
   output->points.resize(m);
 }
 
+// The Filter body of FilterChainB200 and StatisticRemovalB200: CHECK-fails with last_error(h) when run (sm_*_run) fails
+template <typename Handle, typename Run, typename LastError>
+inline void FilterRecordsB200(Handle* h, Run run, LastError last_error, const char* run_name,
+                              const data::InnerCloudType& input, data::InnerCloudType* const output,
+                              std::vector<int>* const inliers) {
+  CHECK(output);
+  const int64_t n = static_cast<int64_t>(input.points.size());
+  output->points.resize(input.points.size());
+  std::vector<int32_t> index(input.points.size());
+  int64_t m = 0;
+  if (n > 0) {
+    const int rc = run(h, &input.points[0].x, n, sizeof(data::InnerPointType), &output->points[0].x, &m, index.data());
+    CHECK_EQ(rc, 0) << run_name << " failed (" << rc << "): " << last_error(h);
+  }
+  output->points.resize(m);
+  if (inliers) inliers->assign(index.begin(), index.begin() + m);
+}
+
 // pre_processers::filter::Factory on the GPU (pre_processors/filter_factory.cc:63-106): one chain per Factory.  The
 // body of Factory::InitFromXmlNode becomes one Add per <filter> and one SetParam per <param>, and the body of
 // Factory::Filter (the call in DataCollector::CloudPreProcessing, builder/data/data_collector.cc:137-141)
@@ -304,18 +322,8 @@ class FilterChainB200 {
 
   void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,
               std::vector<int>* const inliers = nullptr) {
-    CHECK(output);
-    const int64_t n = static_cast<int64_t>(input.points.size());
-    output->points.resize(input.points.size());
-    std::vector<int32_t> index(input.points.size());
-    int64_t m = 0;
-    if (n > 0) {
-      const int rc = sm_filter_chain_run(chain_, &input.points[0].x, n, sizeof(data::InnerPointType),
-                                         &output->points[0].x, &m, index.data());
-      CHECK_EQ(rc, 0) << "sm_filter_chain_run failed (" << rc << "): " << sm_filter_chain_last_error(chain_);
-    }
-    output->points.resize(m);
-    if (inliers) inliers->assign(index.begin(), index.begin() + m);
+    FilterRecordsB200(chain_, sm_filter_chain_run, sm_filter_chain_last_error, "sm_filter_chain_run", input, output,
+                      inliers);
   }
 
   // RangeImage::DepthCluster (pre_processors/filter_range_image.cc:143-173) of the chain's RangeImage `filter` over
@@ -369,18 +377,8 @@ class StatisticRemovalB200 {
   // outside 1..63
   void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,
               std::vector<int>* const inliers = nullptr) {
-    CHECK(output);
-    const int64_t n = static_cast<int64_t>(input.points.size());
-    output->points.resize(input.points.size());
-    std::vector<int32_t> index(input.points.size());
-    int64_t m = 0;
-    if (n > 0) {
-      const int rc = sm_statistic_removal_run(filter_, &input.points[0].x, n, sizeof(data::InnerPointType),
-                                              &output->points[0].x, &m, index.data());
-      CHECK_EQ(rc, 0) << "sm_statistic_removal_run failed (" << rc << "): " << sm_statistic_removal_last_error(filter_);
-    }
-    output->points.resize(m);
-    if (inliers) inliers->assign(index.begin(), index.begin() + m);
+    FilterRecordsB200(filter_, sm_statistic_removal_run, sm_statistic_removal_last_error, "sm_statistic_removal_run",
+                      input, output, inliers);
   }
 
  private:

@@ -23,6 +23,7 @@
 #include "common.cuh"
 #include "compact.cuh"
 #include "kernels.h"
+#include "record_filter.h"
 
 namespace smb {
 namespace {
@@ -729,49 +730,21 @@ int FilterChain::run(const char* in, int64_t n, int64_t stride, float* out, int3
 // ---- C ABI ------------------------------------------------------------------------------------------------------
 using namespace smb;
 
-struct sm_filter_chain {
-  int device = 0;
+struct sm_filter_chain : RecordFilter {
   FilterChain chain;
   DepthCluster depth;
-  cudaStream_t stream = nullptr;
-  DevBuf host_in, host_out, host_idx;
-  char error[256] = {0};
+  explicit sm_filter_chain(int device) : RecordFilter(device, "the filter chain") {}
 };
 
 namespace smb {
 const FilterChain* filter_chain_of(const ::sm_filter_chain* c) { return c ? &c->chain : nullptr; }
 }  // namespace smb
 
-namespace {
-int chain_fail(sm_filter_chain* c, int rc, const char* fmt, const char* arg) {
-  snprintf(c->error, sizeof(c->error), fmt, arg);
-  return rc;
-}
-int chain_device(sm_filter_chain* c) {
-  const int rc = select_device(c->device);
-  if (rc == SM_ERR_NO_DEVICE)
-    return chain_fail(c, rc, "no CUDA device: the filter chain has no CPU fallback%s", "");
-  if (rc == SM_ERR_BAD_ARGUMENT)
-    snprintf(c->error, sizeof(c->error), "device %d is out of range: the filter chain has no CPU fallback", c->device);
-  return rc;
-}
-}  // namespace
-
 extern "C" {
 
-int sm_filter_chain_create(int device, sm_filter_chain** out) {
-  if (!out || device < 0) return SM_ERR_BAD_ARGUMENT;
-  *out = new sm_filter_chain;
-  (*out)->device = device;
-  return SM_OK;
-}
+int sm_filter_chain_create(int device, sm_filter_chain** out) { return create_record_filter(device, out); }
 
-int sm_filter_chain_destroy(sm_filter_chain* c) {
-  if (!c) return SM_ERR_BAD_ARGUMENT;
-  if (c->stream) { cudaSetDevice(c->device); cudaStreamDestroy(c->stream); }
-  delete c;
-  return SM_OK;
-}
+int sm_filter_chain_destroy(sm_filter_chain* c) { return destroy_record_filter(c); }
 
 int sm_filter_chain_add(sm_filter_chain* c, const char* filter_name) {
   if (!c || !filter_name) return SM_ERR_BAD_ARGUMENT;
@@ -784,18 +757,13 @@ int sm_filter_chain_add(sm_filter_chain* c, const char* filter_name) {
     }
   for (const char* name : {"GroundRemoval", "StatisticRemoval", "VoxelGrid"})
     if (strcmp(filter_name, name) == 0)
-      return chain_fail(c, SM_ERR_UNSUPPORTED_TYPE, "filter %s is not built into the chain", filter_name);
-  return chain_fail(c, SM_ERR_UNKNOWN_OPTION, "%s not supported yet.", filter_name);
+      return c->fail(SM_ERR_UNSUPPORTED_TYPE, "filter %s is not built into the chain", filter_name);
+  return c->fail(SM_ERR_UNKNOWN_OPTION, "%s not supported yet.", filter_name);
 }
 
 int sm_filter_chain_set_param(sm_filter_chain* c, int filter, const char* name, int type, const char* text) {
   if (!c || !name || !text || filter < 0 || filter >= (int)c->chain.filters.size()) return SM_ERR_BAD_ARGUMENT;
-  const int rc = filter_set_param(c->chain.filters[filter], name, type, text);
-  if (rc == SM_ERR_UNKNOWN_OPTION)
-    return chain_fail(c, rc, "Check failed: all_right (unknown param %s)", name);
-  if (rc == SM_ERR_BAD_ARGUMENT)
-    return chain_fail(c, rc, "Check failed: all_right (param %s without a type of 0 or 1)", name);
-  return rc;
+  return c->set_param(c->chain.filters[filter], name, type, text);
 }
 
 int sm_filter_chain_validate(sm_filter_chain* c, int filter) {
@@ -805,91 +773,64 @@ int sm_filter_chain_validate(sm_filter_chain* c, int filter) {
 
 int sm_filter_chain_set_option(sm_filter_chain* c, const char* name, const char* text) {
   if (!c || !name || !text) return SM_ERR_BAD_ARGUMENT;
-  if (strcmp(name, "sample_seed") != 0) return chain_fail(c, SM_ERR_UNKNOWN_OPTION, "unknown chain option %s", name);
+  if (strcmp(name, "sample_seed") != 0) return c->fail(SM_ERR_UNKNOWN_OPTION, "unknown chain option %s", name);
   c->chain.sample_seed = (uint32_t)strtoul(text, nullptr, 10);
   return SM_OK;
 }
 
 int sm_filter_chain_run_device(sm_filter_chain* c, const float* dev_points, int64_t n, int64_t stride_bytes,
                                float* dev_out, int64_t* m_out, int32_t* dev_inlier_index, void* cuda_stream) {
-  if (!c || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 ||
-      (n > 0 && (!dev_points || !dev_out)))
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(chain_device(c));
+  if (!c || !records_ok(dev_points, n, stride_bytes, dev_out, m_out)) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(c->use_device());
   const int rc = c->chain.run((const char*)dev_points, n, stride_bytes, dev_out, dev_inlier_index, m_out,
                               (cudaStream_t)cuda_stream);
   if (rc == SM_ERR_CHECK_FAILED)
-    chain_fail(c, rc, "Check failed: %s", "an inverted BoundingBoxRemoval box or line.start[0] < line.end[0]");
-  else if (rc == SM_ERR_BAD_ARGUMENT)
-    chain_fail(c, rc, "%s", "a RangeImage or GroundRemoval2 grid size the chain cannot run");
-  else if (rc == SM_ERR_CUDA)
-    chain_fail(c, rc, "%s", last_cuda_error());
-  return rc;
+    return c->fail(rc, "Check failed: an inverted BoundingBoxRemoval box or line.start[0] < line.end[0]");
+  if (rc == SM_ERR_BAD_ARGUMENT) return c->fail(rc, "a RangeImage or GroundRemoval2 grid size the chain cannot run");
+  return c->cuda_fail(rc);
 }
 
 int sm_filter_chain_run(sm_filter_chain* c, const float* points, int64_t n, int64_t stride_bytes, float* out,
                         int64_t* m_out, int32_t* inlier_index) {
-  if (!c || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 || (n > 0 && (!points || !out)))
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(chain_device(c));
+  if (!c || !records_ok(points, n, stride_bytes, out, m_out)) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(c->use_device());
   *m_out = 0;
-  if (n == 0) return sm_filter_chain_run_device(c, nullptr, 0, stride_bytes, nullptr, m_out, nullptr, nullptr);
-  if (!c->stream) SMB_CUDA_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-  const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
-  SMB_RC(c->host_in.reserve(in_bytes));
-  SMB_RC(c->host_out.reserve((size_t)n * 20));
-  SMB_RC(c->host_idx.reserve((size_t)n * sizeof(int32_t)));
-  SMB_CUDA_OK(cudaMemcpyAsync(c->host_in.p, points, in_bytes, cudaMemcpyHostToDevice, c->stream));
-  SMB_RC(sm_filter_chain_run_device(c, (const float*)c->host_in.p, n, stride_bytes, (float*)c->host_out.p, m_out,
-                                    (int32_t*)c->host_idx.p, c->stream));
-  if (*m_out > 0) {
-    SMB_CUDA_OK(cudaMemcpyAsync(out, c->host_out.p, (size_t)*m_out * 20, cudaMemcpyDeviceToHost, c->stream));
-    if (inlier_index)
-      SMB_CUDA_OK(cudaMemcpyAsync(inlier_index, c->host_idx.p, (size_t)*m_out * sizeof(int32_t), cudaMemcpyDeviceToHost,
-                                  c->stream));
-    SMB_CUDA_OK(cudaStreamSynchronize(c->stream));
-  }
-  return SM_OK;
+  return run_record_filter(c, sm_filter_chain_run_device, points, n, stride_bytes, out, m_out, inlier_index);
 }
 
 int sm_filter_chain_depth_cluster(sm_filter_chain* c, int filter, const float* points, int64_t n, int64_t stride_bytes,
                                   float* out_xyz, uint32_t* out_label, int32_t* out_index, int64_t* m_out,
                                   uint32_t* point_label) {
-  if (!c || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 ||
-      (n > 0 && (!points || !out_xyz || !out_label || !out_index)))
+  if (!c || !records_ok(points, n, stride_bytes, out_xyz, m_out) || (n > 0 && (!out_label || !out_index)))
     return SM_ERR_BAD_ARGUMENT;
   *m_out = 0;
   if (filter < 0 || filter >= (int)c->chain.filters.size() || c->chain.filters[filter].kind != kFilterRangeImage)
-    return chain_fail(c, SM_ERR_BAD_ARGUMENT, "DepthCluster needs a RangeImage of the chain%s", "");
+    return c->fail(SM_ERR_BAD_ARGUMENT, "DepthCluster needs a RangeImage of the chain");
   // SetInputCloud drops an empty cloud (filter_range_image.cc:67-71), then CHECK(this->inner_cloud_ != nullptr) (:144)
-  if (n == 0) return chain_fail(c, SM_ERR_CHECK_FAILED, "Check failed: this->inner_cloud_ != nullptr%s", "");
+  if (n == 0) return c->fail(SM_ERR_CHECK_FAILED, "Check failed: this->inner_cloud_ != nullptr");
   const FilterParams& f = c->chain.filters[filter];
-  if (!depth_cluster_grid_ok(f))
-    return chain_fail(c, SM_ERR_BAD_ARGUMENT, "%s", "a RangeImage grid DepthCluster cannot run");
-  SMB_RC(chain_device(c));
-  if (!c->stream) SMB_CUDA_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-  const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
-  SMB_RC(c->host_in.reserve(in_bytes));
-  SMB_RC(c->host_out.reserve((size_t)n * 24));    // xyz, label, index, point label
-  float* d_xyz = (float*)c->host_out.p;
-  uint32_t* d_label = (uint32_t*)(d_xyz + 3 * n);
-  int32_t* d_index = (int32_t*)(d_label + n);
-  uint32_t* d_point = (uint32_t*)(d_index + n);
-  SMB_CUDA_OK(cudaMemcpyAsync(c->host_in.p, points, in_bytes, cudaMemcpyHostToDevice, c->stream));
-  const int rc = c->depth.run(f, (const char*)c->host_in.p, (int)n, stride_bytes, d_xyz, d_label, d_index,
-                              point_label ? d_point : nullptr, m_out, c->stream);
-  if (rc == SM_ERR_CUDA) return chain_fail(c, rc, "%s", last_cuda_error());
-  SMB_RC(rc);
-  const size_t m = (size_t)*m_out;
-  if (m > 0) {
-    SMB_CUDA_OK(cudaMemcpyAsync(out_xyz, d_xyz, m * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    SMB_CUDA_OK(cudaMemcpyAsync(out_label, d_label, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-    SMB_CUDA_OK(cudaMemcpyAsync(out_index, d_index, m * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  }
-  if (point_label)
-    SMB_CUDA_OK(cudaMemcpyAsync(point_label, d_point, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-  SMB_CUDA_OK(cudaStreamSynchronize(c->stream));
-  return SM_OK;
+  if (!depth_cluster_grid_ok(f)) return c->fail(SM_ERR_BAD_ARGUMENT, "a RangeImage grid DepthCluster cannot run");
+  SMB_RC(c->use_device());
+  return c->cuda_fail([&]() -> int {
+    SMB_RC(c->stage(points, n, stride_bytes, (size_t)n * 24));    // xyz, label, index, point label
+    float* d_xyz = (float*)c->host_out.p;
+    uint32_t* d_label = (uint32_t*)(d_xyz + 3 * n);
+    int32_t* d_index = (int32_t*)(d_label + n);
+    uint32_t* d_point = (uint32_t*)(d_index + n);
+    SMB_RC(c->depth.run(f, (const char*)c->host_in.p, (int)n, stride_bytes, d_xyz, d_label, d_index,
+                        point_label ? d_point : nullptr, m_out, c->stream));
+    const size_t m = (size_t)*m_out;
+    if (m > 0) {
+      SMB_CUDA_OK(cudaMemcpyAsync(out_xyz, d_xyz, m * 3 * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+      SMB_CUDA_OK(cudaMemcpyAsync(out_label, d_label, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+      SMB_CUDA_OK(cudaMemcpyAsync(out_index, d_index, m * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+    }
+    if (point_label)
+      SMB_CUDA_OK(cudaMemcpyAsync(point_label, d_point, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                                  c->stream));
+    SMB_CUDA_OK(cudaStreamSynchronize(c->stream));
+    return SM_OK;
+  }());
 }
 
 const char* sm_filter_chain_last_error(const sm_filter_chain* c) { return c ? c->error : ""; }

@@ -407,7 +407,7 @@ void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* o
 // ---- filters.cu --------------------------------------------------------------------------
 // pre_processers::filter::Factory (pre_processors/filter_factory.cc:63-106) over the six filters built here
 // kFilterStatisticRemoval is not a kind of the chain (sm_filter_chain_add refuses it): it runs behind its own handle,
-// sm_statistic_removal (statistic_removal.cu), and shares only the parameter parsing.
+// sm_statistic_removal (statistic_removal.cu), built like the chain's on the handle core of record_filter.h.
 enum FilterKind : int {
   kFilterRange = 0, kFilterAxisRange, kFilterBoundingBoxRemoval, kFilterRandomSampler, kFilterRangeImage,
   kFilterGroundRemoval2, kFilterStatisticRemoval

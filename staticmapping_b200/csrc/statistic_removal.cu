@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "compact.cuh"
 #include "kernels.h"
+#include "record_filter.h"
 #include "statistic_removal.cuh"
 
 namespace smb {
@@ -198,69 +199,38 @@ struct StatisticRemoval {
 // ---- C ABI ------------------------------------------------------------------------------------------------------
 using namespace smb;
 
-struct sm_statistic_removal {
-  int device = 0;
+struct sm_statistic_removal : RecordFilter {
   StatisticRemoval f;
-  cudaStream_t stream = nullptr;
-  DevBuf host_in, host_out, host_idx;
-  char error[256] = {0};
+  explicit sm_statistic_removal(int device) : RecordFilter(device, "StatisticRemoval") {}
 };
 
 namespace {
-int sr_fail(sm_statistic_removal* h, int rc, const char* fmt, const char* arg) {
-  snprintf(h->error, sizeof(h->error), fmt, arg);
-  return rc;
-}
-int sr_device(sm_statistic_removal* h) {
-  const int rc = select_device(h->device);
-  if (rc == SM_ERR_NO_DEVICE) return sr_fail(h, rc, "no CUDA device: StatisticRemoval has no CPU fallback%s", "");
-  if (rc == SM_ERR_BAD_ARGUMENT)
-    snprintf(h->error, sizeof(h->error), "device %d is out of range: StatisticRemoval has no CPU fallback", h->device);
-  return rc;
-}
 // the checks both run entry points make before a device is selected
 int sr_check(sm_statistic_removal* h, const void* points, int64_t n, int64_t stride_bytes, const void* out,
              const int64_t* m_out) {
-  if (!h || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 20 || stride_bytes % 4 || (n > 0 && (!points || !out)))
-    return SM_ERR_BAD_ARGUMENT;
+  if (!h || !records_ok(points, n, stride_bytes, out, m_out)) return SM_ERR_BAD_ARGUMENT;
   const int K = h->f.params.point_num_meank;
-  if (K < 1 || K > kSrMaxMeanK) {
-    snprintf(h->error, sizeof(h->error), "point_num_meank %d is outside 1..%d", K, kSrMaxMeanK);
-    return SM_ERR_BAD_ARGUMENT;
-  }
+  if (K < 1 || K > kSrMaxMeanK)
+    return h->fail(SM_ERR_BAD_ARGUMENT, "point_num_meank %d is outside 1..%d", K, kSrMaxMeanK);
   return SM_OK;
 }
 }  // namespace
 
 extern "C" {
 
-int sm_statistic_removal_create(int device, sm_statistic_removal** out) {
-  if (!out || device < 0) return SM_ERR_BAD_ARGUMENT;
-  *out = new sm_statistic_removal;
-  (*out)->device = device;
-  return SM_OK;
-}
+int sm_statistic_removal_create(int device, sm_statistic_removal** out) { return create_record_filter(device, out); }
 
-int sm_statistic_removal_destroy(sm_statistic_removal* h) {
-  if (!h) return SM_ERR_BAD_ARGUMENT;
-  if (h->stream) { cudaSetDevice(h->device); cudaStreamDestroy(h->stream); }
-  delete h;
-  return SM_OK;
-}
+int sm_statistic_removal_destroy(sm_statistic_removal* h) { return destroy_record_filter(h); }
 
 int sm_statistic_removal_set_param(sm_statistic_removal* h, const char* name, int type, const char* text) {
   if (!h || !name || !text) return SM_ERR_BAD_ARGUMENT;
-  const int rc = filter_set_param(h->f.params, name, type, text);
-  if (rc == SM_ERR_UNKNOWN_OPTION) return sr_fail(h, rc, "Check failed: all_right (unknown param %s)", name);
-  if (rc == SM_ERR_BAD_ARGUMENT)
-    return sr_fail(h, rc, "Check failed: all_right (param %s without a type of 0 or 1)", name);
-  return rc;
+  return h->set_param(h->f.params, name, type, text);
 }
 
 int sm_statistic_removal_run_device(sm_statistic_removal* h, const float* dev_points, int64_t n, int64_t stride_bytes,
                                     float* dev_out, int64_t* m_out, int32_t* dev_inlier_index, void* cuda_stream) {
   SMB_RC(sr_check(h, dev_points, n, stride_bytes, dev_out, m_out));
-  SMB_RC(sr_device(h));
+  SMB_RC(h->use_device());
   if (n == 0) {
     *m_out = 0;
     h->f.last_n = 0;
@@ -270,42 +240,21 @@ int sm_statistic_removal_run_device(sm_statistic_removal* h, const float* dev_po
   }
   uint32_t* idx = (uint32_t*)dev_inlier_index;
   if (!idx) {
-    if (h->host_idx.reserve((size_t)n * sizeof(int32_t)) < 0) return sr_fail(h, SM_ERR_CUDA, "%s", last_cuda_error());
+    SMB_RC(h->cuda_fail(h->host_idx.reserve((size_t)n * sizeof(int32_t))));
     idx = (uint32_t*)h->host_idx.p;
   }
   const int rc = h->f.run((const char*)dev_points, n, stride_bytes, dev_out, idx, m_out, (cudaStream_t)cuda_stream);
   if (rc == SM_ERR_CHECK_FAILED)
-    sr_fail(h, rc, "Check failed: %s", "between 1 and point_num_meank finite points (PCL reads past its k-list)");
-  else if (rc == SM_ERR_BAD_ARGUMENT)
-    sr_fail(h, rc, "%s", "more finite points than the 24-level k-d tree holds");
-  else if (rc == SM_ERR_CUDA)
-    sr_fail(h, rc, "%s", last_cuda_error());
-  return rc;
+    return h->fail(rc, "Check failed: between 1 and point_num_meank finite points (PCL reads past its k-list)");
+  if (rc == SM_ERR_BAD_ARGUMENT) return h->fail(rc, "more finite points than the 24-level k-d tree holds");
+  return h->cuda_fail(rc);
 }
 
 int sm_statistic_removal_run(sm_statistic_removal* h, const float* points, int64_t n, int64_t stride_bytes, float* out,
                              int64_t* m_out, int32_t* inlier_index) {
   SMB_RC(sr_check(h, points, n, stride_bytes, out, m_out));
-  SMB_RC(sr_device(h));
-  if (n == 0) return sm_statistic_removal_run_device(h, nullptr, 0, stride_bytes, nullptr, m_out, nullptr, nullptr);
-  if (!h->stream) SMB_CUDA_OK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
-  SMB_RC(h->host_in.reserve(in_bytes));
-  SMB_RC(h->host_out.reserve((size_t)n * 20));
-  SMB_RC(h->host_idx.reserve((size_t)n * sizeof(int32_t)));
-  SMB_CUDA_OK(cudaMemcpyAsync(h->host_in.p, points, in_bytes, cudaMemcpyHostToDevice, h->stream));
-  int64_t m = 0;
-  SMB_RC(sm_statistic_removal_run_device(h, (const float*)h->host_in.p, n, stride_bytes, (float*)h->host_out.p, &m,
-                                         (int32_t*)h->host_idx.p, h->stream));
-  if (m > 0) {
-    SMB_CUDA_OK(cudaMemcpyAsync(out, h->host_out.p, (size_t)m * 20, cudaMemcpyDeviceToHost, h->stream));
-    if (inlier_index)
-      SMB_CUDA_OK(cudaMemcpyAsync(inlier_index, h->host_idx.p, (size_t)m * sizeof(int32_t), cudaMemcpyDeviceToHost,
-                                  h->stream));
-    SMB_CUDA_OK(cudaStreamSynchronize(h->stream));
-  }
-  *m_out = m;
-  return SM_OK;
+  SMB_RC(h->use_device());
+  return run_record_filter(h, sm_statistic_removal_run_device, points, n, stride_bytes, out, m_out, inlier_index);
 }
 
 int sm_statistic_removal_stats(const sm_statistic_removal* h, double* out4) {

@@ -22,31 +22,96 @@ class DepthClusters(NamedTuple):
     point_label: np.ndarray    # (n,) uint32, the label of every pixel owner of the input (small clusters too), else 0
 
 
-class Factory:
-    """filter::Factory.  InitFromXmlText / InitFromXmlNode take the <filters> node; SetInputCloud + Filter run the
-    chain on the GPU.  `Filter` returns the inlier InnerCloud; Inliers() / Outliers() are indices into the input."""
+def _records(cloud):
+    pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
+    if pts.ndim != 2 or pts.shape[1] != 5:
+        raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
+    return pts
+
+
+def _param_type(text):
+    """a <param>'s type attribute, -1 when it is missing or not an integer (the ABI refuses it)"""
+    try:
+        return int(text)
+    except (TypeError, ValueError):
+        return -1
+
+
+class _RecordFilter:
+    """A GPU filter over (N,5) records behind a C handle, whose functions are named `_abi`_create, _run and so on.
+    SetInputCloud + Filter run it; `Filter` returns the kept InnerCloud, Inliers() / Outliers() are indices into the
+    input."""
+    _abi = ""
 
     def __init__(self, device: int = 0):
         self._lib = _lib.lib()
         self._h = C.c_void_p()
-        if self._lib.sm_filter_chain_create(device, C.byref(self._h)) != 0:
-            raise RuntimeError("sm_filter_chain_create failed")
+        if self._fn("create")(device, C.byref(self._h)) != 0:
+            raise RuntimeError(f"{self._abi}_create failed")
         self._cloud = None
         self._inliers = np.zeros(0, np.int32)
         self._outliers = np.zeros(0, np.int32)
-        self.filter_names = []
-        self.messages = []
 
     def __del__(self):
         if getattr(self, "_h", None):
-            self._lib.sm_filter_chain_destroy(self._h)
+            self._fn("destroy")(self._h)
             self._h = None
 
+    def _fn(self, name):
+        return getattr(self._lib, f"{self._abi}_{name}")
+
     def _error(self):
-        return (self._lib.sm_filter_chain_last_error(self._h) or b"").decode()
+        return (self._fn("last_error")(self._h) or b"").decode()
+
+    def _check(self, rc, name):
+        """the exception for return code `rc` of the entry point `name`"""
+        if rc == -20:
+            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
+        if rc == -5:
+            raise CheckFailure(self._error())
+        if rc == -1:       # e.g. a RangeImage size of 0, where the reference keeps its previous cloud without a CHECK
+            raise ValueError(self._error())
+        if rc != 0:
+            raise RuntimeError(f"{self._abi}_{name} failed with {rc}: {self._error()}")
 
     def InitFromXmlText(self, text):
         self.InitFromXmlNode(ET.fromstring(text))
+
+    def SetInputCloud(self, cloud):
+        self._cloud = _records(cloud)
+
+    def Filter(self):
+        if self._cloud is None:
+            return None
+        pts = self._cloud
+        n = pts.shape[0]
+        out = np.empty_like(pts)
+        index = np.empty(n, np.int32)
+        m = C.c_int64(0)
+        self._check(self._fn("run")(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m), index.ctypes.data),
+                    "run")
+        self._inliers = index[:m.value].copy()
+        mask = np.ones(n, bool)
+        mask[self._inliers] = False
+        self._outliers = np.nonzero(mask)[0].astype(np.int32)
+        return InnerCloud(out[:m.value].copy())
+
+    def Inliers(self):
+        return self._inliers
+
+    def Outliers(self):
+        return self._outliers
+
+
+class Factory(_RecordFilter):
+    """filter::Factory.  InitFromXmlText / InitFromXmlNode take the <filters> node; SetInputCloud + Filter run the
+    chain on the GPU.  `Filter` returns the inlier InnerCloud; Inliers() / Outliers() are indices into the input."""
+    _abi = "sm_filter_chain"
+
+    def __init__(self, device: int = 0):
+        super().__init__(device)
+        self.filter_names = []
+        self.messages = []
 
     def InitFromXmlNode(self, filters_node):
         """filter_factory.cc:63-81.  A name the reference does not register is skipped with a message; a <param> with
@@ -64,11 +129,8 @@ class Factory:
                 raise CheckFailure(self._error())
             self.filter_names.append(name)
             for param in node.findall("param"):
-                try:
-                    ptype = int(param.attrib["type"])
-                except (KeyError, ValueError):
-                    ptype = -1
-                rc = self._lib.sm_filter_chain_set_param(self._h, index, param.attrib.get("name", "").encode(), ptype,
+                rc = self._lib.sm_filter_chain_set_param(self._h, index, param.attrib.get("name", "").encode(),
+                                                         _param_type(param.attrib.get("type")),
                                                          (param.text or "").strip().encode())
                 if rc != 0:
                     raise CheckFailure(self._error())
@@ -79,96 +141,33 @@ class Factory:
     def SetSampleSeed(self, seed):
         self._lib.sm_filter_chain_set_option(self._h, b"sample_seed", str(int(seed)).encode())
 
-    def SetInputCloud(self, cloud):
-        pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
-        if pts.ndim != 2 or pts.shape[1] != 5:
-            raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
-        self._cloud = pts
-
-    def Filter(self):
-        if self._cloud is None:
-            return None
-        pts = self._cloud
-        n = pts.shape[0]
-        out = np.empty_like(pts)
-        index = np.empty(n, np.int32)
-        m = C.c_int64(0)
-        rc = self._lib.sm_filter_chain_run(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m), index.ctypes.data)
-        if rc == -20:
-            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
-        if rc == -5:
-            raise CheckFailure(self._error())
-        if rc == -1:       # e.g. a RangeImage size of 0, where the reference keeps its previous cloud without a CHECK
-            raise ValueError(self._error())
-        if rc != 0:
-            raise RuntimeError(f"sm_filter_chain_run failed with {rc}: {self._error()}")
-        self._inliers = index[:m.value].copy()
-        mask = np.ones(n, bool)
-        mask[self._inliers] = False
-        self._outliers = np.nonzero(mask)[0].astype(np.int32)
-        return InnerCloud(out[:m.value].copy())
-
-    def Inliers(self):
-        return self._inliers
-
-    def Outliers(self):
-        return self._outliers
-
     def DepthCluster(self, filter_index, cloud):
         """RangeImage::DepthCluster (filter_range_image.cc:143-173) after SetInputCloud(cloud) + Filter on the chain's
         filter `filter_index`, which must be a RangeImage; `cloud` is that filter's own input, (N,5) records.  An empty
         cloud raises CheckFailure (CHECK(inner_cloud_ != nullptr)); a filter that is not a RangeImage or a grid with
         horizontal_line_num < 2 raises ValueError."""
-        pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
-        if pts.ndim != 2 or pts.shape[1] != 5:
-            raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
+        pts = _records(cloud)
         n = pts.shape[0]
         xyz = np.empty((max(n, 1), 3), np.float32)
         label = np.empty(max(n, 1), np.uint32)
         index = np.empty(max(n, 1), np.int32)
         point_label = np.zeros(max(n, 1), np.uint32)
         m = C.c_int64(0)
-        rc = self._lib.sm_filter_chain_depth_cluster(self._h, int(filter_index), pts.ctypes.data, n, 20, xyz.ctypes.data,
-                                                     label.ctypes.data, index.ctypes.data, C.byref(m),
-                                                     point_label.ctypes.data)
-        if rc == -20:
-            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
-        if rc == -5:
-            raise CheckFailure(self._error())
-        if rc == -1:
-            raise ValueError(self._error())
-        if rc != 0:
-            raise RuntimeError(f"sm_filter_chain_depth_cluster failed with {rc}: {self._error()}")
+        self._check(self._lib.sm_filter_chain_depth_cluster(self._h, int(filter_index), pts.ctypes.data, n, 20,
+                                                            xyz.ctypes.data, label.ctypes.data, index.ctypes.data,
+                                                            C.byref(m), point_label.ctypes.data), "depth_cluster")
         k = m.value
         return DepthClusters(xyz[:k].copy(), label[:k].copy(), index[:k].copy(), point_label[:n].copy())
 
 
-class StatisticRemoval:
+class StatisticRemoval(_RecordFilter):
     """pre_processers::filter::StatisticRemoval as PCL's StatisticalOutlierRemoval (setMeanK(point_num_meank),
     setStddevMulThresh(std_mul)), the call the reference leaves as a TODO, on the GPU (sm_statistic_removal_*,
     include/sm_b200.h).  InitFromXmlText / InitFromXmlNode take one <filter name="StatisticRemoval"> node and parse its
-    <param>s as Factory does; SetInputCloud + Filter run it.  `Filter` returns the kept InnerCloud; Inliers() /
+    <param>s as Factory does; SetInputCloud + Filter run it.  `Filter` returns the kept InnerCloud and raises
+    CheckFailure for 1..point_num_meank finite points, ValueError for a point_num_meank outside 1..63; Inliers() /
     Outliers() are indices into the input and Stats() is (mean, stddev, threshold, valid) of the last run."""
-
-    def __init__(self, device: int = 0):
-        self._lib = _lib.lib()
-        self._h = C.c_void_p()
-        if self._lib.sm_statistic_removal_create(device, C.byref(self._h)) != 0:
-            raise RuntimeError("sm_statistic_removal_create failed")
-        self._cloud = None
-        self._inliers = np.zeros(0, np.int32)
-        self._outliers = np.zeros(0, np.int32)
-
-    def __del__(self):
-        if getattr(self, "_h", None):
-            self._lib.sm_statistic_removal_destroy(self._h)
-            self._h = None
-
-    def _error(self):
-        return (self._lib.sm_statistic_removal_last_error(self._h) or b"").decode()
-
-    def InitFromXmlText(self, text):
-        self.InitFromXmlNode(ET.fromstring(text))
+    _abi = "sm_statistic_removal"
 
     def InitFromXmlNode(self, filter_node):
         """A <param> with an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57);
@@ -181,54 +180,13 @@ class StatisticRemoval:
             self.SetParam(param.attrib.get("name", ""), param.attrib.get("type"), (param.text or "").strip())
 
     def SetParam(self, name, ptype, text):
-        try:
-            ptype = int(ptype)
-        except (TypeError, ValueError):
-            ptype = -1
-        rc = self._lib.sm_statistic_removal_set_param(self._h, str(name).encode(), ptype, str(text).encode())
+        rc = self._lib.sm_statistic_removal_set_param(self._h, str(name).encode(), _param_type(ptype),
+                                                      str(text).encode())
         if rc != 0:
             raise CheckFailure(self._error())
-
-    def SetInputCloud(self, cloud):
-        pts = cloud.points if isinstance(cloud, InnerCloud) else np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
-        if pts.ndim != 2 or pts.shape[1] != 5:
-            raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
-        self._cloud = pts
-
-    def Filter(self):
-        """CheckFailure for 1..point_num_meank finite points; ValueError for a point_num_meank outside 1..63."""
-        if self._cloud is None:
-            return None
-        pts = self._cloud
-        n = pts.shape[0]
-        out = np.empty_like(pts)
-        index = np.empty(n, np.int32)
-        m = C.c_int64(0)
-        rc = self._lib.sm_statistic_removal_run(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m),
-                                                index.ctypes.data)
-        if rc == -20:
-            raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
-        if rc == -5:
-            raise CheckFailure(self._error())
-        if rc == -1:
-            raise ValueError(self._error())
-        if rc != 0:
-            raise RuntimeError(f"sm_statistic_removal_run failed with {rc}: {self._error()}")
-        self._inliers = index[:m.value].copy()
-        mask = np.ones(n, bool)
-        mask[self._inliers] = False
-        self._outliers = np.nonzero(mask)[0].astype(np.int32)
-        return InnerCloud(out[:m.value].copy())
-
-    def Inliers(self):
-        return self._inliers
-
-    def Outliers(self):
-        return self._outliers
 
     def Stats(self):
         """(mean, stddev, threshold, valid) of the last run"""
         s = (C.c_double * 4)()
         self._lib.sm_statistic_removal_stats(self._h, s)
         return tuple(s)
-
