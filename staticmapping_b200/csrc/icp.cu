@@ -143,6 +143,14 @@ __device__ __forceinline__ void load_query(const IcpBuffers& b, const double* T,
   }
 }
 
+// the match of source point i for phase B, and its d2 counted in the 2048-bin global histogram (a fire-and-forget
+// reduction, L2-resident)
+__device__ __forceinline__ void store_match(const IcpBuffers& b, int i, int slot, double d2) {
+  b.slot[i] = slot;
+  b.d2[i] = d2;
+  if (finite_d2(d2)) atomicAdd(&b.hist[dist_bin(d2)], 1u);
+}
+
 template <bool kAllSmem, bool kComp>
 __global__ void __launch_bounds__(kKnnCtaThreads, SMB_KNN_MIN_CTAS)
 icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __restrict__ deskewed) {
@@ -153,20 +161,10 @@ icp_knn_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __restrict_
   if (threadIdx.x < 16) T[threadIdx.x] = b.state->T_iter[threadIdx.x];
   __syncthreads();
   const int begin = blockIdx.x * per_cta, end = min(begin + per_cta, p.n_source);
-  int i = begin + threadIdx.x;
-  double px = 0.0, py = 0.0, pz = 0.0;
-  if (i < end) load_query<kComp>(b, T, deskewed, i, px, py, pz);
-  mbar_wait(bar, 0);      // every thread waits: the CTA must not retire while the copy engine writes its smem
-  while (i < end) {
-    int slot; double d2;
-    knn1_smem<kAllSmem>(tree, px, py, pz, p.max_error2, slot, d2);
-    b.slot[i] = slot;
-    b.d2[i] = d2;
-    // fire-and-forget reduction straight into the 2048-bin global histogram (L2-resident)
-    if (finite_d2(d2)) atomicAdd(&b.hist[dist_bin(d2)], 1u);
-    i += kKnnCtaThreads;
-    if (i < end) load_query<kComp>(b, T, deskewed, i, px, py, pz);
-  }
+  knn1_cta<kAllSmem>(
+      tree, bar, begin, end, p.max_error2,
+      [&](int i, double& x, double& y, double& z) { load_query<kComp>(b, T, deskewed, i, x, y, z); },
+      [&](int i, int slot, double d2) { store_match(b, i, slot, d2); });
 }
 
 // Phase A with several queries per thread (many alignments in flight: queries_per_cta > 256): lockstep root
@@ -189,12 +187,7 @@ icp_knn_batch_kernel(IcpBuffers b, IcpParams p, int per_cta, const double* __res
       [&](int i, double& x, double& y, double& z) { load_query<kComp>(b, T, deskewed, i, x, y, z); },
       [&](int i, int best, double head) { b.slot[i] = best; b.d2[i] = head; },
       [&](int i, double& head, int& best) { head = __ldcg(b.d2 + i); best = __ldcg(b.slot + i); },
-      [&](int i, int slot, double d2) {
-        b.slot[i] = slot;
-        b.d2[i] = d2;
-        // fire-and-forget reduction straight into the 2048-bin global histogram (L2-resident)
-        if (finite_d2(d2)) atomicAdd(&b.hist[dist_bin(d2)], 1u);
-      });
+      [&](int i, int slot, double d2) { store_match(b, i, slot, d2); });
 }
 
 // -------------------------------------------------------------------------------- phase B
@@ -355,13 +348,10 @@ knn_query_kernel(KdCompact kc, const double* __restrict__ query, int64_t qstride
   uint64_t* bar; double* extra;
   const SmemTree tree = stage_tree(kc, knn_smem, &bar, &extra);
   const int begin = blockIdx.x * per_cta, end = min(begin + per_cta, nq);
-  mbar_wait(bar, 0);
-  for (int i = begin + threadIdx.x; i < end; i += kKnnCtaThreads) {
-    int slot; double d;
-    knn1_smem<kAllSmem>(tree, query[i], query[qstride + i], query[2 * qstride + i], max_error2, slot, d);
-    ids[i] = slot >= 0 ? kc.pid[slot] : -1;
-    d2[i] = d;
-  }
+  knn1_cta<kAllSmem>(
+      tree, bar, begin, end, max_error2,
+      [&](int i, double& x, double& y, double& z) { x = query[i]; y = query[qstride + i]; z = query[2 * qstride + i]; },
+      [&](int i, int slot, double d) { ids[i] = slot >= 0 ? kc.pid[slot] : -1; d2[i] = d; });
 }
 
 

@@ -58,6 +58,13 @@ struct RegList {
     for (int j = 0; j < K; ++j)
       if (j >= K - k) { ids[j - (K - k)] = e[j] >= 0 ? pid[e[j]] : -1; d2[j - (K - k)] = d[j]; }
   }
+  // f(j, entry) for the list's entries j = 0 .. k - 1 in order
+  template <class F>
+  __device__ __forceinline__ void for_each(int k, F f) const {
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+      if (j >= K - k) f(j - (K - k), e[j]);
+  }
 };
 
 // the same list in this thread's shared-memory columns: entry j at d[j * kKnnCtaThreads]
@@ -86,6 +93,10 @@ struct SmemList {
       ids[j] = en >= 0 ? pid[en] : -1;
       d2[j] = d[j * kKnnCtaThreads];
     }
+  }
+  template <class F>
+  __device__ __forceinline__ void for_each(int k, F f) const {
+    for (int j = 0; j < k; ++j) f(j, e[j * kKnnCtaThreads]);
   }
 };
 
@@ -118,31 +129,14 @@ __device__ __forceinline__ void scan_bucket_k(const double* __restrict__ pb, int
   }
 }
 
-// recurseKnn for one query: the root visit (as knn_root_visit, with the k-entry list and both far-side tests), then the
+// recurseKnn for one query: the root visit (knn_root_visit's, with the k-entry list and both far-side tests), then the
 // far visits deepest pending level first
 template <bool kAllSmem, class List>
 __device__ __forceinline__ void knn_k_search(const SmemTree& t, double qx, double qy, double qz, const KnnKParams& p,
                                              List& list) {
   double head = kInfD;
-  t.sq[0] = qx; t.sq[kKnnCtaThreads] = qy; t.sq[2 * kKnnCtaThreads] = qz;
-  const int lsm = kAllSmem ? t.levels : min(t.levels, kKnnSmemLevels);
-  int h = 0, l = 0;
-  bool leaf = false;
-  while (l < lsm) {
-    const int cd = t.s_dim[h];
-    if (cd == 3) { leaf = true; break; }
-    h = 2 * h + 1 + (t.sq[cd * kKnnCtaThreads] > t.s_cut[h] ? 1 : 0);
-    ++l;
-  }
-  if (!kAllSmem && !leaf) {
-    while (l < t.levels) {
-      double cut; int cd;
-      ldg_node(t.g_node, h, cut, cd);
-      if (cd == 3) break;
-      h = 2 * h + 1 + (t.sq[cd * kKnnCtaThreads] > cut ? 1 : 0);
-      ++l;
-    }
-  }
+  int h, l;
+  knn_root_descent<kAllSmem>(t, qx, qy, qz, h, l);
   scan_bucket_k(t.pb, (h + 1 - (1 << l)) << (t.levels - l), qx, qy, qz, p, list, head);
   int hp1 = h + 1, ll = l;
   uint32_t pending = 0u, turns = 0u;
@@ -163,45 +157,51 @@ __device__ __forceinline__ void knn_k_search(const SmemTree& t, double qx, doubl
   }
 }
 
-// one query per thread; K = 4 / 8: the list in registers (k <= K), K = 0: in shared memory behind the staged tree
-template <int K, bool kAllSmem>
-__global__ void __launch_bounds__(kKnnCtaThreads)
-knn_k_kernel(KdCompact kc, const double* __restrict__ query, int64_t qstride, int nq, KnnKParams p,
-             int32_t* __restrict__ ids, double* __restrict__ d2) {
-  extern __shared__ __align__(128) unsigned char knn_smem[];
-  uint64_t* bar; double* extra;
-  const SmemTree tree = stage_tree(kc, knn_smem, &bar, &extra);
-  const int i = blockIdx.x * kKnnCtaThreads + threadIdx.x;
-  const double qx = i < nq ? query[i] : 0.0, qy = i < nq ? query[qstride + i] : 0.0,
-               qz = i < nq ? query[2 * qstride + i] : 0.0;
-  mbar_wait(bar, 0);
-  if (i >= nq) return;
-  int32_t* out_ids = ids + (int64_t)i * p.k;
-  double* out_d2 = d2 + (int64_t)i * p.k;
-  if constexpr (K > 0) {
-    RegList<K> list;
-    list.init(p.k);
-    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
-    list.store(kc.pid, p.k, out_ids, out_d2);
-  } else {
-    const size_t at = (knn_smem_bytes(kc.levels) + 15) & ~(size_t)15;
-    SmemList list{reinterpret_cast<double*>(knn_smem + at) + threadIdx.x,
-                  reinterpret_cast<int*>(knn_smem + at + (size_t)p.k * kKnnCtaThreads * sizeof(double)) + threadIdx.x};
-    list.init(p.k);
-    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
-    list.store(kc.pid, p.k, out_ids, out_d2);
+// What a query keeps of its finished list.  at(kc, p, i, qx, qy, qz) is called before the search and returns the
+// function the finished list is handed to.  KnnRows forms the row's address there, ahead of the search: formed after
+// it, ptxas schedules the shared-memory list's search differently.  The returned functions capture copies, not `this`:
+// capturing `this` costs the register-list mean-distance kernels 20 to 22 registers.
+// KnnRows: the query's k-row, original ids (-1: no entry) and squared distances.
+struct KnnRows {
+  static constexpr int kMinCtasPerSm = 0;      // no minimum
+  int32_t* ids;
+  double* d2;
+  __device__ __forceinline__ auto at(const KdCompact& kc, const KnnKParams& p, int i, double, double, double) const {
+    int32_t* out_ids = ids + (int64_t)i * p.k;
+    double* out_d2 = d2 + (int64_t)i * p.k;
+    return [&kc, &p, out_ids, out_d2](const auto& list) { list.store(kc.pid, p.k, out_ids, out_d2); };
   }
-}
+};
 
-// StatisticalOutlierRemoval's per-point mean distance (statistic_removal.cuh): the same search as knn_k_kernel for
-// k = K + 1 (eps = 0, self-match allowed, no radius), but instead of the k-row it reads each list entry's point back
-// from the padded bucket the entry names and writes one float per query, at dist[qindex[i]].  Entry 0 (d2 = 0: the
-// query or a duplicate of it) is dropped.  The minimum of one CTA per SM leaves ptxas room for the shared-memory list
-// variant's epilogue without a spill (it holds two CTAs per SM at K = 30 by its shared memory anyway).
-template <int K, bool kAllSmem>
-__global__ void __launch_bounds__(kKnnCtaThreads, 1)
-knn_mean_distance_kernel(KdCompact kc, const double* __restrict__ query, int64_t qstride, int nq, KnnKParams p,
-                         const uint32_t* __restrict__ qindex, float* __restrict__ dist) {
+// KnnMeanDistance: StatisticalOutlierRemoval's per-point mean distance (statistic_removal.cuh), for k = K + 1 (eps = 0,
+// self-match allowed, no radius): instead of the k-row it reads each list entry's point back from the padded bucket the
+// entry names and writes one float per query, at dist[qindex[i]].  Entry 0 (d2 = 0: the query or a duplicate of it) is
+// dropped.  The minimum of one CTA per SM leaves ptxas room for the shared-memory list variant's epilogue without a
+// spill (it holds two CTAs per SM at K = 30 by its shared memory anyway).
+struct KnnMeanDistance {
+  static constexpr int kMinCtasPerSm = 1;
+  const uint32_t* qindex;
+  float* dist;
+  __device__ __forceinline__ auto at(const KdCompact& kc, const KnnKParams& p, int i, double qx, double qy,
+                                     double qz) const {
+    return [&kc, &p, i, qx, qy, qz, qindex = qindex, dist = dist](const auto& list) {
+      const float fx = (float)qx, fy = (float)qy, fz = (float)qz;   // exact: the coordinates are widened floats
+      double sum = 0.0;
+      list.for_each(p.k, [&](int j, int en) {
+        if (j == 0 || en < 0) return;            // en < 0 is not reached: the tree holds more than K points
+        const double* b = kc.pb + (int64_t)(en >> 3) * 24 + (en & 7);
+        sum = sr_dadd(sum, sr_neighbour_term(fx, fy, fz, (float)__ldg(b), (float)__ldg(b + 8), (float)__ldg(b + 16)));
+      });
+      dist[qindex[i]] = sr_mean_distance(sum, p.k - 1);
+    };
+  }
+};
+
+// one query per thread; K = 4 / 8: the list in registers (k <= K), K = 0: in shared memory behind the staged tree
+template <int K, bool kAllSmem, class Epilogue>
+__global__ void __launch_bounds__(kKnnCtaThreads, Epilogue::kMinCtasPerSm)
+knn_k_kernel(KdCompact kc, const double* __restrict__ query, int64_t qstride, int nq, KnnKParams p,
+             Epilogue epilogue) {
   extern __shared__ __align__(128) unsigned char knn_smem[];
   uint64_t* bar; double* extra;
   const SmemTree tree = stage_tree(kc, knn_smem, &bar, &extra);
@@ -210,29 +210,21 @@ knn_mean_distance_kernel(KdCompact kc, const double* __restrict__ query, int64_t
                qz = i < nq ? query[2 * qstride + i] : 0.0;
   mbar_wait(bar, 0);
   if (i >= nq) return;
-  const float fx = (float)qx, fy = (float)qy, fz = (float)qz;     // exact: the coordinates are widened floats
-  double sum = 0.0;
-  auto add = [&](int en) {
-    if (en < 0) return;                                            // not reached: the tree holds more than K points
-    const double* b = kc.pb + (int64_t)(en >> 3) * 24 + (en & 7);
-    sum = sr_dadd(sum, sr_neighbour_term(fx, fy, fz, (float)__ldg(b), (float)__ldg(b + 8), (float)__ldg(b + 16)));
+  const auto finish = epilogue.at(kc, p, i, qx, qy, qz);
+  const auto search = [&](auto& list) {
+    list.init(p.k);
+    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
+    finish(list);
   };
   if constexpr (K > 0) {
     RegList<K> list;
-    list.init(p.k);
-    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
-#pragma unroll
-    for (int j = 0; j < K; ++j)
-      if (j > K - p.k) add(list.e[j]);
+    search(list);
   } else {
     const size_t at = (knn_smem_bytes(kc.levels) + 15) & ~(size_t)15;
     SmemList list{reinterpret_cast<double*>(knn_smem + at) + threadIdx.x,
                   reinterpret_cast<int*>(knn_smem + at + (size_t)p.k * kKnnCtaThreads * sizeof(double)) + threadIdx.x};
-    list.init(p.k);
-    knn_k_search<kAllSmem>(tree, qx, qy, qz, p, list);
-    for (int j = 1; j < p.k; ++j) add(list.e[j * kKnnCtaThreads]);
+    search(list);
   }
-  dist[qindex[i]] = sr_mean_distance(sum, p.k - 1);
 }
 
 size_t knn_k_smem_bytes(int levels, int k) {
@@ -240,28 +232,22 @@ size_t knn_k_smem_bytes(int levels, int k) {
   return k <= 8 ? knn_smem_bytes(levels) : tree + (size_t)k * kKnnCtaThreads * (sizeof(double) + sizeof(int));
 }
 
-template <int K, bool kAllSmem>
-int launch_k(const KdCompact& kc, const double* query, int64_t qstride, int nq, const KnnKParams& p, int32_t* ids,
-             double* d2, cudaStream_t s) {
+// the kernel for p.k (list in registers up to k = 8) and the tree's depth (all inner levels staged or not)
+template <class Epilogue>
+int launch_k(const KdCompact& kc, const double* query, int64_t qstride, int nq, const KnnKParams& p,
+             const Epilogue& epilogue, cudaStream_t s) {
   const size_t smem = knn_k_smem_bytes(kc.levels, p.k);
-  if (smem > 48 * 1024)
-    SMB_CUDA_OK(cudaFuncSetAttribute(knn_k_kernel<K, kAllSmem>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  knn_k_kernel<K, kAllSmem><<<ceil_div(nq, kKnnCtaThreads), kKnnCtaThreads, smem, s>>>(kc, query, qstride, nq, p, ids, d2);
-  SMB_CUDA_OK(cudaGetLastError());
-  return 0;
-}
-
-template <int K, bool kAllSmem>
-int launch_mean_distance(const KdCompact& kc, const double* query, int64_t qstride, int nq, const KnnKParams& p,
-                         const uint32_t* qindex, float* dist, cudaStream_t s) {
-  const size_t smem = knn_k_smem_bytes(kc.levels, p.k);
-  if (smem > 48 * 1024)
-    SMB_CUDA_OK(cudaFuncSetAttribute(knn_mean_distance_kernel<K, kAllSmem>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem));
-  knn_mean_distance_kernel<K, kAllSmem><<<ceil_div(nq, kKnnCtaThreads), kKnnCtaThreads, smem, s>>>(kc, query, qstride, nq,
-                                                                                                   p, qindex, dist);
-  SMB_CUDA_OK(cudaGetLastError());
-  return 0;
+  const auto launch = [&](auto kernel) {
+    if (smem > 48 * 1024)
+      SMB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<ceil_div(nq, kKnnCtaThreads), kKnnCtaThreads, smem, s>>>(kc, query, qstride, nq, p, epilogue);
+    SMB_CUDA_OK(cudaGetLastError());
+    return 0;
+  };
+  const bool all = kc.levels <= kKnnSmemLevels;
+  if (p.k <= 4) return all ? launch(knn_k_kernel<4, true, Epilogue>) : launch(knn_k_kernel<4, false, Epilogue>);
+  if (p.k <= 8) return all ? launch(knn_k_kernel<8, true, Epilogue>) : launch(knn_k_kernel<8, false, Epilogue>);
+  return all ? launch(knn_k_kernel<0, true, Epilogue>) : launch(knn_k_kernel<0, false, Epilogue>);
 }
 
 }  // namespace
@@ -270,28 +256,15 @@ int knn_k_query(const KdCompact& kc, const double* query, int64_t qstride, int n
                 double max_radius2, bool allow_self_match, int32_t* ids, double* d2, cudaStream_t stream) {
   if (nq <= 0) return 0;
   if (k < 1 || k > kKnnMaxK) return -1;
-  const KnnKParams p{k, allow_self_match ? 1 : 0, max_error2, max_radius2};
-  const bool all = kc.levels <= kKnnSmemLevels;
-  if (k <= 4) return all ? launch_k<4, true>(kc, query, qstride, nq, p, ids, d2, stream)
-                         : launch_k<4, false>(kc, query, qstride, nq, p, ids, d2, stream);
-  if (k <= 8) return all ? launch_k<8, true>(kc, query, qstride, nq, p, ids, d2, stream)
-                         : launch_k<8, false>(kc, query, qstride, nq, p, ids, d2, stream);
-  return all ? launch_k<0, true>(kc, query, qstride, nq, p, ids, d2, stream)
-             : launch_k<0, false>(kc, query, qstride, nq, p, ids, d2, stream);
+  return launch_k(kc, query, qstride, nq, KnnKParams{k, allow_self_match ? 1 : 0, max_error2, max_radius2},
+                  KnnRows{ids, d2}, stream);
 }
 
 int knn_mean_distance_query(const KdCompact& kc, const double* query, int64_t qstride, int nq, int mean_k,
                             const uint32_t* qindex, float* dist, cudaStream_t stream) {
   if (nq <= 0) return 0;
   if (mean_k < 1 || mean_k >= kKnnMaxK) return -1;
-  const KnnKParams p{mean_k + 1, 1, 1.0, kInfD};
-  const bool all = kc.levels <= kKnnSmemLevels;
-  if (p.k <= 4) return all ? launch_mean_distance<4, true>(kc, query, qstride, nq, p, qindex, dist, stream)
-                           : launch_mean_distance<4, false>(kc, query, qstride, nq, p, qindex, dist, stream);
-  if (p.k <= 8) return all ? launch_mean_distance<8, true>(kc, query, qstride, nq, p, qindex, dist, stream)
-                           : launch_mean_distance<8, false>(kc, query, qstride, nq, p, qindex, dist, stream);
-  return all ? launch_mean_distance<0, true>(kc, query, qstride, nq, p, qindex, dist, stream)
-             : launch_mean_distance<0, false>(kc, query, qstride, nq, p, qindex, dist, stream);
+  return launch_k(kc, query, qstride, nq, KnnKParams{mean_k + 1, 1, 1.0, kInfD}, KnnMeanDistance{qindex, dist}, stream);
 }
 
 }  // namespace smb

@@ -289,16 +289,11 @@ __device__ __forceinline__ int knn_descend(const SmemTree& t, double me2, double
   return (h + 1 - (1 << l)) << (t.levels - l);
 }
 
-// First visit of a query: the descent from the root (staged levels from shared memory, the rest one
-// packed record per level), the first bucket, and the mask of the path levels whose far side passes
-// with the head that bucket left, each tested exactly (node re-read: shared memory or L1).  rd = 0 and
-// off = 0 along the whole root path, so rd_new(a) = 0 + (-(0*0) + off^2) = off^2 exactly, and the pop
-// re-tests every level of the mask with the head of its moment.
+// The descent of a query from the root to its leaf (heap index h, level l): the staged levels from shared
+// memory, the rest one packed record per level.  Leaves the query in its t.sq column.
 template <bool kAllSmem>
-__device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, double qy, double qz, double me2,
-                                               double& head, int& best, int& hp1_out, int& ll_out, uint32_t& mask_out) {
-  head = __longlong_as_double(0x7ff0000000000000ll);
-  best = -1;
+__device__ __forceinline__ void knn_root_descent(const SmemTree& t, double qx, double qy, double qz, int& h_out,
+                                                 int& l_out) {
   t.sq[0] = qx; t.sq[kKnnCtaThreads] = qy; t.sq[2 * kKnnCtaThreads] = qz;
   const int lsm = kAllSmem ? t.levels : min(t.levels, kKnnSmemLevels);    // levels staged in shared memory
   int h = 0, l = 0;
@@ -318,6 +313,20 @@ __device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, dou
       ++l;
     }
   }
+  h_out = h; l_out = l;
+}
+
+// First visit of a query: the root descent, the first bucket, and the mask of the path levels whose far
+// side passes with the head that bucket left, each tested exactly (node re-read: shared memory or L1).
+// rd = 0 and off = 0 along the whole root path, so rd_new(a) = 0 + (-(0*0) + off^2) = off^2 exactly, and
+// the pop re-tests every level of the mask with the head of its moment.
+template <bool kAllSmem>
+__device__ __forceinline__ void knn_root_visit(const SmemTree& t, double qx, double qy, double qz, double me2,
+                                               double& head, int& best, int& hp1_out, int& ll_out, uint32_t& mask_out) {
+  head = __longlong_as_double(0x7ff0000000000000ll);
+  best = -1;
+  int h, l;
+  knn_root_descent<kAllSmem>(t, qx, qy, qz, h, l);
   scan_bucket(t.pb, (h + 1 - (1 << l)) << (t.levels - l), qx, qy, qz, head, best);
   const int hp1 = h + 1, ll = l;
   uint32_t mask = 0u;
@@ -342,6 +351,25 @@ __device__ __forceinline__ void knn1_smem(const SmemTree& t, double qx, double q
   }
   best_out = best;
   d2_out = head;
+}
+
+// One CTA's range [begin, end), one query per thread (consecutive threads = consecutive queries).  The first
+// query is loaded while the tree top is being staged, each next one right after the previous result is stored.
+// load_q(i, x, y, z), store(i, best, d2).
+template <bool kAllSmem, typename LoadQ, typename Store>
+__device__ __forceinline__ void knn1_cta(const SmemTree& tree, uint64_t* bar, int begin, int end, double me2,
+                                         LoadQ load_q, Store store) {
+  int i = begin + threadIdx.x;
+  double3 q = make_double3(0.0, 0.0, 0.0);
+  if (i < end) load_q(i, q.x, q.y, q.z);
+  mbar_wait(bar, 0);      // every thread waits: the CTA must not retire while the copy engine writes its smem
+  while (i < end) {
+    int slot; double d2;
+    knn1_smem<kAllSmem>(tree, q.x, q.y, q.z, me2, slot, d2);
+    store(i, slot, d2);
+    i += kKnnCtaThreads;
+    if (i < end) load_q(i, q.x, q.y, q.z);
+  }
 }
 
 // ---- far visits of a batch of queries, one WARP working through a list ---------------------------

@@ -753,6 +753,33 @@ int set_f64(sm_handle* h, bool target, bool on_device, const double* pts, int64_
   return target ? icp_set_target(h, *f, pts, nrm, n, on_device) : icp_set_source(h, *f, pts, n, on_device);
 }
 
+// The set-up the stand-alone searches share: the target uploaded AoS -> SoA and its kIds tree built, then, for nq > 0,
+// the queries uploaded and search(tree, queries, query stride) run, all on stream s, which is synchronised after the
+// target's upload and again before returning.  Host clouds go through one staging buffer; device clouds are read in
+// place.
+template <class Search>
+int knn_on_target(const double* target, int64_t nt, const double* query, int64_t nq, int bucket, bool on_device,
+                  cudaStream_t s, Search search) {
+  const int64_t ts = pad64(nt), qs = pad64(nq > 0 ? nq : 1);
+  DevBuf stage, tgt, qry, kdws;
+  KdCompactTree tree;
+  if (!on_device) SMB_RC(stage.reserve((size_t)3 * (size_t)(nt > nq ? nt : nq) * sizeof(double)));   // both uploads
+  SMB_RC(tgt.reserve((size_t)3 * ts * sizeof(double)));
+  SMB_RC(qry.reserve((size_t)3 * qs * sizeof(double)));
+  SMB_RC(tree.reserve((int)nt, bucket, KdCompactTree::kIds));
+  KdWorkspace ws;
+  SMB_RC(ws.carve(kdws, (int)nt, bucket));
+  SMB_RC(upload_soa(target, nt, on_device, stage, (double*)tgt.p, ts, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  SMB_RC(tree.build((const double*)tgt.p, nullptr, ts, (int)nt, bucket, ws, s));
+  if (nq > 0) {
+    SMB_RC(upload_soa(query, nq, on_device, stage, (double*)qry.p, qs, s));
+    SMB_RC(search(tree.view(), (const double*)qry.p, qs));
+  }
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  return SM_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1058,8 +1085,29 @@ int sm_calculate_normals(int device, const double* points, int64_t n, double* ou
   return SM_OK;
 }
 
+// sm_knn1 / sm_debug_knn1_batched: host clouds, the default stream, synchronised before returning
 static int knn1_impl(int device, const double* target, int64_t nt, const double* query, int64_t nq,
-                     double epsilon, int bucket, int queries_per_cta, int32_t* ids, double* d2);
+                     double epsilon, int bucket, int queries_per_cta, int32_t* ids, double* d2) {
+  // buckets hold at most 8 points (one padded bucket = x[8] y[8] z[8]); libnabo's default is 8
+  if (!target || !query || nt <= 0 || nt > (1 << 30) || nq < 0 || nq > (1 << 30) || bucket < 2 || bucket > 8 ||
+      !(epsilon >= 0.0))
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  if (kd_num_levels((int)nt, bucket) > 24) return SM_ERR_BAD_ARGUMENT;
+  cudaStream_t s = nullptr;
+  DevBuf ids_d, d2_d, items;
+  SMB_RC(ids_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(int32_t)));
+  SMB_RC(d2_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(double)));
+  SMB_RC(items.reserve(knn_items_bytes((int)nq)));
+  const auto search = [&](const KdCompact& kc, const double* q, int64_t qs) -> int {
+    SMB_RC(knn_query(kc, q, qs, (int)nq, (1.0 + epsilon) * (1.0 + epsilon), (int32_t*)ids_d.p, (double*)d2_d.p, s,
+                     queries_per_cta, (int4*)items.p));
+    SMB_CUDA_OK(cudaMemcpyAsync(ids, ids_d.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    SMB_CUDA_OK(cudaMemcpyAsync(d2, d2_d.p, (size_t)nq * sizeof(double), cudaMemcpyDeviceToHost, s));
+    return SM_OK;
+  };
+  return knn_on_target(target, nt, query, nq, bucket, false, s, search);
+}
 
 int sm_knn1(int device, const double* target, int64_t nt, const double* query, int64_t nq,
             double epsilon, int bucket, int32_t* ids, double* d2) {
@@ -1074,44 +1122,9 @@ int sm_debug_knn1_batched(int device, const double* target, int64_t nt, const do
   return knn1_impl(device, target, nt, query, nq, epsilon, bucket, queries_per_cta, ids, d2);
 }
 
-static int knn1_impl(int device, const double* target, int64_t nt, const double* query, int64_t nq,
-                     double epsilon, int bucket, int queries_per_cta, int32_t* ids, double* d2) {
-  // buckets hold at most 8 points (one padded bucket = x[8] y[8] z[8]); libnabo's default is 8
-  if (!target || !query || nt <= 0 || nt > (1 << 30) || nq < 0 || nq > (1 << 30) || bucket < 2 || bucket > 8 ||
-      !(epsilon >= 0.0))
-    return SM_ERR_BAD_ARGUMENT;
-  SMB_RC(select_device(device));
-  cudaStream_t s = nullptr;
-  const int64_t ts = pad64(nt), qs = pad64(nq > 0 ? nq : 1);
-  const int levels = kd_num_levels((int)nt, bucket);
-  if (levels > 24) return SM_ERR_BAD_ARGUMENT;
-  DevBuf stage, tgt, qry, kdws, ids_d, d2_d, items;
-  KdCompactTree tree;
-  SMB_RC(stage.reserve((size_t)3 * (size_t)(nt > nq ? nt : nq) * sizeof(double)));   // shared by both uploads
-  SMB_RC(tgt.reserve((size_t)3 * ts * sizeof(double)));
-  SMB_RC(qry.reserve((size_t)3 * qs * sizeof(double)));
-  SMB_RC(tree.reserve((int)nt, bucket, KdCompactTree::kIds));
-  KdWorkspace ws;
-  SMB_RC(ws.carve(kdws, (int)nt, bucket));
-  SMB_RC(ids_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(int32_t)));
-  SMB_RC(d2_d.reserve((size_t)(nq > 0 ? nq : 1) * sizeof(double)));
-  SMB_RC(items.reserve(knn_items_bytes((int)nq)));
-  SMB_RC(upload_soa(target, nt, false, stage, (double*)tgt.p, ts, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  SMB_RC(tree.build((const double*)tgt.p, nullptr, ts, (int)nt, bucket, ws, s));
-  if (nq > 0) {
-    SMB_RC(upload_soa(query, nq, false, stage, (double*)qry.p, qs, s));
-    SMB_RC(knn_query(tree.view(), (const double*)qry.p, qs, (int)nq, (1.0 + epsilon) * (1.0 + epsilon), (int32_t*)ids_d.p,
-                     (double*)d2_d.p, s, queries_per_cta, (int4*)items.p));
-    SMB_CUDA_OK(cudaMemcpyAsync(ids, ids_d.p, (size_t)nq * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    SMB_CUDA_OK(cudaMemcpyAsync(d2, d2_d.p, (size_t)nq * sizeof(double), cudaMemcpyDeviceToHost, s));
-  }
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  return SM_OK;
-}
-
 // sm_knn / sm_knn_device: the tree of sm_knn1, then knn_k_query.  Host clouds go through a staging buffer on the
 // default stream; device clouds are read in place and the results written to the caller's buffers on its stream.
+// Either way the stream is synchronised before returning.
 static int knn_impl(int device, const double* target, int64_t nt, const double* query, int64_t nq, int32_t k,
                     double epsilon, double max_radius, uint32_t flags, int bucket, int32_t* ids, double* d2,
                     bool on_device, cudaStream_t s) {
@@ -1121,36 +1134,24 @@ static int knn_impl(int device, const double* target, int64_t nt, const double* 
     return SM_ERR_BAD_ARGUMENT;
   if (kd_num_levels((int)nt, bucket) > 24) return SM_ERR_BAD_ARGUMENT;
   SMB_RC(select_device(device));
-  const int64_t ts = pad64(nt), qs = pad64(nq > 0 ? nq : 1);
-  DevBuf stage, tgt, qry, kdws, ids_d, d2_d;
-  KdCompactTree tree;
-  if (!on_device) SMB_RC(stage.reserve((size_t)3 * (size_t)(nt > nq ? nt : nq) * sizeof(double)));
-  SMB_RC(tgt.reserve((size_t)3 * ts * sizeof(double)));
-  SMB_RC(qry.reserve((size_t)3 * qs * sizeof(double)));
-  SMB_RC(tree.reserve((int)nt, bucket, KdCompactTree::kIds));
-  KdWorkspace ws;
-  SMB_RC(ws.carve(kdws, (int)nt, bucket));
-  const size_t n_out = (size_t)(nq > 0 ? nq : 1) * (size_t)k;
+  DevBuf ids_d, d2_d;
   if (!on_device) {
+    const size_t n_out = (size_t)(nq > 0 ? nq : 1) * (size_t)k;
     SMB_RC(ids_d.reserve(n_out * sizeof(int32_t)));
     SMB_RC(d2_d.reserve(n_out * sizeof(double)));
   }
-  SMB_RC(upload_soa(target, nt, on_device, stage, (double*)tgt.p, ts, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  SMB_RC(tree.build((const double*)tgt.p, nullptr, ts, (int)nt, bucket, ws, s));
-  if (nq > 0) {
-    SMB_RC(upload_soa(query, nq, on_device, stage, (double*)qry.p, qs, s));
+  const auto search = [&](const KdCompact& kc, const double* q, int64_t qs) -> int {
     int32_t* ids_out = on_device ? ids : (int32_t*)ids_d.p;
     double* d2_out = on_device ? d2 : (double*)d2_d.p;
-    SMB_RC(knn_k_query(tree.view(), (const double*)qry.p, qs, (int)nq, k, (1.0 + epsilon) * (1.0 + epsilon),
-                       max_radius * max_radius, (flags & SM_KNN_ALLOW_SELF_MATCH) != 0u, ids_out, d2_out, s));
+    SMB_RC(knn_k_query(kc, q, qs, (int)nq, k, (1.0 + epsilon) * (1.0 + epsilon), max_radius * max_radius,
+                       (flags & SM_KNN_ALLOW_SELF_MATCH) != 0u, ids_out, d2_out, s));
     if (!on_device) {
       SMB_CUDA_OK(cudaMemcpyAsync(ids, ids_d.p, (size_t)nq * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
       SMB_CUDA_OK(cudaMemcpyAsync(d2, d2_d.p, (size_t)nq * k * sizeof(double), cudaMemcpyDeviceToHost, s));
     }
-  }
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  return SM_OK;
+    return SM_OK;
+  };
+  return knn_on_target(target, nt, query, nq, bucket, on_device, s, search);
 }
 
 int sm_knn(int device, const double* target_3xn, int64_t n_target, const double* query_3xn, int64_t n_query,
