@@ -276,7 +276,7 @@ inline void VoxelGridFilterB200(const data::InnerCloudType& input, float voxel_s
   output->points.resize(m);
 }
 
-// The Filter body of FilterChainB200 and StatisticRemovalB200: CHECK-fails with last_error(h) when run (sm_*_run) fails
+// The Filter body of FilterChainB200, StatisticRemovalB200 and GroundRemovalB200: CHECK-fails with last_error(h) when run (sm_*_run) fails
 template <typename Handle, typename Run, typename LastError>
 inline void FilterRecordsB200(Handle* h, Run run, LastError last_error, const char* run_name,
                               const data::InnerCloudType& input, data::InnerCloudType* const output,
@@ -383,6 +383,45 @@ class StatisticRemovalB200 {
 
  private:
   sm_statistic_removal* filter_ = nullptr;
+};
+
+// pre_processers::filter::GroundRemoval (v1, pre_processors/filter_ground_removal.{h,cc}) on the GPU: one per
+// GroundRemoval.  The body of its InitFromXmlNode becomes one SetParam per <param>, and that of Filter
+//   this->FilterPrepare(cloud);
+//   filter_.Filter(*this->inner_cloud_, cloud.get(), &this->inliers_, &this->outliers_);
+// The output is in the reference's voxel (std::map) order; inliers and outliers are ascending, and the points of a
+// voxel below min_point_num_in_voxel are in neither.
+class GroundRemovalB200 {
+ public:
+  explicit GroundRemovalB200(int device = 0) { CHECK_EQ(sm_ground_removal_create(device, &filter_), 0); }
+  ~GroundRemovalB200() { sm_ground_removal_destroy(filter_); }
+  GroundRemovalB200(const GroundRemovalB200&) = delete;
+  GroundRemovalB200& operator=(const GroundRemovalB200&) = delete;
+
+  // min_point_num_in_voxel (type 0), leaf_size or height_threshold (type 1); type -1 when the <param> has none (the
+  // reference CHECK-fails, filter_interface.cc:57)
+  void SetParam(const std::string& name, int type, const std::string& text) {
+    CHECK_EQ(sm_ground_removal_set_param(filter_, name.c_str(), type, text.c_str()), 0)
+        << sm_ground_removal_last_error(filter_);
+  }
+
+  // CHECK-fails when the voxel indices of an axis span more than 2^21 - 1 voxels (include/sm_b200.h)
+  void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,
+              std::vector<int>* const inliers = nullptr, std::vector<int>* const outliers = nullptr) {
+    FilterRecordsB200(filter_, sm_ground_removal_run, sm_ground_removal_last_error, "sm_ground_removal_run", input,
+                      output, nullptr);
+    int64_t n_in = 0, n_out = 0;
+    if (!input.points.empty()) CHECK_EQ(sm_ground_removal_indices(filter_, nullptr, &n_in, nullptr, &n_out), 0);
+    std::vector<int32_t> in(static_cast<size_t>(n_in)), out(static_cast<size_t>(n_out));
+    if (n_in + n_out > 0)
+      CHECK_EQ(sm_ground_removal_indices(filter_, in.data(), &n_in, out.data(), &n_out), 0)
+          << "sm_ground_removal_indices failed";
+    if (inliers) inliers->assign(in.begin(), in.end());
+    if (outliers) outliers->assign(out.begin(), out.end());
+  }
+
+ private:
+  sm_ground_removal* filter_ = nullptr;
 };
 
 // descriptor::M2dp::setInputCloud + getFinalDescriptor on the GPU (descriptor/m2dp.cc:129-153): the body of

@@ -407,10 +407,9 @@ typedef struct sm_filter_chain sm_filter_chain;
 int sm_filter_chain_create(int device, sm_filter_chain** out);
 int sm_filter_chain_destroy(sm_filter_chain* chain);
 /* One <filter name=...> of Factory::InitFromXmlNode (filter_factory.cc:64-80): appends the filter at its constructor's
- * defaults and returns its index.  GroundRemoval, StatisticRemoval (an empty body in the reference,
- * filter_statistic_removal.cc:44-59; PCL's filter is sm_statistic_removal_*) and VoxelGrid (see sm_voxel_grid_filter)
- * are not built into the chain:
- * SM_ERR_UNSUPPORTED_TYPE.  A name the reference does not register either (it skips it, :68-71):
+ * defaults and returns its index.  GroundRemoval (see sm_ground_removal_*), StatisticRemoval (an empty body in the
+ * reference, filter_statistic_removal.cc:44-59; PCL's filter is sm_statistic_removal_*) and VoxelGrid (see
+ * sm_voxel_grid_filter) are not built into the chain: SM_ERR_UNSUPPORTED_TYPE.  A name the reference does not register either (it skips it, :68-71):
  * SM_ERR_UNKNOWN_OPTION; the chain is unchanged. */
 int sm_filter_chain_add(sm_filter_chain* chain, const char* filter_name);
 /* One <param type=... name=...>text</param> of Interface::InitFromXmlNode (filter_interface.cc:38-58): `text` is read
@@ -506,6 +505,47 @@ int sm_statistic_removal_run_device(sm_statistic_removal* filter, const float* d
 /* The last successful run's mean, stddev, threshold and valid (step 4), as four doubles. */
 int sm_statistic_removal_stats(const sm_statistic_removal* filter, double* out4);
 const char* sm_statistic_removal_last_error(const sm_statistic_removal* filter);
+
+/* ---- pre_processers::filter::GroundRemoval: the voxel height-range ground filter ---------------------------------
+ * GroundRemoval (v1, filter_ground_removal.{h,cc}) with min_point_num_in_voxel (int32, 10), leaf_size (float, 0.8) and
+ * height_threshold (float, 0.15).  It is not part of the chain (sm_filter_chain_add refuses it); it has its own handle,
+ * used by one thread at a time.  Its device buffers belong to the handle and only grow.
+ *   1. Voxel index per axis: (int)(coordinate / leaf_size), a float division truncated toward zero; a NaN quotient or
+ *      one outside int's range gives INT_MIN (the reference's x86 build).  Such points are kept in that voxel, so
+ *      leaf_size = 0 puts every point into (INT_MIN, INT_MIN, INT_MIN).
+ *   2. Voxels in the order of the reference's std::map: lexicographic on signed (ix, iy, iz); a voxel holds its points
+ *      in input order.
+ *   3. Per voxel: fewer than min_point_num_in_voxel points -> skipped (neither inlier nor outlier).  Else, if iz <= 0:
+ *      max_z / min_z from -1e9 / 1e9 with strict > / < (a NaN z updates neither), delta = max_z - min_z in float, and
+ *      the voxel is ground iff delta >= 0 && delta <= height_threshold: its points are outliers.  Every other voxel
+ *      emits its whole records (x, y, z, intensity, factor) in input order and its points are inliers.
+ * LIMIT: the voxel key has 21 bits per axis.  Per axis, the indices other than INT_MIN must span at most 2^21 - 1
+ * voxels (about 1 677 km at leaf_size 0.8); past that the run returns SM_ERR_BAD_ARGUMENT where the reference runs. */
+typedef struct sm_ground_removal sm_ground_removal;
+/* Needs no device; the first run binds CUDA ordinal `device`. */
+int sm_ground_removal_create(int device, sm_ground_removal** out);
+int sm_ground_removal_destroy(sm_ground_removal* filter);
+/* One <param type=... name=...>text</param> of the filter's XML node, parsed exactly as sm_filter_chain_set_param parses
+ * it: SM_ERR_UNKNOWN_OPTION for a name other than min_point_num_in_voxel / leaf_size / height_threshold,
+ * SM_ERR_BAD_ARGUMENT for a type other than 0 / 1.  Every value is accepted, as in the reference (no ConfigsValid). */
+int sm_ground_removal_set_param(sm_ground_removal* filter, const char* name, int type, const char* text);
+/* SetInputCloud + Filter.  `points`: n records `stride_bytes` (>= 20, a multiple of 4) apart, float x, y, z,
+ * intensity, factor first; `out`: capacity n packed 5-float records, the emitted ones in voxel order; *m_out = their
+ * number; index (optional, capacity n): the input index of each emitted record, in emission order, so NOT ascending
+ * (Inliers() is sm_ground_removal_indices).  n = 0: *m_out = 0 and empty index lists.  SM_ERR_BAD_ARGUMENT: a bad
+ * stride, null pointers with n > 0, more than 2^30 points, or a span past the key limit above.
+ * The _device form takes device pointers (in and out may not overlap), runs on `cuda_stream` (a cudaStream_t, NULL =
+ * default stream) and returns after the stream has finished; it reads the stream's results back once (the counts and
+ * the per-axis index bounds).  Its output feeds sm_set_input_source_f32_device (stride 20). */
+int sm_ground_removal_run(sm_ground_removal* filter, const float* points, int64_t n, int64_t stride_bytes, float* out,
+                          int64_t* m_out, int32_t* index_or_null);
+int sm_ground_removal_run_device(sm_ground_removal* filter, const float* dev_points, int64_t n, int64_t stride_bytes,
+                                 float* dev_out, int64_t* m_out, int32_t* dev_index_or_null, void* cuda_stream);
+/* Inliers() / Outliers() of the last successful run, ascending input indices: the points of the emitted voxels and of
+ * the ground voxels.  *n_inliers / *n_outliers = their numbers; null arrays return the counts only. */
+int sm_ground_removal_indices(const sm_ground_removal* filter, int32_t* inliers_or_null, int64_t* n_inliers,
+                              int32_t* outliers_or_null, int64_t* n_outliers);
+const char* sm_ground_removal_last_error(const sm_ground_removal* filter);
 
 int sm_device_count(void);
 const char* sm_version(void);

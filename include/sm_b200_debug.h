@@ -28,6 +28,8 @@
  *     sm_debug_depth_edge_host RangeImage::DepthCluster's edge predicate
  *     sm_debug_statistic_removal_exact_sum_host  StatisticRemoval's correctly rounded sum of non-negative floats
  *     sm_debug_statistic_removal_distance_host   StatisticRemoval's per-point mean distance over a neighbour list
+ *     sm_debug_ground_removal_index_host, sm_debug_ground_removal_voxel_host  GroundRemoval's voxel index of a point
+ *                              and its decision for one voxel
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -395,6 +397,16 @@ int sm_debug_statistic_removal_distance_host(const float* query_3, const float* 
  * run's point count (0 before any run); SM_ERR_BAD_ARGUMENT when capacity < *n. */
 int sm_debug_statistic_removal_distances(const struct sm_statistic_removal* filter, float* out, int64_t capacity,
                                          int64_t* n);
+
+/* GroundRemoval's voxel index (csrc/ground_removal.cu gr_index) compiled for the host: ixyz[3i + d] = the index along
+ * axis d of record i of n records `stride_bytes` apart, (int)(coordinate / leaf_size) or INT_MIN. */
+int sm_debug_ground_removal_index_host(const float* points, int64_t n, int64_t stride_bytes, float leaf_size,
+                                       int32_t* ixyz);
+/* GroundRemoval's decision for one voxel (gr_z_update, gr_voxel_status) compiled for the host, over the z of its
+ * `count` points in input order and its z index iz: *status 0 skipped, 1 ground (outliers), 2 kept (inliers);
+ * max_min_2 = max_z, min_z as the reference's loop leaves them (-1e9, 1e9 when the loop does not run). */
+int sm_debug_ground_removal_voxel_host(const float* z, int64_t count, int32_t iz, int32_t min_point_num_in_voxel,
+                                       float height_threshold, int32_t* status, float* max_min_2);
 
 #ifdef __cplusplus
 }

@@ -96,6 +96,13 @@ SIGNATURES = {
                                                   _VP]),
     "sm_statistic_removal_stats": (C.c_int, [_VP, _DP]),
     "sm_statistic_removal_last_error": (C.c_char_p, [_VP]),
+    "sm_ground_removal_create": (C.c_int, [C.c_int, C.POINTER(_VP)]),
+    "sm_ground_removal_destroy": (C.c_int, [_VP]),
+    "sm_ground_removal_set_param": (C.c_int, [_VP, C.c_char_p, C.c_int, C.c_char_p]),
+    "sm_ground_removal_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
+    "sm_ground_removal_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
+    "sm_ground_removal_indices": (C.c_int, [_VP, _VP, C.POINTER(C.c_int64), _VP, C.POINTER(C.c_int64)]),
+    "sm_ground_removal_last_error": (C.c_char_p, [_VP]),
     # include/sm_b200_debug.h (test hooks)
     "sm_debug_solve6": (C.c_int, [C.c_int, _VP, _VP, _VP, _VP]),
     "sm_debug_solve6_host": (C.c_int, [_VP, _VP, _VP, _VP]),
@@ -152,6 +159,8 @@ SIGNATURES = {
     "sm_debug_statistic_removal_exact_sum_host": (C.c_int, [_VP, C.c_int64, _DP]),
     "sm_debug_statistic_removal_distance_host": (C.c_int, [_VP, _VP, C.c_int32, _VP]),
     "sm_debug_statistic_removal_distances": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "sm_debug_ground_removal_index_host": (C.c_int, [_VP, C.c_int64, C.c_int64, C.c_float, _VP]),
+    "sm_debug_ground_removal_voxel_host": (C.c_int, [_VP, C.c_int64, C.c_int32, C.c_int32, C.c_float, _VP, _VP]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

@@ -3,6 +3,7 @@
 #define SM_B200_COMMON_CUH_
 
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -37,6 +38,12 @@ inline int select_device(int device) {
   if (device < 0 || device >= ndev) return SM_ERR_BAD_ARGUMENT;
   SMB_CUDA_OK(cudaSetDevice(device));
   return SM_OK;
+}
+
+// A float / double -> int conversion outside int's range is undefined in C++; the reference's x86 build yields INT_MIN
+// there (also for NaN), which its clamps and range tests then read as "below 0".  Restated so on every side.
+__host__ __device__ __forceinline__ int to_int(double q) {
+  return (q > -2147483649.0 && q < 2147483648.0) ? (int)q : INT_MIN;
 }
 
 constexpr int kNumSMs = 132;  // H100 SXM; grids are sized in multiples

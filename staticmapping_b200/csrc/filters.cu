@@ -33,12 +33,6 @@ constexpr int kMaxCells = 1 << 24;      // RangeImage pixels / GroundRemoval2 ce
 
 struct PredicateRun { int count; uint32_t seed; FilterParams f[kMaxRun]; };
 
-// A float / double -> int conversion outside int's range is undefined in C++; the reference's x86 build yields INT_MIN
-// there (also for NaN), which its clamps and range tests then read as "below 0".  Restated so on every side.
-__host__ __device__ __forceinline__ int to_int(double q) {
-  return (q > -2147483649.0 && q < 2147483648.0) ? (int)q : INT_MIN;
-}
-
 __host__ __device__ __forceinline__ uint32_t fmix32(uint32_t x) {   // MurmurHash3's 32-bit finaliser
   x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
   return x;
@@ -463,6 +457,9 @@ FilterParams filter_defaults(int kind) {
   f.max_start_height = 0.2f; f.max_error = 0.05f; f.max_slope = (float)tan(M_PI / 12.); f.max_b = 0.1f;
   f.max_dist_to_line = 0.05f; f.search_angle = 10.f; f.thread_num = 4;
   if (kind == kFilterStatisticRemoval) { f.point_num_meank = 30; f.std_mul = 1.f; }   // in Range's storage
+  if (kind == kFilterGroundRemoval) {                                                  // in AxisRange's storage
+    f.min_point_num_in_voxel = 10; f.leaf_size = 0.8f; f.height_threshold = 0.15f;
+  }
   return f;
 }
 
@@ -494,6 +491,9 @@ bool filter_param(FilterParams& f, const char* name, void** target, int* type) {
       {kFilterGroundRemoval2, "thread_num", 0, &f.thread_num},
       {kFilterStatisticRemoval, "point_num_meank", 0, &f.point_num_meank},
       {kFilterStatisticRemoval, "std_mul", 1, &f.std_mul},
+      {kFilterGroundRemoval, "min_point_num_in_voxel", 0, &f.min_point_num_in_voxel},
+      {kFilterGroundRemoval, "leaf_size", 1, &f.leaf_size},
+      {kFilterGroundRemoval, "height_threshold", 1, &f.height_threshold},
   };
   for (const Entry& e : table)
     if (e.kind == f.kind && strcmp(e.name, name) == 0) { *target = e.p; *type = e.type; return true; }

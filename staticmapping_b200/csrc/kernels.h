@@ -406,24 +406,29 @@ void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* o
 
 // ---- filters.cu --------------------------------------------------------------------------
 // pre_processers::filter::Factory (pre_processors/filter_factory.cc:63-106) over the six filters built here
-// kFilterStatisticRemoval is not a kind of the chain (sm_filter_chain_add refuses it): it runs behind its own handle,
-// sm_statistic_removal (statistic_removal.cu), built like the chain's on the handle core of record_filter.h.
+// kFilterStatisticRemoval and kFilterGroundRemoval are not kinds of the chain (sm_filter_chain_add refuses them): each
+// runs behind its own handle, sm_statistic_removal (statistic_removal.cu) and sm_ground_removal (ground_removal.cu),
+// built like the chain's on the handle core of record_filter.h.
 enum FilterKind : int {
   kFilterRange = 0, kFilterAxisRange, kFilterBoundingBoxRemoval, kFilterRandomSampler, kFilterRangeImage,
-  kFilterGroundRemoval2, kFilterStatisticRemoval
+  kFilterGroundRemoval2, kFilterStatisticRemoval, kFilterGroundRemoval
 };
 // One filter of the chain: the members of the reference class of its kind under their XML names, at the
 // constructors' defaults (filter_range.cc:31-38, filter_axis_range.h:56-57, filter_bounding_box.h,
 // filter_random_sample.cc:29, filter_range_image.cc:29-37, filter_ground_removal2.cc:74-89,
-// filter_statistic_removal.h).  Passed to the kernels by value.  StatisticRemoval's two members share Range's storage:
-// a FilterParams holds the parameters of one kind, and its size and layout are what the chain's kernels take.
+// filter_statistic_removal.h, filter_ground_removal.cc:29-39).  Passed to the kernels by value.  StatisticRemoval's
+// two members share Range's storage and GroundRemoval's three AxisRange's: a FilterParams holds the parameters of one
+// kind, and its size and layout are what the chain's kernels take.
 struct FilterParams {
   int kind;
   union {
     struct { float min_range, max_range; };                         // Range
     struct { int32_t point_num_meank; float std_mul; };             // StatisticRemoval
   };
-  float min, max; int axis_index;                                   // AxisRange
+  union {
+    struct { float min, max; int axis_index; };                     // AxisRange
+    struct { int32_t min_point_num_in_voxel; float leaf_size, height_threshold; };   // GroundRemoval
+  };
   float min_x, min_y, min_z, max_x, max_y, max_z;                   // BoundingBoxRemoval
   float sampling_rate;                                              // RandomSampler
   float top_angle, btm_angle, offset_x, offset_y, offset_z;         // RangeImage
@@ -463,6 +468,16 @@ const FilterChain* filter_chain_of(const ::sm_filter_chain* c);   // the chain b
 // leaves their number in *m (device memory).  tile_cnt: compact_count_bytes(n), turned into offsets in place.
 void filter_compact_records(const char* pts, int64_t stride, const uint32_t* index_in, int n, const uint8_t* flag,
                             uint32_t* tile_cnt, float* out, uint32_t* index_out, uint32_t* m, cudaStream_t s);
+
+// ---- ground_removal.cu -------------------------------------------------------------------------
+// the fate of a GroundRemoval voxel (filter_ground_removal.cc:74-108): skipped (in neither list), ground (its points
+// are outliers) or kept (its records are emitted, its points are inliers)
+enum GrStatus : int { kGrSkipped = 0, kGrGround = 1, kGrKept = 2 };
+// host builds of the per-point voxel index and of the per-voxel decision over the voxel's z in input order (test hooks
+// sm_debug_ground_removal_index_host / _voxel_host); max_min: the z loop's max_z, min_z
+void gr_debug_index_host(const float* p, float leaf, int* ixyz);
+int gr_debug_voxel_host(const float* z, int64_t count, int iz, int32_t min_points, float height_threshold,
+                        float* max_min);
 
 // ---- depth_cluster.cu --------------------------------------------------------------------------
 // sinf / cosf of RangeImage::LabelOneComponent's horizontal and vertical resolution (filter_range_image.cc:255-259)

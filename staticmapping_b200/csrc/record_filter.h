@@ -1,5 +1,6 @@
 // The C handle core of the filters over records (sm_filter_chain in filters.cu, sm_statistic_removal in
-// statistic_removal.cu): each handle derives from RecordFilter and adds its filter's state.
+// statistic_removal.cu, sm_ground_removal in ground_removal.cu): each handle derives from RecordFilter and adds its
+// filter's state.
 #ifndef SM_B200_RECORD_FILTER_H_
 #define SM_B200_RECORD_FILTER_H_
 

@@ -137,6 +137,21 @@ int sm_debug_pm_surface_normal_leaf_host(const float* members_3k, int32_t count,
 }
 
 // test hook: the voxel index of a point as the three voxelisations compute it, compiled for the host
+int sm_debug_ground_removal_index_host(const float* points, int64_t n, int64_t stride_bytes, float leaf_size,
+                                       int32_t* ixyz) {
+  if ((n > 0 && (!points || !ixyz)) || n < 0 || stride_bytes < 12 || stride_bytes % 4) return SM_ERR_BAD_ARGUMENT;
+  for (int64_t i = 0; i < n; ++i)
+    gr_debug_index_host(points + i * (stride_bytes / 4), leaf_size, ixyz + 3 * i);
+  return SM_OK;
+}
+
+int sm_debug_ground_removal_voxel_host(const float* z, int64_t count, int32_t iz, int32_t min_point_num_in_voxel,
+                                       float height_threshold, int32_t* status, float* max_min_2) {
+  if ((count > 0 && !z) || count < 0 || count > INT32_MAX || !status || !max_min_2) return SM_ERR_BAD_ARGUMENT;
+  *status = gr_debug_voxel_host(z, count, iz, min_point_num_in_voxel, height_threshold, max_min_2);
+  return SM_OK;
+}
+
 int sm_debug_voxel_index(int32_t op, const float* p3, float param, int32_t min_b, int64_t* out4) {
   if (!p3 || !out4) return SM_ERR_BAD_ARGUMENT;
   switch (op) {

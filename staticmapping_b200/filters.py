@@ -1,7 +1,8 @@
 """pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
 chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
 deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster.  StatisticRemoval,
-PCL's statistical outlier removal, runs on its own handle (sm_statistic_removal_*).  There is no CPU fallback."""
+PCL's statistical outlier removal, and GroundRemoval, the voxel height-range ground filter, run on their own handles
+(sm_statistic_removal_*, sm_ground_removal_*).  There is no CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -116,7 +117,8 @@ class Factory(_RecordFilter):
     def InitFromXmlNode(self, filters_node):
         """filter_factory.cc:63-81.  A name the reference does not register is skipped with a message; a <param> with
         an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57), and so does a filter
-        the reference has but this chain does not build (GroundRemoval, StatisticRemoval, VoxelGrid)."""
+        the reference has but this chain does not build: GroundRemoval (see GroundRemoval), StatisticRemoval (see
+        StatisticRemoval) and VoxelGrid."""
         if isinstance(filters_node, (str, bytes)):
             filters_node = ET.fromstring(filters_node)
         for node in filters_node.findall("filter"):
@@ -160,7 +162,27 @@ class Factory(_RecordFilter):
         return DepthClusters(xyz[:k].copy(), label[:k].copy(), index[:k].copy(), point_label[:n].copy())
 
 
-class StatisticRemoval(_RecordFilter):
+class _OwnHandleFilter(_RecordFilter):
+    """A filter the chain does not build, on its own handle: configured from its one <filter name=`_name`> node."""
+    _name = ""
+
+    def InitFromXmlNode(self, filter_node):
+        """A <param> with an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57);
+        a node that is not <filter name=`_name`> raises ValueError."""
+        if isinstance(filter_node, (str, bytes)):
+            filter_node = ET.fromstring(filter_node)
+        if filter_node.tag != "filter" or filter_node.attrib.get("name", "") != self._name:
+            raise ValueError(f'expected a <filter name="{self._name}"> node')
+        for param in filter_node.findall("param"):
+            self.SetParam(param.attrib.get("name", ""), param.attrib.get("type"), (param.text or "").strip())
+
+    def SetParam(self, name, ptype, text):
+        rc = self._fn("set_param")(self._h, str(name).encode(), _param_type(ptype), str(text).encode())
+        if rc != 0:
+            raise CheckFailure(self._error())
+
+
+class StatisticRemoval(_OwnHandleFilter):
     """pre_processers::filter::StatisticRemoval as PCL's StatisticalOutlierRemoval (setMeanK(point_num_meank),
     setStddevMulThresh(std_mul)), the call the reference leaves as a TODO, on the GPU (sm_statistic_removal_*,
     include/sm_b200.h).  InitFromXmlText / InitFromXmlNode take one <filter name="StatisticRemoval"> node and parse its
@@ -168,25 +190,39 @@ class StatisticRemoval(_RecordFilter):
     CheckFailure for 1..point_num_meank finite points, ValueError for a point_num_meank outside 1..63; Inliers() /
     Outliers() are indices into the input and Stats() is (mean, stddev, threshold, valid) of the last run."""
     _abi = "sm_statistic_removal"
-
-    def InitFromXmlNode(self, filter_node):
-        """A <param> with an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57);
-        a node that is not <filter name="StatisticRemoval"> raises ValueError."""
-        if isinstance(filter_node, (str, bytes)):
-            filter_node = ET.fromstring(filter_node)
-        if filter_node.tag != "filter" or filter_node.attrib.get("name", "") != "StatisticRemoval":
-            raise ValueError('expected a <filter name="StatisticRemoval"> node')
-        for param in filter_node.findall("param"):
-            self.SetParam(param.attrib.get("name", ""), param.attrib.get("type"), (param.text or "").strip())
-
-    def SetParam(self, name, ptype, text):
-        rc = self._lib.sm_statistic_removal_set_param(self._h, str(name).encode(), _param_type(ptype),
-                                                      str(text).encode())
-        if rc != 0:
-            raise CheckFailure(self._error())
+    _name = "StatisticRemoval"
 
     def Stats(self):
         """(mean, stddev, threshold, valid) of the last run"""
         s = (C.c_double * 4)()
         self._lib.sm_statistic_removal_stats(self._h, s)
         return tuple(s)
+
+
+class GroundRemoval(_OwnHandleFilter):
+    """pre_processers::filter::GroundRemoval (v1, pre_processors/filter_ground_removal.{h,cc}) on the GPU
+    (sm_ground_removal_*, include/sm_b200.h): voxels of leaf_size in the reference's std::map order; a voxel of fewer
+    than min_point_num_in_voxel points is skipped, one with z index <= 0 and a z range in [0, height_threshold] is
+    ground, every other one is emitted.  InitFromXmlText / InitFromXmlNode take one <filter name="GroundRemoval"> node
+    and parse its <param>s as Factory does; SetInputCloud + Filter run it.  `Filter` returns the emitted InnerCloud in
+    voxel order; Inliers() / Outliers() are the points of the emitted and of the ground voxels, ascending indices into
+    the input (a skipped voxel's points are in neither).  A span of voxel indices past the 63-bit key raises
+    ValueError."""
+    _abi = "sm_ground_removal"
+    _name = "GroundRemoval"
+
+    def Filter(self):
+        if self._cloud is None:
+            return None
+        pts = self._cloud
+        n = pts.shape[0]
+        out = np.empty_like(pts)
+        m = C.c_int64(0)
+        self._check(self._fn("run")(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m), None), "run")
+        inliers, outliers = np.empty(n, np.int32), np.empty(n, np.int32)
+        ni, no = C.c_int64(0), C.c_int64(0)
+        self._check(self._fn("indices")(self._h, inliers.ctypes.data, C.byref(ni), outliers.ctypes.data, C.byref(no)),
+                    "indices")
+        self._inliers = inliers[:ni.value].copy()
+        self._outliers = outliers[:no.value].copy()
+        return InnerCloud(out[:m.value].copy())
