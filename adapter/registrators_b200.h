@@ -424,6 +424,64 @@ class GroundRemovalB200 {
   sm_ground_removal* filter_ = nullptr;
 };
 
+// The submap sampler RandomSamplerWithPlaneDetect (pre_processors/random_sample_with_plane_detect.h) on the GPU: one
+// per sampler, with the class's setters.  Filter keeps the plane points of PlaneDetector and samples the rest at the
+// rate, in input order; Inliers() / Outliers() / PlaneIndices() are ascending.  FilterDevice takes a device cloud and
+// leaves its output on the device, where sm_set_input_target_f32_device (stride 20) reads it; Submap::InsertFrame's
+// next step, CalculateNormals, reads the host output of Filter.  CHECK-fails past 2^24 points or the voxel key's span
+// (include/sm_b200.h).
+class RandomSamplerWithPlaneDetectB200 {
+ public:
+  explicit RandomSamplerWithPlaneDetectB200(int device = 0) { CHECK_EQ(sm_plane_sampler_create(device, &sampler_), 0); }
+  ~RandomSamplerWithPlaneDetectB200() { sm_plane_sampler_destroy(sampler_); }
+  RandomSamplerWithPlaneDetectB200(const RandomSamplerWithPlaneDetectB200&) = delete;
+  RandomSamplerWithPlaneDetectB200& operator=(const RandomSamplerWithPlaneDetectB200&) = delete;
+
+  void SetSamplingRate(float rate) { Warn(sm_plane_sampler_set_sampling_rate(sampler_, rate)); }
+  void SetLeafSize(float size) { Warn(sm_plane_sampler_set_leaf_size(sampler_, size)); }
+  void SetMinPointNumInVoxel(size_t num) { Warn(sm_plane_sampler_set_min_point_num_in_voxel(sampler_, num)); }
+
+  void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output) {
+    FilterRecordsB200(sampler_, sm_plane_sampler_run, sm_plane_sampler_last_error, "sm_plane_sampler_run", input,
+                      output, nullptr);
+  }
+  // n records of `stride_bytes` in device memory -> dev_out (capacity n 5-float records); the number kept
+  int64_t FilterDevice(const float* dev_points, int64_t n, int64_t stride_bytes, float* dev_out,
+                       void* cuda_stream = nullptr) {
+    int64_t m = 0;
+    const int rc = sm_plane_sampler_run_device(sampler_, dev_points, n, stride_bytes, dev_out, &m, nullptr,
+                                               cuda_stream);
+    CHECK_EQ(rc, 0) << "sm_plane_sampler_run_device failed (" << rc << "): " << sm_plane_sampler_last_error(sampler_);
+    return m;
+  }
+
+  std::vector<int> Inliers() const { return Lists(0); }
+  std::vector<int> Outliers() const { return Lists(1); }
+  std::vector<int> PlaneIndices() const { return Lists(2); }
+
+ private:
+  void Warn(int rc) {
+    CHECK_EQ(rc, 0);
+    const char* message = sm_plane_sampler_last_error(sampler_);
+    if (message && message[0]) LOG(WARNING) << message;
+  }
+  std::vector<int> Lists(int which) const {
+    int64_t n[3] = {0, 0, 0};
+    CHECK_EQ(sm_plane_sampler_indices(sampler_, nullptr, &n[0], nullptr, &n[1]), 0);
+    CHECK_EQ(sm_plane_sampler_plane_indices(sampler_, nullptr, &n[2]), 0);
+    std::vector<int32_t> list(static_cast<size_t>(n[which]));
+    if (!list.empty() && which == 2) {
+      CHECK_EQ(sm_plane_sampler_plane_indices(sampler_, list.data(), &n[2]), 0);
+    } else if (!list.empty()) {
+      CHECK_EQ(sm_plane_sampler_indices(sampler_, which == 0 ? list.data() : nullptr, &n[0],
+                                        which == 1 ? list.data() : nullptr, &n[1]), 0);
+    }
+    return std::vector<int>(list.begin(), list.end());
+  }
+
+  sm_plane_sampler* sampler_ = nullptr;
+};
+
 // descriptor::M2dp::setInputCloud + getFinalDescriptor on the GPU (descriptor/m2dp.cc:129-153): the body of
 // setInputCloud becomes   return registrator::M2dpB200(*source, r_, max_distance_, t_, p_, q_, &descriptor_);
 inline bool M2dpB200(const data::InnerCloudType& source, double r, double max_distance, int32_t t, int32_t p,

@@ -547,6 +547,63 @@ int sm_ground_removal_indices(const sm_ground_removal* filter, int32_t* inliers_
                               int32_t* outliers_or_null, int64_t* n_outliers);
 const char* sm_ground_removal_last_error(const sm_ground_removal* filter);
 
+/* ---- RandomSamplerWithPlaneDetect: keep the plane points, sample the rest ------------------------------------------
+ * The submap sampler RandomSamplerWithPlaneDetect (random_sample_with_plane_detect.h) with its PlaneDetector
+ * (plane_detector.h).  Parameters are the class's setters (no XML node): sampling_rate (float, 1), leaf_size (float,
+ * 0.8: the sampler's constructor overrides the detector's 0.5) and min_point_num_in_voxel (size_t, 10).  The ground
+ * height threshold is fixed at 0.2 and the RANSAC distance threshold at 0.1.  It is not part of the chain
+ * (sm_filter_chain_add refuses the name, as filter::Factory does not register it); it has its own handle, used by one
+ * thread at a time, whose device buffers only grow.  A run, in order:
+ *   1. n = 0: nothing is emitted.
+ *   2. rate > 0.999999 (in double): every record is copied and no detection runs; no plane indices.
+ *   3. Voxels: GroundRemoval's keys and order (sm_ground_removal_* steps 1-2), INT_MIN for a NaN or out-of-range
+ *      quotient included.
+ *   4. Detect: if 0.2 >= leaf_size there are no plane points.  Otherwise, per voxel in map order: fewer than min points
+ *      -> skipped; iz <= 0 -> GroundRemoval's z-range rule with threshold 0.2: all its points are plane points, or
+ *      none are; iz > 0 with fewer than 2 min points -> skipped; else PCL's SACSegmentation (SACMODEL_PLANE, SAC_RANSAC,
+ *      threshold 0.1, optimised coefficients, 50 iterations, probability 0.99, generator seeded 12345u) on its points
+ *      in input order, and the refined inliers are plane points iff (float)inliers / (float)count > 0.85 (in double).
+ *      DESIGN §4l restates the RANSAC step by step.
+ *   5. Sampler, over the input in index order: a plane point is kept; any other point increments other_sum and is kept
+ *      iff (float)sampled / (float)other_sum < rate, which then increments sampled.
+ * Output: the kept records in input order; Inliers() = the kept indices, Outliers() = the rest, PlaneIndices() = the
+ * sorted output of Detect, all ascending.
+ * Where the reference is undefined or leaks state, this settles it:
+ *   - plane_indices.front() on an empty vector (after the last plane point, or with none) means "no further plane
+ *     point";
+ *   - PlaneDetector::voxels_ is never cleared, so a reused reference sampler mixes in the voxels of earlier clouds;
+ *     every run here starts fresh, as the reference's first call on a new object does;
+ *   - PlaneDetector's min_z_ / max_z_ are computed and never read: they do not exist here.
+ * LIMITS: the float other_sum is exact up to 2^24, so a run of more than 2^24 points returns SM_ERR_BAD_ARGUMENT; the
+ * voxel key's span limit of sm_ground_removal_* applies (SM_ERR_BAD_ARGUMENT) whenever Detect runs.
+ * Difference: computeRoots' atan2, cos and sin are evaluated in double and rounded to float (DESIGN §4l). */
+typedef struct sm_plane_sampler sm_plane_sampler;
+/* Needs no device; the first run binds CUDA ordinal `device`. */
+int sm_plane_sampler_create(int device, sm_plane_sampler** out);
+int sm_plane_sampler_destroy(sm_plane_sampler* sampler);
+/* SetSamplingRate: above 1 -> 1, below 1e-6 (in double) -> (float)1e-6, with the reference's warning as the last
+ * error; SM_OK either way. */
+int sm_plane_sampler_set_sampling_rate(sm_plane_sampler* sampler, float rate);
+int sm_plane_sampler_set_leaf_size(sm_plane_sampler* sampler, float leaf_size);
+/* SetMinPointNumInVoxel (size_t): below 5 -> 5, with the reference's warning as the last error. */
+int sm_plane_sampler_set_min_point_num_in_voxel(sm_plane_sampler* sampler, uint64_t num);
+/* SetInputCloud + Filter.  `points`: n records `stride_bytes` (>= 20, a multiple of 4) apart, float x, y, z,
+ * intensity, factor first; `out`: capacity n packed 5-float records, the kept ones in input order; *m_out = their
+ * number; index (optional, capacity n): their input indices (= Inliers()).  SM_ERR_BAD_ARGUMENT: a bad stride, null
+ * pointers with n > 0, more than 2^24 points, or the span limit.  The _device form takes device pointers (in and out
+ * may not overlap), runs on `cuda_stream` (NULL = default stream) and returns after the stream has finished, with one
+ * read-back of the counts.  Its output feeds sm_calculate_normals and sm_set_input_target_f32_device (stride 20). */
+int sm_plane_sampler_run(sm_plane_sampler* sampler, const float* points, int64_t n, int64_t stride_bytes, float* out,
+                         int64_t* m_out, int32_t* index_or_null);
+int sm_plane_sampler_run_device(sm_plane_sampler* sampler, const float* dev_points, int64_t n, int64_t stride_bytes,
+                                float* dev_out, int64_t* m_out, int32_t* dev_index_or_null, void* cuda_stream);
+/* Inliers() / Outliers() of the last successful run, ascending; null arrays return the counts only. */
+int sm_plane_sampler_indices(const sm_plane_sampler* sampler, int32_t* inliers_or_null, int64_t* n_inliers,
+                             int32_t* outliers_or_null, int64_t* n_outliers);
+/* The sorted plane indices of the last successful run (empty on the copy path); a null array returns the count. */
+int sm_plane_sampler_plane_indices(const sm_plane_sampler* sampler, int32_t* plane_or_null, int64_t* n_plane);
+const char* sm_plane_sampler_last_error(const sm_plane_sampler* sampler);
+
 int sm_device_count(void);
 const char* sm_version(void);
 

@@ -408,6 +408,22 @@ int sm_debug_ground_removal_index_host(const float* points, int64_t n, int64_t s
 int sm_debug_ground_removal_voxel_host(const float* z, int64_t count, int32_t iz, int32_t min_point_num_in_voxel,
                                        float height_threshold, int32_t* status, float* max_min_2);
 
+/* RandomSamplerWithPlaneDetect's single-hypothesis pieces (csrc/plane_sampler.cu) compiled for the host.  op 0:
+ * isSampleGood over in = p0, p1, p2 (x, y, z each): out[0] = 1 or 0.  op 1: computeModelCoefficients over the same:
+ * out[0..3].  op 2: in = c[4], p[3]: out[0] = |c . (p, 1)|, out[1] = 1 iff it is an inlier (< 0.1 in double).
+ * op 3: pcl::eigen33 of the row-major symmetric 3x3 in: out[0..2] = the eigenvector of the smallest eigenvalue. */
+int sm_debug_plane_sampler_piece_host(int32_t op, const float* in, float* out);
+/* The ratio rule in closed form compiled for the host: out[k - k0] = 1 iff non-plane point k (1-based) is kept at
+ * `rate`, for k0 <= k < k1, 1 <= k0, k1 <= 2^24 + 1. */
+int sm_debug_plane_sampler_keep_host(float rate, int64_t k0, int64_t k1, uint8_t* out);
+/* Keep (on = 1) or stop keeping the per-voxel trace of the sampler's runs. */
+int sm_debug_plane_sampler_trace(struct sm_plane_sampler* sampler, int32_t on);
+/* The trace of the last successful run with the trace on: one record of 8 words per voxel in map order (int32
+ * status, iterations, best count, final count; float refined coefficients[4]); status 0 skipped, 1 / 2 z-range rule
+ * with / without plane points, 3 skipped before RANSAC, 4 / 5 RANSAC with / without.  *n = the voxels (0 when Detect
+ * did not run); SM_ERR_BAD_ARGUMENT when capacity < *n. */
+int sm_debug_plane_sampler_voxels(struct sm_plane_sampler* sampler, void* out, int64_t capacity, int64_t* n);
+
 #ifdef __cplusplus
 }
 #endif

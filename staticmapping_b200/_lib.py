@@ -103,6 +103,16 @@ SIGNATURES = {
     "sm_ground_removal_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
     "sm_ground_removal_indices": (C.c_int, [_VP, _VP, C.POINTER(C.c_int64), _VP, C.POINTER(C.c_int64)]),
     "sm_ground_removal_last_error": (C.c_char_p, [_VP]),
+    "sm_plane_sampler_create": (C.c_int, [C.c_int, C.POINTER(_VP)]),
+    "sm_plane_sampler_destroy": (C.c_int, [_VP]),
+    "sm_plane_sampler_set_sampling_rate": (C.c_int, [_VP, C.c_float]),
+    "sm_plane_sampler_set_leaf_size": (C.c_int, [_VP, C.c_float]),
+    "sm_plane_sampler_set_min_point_num_in_voxel": (C.c_int, [_VP, C.c_uint64]),
+    "sm_plane_sampler_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
+    "sm_plane_sampler_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
+    "sm_plane_sampler_indices": (C.c_int, [_VP, _VP, C.POINTER(C.c_int64), _VP, C.POINTER(C.c_int64)]),
+    "sm_plane_sampler_plane_indices": (C.c_int, [_VP, _VP, C.POINTER(C.c_int64)]),
+    "sm_plane_sampler_last_error": (C.c_char_p, [_VP]),
     # include/sm_b200_debug.h (test hooks)
     "sm_debug_solve6": (C.c_int, [C.c_int, _VP, _VP, _VP, _VP]),
     "sm_debug_solve6_host": (C.c_int, [_VP, _VP, _VP, _VP]),
@@ -161,6 +171,10 @@ SIGNATURES = {
     "sm_debug_statistic_removal_distances": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
     "sm_debug_ground_removal_index_host": (C.c_int, [_VP, C.c_int64, C.c_int64, C.c_float, _VP]),
     "sm_debug_ground_removal_voxel_host": (C.c_int, [_VP, C.c_int64, C.c_int32, C.c_int32, C.c_float, _VP, _VP]),
+    "sm_debug_plane_sampler_piece_host": (C.c_int, [C.c_int32, _VP, _VP]),
+    "sm_debug_plane_sampler_keep_host": (C.c_int, [C.c_float, C.c_int64, C.c_int64, _VP]),
+    "sm_debug_plane_sampler_trace": (C.c_int, [_VP, C.c_int32]),
+    "sm_debug_plane_sampler_voxels": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

@@ -6,7 +6,7 @@
 // key order (.cc:74-108): a voxel of fewer than min_point_num_in_voxel points is skipped (in neither list); a voxel with
 // iz <= 0 whose z range max_z - min_z (from -1e9 / 1e9, strict > / <) lies in [0, height_threshold] is ground and its
 // points are outliers; every other voxel emits its records in input order and its points are inliers.  Both lists are
-// sorted.  Here:
+// sorted.  Here (bounds to voxels: voxel_sort, which plane_sampler.cu shares; lists: flag_list, which it shares too):
 //   bounds   per-point voxel index (gr_index), per-axis min / max of the indices other than INT_MIN (grid-strided,
 //            warp and block reductions, then one atomic per block on an order-preserving unsigned encoding)
 //   key      63-bit key, 21 bits per axis: 0 for INT_MIN, else index - min + 1, so the keys ascend in the map's order
@@ -40,38 +40,9 @@ namespace {
 constexpr int kGrSlotBits = 21;
 constexpr uint32_t kGrSlots = 1u << kGrSlotBits;   // slot 0: INT_MIN; slots 1 .. 2^21 - 1: index - min + 1
 constexpr uint32_t kGrSign = 0x80000000u;           // int -> order-preserving unsigned
-// meta[0..2]: ~enc(min index) per axis, meta[3..5]: enc(max index), both over the indices other than INT_MIN (0: none);
-// meta[8]: records emitted, meta[9]: inliers, meta[10]: outliers
+// meta[0..2]: ~enc(min index) per axis, meta[3..5]: enc(max index), both over the indices other than INT_MIN (0: none)
+// (voxel_sort); meta[8]: records emitted, meta[9]: inliers, meta[10]: outliers
 constexpr int kGrMeta = 12;
-
-inline int64_t gr_pad64(int64_t n) { return (n + 63) & ~(int64_t)63; }
-
-// (int)(coordinate / leaf_size) per axis: a float division, truncated toward zero, INT_MIN for a NaN quotient or one
-// outside int's range (to_int)
-__host__ __device__ __forceinline__ void gr_index(const float* p, float leaf, int* ixyz) {
-  ixyz[0] = to_int(p[0] / leaf);
-  ixyz[1] = to_int(p[1] / leaf);
-  ixyz[2] = to_int(p[2] / leaf);
-}
-
-// one step of the reference's z loop (.cc:81-89): a NaN z updates neither
-__host__ __device__ __forceinline__ void gr_z_update(float z_max, float z_min, float* max_z, float* min_z) {
-  if (z_max > *max_z) *max_z = z_max;
-  if (z_min < *min_z) *min_z = z_min;
-}
-
-// the voxel's fate (.cc:77-107); max_z / min_z are read only when the size test passes and iz <= 0
-__host__ __device__ __forceinline__ int gr_voxel_status(int32_t count, int iz, float max_z, float min_z,
-                                                        int32_t min_points, float height_threshold) {
-  if (count < min_points) return kGrSkipped;
-  if (iz > 0) return kGrKept;
-  const float delta = max_z - min_z;
-  return (delta >= 0.f && delta <= height_threshold) ? kGrGround : kGrKept;
-}
-
-__device__ __forceinline__ const float* gr_point(const char* pts, int64_t stride, uint32_t i) {
-  return reinterpret_cast<const float*>(pts + (int64_t)i * stride);
-}
 
 // grid-strided, a few blocks per SM: one atomic per block and bound, so that the atomics do not serialise on meta
 __global__ void __launch_bounds__(256)
@@ -213,6 +184,37 @@ gr_list_scatter_kernel(const uint8_t* __restrict__ status, int n, int want, cons
 
 }  // namespace
 
+int voxel_sort(const char* pts, int n, int64_t stride, float leaf, const RadixPairs& rp, uint32_t* meta,
+               uint32_t* tile_cnt, uint32_t* voxel_start, cudaStream_t s) {
+  const int tiles = compact_tiles(n);
+  const int blocks = ceil_div(n, 256);
+  gr_bounds_kernel<<<std::min(blocks, 4 * kNumSMs), 256, 0, s>>>(pts, stride, n, leaf, meta);
+  gr_key_kernel<<<blocks, 256, 0, s>>>(pts, stride, n, leaf, meta, rp.keys[0], rp.vals[0]);
+  SMB_RC(radix_sort_pairs_u64(rp.keys[0], rp.vals[0], rp.keys[1], rp.vals[1], n, 1, voxel_sort_stride(n), rp.scratch,
+                              s, 8));
+  // 8 passes: the sorted pairs are back in the first buffers
+  gr_heads_count_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], n, tile_cnt);
+  compact_scan(tile_cnt, tiles, s);                     // tile_cnt[tiles] = the number of voxels
+  gr_heads_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], n, tile_cnt, voxel_start);
+  return SM_OK;
+}
+
+bool voxel_span_ok(const uint32_t* host_meta) {
+  for (int d = 0; d < 3; ++d) {
+    if (!host_meta[3 + d]) continue;                    // no index but INT_MIN on this axis
+    const int64_t lo = (int)(~host_meta[d] ^ kGrSign), hi = (int)(host_meta[3 + d] ^ kGrSign);
+    if (hi - lo + 1 > (int64_t)kGrSlots - 1) return false;
+  }
+  return true;
+}
+
+void flag_list(const uint8_t* flag, int n, int want, uint32_t* tile_cnt, int32_t* list, uint32_t* m, cudaStream_t s) {
+  const int tiles = compact_tiles(n);
+  gr_list_count_kernel<<<tiles, kCompactThreads, 0, s>>>(flag, n, want, tile_cnt);
+  compact_scan(tile_cnt, tiles, s);
+  gr_list_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(flag, n, want, tile_cnt, list, m);
+}
+
 // host builds of the per-point index and the per-voxel decision (test hooks sm_debug_ground_removal_*_host)
 void gr_debug_index_host(const float* p, float leaf, int* ixyz) { gr_index(p, leaf, ixyz); }
 int gr_debug_voxel_host(const float* z, int64_t count, int iz, int32_t min_points, float height_threshold,
@@ -234,7 +236,7 @@ struct GroundRemoval {
   int64_t n_inliers = 0, n_outliers = 0;
 
   int reserve(int64_t n) {
-    SMB_RC(sort.reserve(RadixPairs::bytes(gr_pad64(n), (int)n)));
+    SMB_RC(sort.reserve(RadixPairs::bytes(voxel_sort_stride(n), (int)n)));
     SMB_RC(tile_cnt.reserve(4 * compact_count_bytes(n)));
     SMB_RC(voxel_start.reserve(((size_t)n + 1) * sizeof(uint32_t)));
     SMB_RC(emit.reserve((size_t)n));
@@ -252,22 +254,15 @@ struct GroundRemoval {
     const float leaf = params.leaf_size;
     const int ni = (int)n;
     const int tiles = compact_tiles(n);
-    const int64_t st = gr_pad64(n);
     SMB_RC(reserve(n));
     RadixPairs rp;
-    rp.carve(sort.p, st);
+    rp.carve(sort.p, voxel_sort_stride(n));
     uint32_t* mt = (uint32_t*)meta.p;
     uint32_t* tc[4];
     for (int j = 0; j < 4; ++j) tc[j] = (uint32_t*)tile_cnt.p + (size_t)j * (tiles + 1);
-    const int blocks = ceil_div(n, 256);
     SMB_CUDA_OK(cudaMemsetAsync(mt, 0, kGrMeta * sizeof(uint32_t), s));
-    gr_bounds_kernel<<<std::min(blocks, 4 * kNumSMs), 256, 0, s>>>(pts, stride, ni, leaf, mt);
-    gr_key_kernel<<<blocks, 256, 0, s>>>(pts, stride, ni, leaf, mt, rp.keys[0], rp.vals[0]);
-    SMB_RC(radix_sort_pairs_u64(rp.keys[0], rp.vals[0], rp.keys[1], rp.vals[1], ni, 1, st, rp.scratch, s, 8));
-    const uint32_t* order = rp.vals[0];                 // 8 passes: the sorted pairs are back in the first buffers
-    gr_heads_count_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], ni, tc[0]);
-    compact_scan(tc[0], tiles, s);                      // tc[0][tiles] = the number of voxels
-    gr_heads_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], ni, tc[0], (uint32_t*)voxel_start.p);
+    SMB_RC(voxel_sort(pts, ni, stride, leaf, rp, mt, tc[0], (uint32_t*)voxel_start.p, s));
+    const uint32_t* order = rp.vals[0];
     const int decide_blocks = (int)std::min<int64_t>(ceil_div(n, 8), 32 * kNumSMs);
     gr_decide_kernel<<<decide_blocks, 256, 0, s>>>(pts, stride, order, (const uint32_t*)voxel_start.p, tc[0] + tiles,
                                                    leaf, params.min_point_num_in_voxel, params.height_threshold,
@@ -277,21 +272,13 @@ struct GroundRemoval {
     filter_compact_records((const char*)sorted.p, 20, order, ni, (const uint8_t*)emit.p, tc[1], out, out_index, mt + 8,
                            s);
     const std::pair<int, DevBuf*> lists[2] = {{kGrKept, &inliers_next}, {kGrGround, &outliers_next}};
-    for (int j = 0; j < 2; ++j) {
-      gr_list_count_kernel<<<tiles, kCompactThreads, 0, s>>>((const uint8_t*)status.p, ni, lists[j].first, tc[2 + j]);
-      compact_scan(tc[2 + j], tiles, s);
-      gr_list_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>((const uint8_t*)status.p, ni, lists[j].first,
-                                                               tc[2 + j], (int32_t*)lists[j].second->p, mt + 9 + j);
-    }
+    for (int j = 0; j < 2; ++j)
+      flag_list((const uint8_t*)status.p, ni, lists[j].first, tc[2 + j], (int32_t*)lists[j].second->p, mt + 9 + j, s);
     SMB_CUDA_OK(cudaGetLastError());
     uint32_t host[11];
     SMB_CUDA_OK(cudaMemcpyAsync(host, mt, sizeof(host), cudaMemcpyDeviceToHost, s));
     SMB_CUDA_OK(cudaStreamSynchronize(s));
-    for (int d = 0; d < 3; ++d) {
-      if (!host[3 + d]) continue;                       // no index but INT_MIN on this axis
-      const int64_t lo = (int)(~host[d] ^ kGrSign), hi = (int)(host[3 + d] ^ kGrSign);
-      if (hi - lo + 1 > (int64_t)kGrSlots - 1) return SM_ERR_BAD_ARGUMENT;
-    }
+    if (!voxel_span_ok(host)) return SM_ERR_BAD_ARGUMENT;
     std::swap(inliers, inliers_next);
     std::swap(outliers, outliers_next);
     n_inliers = host[9];

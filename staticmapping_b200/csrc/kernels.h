@@ -11,6 +11,7 @@
 #include "common.cuh"
 
 struct sm_filter_chain;
+struct sm_plane_sampler;
 
 namespace smb {
 
@@ -473,11 +474,87 @@ void filter_compact_records(const char* pts, int64_t stride, const uint32_t* ind
 // the fate of a GroundRemoval voxel (filter_ground_removal.cc:74-108): skipped (in neither list), ground (its points
 // are outliers) or kept (its records are emitted, its points are inliers)
 enum GrStatus : int { kGrSkipped = 0, kGrGround = 1, kGrKept = 2 };
+
+// (int)(coordinate / leaf_size) per axis: a float division, truncated toward zero, INT_MIN for a NaN quotient or one
+// outside int's range (to_int).  GroundRemoval and PlaneDetector (plane_detector.h:80-83) key their voxels so.
+__host__ __device__ __forceinline__ void gr_index(const float* p, float leaf, int* ixyz) {
+  ixyz[0] = to_int(p[0] / leaf);
+  ixyz[1] = to_int(p[1] / leaf);
+  ixyz[2] = to_int(p[2] / leaf);
+}
+
+// one step of the reference's z loop (.cc:81-89, plane_detector.h:109-118): a NaN z updates neither
+__host__ __device__ __forceinline__ void gr_z_update(float z_max, float z_min, float* max_z, float* min_z) {
+  if (z_max > *max_z) *max_z = z_max;
+  if (z_min < *min_z) *min_z = z_min;
+}
+
+// the voxel's fate (.cc:77-107); max_z / min_z are read only when the size test passes and iz <= 0
+__host__ __device__ __forceinline__ int gr_voxel_status(int32_t count, int iz, float max_z, float min_z,
+                                                        int32_t min_points, float height_threshold) {
+  if (count < min_points) return kGrSkipped;
+  if (iz > 0) return kGrKept;
+  const float delta = max_z - min_z;
+  return (delta >= 0.f && delta <= height_threshold) ? kGrGround : kGrKept;
+}
+
+__device__ __forceinline__ const float* gr_point(const char* pts, int64_t stride, uint32_t i) {
+  return reinterpret_cast<const float*>(pts + (int64_t)i * stride);
+}
+
+// The voxels of GroundRemoval and PlaneDetector (plane_sampler.cu) in the reference's std::map order, lexicographic
+// on signed (ix, iy, iz).  For n >= 1 records, after the caller has zeroed meta[0..5]: meta[0..5] = the
+// per-axis index bounds (voxel_span_ok reads them), the sorted 63-bit keys in rp.keys[0] with the input indices in
+// rp.vals[0] (stable: a voxel keeps its points in input order), voxel_start[v] = the first sorted position of voxel
+// v, voxel_start[voxels] = n, and tile_cnt[compact_tiles(n)] = the number of voxels.  rp: carved with
+// voxel_sort_stride(n); tile_cnt: compact_count_bytes(n).
+inline int64_t voxel_sort_stride(int64_t n) { return (n + 63) & ~(int64_t)63; }
+int voxel_sort(const char* pts, int n, int64_t stride, float leaf, const RadixPairs& rp, uint32_t* meta,
+               uint32_t* tile_cnt, uint32_t* voxel_start, cudaStream_t s);
+// false when the indices other than INT_MIN of an axis span more than 2^21 - 1 voxels (the key cannot hold them);
+// host_meta: meta[0..5] read back after voxel_sort
+bool voxel_span_ok(const uint32_t* host_meta);
+// list = the i < n with flag[i] == want, ascending, and *m their number (device memory); tile_cnt:
+// compact_count_bytes(n)
+void flag_list(const uint8_t* flag, int n, int want, uint32_t* tile_cnt, int32_t* list, uint32_t* m, cudaStream_t s);
 // host builds of the per-point voxel index and of the per-voxel decision over the voxel's z in input order (test hooks
 // sm_debug_ground_removal_index_host / _voxel_host); max_min: the z loop's max_z, min_z
 void gr_debug_index_host(const float* p, float leaf, int* ixyz);
 int gr_debug_voxel_host(const float* z, int64_t count, int iz, int32_t min_points, float height_threshold,
                         float* max_min);
+
+// ---- plane_sampler.cu --------------------------------------------------------------------------
+// what Detect did with a voxel (plane_detector.h:103-152): skipped (fewer than min points), the z-range rule (iz <= 0)
+// with or without plane points, skipped before RANSAC (iz > 0, fewer than 2 min points), RANSAC with or without
+enum PsStatus : int32_t {
+  kPsSkipped = 0, kPsGroundPlane = 1, kPsGroundNot = 2, kPsSkippedRansac = 3, kPsRansacPlane = 4, kPsRansacNot = 5
+};
+// one voxel of the last run, in map order (test hook sm_debug_plane_sampler_voxels): its status; for a RANSAC voxel
+// the loop's iterations, the best count (-INT_MAX when no sample was found), the refined coefficients (the best
+// model's when there were 3 inliers or fewer); the plane points it gave
+struct PsTrace {
+  int32_t status, iterations, best, final_count;
+  float coef[4];
+};
+// host builds (test hooks sm_debug_plane_sampler_piece_host / _keep_host)
+int ps_debug_piece_host(int op, const float* in, float* out);
+void ps_debug_keep_host(float rate, int64_t k0, int64_t k1, uint8_t* out);
+// The device buffers and parameters of one RandomSamplerWithPlaneDetect; the buffers only grow.  run(): n in
+// 1..2^24 records of `stride` bytes in device memory -> out (capacity n records) and out_index (capacity n), the
+// kept records in input order, *m; returns after the stream has finished.  SM_ERR_BAD_ARGUMENT: a voxel span past
+// voxel_sort's key.  The lists (inliers, outliers, plane indices) of a run are written into lists_next and swapped in
+// when it succeeds.
+struct PlaneSampler {
+  float rate = 1.f, leaf_size = 0.8f;
+  uint64_t min_points = 10;
+  bool trace_on = false;                 // sm_debug_plane_sampler_trace: keep the per-voxel trace of every run
+  DevBuf sort, tile_cnt, voxel_start, scratch, cta_list, plane, keep, meta, rnd, trace, lists[3], lists_next[3];
+  int64_t n_lists[3] = {0, 0, 0};
+  int64_t n_voxels = 0;                  // traced voxels of the last run
+  int reserve(int64_t n);
+  int run(const char* pts, int64_t n, int64_t stride, float* out, uint32_t* out_index, int64_t* m, cudaStream_t s);
+};
+PlaneSampler* plane_sampler_of(::sm_plane_sampler* h);   // the state behind the C handle, null for null
 
 // ---- depth_cluster.cu --------------------------------------------------------------------------
 // sinf / cosf of RangeImage::LabelOneComponent's horizontal and vertical resolution (filter_range_image.cc:255-259)

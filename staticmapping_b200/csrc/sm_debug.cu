@@ -152,6 +152,35 @@ int sm_debug_ground_removal_voxel_host(const float* z, int64_t count, int32_t iz
   return SM_OK;
 }
 
+// test hooks: RandomSamplerWithPlaneDetect's pieces and closed-form ratio rule compiled for the host, its trace
+int sm_debug_plane_sampler_piece_host(int32_t op, const float* in, float* out) {
+  if (!in || !out) return SM_ERR_BAD_ARGUMENT;
+  return ps_debug_piece_host(op, in, out) == 0 ? SM_OK : SM_ERR_BAD_ARGUMENT;
+}
+
+int sm_debug_plane_sampler_keep_host(float rate, int64_t k0, int64_t k1, uint8_t* out) {
+  if (k0 < 1 || k1 < k0 || k1 > (1 << 24) + 1 || (k1 > k0 && !out)) return SM_ERR_BAD_ARGUMENT;
+  ps_debug_keep_host(rate, k0, k1, out);
+  return SM_OK;
+}
+
+int sm_debug_plane_sampler_trace(sm_plane_sampler* sampler, int32_t on) {
+  PlaneSampler* f = plane_sampler_of(sampler);
+  if (!f) return SM_ERR_BAD_ARGUMENT;
+  f->trace_on = on != 0;
+  return SM_OK;
+}
+
+int sm_debug_plane_sampler_voxels(sm_plane_sampler* sampler, void* out, int64_t capacity, int64_t* n) {
+  PlaneSampler* f = plane_sampler_of(sampler);
+  if (!f || !n) return SM_ERR_BAD_ARGUMENT;
+  *n = f->n_voxels;
+  if (f->n_voxels == 0) return SM_OK;
+  if (!out || capacity < f->n_voxels) return SM_ERR_BAD_ARGUMENT;
+  SMB_CUDA_OK(cudaMemcpy(out, f->trace.p, (size_t)f->n_voxels * sizeof(PsTrace), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
 int sm_debug_voxel_index(int32_t op, const float* p3, float param, int32_t min_b, int64_t* out4) {
   if (!p3 || !out4) return SM_ERR_BAD_ARGUMENT;
   switch (op) {

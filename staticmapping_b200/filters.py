@@ -1,8 +1,9 @@
 """pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
 chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
 deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster.  StatisticRemoval,
-PCL's statistical outlier removal, and GroundRemoval, the voxel height-range ground filter, run on their own handles
-(sm_statistic_removal_*, sm_ground_removal_*).  There is no CPU fallback."""
+PCL's statistical outlier removal, GroundRemoval, the voxel height-range ground filter, and the submap sampler
+RandomSamplerWithPlaneDetect run on their own handles (sm_statistic_removal_*, sm_ground_removal_*,
+sm_plane_sampler_*).  There is no CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -226,3 +227,58 @@ class GroundRemoval(_OwnHandleFilter):
         self._inliers = inliers[:ni.value].copy()
         self._outliers = outliers[:no.value].copy()
         return InnerCloud(out[:m.value].copy())
+
+
+class RandomSamplerWithPlaneDetect(_RecordFilter):
+    """The submap sampler RandomSamplerWithPlaneDetect (pre_processors/random_sample_with_plane_detect.h) with its
+    PlaneDetector on the GPU (sm_plane_sampler_*, include/sm_b200.h): the points of flat low voxels and of voxels whose
+    RANSAC plane holds more than 85 % of their points are kept, and the other points are sampled at SetSamplingRate's
+    rate in input order.  Configured by its setters (no XML node); SetInputCloud + Filter run it.  `Filter` returns the
+    kept InnerCloud in input order; Inliers() / Outliers() are the kept and the dropped input indices and
+    PlaneIndices() the plane points, all ascending.  More than 2^24 points, or a span of voxel indices past the 63-bit
+    key, raise ValueError."""
+    _abi = "sm_plane_sampler"
+
+    def __init__(self, device: int = 0):
+        super().__init__(device)
+        self._plane = np.zeros(0, np.int32)
+        self.messages = []
+
+    def _setter(self, name, value):
+        self._check(self._fn(name)(self._h, value), name)
+        message = self._error()
+        if message:
+            self.messages.append(message)
+
+    def SetSamplingRate(self, rate):
+        """above 1 -> 1, below 1e-6 -> 1e-6, with the reference's warning in `messages`"""
+        self._setter("set_sampling_rate", float(rate))
+
+    def SetLeafSize(self, size):
+        self._setter("set_leaf_size", float(size))
+
+    def SetMinPointNumInVoxel(self, num):
+        """a size_t: below 5 -> 5, with the reference's warning in `messages`"""
+        self._setter("set_min_point_num_in_voxel", int(num) % (1 << 64))
+
+    def Filter(self):
+        if self._cloud is None:
+            return None
+        pts = self._cloud
+        n = pts.shape[0]
+        out = np.empty_like(pts)
+        m = C.c_int64(0)
+        self._check(self._fn("run")(self._h, pts.ctypes.data, n, 20, out.ctypes.data, C.byref(m), None), "run")
+        inliers, outliers = np.empty(n, np.int32), np.empty(n, np.int32)
+        ni, no, npl = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        self._check(self._fn("indices")(self._h, inliers.ctypes.data, C.byref(ni), outliers.ctypes.data, C.byref(no)),
+                    "indices")
+        plane = np.empty(n, np.int32)
+        self._check(self._fn("plane_indices")(self._h, plane.ctypes.data, C.byref(npl)), "plane_indices")
+        self._inliers = inliers[:ni.value].copy()
+        self._outliers = outliers[:no.value].copy()
+        self._plane = plane[:npl.value].copy()
+        return InnerCloud(out[:m.value].copy())
+
+    def PlaneIndices(self):
+        return self._plane
