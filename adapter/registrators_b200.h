@@ -319,7 +319,11 @@ class FilterChainB200 {
         << sm_filter_chain_last_error(chain_);
   }
   bool ConfigsValid(int filter) { return sm_filter_chain_validate(chain_, filter) == 1; }
+  // true: Add also accepts GroundRemoval, StatisticRemoval and VoxelGrid (the chain option all_filters); false
+  // restores their refusal.  Filters already added stay.
+  void SetAllFilters(bool on) { CHECK_EQ(sm_filter_chain_set_option(chain_, "all_filters", on ? "1" : "0"), 0); }
 
+  // inliers: the indices in `input` of the output records, in emission order (include/sm_b200.h)
   void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,
               std::vector<int>* const inliers = nullptr) {
     FilterRecordsB200(chain_, sm_filter_chain_run, sm_filter_chain_last_error, "sm_filter_chain_run", input, output,

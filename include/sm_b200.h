@@ -401,7 +401,25 @@ double sm_m2dp_match(const float* P, const float* Q, int64_t n);
  *                       max_dist_to_line (0.05), search_angle (10), thread_num (4, unused).
  * atan2f is CUDA's here and glibc's in the reference: a point within a few float ulps of a RangeImage row / column
  * border or a GroundRemoval2 segment border can land in the neighbouring pixel / segment.  A float -> int conversion
- * outside int's range (undefined in C++) gives INT_MIN, as the reference's x86 build does. */
+ * outside int's range (undefined in C++) gives INT_MIN, as the reference's x86 build does.
+ * With the chain option all_filters, the reference's other three filters are built too, as the GPU filters of their
+ * own entry points.  None of them gives the reference Factory's result, which is why the option is off by default:
+ * the reference's StatisticRemoval::Filter is an empty body (filter_statistic_removal.cc:44-59), its VoxelGrid emits
+ * in std::unordered_map order, and its GroundRemoval breaks the ascending order above.  With the option on, each
+ * stage reads the previous stage's records in their order, and a run's inlier_index holds the scan index of every
+ * emitted record in emission order; the six kinds above emit in ascending order, so their chains are unchanged.
+ *   GroundRemoval       min_point_num_in_voxel (10), leaf_size (0.8), height_threshold (0.15): sm_ground_removal_*
+ *                       steps 1-3 on the stage's input, records in map order, each index the scan index of the
+ *                       record's input point.  A voxel span past 2^21 - 1: SM_ERR_BAD_ARGUMENT.
+ *   StatisticRemoval    point_num_meank (30), std_mul (1): sm_statistic_removal_* on the stage's input, kept records in
+ *                       input order.  point_num_meank outside 1..63: SM_ERR_BAD_ARGUMENT before any work; 1..K finite
+ *                       points: SM_ERR_CHECK_FAILED.
+ *   VoxelGrid           voxel_size (0.1): sm_voxel_grid_filter on the stage's input, the same voxel means bit for bit
+ *                       (factor 0) in ascending (ix, iy, iz), non-finite points dropped; each record's index is the
+ *                       scan index of its voxel's first member in the stage's input order, which a later RandomSampler
+ *                       keys on.  voxel_size <= 1e-6 (ConfigsValid, where the reference would run with an undefined
+ *                       lround): SM_ERR_BAD_ARGUMENT before any work; finite points spanning 2^21 voxels or more
+ *                       along an axis: SM_ERR_BAD_ARGUMENT. */
 typedef struct sm_filter_chain sm_filter_chain;
 /* filter::Factory::Factory (filter_factory.h).  Needs no device; the first run binds CUDA ordinal `device`. */
 int sm_filter_chain_create(int device, sm_filter_chain** out);
@@ -409,8 +427,8 @@ int sm_filter_chain_destroy(sm_filter_chain* chain);
 /* One <filter name=...> of Factory::InitFromXmlNode (filter_factory.cc:64-80): appends the filter at its constructor's
  * defaults and returns its index.  GroundRemoval (see sm_ground_removal_*), StatisticRemoval (an empty body in the
  * reference, filter_statistic_removal.cc:44-59; PCL's filter is sm_statistic_removal_*) and VoxelGrid (see
- * sm_voxel_grid_filter) are not built into the chain: SM_ERR_UNSUPPORTED_TYPE.  A name the reference does not register either (it skips it, :68-71):
- * SM_ERR_UNKNOWN_OPTION; the chain is unchanged. */
+ * sm_voxel_grid_filter) are added only while the option all_filters is on, else SM_ERR_UNSUPPORTED_TYPE.  A name the
+ * reference does not register either (it skips it, :68-71): SM_ERR_UNKNOWN_OPTION; the chain is unchanged. */
 int sm_filter_chain_add(sm_filter_chain* chain, const char* filter_name);
 /* One <param type=... name=...>text</param> of Interface::InitFromXmlNode (filter_interface.cc:38-58): `text` is read
  * as pugixml's as_int (type 0) or as_float (type 1), then cast to the parameter's declared type
@@ -418,14 +436,20 @@ int sm_filter_chain_add(sm_filter_chain* chain, const char* filter_name);
  * name the filter does not register, SM_ERR_BAD_ARGUMENT for a type other than 0 / 1 (a <param> without `type`). */
 int sm_filter_chain_set_param(sm_filter_chain* chain, int filter, const char* name, int type, const char* text);
 /* Interface::ConfigsValid of the filter (filter_interface.cc:59; AxisRange filter_axis_range.cc:41-43,
- * BoundingBoxRemoval filter_bounding_box.cc:49-51, RandomSampler filter_random_sample.cc:35-37): 1 / 0.  As in the
- * reference's Factory (filter_factory.cc:77), an invalid filter still runs. */
+ * BoundingBoxRemoval filter_bounding_box.cc:49-51, RandomSampler filter_random_sample.cc:35-37, VoxelGrid
+ * filter_voxel_grid.cc:35): 1 / 0.  As in the reference's Factory (filter_factory.cc:77), an invalid filter still
+ * runs, except a VoxelGrid (see above). */
 int sm_filter_chain_validate(sm_filter_chain* chain, int filter);
-/* Chain options, no reference counterpart: sample_seed (unsigned, 1), the seed of RandomSampler's stand-in. */
+/* Chain options, no reference counterpart: sample_seed (unsigned, 1), the seed of RandomSampler's stand-in;
+ * all_filters (unsigned, 0): non-zero makes sm_filter_chain_add accept GroundRemoval, StatisticRemoval and VoxelGrid,
+ * 0 restores their refusal.  all_filters affects sm_filter_chain_add only: filters already added stay. */
 int sm_filter_chain_set_option(sm_filter_chain* chain, const char* name, const char* text);
 /* Factory::SetInputCloud + Factory::Filter (filter_factory.cc:83-106).  `points`: n records `stride_bytes` (>= 20)
  * apart; `out`: capacity n packed 5-float records; *m_out = the number of inliers; inlier_index (optional, capacity
- * n): their indices in `points`, ascending.  An empty chain copies the input (:90-93).  SM_ERR_BAD_ARGUMENT: a
+ * n): their indices in `points`, in emission order (ascending without GroundRemoval and VoxelGrid).  An empty chain
+ * copies the input (:90-93); an empty intermediate cloud ends the chain.  `out` and inlier_index are written on
+ * success only, except by a failing GroundRemoval2 stage of the _device form.
+ * SM_ERR_BAD_ARGUMENT: the errors of the three stages above, a
  * RangeImage with vertical_line_num <= 0 or horizontal_line_num <= 0 (its SetInputCloud keeps the previous cloud,
  * filter_range_image.cc:72-74) or a grid of more than 2^24 pixels / cells.  SM_ERR_CHECK_FAILED: an inverted
  * BoundingBoxRemoval box (CHECK in common/bounding_box.cc:114) or a fitted ground line that does not run outward
@@ -463,7 +487,7 @@ const char* sm_filter_chain_last_error(const sm_filter_chain* chain);
  * (float, 1.0), but its Filter body is a commented-out pcl::StatisticalOutlierRemoval call (setMeanK(point_num_meank),
  * setStddevMulThresh(std_mul)) under a TODO (filter_statistic_removal.cc:44-59): there the filter does nothing.  This
  * is that PCL filter (StatisticalOutlierRemoval::applyFilterIndices of PCL 1.8 / 1.10), restated from upstream PCL and
- * FLANN; no PCL is compiled to check it.  It is not part of the chain (sm_filter_chain_add refuses it); it has its own
+ * FLANN; no PCL is compiled to check it.  It is a chain stage only with the chain option all_filters; it has its own
  * handle, used by one thread at a time.  Its device buffers belong to the handle and only grow.
  *   1. A point is finite when x, y and z are; only finite points are searched.  A non-finite point gets distance 0.
  *   2. The K + 1 nearest finite points of each finite point, K = point_num_meank: exact search, self-match allowed, over
@@ -508,7 +532,7 @@ const char* sm_statistic_removal_last_error(const sm_statistic_removal* filter);
 
 /* ---- pre_processers::filter::GroundRemoval: the voxel height-range ground filter ---------------------------------
  * GroundRemoval (v1, filter_ground_removal.{h,cc}) with min_point_num_in_voxel (int32, 10), leaf_size (float, 0.8) and
- * height_threshold (float, 0.15).  It is not part of the chain (sm_filter_chain_add refuses it); it has its own handle,
+ * height_threshold (float, 0.15).  It is a chain stage only with the chain option all_filters; it has its own handle,
  * used by one thread at a time.  Its device buffers belong to the handle and only grow.
  *   1. Voxel index per axis: (int)(coordinate / leaf_size), a float division truncated toward zero; a NaN quotient or
  *      one outside int's range gives INT_MIN (the reference's x86 build).  Such points are kept in that voxel, so

@@ -11,6 +11,9 @@
 //     a cell stay in input order) -> one thread per cell walks its points in order (running minimum and membership
 //     are order dependent, :195-209) -> one thread per segment runs FitLines' sequential scan (:240-316) -> one
 //     thread per point for ClusterGround (:337-396) -> ordered compaction of the non-ground points.
+// With the chain option all_filters: GroundRemoval, StatisticRemoval and VoxelGrid, each one stage run by the stage
+// object its own entry point uses (ground_removal.cu, statistic_removal.cu, voxel_filter.cu), on the stage's input with
+// its scan indices; GroundRemoval and VoxelGrid emit in voxel order (FilterChain::record_stage).
 // Compiled with -fmad=false: the float expressions are the reference's, operation by operation.  sqrtf and the
 // divisions are correctly rounded on both sides; atan2f is CUDA's here and glibc's there, so a point within a few
 // ulps of a row / column / segment border can land next door (DESIGN.md section 4h).
@@ -460,6 +463,7 @@ FilterParams filter_defaults(int kind) {
   if (kind == kFilterGroundRemoval) {                                                  // in AxisRange's storage
     f.min_point_num_in_voxel = 10; f.leaf_size = 0.8f; f.height_threshold = 0.15f;
   }
+  if (kind == kFilterVoxelGrid) f.voxel_size = 0.1f;                                   // in Range's storage
   return f;
 }
 
@@ -494,6 +498,7 @@ bool filter_param(FilterParams& f, const char* name, void** target, int* type) {
       {kFilterGroundRemoval, "min_point_num_in_voxel", 0, &f.min_point_num_in_voxel},
       {kFilterGroundRemoval, "leaf_size", 1, &f.leaf_size},
       {kFilterGroundRemoval, "height_threshold", 1, &f.height_threshold},
+      {kFilterVoxelGrid, "voxel_size", 1, &f.voxel_size},
   };
   for (const Entry& e : table)
     if (e.kind == f.kind && strcmp(e.name, name) == 0) { *target = e.p; *type = e.type; return true; }
@@ -517,6 +522,7 @@ bool filter_configs_valid(const FilterParams& f) {
     case kFilterAxisRange: return f.max > f.min && f.axis_index >= 0 && f.axis_index <= 2;   // filter_axis_range.cc:41-43
     case kFilterBoundingBoxRemoval: return f.min_x < f.max_x && f.min_y < f.max_y && f.min_z < f.max_z;   // filter_bounding_box.cc:49-51
     case kFilterRandomSampler: return f.sampling_rate >= 0.f && f.sampling_rate <= 1.f;       // filter_random_sample.cc:35-37
+    case kFilterVoxelGrid: return (double)f.voxel_size > 1.e-6;                              // filter_voxel_grid.cc:35
     default: return true;                                                                    // Interface::ConfigsValid
   }
 }
@@ -677,20 +683,54 @@ int FilterChain::ground_removal2_stage(const FilterParams& f, const char* in, co
   return 0;
 }
 
+// GroundRemoval, StatisticRemoval and VoxelGrid: their stage objects, on the stage's input; *m is the stage's count
+int FilterChain::record_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,
+                              float* out, uint32_t* index_out, int64_t* m, cudaStream_t s) {
+  int rc;
+  if (f.kind == kFilterGroundRemoval) {
+    ground.params = f;
+    rc = ground.run(in, n, stride, index_in, out, index_out, m, s, false);
+    if (rc == SM_ERR_BAD_ARGUMENT)
+      fault = "GroundRemoval: the voxel indices of an axis span more than 2^21 - 1 voxels (the 63-bit voxel key)";
+  } else if (f.kind == kFilterStatisticRemoval) {
+    statistic.params = f;
+    rc = statistic.run(in, n, stride, index_in, out, index_out, m, s);
+    if (rc == SM_ERR_CHECK_FAILED)
+      fault = "Check failed: StatisticRemoval between 1 and point_num_meank finite points (PCL reads past its k-list)";
+    if (rc == SM_ERR_BAD_ARGUMENT) fault = "StatisticRemoval: more finite points than the 24-level k-d tree holds";
+  } else {
+    rc = voxel.run(in, n, stride, f.voxel_size, index_in, out, index_out, m, s);
+    if (rc == SM_ERR_BAD_ARGUMENT) fault = "VoxelGrid: the finite points span 2^21 voxels or more along an axis";
+  }
+  return rc;
+}
+
 int FilterChain::run(const char* in, int64_t n, int64_t stride, float* out, int32_t* out_index, int64_t* m,
                      cudaStream_t s) {
   *m = 0;
+  fault = "";
   for (const FilterParams& f : filters) {
     // RangeImage::SetInputCloud keeps its previous cloud for such a size (filter_range_image.cc:72-74); the box of an
     // invalid BoundingBoxRemoval CHECK-fails in its constructor (common/bounding_box.cc:114)
     if (f.kind == kFilterRangeImage && (f.vertical_line_num <= 0 || f.horizontal_line_num <= 0 ||
                                         (int64_t)f.vertical_line_num * f.horizontal_line_num > kMaxCells))
-      return SM_ERR_BAD_ARGUMENT;
+      return bad_grid();
     if (f.kind == kFilterGroundRemoval2 &&
         (f.bin_num <= 0 || f.segment_num <= 0 || (int64_t)f.bin_num * f.segment_num > kMaxCells ||
          gr2_consts(f).search_steps < 0 || gr2_consts(f).search_steps >= f.segment_num))
+      return bad_grid();
+    if (f.kind == kFilterBoundingBoxRemoval && !filter_configs_valid(f)) return check_failed();
+    if (f.kind == kFilterStatisticRemoval) {
+      statistic.params = f;
+      if (!statistic.k_ok()) {
+        fault = "StatisticRemoval: point_num_meank is outside 1..63";
+        return SM_ERR_BAD_ARGUMENT;
+      }
+    }
+    if (f.kind == kFilterVoxelGrid && !filter_configs_valid(f)) {   // the reference would run with an undefined lround
+      fault = "VoxelGrid: voxel_size <= 1e-6 (ConfigsValid)";
       return SM_ERR_BAD_ARGUMENT;
-    if (f.kind == kFilterBoundingBoxRemoval && !filter_configs_valid(f)) return SM_ERR_CHECK_FAILED;
+    }
   }
   if (n == 0) return 0;
   SMB_RC(reserve(n));
@@ -705,10 +745,30 @@ int FilterChain::run(const char* in, int64_t n, int64_t stride, float* out, int3
     const bool last = end >= n_filters;
     float* dst = last ? out : (float*)rec[stage & 1].p;
     uint32_t* dst_idx = (last && out_index) ? (uint32_t*)out_index : (uint32_t*)idx[stage & 1].p;
+    const int kind = n_filters ? filters[first].kind : kFilterRange;
+    if (kind >= kFilterStatisticRemoval) {
+      // GroundRemoval and VoxelGrid find their span limit after writing their output: as the last stage, they write
+      // into the chain's buffers, copied out on success
+      const bool staged = last && kind != kFilterStatisticRemoval;
+      float* rec_out = staged ? (float*)rec[stage & 1].p : dst;
+      uint32_t* idx_out = staged ? (uint32_t*)idx[stage & 1].p : dst_idx;
+      int64_t stage_m = 0;
+      SMB_RC(record_stage(filters[first], cur, cur_idx, (int)cur_n, cur_stride, rec_out, idx_out, &stage_m, s));
+      if (staged && stage_m > 0) {
+        SMB_CUDA_OK(cudaMemcpyAsync(dst, rec_out, (size_t)stage_m * 20, cudaMemcpyDeviceToDevice, s));
+        if (out_index)
+          SMB_CUDA_OK(cudaMemcpyAsync(out_index, idx_out, (size_t)stage_m * sizeof(uint32_t),
+                                      cudaMemcpyDeviceToDevice, s));
+        SMB_CUDA_OK(cudaStreamSynchronize(s));
+      }
+      cur = (const char*)rec_out; cur_idx = idx_out; cur_stride = 20; cur_n = (uint32_t)stage_m;
+      first = end; ++stage;
+      continue;
+    }
     int gr2_status = 0;
-    if (!n_filters || filters[first].kind <= kFilterRandomSampler) {
+    if (kind <= kFilterRandomSampler) {
       SMB_RC(predicate_stage(first, end - first, cur, cur_idx, (int)cur_n, cur_stride, dst, dst_idx, s));
-    } else if (filters[first].kind == kFilterRangeImage) {
+    } else if (kind == kFilterRangeImage) {
       SMB_RC(range_image_stage(filters[first], cur, cur_idx, (int)cur_n, cur_stride, dst, dst_idx, s));
     } else {
       SMB_RC(ground_removal2_stage(filters[first], cur, cur_idx, (int)cur_n, cur_stride, dst, dst_idx, s));
@@ -717,7 +777,7 @@ int FilterChain::run(const char* in, int64_t n, int64_t stride, float* out, int3
     uint32_t host[2] = {0, 0};    // the stage's count sizes the next stage's grids
     SMB_CUDA_OK(cudaMemcpyAsync(host, count.p, sizeof(host), cudaMemcpyDeviceToHost, s));
     SMB_CUDA_OK(cudaStreamSynchronize(s));
-    if (gr2_status && host[1]) { gr2.status = 1; return SM_ERR_CHECK_FAILED; }   // CHECK(line.start[0] < line.end[0])
+    if (gr2_status && host[1]) { gr2.status = 1; return check_failed(); }   // CHECK(line.start[0] < line.end[0])
     cur = (const char*)dst; cur_idx = dst_idx; cur_stride = 20; cur_n = host[0];
     first = end; ++stage;
   } while (first < n_filters && cur_n > 0);   // a filter handed an empty cloud does nothing (its SetInputCloud)
@@ -755,9 +815,14 @@ int sm_filter_chain_add(sm_filter_chain* c, const char* filter_name) {
       c->chain.filters.push_back(filter_defaults(k));
       return (int)c->chain.filters.size() - 1;
     }
-  for (const char* name : {"GroundRemoval", "StatisticRemoval", "VoxelGrid"})
-    if (strcmp(filter_name, name) == 0)
-      return c->fail(SM_ERR_UNSUPPORTED_TYPE, "filter %s is not built into the chain", filter_name);
+  static const char* const more[] = {"StatisticRemoval", "GroundRemoval", "VoxelGrid"};   // kinds 6, 7, 8
+  for (int k = 0; k < 3; ++k)
+    if (strcmp(filter_name, more[k]) == 0) {
+      if (!c->chain.all_filters)
+        return c->fail(SM_ERR_UNSUPPORTED_TYPE, "filter %s is not built into the chain", filter_name);
+      c->chain.filters.push_back(filter_defaults(kFilterStatisticRemoval + k));
+      return (int)c->chain.filters.size() - 1;
+    }
   return c->fail(SM_ERR_UNKNOWN_OPTION, "%s not supported yet.", filter_name);
 }
 
@@ -773,8 +838,11 @@ int sm_filter_chain_validate(sm_filter_chain* c, int filter) {
 
 int sm_filter_chain_set_option(sm_filter_chain* c, const char* name, const char* text) {
   if (!c || !name || !text) return SM_ERR_BAD_ARGUMENT;
-  if (strcmp(name, "sample_seed") != 0) return c->fail(SM_ERR_UNKNOWN_OPTION, "unknown chain option %s", name);
-  c->chain.sample_seed = (uint32_t)strtoul(text, nullptr, 10);
+  uint32_t* option = strcmp(name, "sample_seed") == 0   ? &c->chain.sample_seed
+                     : strcmp(name, "all_filters") == 0 ? &c->chain.all_filters
+                                                        : nullptr;
+  if (!option) return c->fail(SM_ERR_UNKNOWN_OPTION, "unknown chain option %s", name);
+  *option = (uint32_t)strtoul(text, nullptr, 10);
   return SM_OK;
 }
 
@@ -784,9 +852,7 @@ int sm_filter_chain_run_device(sm_filter_chain* c, const float* dev_points, int6
   SMB_RC(c->use_device());
   const int rc = c->chain.run((const char*)dev_points, n, stride_bytes, dev_out, dev_inlier_index, m_out,
                               (cudaStream_t)cuda_stream);
-  if (rc == SM_ERR_CHECK_FAILED)
-    return c->fail(rc, "Check failed: an inverted BoundingBoxRemoval box or line.start[0] < line.end[0]");
-  if (rc == SM_ERR_BAD_ARGUMENT) return c->fail(rc, "a RangeImage or GroundRemoval2 grid size the chain cannot run");
+  if (rc == SM_ERR_CHECK_FAILED || rc == SM_ERR_BAD_ARGUMENT) return c->fail(rc, "%s", c->chain.fault);
   return c->cuda_fail(rc);
 }
 

@@ -16,8 +16,8 @@
 //            strict comparisons), gr_voxel_status; writes the emit flag of every sorted position and the status of
 //            every input point
 //   emit     emitted records gathered into sorted order with the flag counts, then filter_compact_records with the
-//            sorted input indices as index_in
-//   lists    inliers and outliers: two ordered compactions of the status over the input
+//            sorted input indices as index_in (in the chain's stage, their scan indices: gr_scan_index_kernel)
+//   lists    inliers and outliers: two ordered compactions of the status over the input (the own handle only)
 // One read-back, at the end: the per-axis bounds (the span check), the number emitted and the two list lengths.
 // Compiled with -fmad=false.
 #include <limits.h>
@@ -182,6 +182,14 @@ gr_list_scatter_kernel(const uint8_t* __restrict__ status, int n, int want, cons
   if (blockIdx.x == 0 && threadIdx.x == 0) *m = tile_off[gridDim.x];
 }
 
+// scan[k] = index_in[order[k]]: the scan index of the point at sorted position k, when the input is a chain stage's
+__global__ void __launch_bounds__(256)
+gr_scan_index_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ index_in, int n,
+                     uint32_t* __restrict__ scan) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) scan[k] = index_in[order[k]];
+}
+
 }  // namespace
 
 int voxel_sort(const char* pts, int n, int64_t stride, float leaf, const RadixPairs& rp, uint32_t* meta,
@@ -227,66 +235,65 @@ int gr_debug_voxel_host(const float* z, int64_t count, int iz, int32_t min_point
   return gr_voxel_status((int32_t)count, iz, max_z, min_z, min_points, height_threshold);
 }
 
-// The device buffers of one GroundRemoval.  reserve() sizes them for n records; they only grow.  The inlier and
-// outlier lists of a run are written into the *_next buffers and swapped in when the run succeeds, so that
-// inliers / outliers always hold the last successful run's.
-struct GroundRemoval {
-  FilterParams params = filter_defaults(kFilterGroundRemoval);
-  DevBuf sort, tile_cnt, voxel_start, emit, status, sorted, meta, inliers, outliers, inliers_next, outliers_next;
-  int64_t n_inliers = 0, n_outliers = 0;
+int GroundRemoval::reserve(int64_t n) {
+  SMB_RC(sort.reserve(RadixPairs::bytes(voxel_sort_stride(n), (int)n)));
+  SMB_RC(tile_cnt.reserve(4 * compact_count_bytes(n)));
+  SMB_RC(voxel_start.reserve(((size_t)n + 1) * sizeof(uint32_t)));
+  SMB_RC(emit.reserve((size_t)n));
+  SMB_RC(status.reserve((size_t)n));
+  SMB_RC(sorted.reserve((size_t)n * 20));
+  SMB_RC(meta.reserve(kGrMeta * sizeof(uint32_t)));
+  SMB_RC(inliers_next.reserve((size_t)n * sizeof(int32_t)));
+  return outliers_next.reserve((size_t)n * sizeof(int32_t));
+}
 
-  int reserve(int64_t n) {
-    SMB_RC(sort.reserve(RadixPairs::bytes(voxel_sort_stride(n), (int)n)));
-    SMB_RC(tile_cnt.reserve(4 * compact_count_bytes(n)));
-    SMB_RC(voxel_start.reserve(((size_t)n + 1) * sizeof(uint32_t)));
-    SMB_RC(emit.reserve((size_t)n));
-    SMB_RC(status.reserve((size_t)n));
-    SMB_RC(sorted.reserve((size_t)n * 20));
-    SMB_RC(meta.reserve(kGrMeta * sizeof(uint32_t)));
-    SMB_RC(inliers_next.reserve((size_t)n * sizeof(int32_t)));
-    return outliers_next.reserve((size_t)n * sizeof(int32_t));
+int GroundRemoval::run(const char* pts, int64_t n, int64_t stride, const uint32_t* index_in, float* out,
+                       uint32_t* out_index, int64_t* m, cudaStream_t s, bool lists) {
+  const float leaf = params.leaf_size;
+  const int ni = (int)n;
+  const int tiles = compact_tiles(n);
+  SMB_RC(reserve(n));
+  RadixPairs rp;
+  rp.carve(sort.p, voxel_sort_stride(n));
+  uint32_t* mt = (uint32_t*)meta.p;
+  uint32_t* tc[4];
+  for (int j = 0; j < 4; ++j) tc[j] = (uint32_t*)tile_cnt.p + (size_t)j * (tiles + 1);
+  SMB_CUDA_OK(cudaMemsetAsync(mt, 0, kGrMeta * sizeof(uint32_t), s));
+  SMB_RC(voxel_sort(pts, ni, stride, leaf, rp, mt, tc[0], (uint32_t*)voxel_start.p, s));
+  const uint32_t* order = rp.vals[0];
+  const int decide_blocks = (int)std::min<int64_t>(ceil_div(n, 8), 32 * kNumSMs);
+  gr_decide_kernel<<<decide_blocks, 256, 0, s>>>(pts, stride, order, (const uint32_t*)voxel_start.p, tc[0] + tiles,
+                                                 leaf, params.min_point_num_in_voxel, params.height_threshold,
+                                                 (uint8_t*)emit.p, (uint8_t*)status.p);
+  gr_gather_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, order, ni, (const uint8_t*)emit.p,
+                                                     (float*)sorted.p, tc[1]);
+  // the scan index of every sorted position, in the sort's free ping-pong buffer, for the scatter to carry
+  const uint32_t* scan = order;
+  if (index_in) {
+    gr_scan_index_kernel<<<ceil_div(n, 256), 256, 0, s>>>(order, index_in, ni, rp.vals[1]);
+    scan = rp.vals[1];
   }
-
-  // n >= 1 records of `stride` bytes in device memory -> out (capacity n records) and out_index (capacity n) in the
-  // map's order, *m; returns after the stream has finished.  SM_ERR_BAD_ARGUMENT: an axis whose indices other than
-  // INT_MIN span more than 2^21 - 1 voxels (the 63-bit key cannot hold them).
-  int run(const char* pts, int64_t n, int64_t stride, float* out, uint32_t* out_index, int64_t* m, cudaStream_t s) {
-    const float leaf = params.leaf_size;
-    const int ni = (int)n;
-    const int tiles = compact_tiles(n);
-    SMB_RC(reserve(n));
-    RadixPairs rp;
-    rp.carve(sort.p, voxel_sort_stride(n));
-    uint32_t* mt = (uint32_t*)meta.p;
-    uint32_t* tc[4];
-    for (int j = 0; j < 4; ++j) tc[j] = (uint32_t*)tile_cnt.p + (size_t)j * (tiles + 1);
-    SMB_CUDA_OK(cudaMemsetAsync(mt, 0, kGrMeta * sizeof(uint32_t), s));
-    SMB_RC(voxel_sort(pts, ni, stride, leaf, rp, mt, tc[0], (uint32_t*)voxel_start.p, s));
-    const uint32_t* order = rp.vals[0];
-    const int decide_blocks = (int)std::min<int64_t>(ceil_div(n, 8), 32 * kNumSMs);
-    gr_decide_kernel<<<decide_blocks, 256, 0, s>>>(pts, stride, order, (const uint32_t*)voxel_start.p, tc[0] + tiles,
-                                                   leaf, params.min_point_num_in_voxel, params.height_threshold,
-                                                   (uint8_t*)emit.p, (uint8_t*)status.p);
-    gr_gather_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, order, ni, (const uint8_t*)emit.p,
-                                                       (float*)sorted.p, tc[1]);
-    filter_compact_records((const char*)sorted.p, 20, order, ni, (const uint8_t*)emit.p, tc[1], out, out_index, mt + 8,
-                           s);
-    const std::pair<int, DevBuf*> lists[2] = {{kGrKept, &inliers_next}, {kGrGround, &outliers_next}};
+  filter_compact_records((const char*)sorted.p, 20, scan, ni, (const uint8_t*)emit.p, tc[1], out, out_index, mt + 8,
+                         s);
+  const std::pair<int, DevBuf*> list_of[2] = {{kGrKept, &inliers_next}, {kGrGround, &outliers_next}};
+  if (lists)
     for (int j = 0; j < 2; ++j)
-      flag_list((const uint8_t*)status.p, ni, lists[j].first, tc[2 + j], (int32_t*)lists[j].second->p, mt + 9 + j, s);
-    SMB_CUDA_OK(cudaGetLastError());
-    uint32_t host[11];
-    SMB_CUDA_OK(cudaMemcpyAsync(host, mt, sizeof(host), cudaMemcpyDeviceToHost, s));
-    SMB_CUDA_OK(cudaStreamSynchronize(s));
-    if (!voxel_span_ok(host)) return SM_ERR_BAD_ARGUMENT;
+      flag_list((const uint8_t*)status.p, ni, list_of[j].first, tc[2 + j], (int32_t*)list_of[j].second->p, mt + 9 + j,
+                s);
+  SMB_CUDA_OK(cudaGetLastError());
+  uint32_t host[11];
+  SMB_CUDA_OK(cudaMemcpyAsync(host, mt, sizeof(host), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  if (!voxel_span_ok(host)) return SM_ERR_BAD_ARGUMENT;
+  if (lists) {
     std::swap(inliers, inliers_next);
     std::swap(outliers, outliers_next);
     n_inliers = host[9];
     n_outliers = host[10];
-    *m = (int64_t)host[8];
-    return SM_OK;
   }
-};
+  *m = (int64_t)host[8];
+  return SM_OK;
+}
 
 }  // namespace smb
 
@@ -323,7 +330,8 @@ int sm_ground_removal_run_device(sm_ground_removal* h, const float* dev_points, 
     SMB_RC(h->cuda_fail(h->host_idx.reserve((size_t)n * sizeof(int32_t))));
     idx = (uint32_t*)h->host_idx.p;
   }
-  const int rc = h->f.run((const char*)dev_points, n, stride_bytes, dev_out, idx, m_out, (cudaStream_t)cuda_stream);
+  const int rc = h->f.run((const char*)dev_points, n, stride_bytes, nullptr, dev_out, idx, m_out,
+                          (cudaStream_t)cuda_stream, true);
   if (rc == SM_ERR_BAD_ARGUMENT)
     return h->fail(rc, "the voxel indices of an axis span more than 2^21 - 1 voxels (the 63-bit voxel key)");
   return h->cuda_fail(rc);

@@ -3,6 +3,7 @@
 #define SM_B200_KERNELS_H_
 
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include <utility>
@@ -406,25 +407,28 @@ void m2dp_axes(const float* cov6, float* E9);
 void m2dp_descriptor(const int* A, const double* G, int rows, int cols, float* out);
 
 // ---- filters.cu --------------------------------------------------------------------------
-// pre_processers::filter::Factory (pre_processors/filter_factory.cc:63-106) over the six filters built here
-// kFilterStatisticRemoval and kFilterGroundRemoval are not kinds of the chain (sm_filter_chain_add refuses them): each
-// runs behind its own handle, sm_statistic_removal (statistic_removal.cu) and sm_ground_removal (ground_removal.cu),
-// built like the chain's on the handle core of record_filter.h.
+// pre_processers::filter::Factory (pre_processors/filter_factory.cc:63-106) over the six filters built here, and
+// with the chain option all_filters over the reference's other three: kFilterStatisticRemoval, kFilterGroundRemoval
+// and kFilterVoxelGrid, whose stages (StatisticRemoval, GroundRemoval, VoxelGrid below) also run behind their own
+// entry points, sm_statistic_removal (statistic_removal.cu), sm_ground_removal (ground_removal.cu) and
+// sm_voxel_grid_filter (voxel_filter.cu).
 enum FilterKind : int {
   kFilterRange = 0, kFilterAxisRange, kFilterBoundingBoxRemoval, kFilterRandomSampler, kFilterRangeImage,
-  kFilterGroundRemoval2, kFilterStatisticRemoval, kFilterGroundRemoval
+  kFilterGroundRemoval2, kFilterStatisticRemoval, kFilterGroundRemoval, kFilterVoxelGrid
 };
 // One filter of the chain: the members of the reference class of its kind under their XML names, at the
 // constructors' defaults (filter_range.cc:31-38, filter_axis_range.h:56-57, filter_bounding_box.h,
 // filter_random_sample.cc:29, filter_range_image.cc:29-37, filter_ground_removal2.cc:74-89,
-// filter_statistic_removal.h, filter_ground_removal.cc:29-39).  Passed to the kernels by value.  StatisticRemoval's
-// two members share Range's storage and GroundRemoval's three AxisRange's: a FilterParams holds the parameters of one
-// kind, and its size and layout are what the chain's kernels take.
+// filter_statistic_removal.h, filter_ground_removal.cc:29-39, filter_voxel_grid.h:55).  Passed to the kernels by
+// value.  StatisticRemoval's two members and VoxelGrid's one share Range's storage and GroundRemoval's three
+// AxisRange's: a FilterParams holds the parameters of one kind, and its size and layout are what the chain's kernels
+// take.
 struct FilterParams {
   int kind;
   union {
     struct { float min_range, max_range; };                         // Range
     struct { int32_t point_num_meank; float std_mul; };             // StatisticRemoval
+    struct { float voxel_size; };                                   // VoxelGrid
   };
   union {
     struct { float min, max; int axis_index; };                     // AxisRange
@@ -522,6 +526,56 @@ void flag_list(const uint8_t* flag, int n, int want, uint32_t* tile_cnt, int32_t
 void gr_debug_index_host(const float* p, float leaf, int* ixyz);
 int gr_debug_voxel_host(const float* z, int64_t count, int iz, int32_t min_points, float height_threshold,
                         float* max_min);
+// The device buffers and parameters of one GroundRemoval, shared by sm_ground_removal_* and the chain's stage.
+// reserve() sizes the buffers for n records; they only grow.  run(): n >= 1 records of `stride` bytes in device memory
+// (index_in: their scan indices, null = identity) -> out (capacity n records) and out_index (capacity n) in the map's
+// order, each index the scan index of the record's input point, *m; returns after the stream has finished.  With
+// `lists`, the run's inlier and outlier lists (input indices, ascending) are written into the *_next buffers and
+// swapped in when it succeeds, so that inliers / outliers always hold the last successful run's.
+// SM_ERR_BAD_ARGUMENT: an axis whose indices other than INT_MIN span more than 2^21 - 1 voxels (the 63-bit key cannot
+// hold them); out and out_index have been written then.
+struct GroundRemoval {
+  FilterParams params = filter_defaults(kFilterGroundRemoval);
+  DevBuf sort, tile_cnt, voxel_start, emit, status, sorted, meta, inliers, outliers, inliers_next, outliers_next;
+  int64_t n_inliers = 0, n_outliers = 0;
+  int reserve(int64_t n);
+  int run(const char* pts, int64_t n, int64_t stride, const uint32_t* index_in, float* out, uint32_t* out_index,
+          int64_t* m, cudaStream_t s, bool lists);
+};
+
+// ---- statistic_removal.cu ----------------------------------------------------------------------
+// The device buffers and parameters of one StatisticRemoval, shared by sm_statistic_removal_* and the chain's stage.
+// reserve() sizes them for n records; they only grow.  run(): n >= 1 records of `stride` bytes in device memory
+// (index_in: their scan indices, null = identity) -> the kept records in input order in out (capacity n records),
+// their scan indices in out_index (capacity n), *m; returns after the stream has finished.  The caller checks k_ok()
+// first.  SM_ERR_CHECK_FAILED: 1..K finite points; SM_ERR_BAD_ARGUMENT: more finite points than a 24-level tree holds;
+// out and out_index are untouched then.
+struct StatisticRemoval {
+  FilterParams params = filter_defaults(kFilterStatisticRemoval);
+  DevBuf flag, tile_cnt, coord, index, dist, bins, stats, count, kdws;
+  KdCompactTree tree;
+  int64_t last_n = 0;                                  // points of the last run (its distances are in dist)
+  double host_stats[4] = {NAN, NAN, NAN, 0.0};
+  bool k_ok() const;                                   // point_num_meank in 1..63: K + 1 neighbours within 64
+  int reserve(int64_t n);
+  int run(const char* pts, int64_t n, int64_t stride, const uint32_t* index_in, float* out, uint32_t* out_index,
+          int64_t* m, cudaStream_t s);
+};
+
+// ---- voxel_filter.cu ---------------------------------------------------------------------------
+// The device buffers of one VoxelGrid::Filter (filter_voxel_grid.cc:37-78), shared by sm_voxel_grid_filter and the
+// chain's stage.  reserve() sizes them for n records; they only grow.  run(): n >= 1 records of `stride` (>= 16)
+// bytes in device memory, x, y, z, intensity first -> one record per voxel in out (capacity n records), in ascending
+// (ix, iy, iz), the voxel's mean with factor 0, *m; returns after the stream has finished.  out_index (optional,
+// capacity n): the scan index (index_in, null = identity) of each voxel's first member in input order.  Points with
+// a NaN / inf quotient are dropped.  voxel > 1e-6 (the caller checks).  SM_ERR_BAD_ARGUMENT: the finite points span
+// 2^21 voxels or more along an axis; out and out_index have been written then.
+struct VoxelGrid {
+  DevBuf sort, tile_cnt, voxel_start, sorted, meta;
+  int reserve(int64_t n);
+  int run(const char* pts, int64_t n, int64_t stride, float voxel, const uint32_t* index_in, float* out,
+          uint32_t* out_index, int64_t* m, cudaStream_t s);
+};
 
 // ---- plane_sampler.cu --------------------------------------------------------------------------
 // what Detect did with a voxel (plane_detector.h:103-152): skipped (fewer than min points), the z-range rule (iz <= 0)
@@ -578,13 +632,20 @@ struct DepthCluster {
 };
 
 // The device buffers and the stages of one filter chain.  reserve() sizes the buffers for n records and the chain's
-// RangeImage / GroundRemoval2 grids; they only grow.  run() applies the filters in order to n records of `stride`
-// bytes in device memory and leaves the inliers, packed, in `out` (capacity n records) with their indices in the
-// input scan in `out_index` (optional); it returns after the stream has finished, with the count in *m.
+// RangeImage / GroundRemoval2 grids; they only grow, and so do those of the GroundRemoval, StatisticRemoval and
+// VoxelGrid stages.  run() applies the filters in order to n records of `stride` bytes in device memory and leaves
+// the records of the last stage, packed, in `out` (capacity n records) with their indices in the input scan in
+// `out_index` (optional), in emission order; it returns after the stream has finished, with the count in *m.  On
+// SM_ERR_BAD_ARGUMENT / SM_ERR_CHECK_FAILED, `fault` says why.
 struct FilterChain {
   std::vector<FilterParams> filters;
   uint32_t sample_seed = 1;
+  uint32_t all_filters = 0;          // chain option: sm_filter_chain_add accepts the three kinds above
+  const char* fault = "";
   DevBuf rec[2], idx[2], flag, block_cnt, count, pixel, owner, sort, cell_of, pt, member, cells, occ, work, lines;
+  GroundRemoval ground;
+  StatisticRemoval statistic;
+  VoxelGrid voxel;
   // the intermediates of the last GroundRemoval2 stage (test hook sm_debug_filter_ground_removal2)
   struct Gr2View {
     const uint32_t* cell_of; const uint8_t* member; const uint32_t* cell_cnt; const float2* cell_min;
@@ -601,7 +662,15 @@ struct FilterChain {
                         float* out, uint32_t* index_out, cudaStream_t s);
   int ground_removal2_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,
                             float* out, uint32_t* index_out, cudaStream_t s);
+  // GroundRemoval, StatisticRemoval and VoxelGrid; *m = the stage's count
+  int record_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride, float* out,
+                   uint32_t* index_out, int64_t* m, cudaStream_t s);
   int stage_end(int first) const;   // one past the last filter of the stage that starts at `first`
+  int bad_grid() { fault = "a RangeImage or GroundRemoval2 grid size the chain cannot run"; return SM_ERR_BAD_ARGUMENT; }
+  int check_failed() {
+    fault = "Check failed: an inverted BoundingBoxRemoval box or line.start[0] < line.end[0]";
+    return SM_ERR_CHECK_FAILED;
+  }
 };
 
 }  // namespace smb

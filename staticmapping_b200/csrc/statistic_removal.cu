@@ -12,7 +12,8 @@
 //   stats   sum and sum of squares of the n distances, each the exact sum rounded once to double (per-exponent int64
 //           bins, shared then global integer atomics, one thread to finish); mean, stddev and threshold stay on the
 //           device.
-//   select  keep iff !(distance > threshold), then the chain's ordered scatter of whole records.  Read back: m.
+//   select  keep iff !(distance > threshold), then the chain's ordered scatter of whole records, which carries the scan
+//           indices of a chain stage's input.  Read back: m.
 // Compiled with -fmad=false.
 #include <math.h>
 #include <string.h>
@@ -128,71 +129,63 @@ sr_select_kernel(const float* __restrict__ dist, int n, const double* __restrict
 
 }  // namespace
 
-// The device buffers of one StatisticRemoval and its stages.  reserve() sizes them for n records; they only grow.
-struct StatisticRemoval {
-  FilterParams params = filter_defaults(kFilterStatisticRemoval);
-  DevBuf flag, tile_cnt, coord, index, dist, bins, stats, count, kdws;
-  KdCompactTree tree;
-  int64_t last_n = 0;                                  // points of the last run (its distances are in dist)
-  double host_stats[4] = {NAN, NAN, NAN, 0.0};
+bool StatisticRemoval::k_ok() const { return params.point_num_meank >= 1 && params.point_num_meank <= kSrMaxMeanK; }
 
-  int reserve(int64_t n) {
-    SMB_RC(flag.reserve((size_t)n));
-    SMB_RC(tile_cnt.reserve(compact_count_bytes(n)));
-    SMB_RC(coord.reserve((size_t)3 * sr_pad64(n) * sizeof(double)));
-    SMB_RC(index.reserve((size_t)n * sizeof(uint32_t)));
-    SMB_RC(dist.reserve((size_t)n * sizeof(float)));
-    SMB_RC(bins.reserve(2 * kSrBins * sizeof(unsigned long long)));
-    SMB_RC(stats.reserve(4 * sizeof(double)));
-    return count.reserve(2 * sizeof(uint32_t));
-  }
+int StatisticRemoval::reserve(int64_t n) {
+  SMB_RC(flag.reserve((size_t)n));
+  SMB_RC(tile_cnt.reserve(compact_count_bytes(n)));
+  SMB_RC(coord.reserve((size_t)3 * sr_pad64(n) * sizeof(double)));
+  SMB_RC(index.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(dist.reserve((size_t)n * sizeof(float)));
+  SMB_RC(bins.reserve(2 * kSrBins * sizeof(unsigned long long)));
+  SMB_RC(stats.reserve(4 * sizeof(double)));
+  return count.reserve(2 * sizeof(uint32_t));
+}
 
-  // n >= 1 records of `stride` bytes in device memory -> out (capacity n records), out_index (capacity n) and *m;
-  // returns after the stream has finished.  SM_ERR_CHECK_FAILED (outputs untouched): 1..K finite points.
-  int run(const char* pts, int64_t n, int64_t stride, float* out, uint32_t* out_index, int64_t* m, cudaStream_t s) {
-    const int K = params.point_num_meank;
-    const int ni = (int)n;
-    const int tiles = compact_tiles(n);
-    const int64_t cs = sr_pad64(n);
-    SMB_RC(reserve(n));
-    last_n = 0;
-    uint32_t* cnt = (uint32_t*)count.p;
-    uint32_t* tc = (uint32_t*)tile_cnt.p;
-    SMB_CUDA_OK(cudaMemsetAsync(bins.p, 0, 2 * kSrBins * sizeof(unsigned long long), s));
-    sr_finite_count_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, ni, (uint8_t*)flag.p, tc);
-    compact_scan(tc, tiles, s);
-    sr_pack_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, ni, (const uint8_t*)flag.p, tc, (double*)coord.p, cs,
-                                                     (uint32_t*)index.p, (float*)dist.p, cnt);
-    SMB_CUDA_OK(cudaGetLastError());
-    uint32_t nf = 0;                                   // sizes the tree
-    SMB_CUDA_OK(cudaMemcpyAsync(&nf, cnt, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    SMB_CUDA_OK(cudaStreamSynchronize(s));
-    if (nf >= 1 && nf <= (uint32_t)K) return SM_ERR_CHECK_FAILED;   // PCL reads past its k-list there
-    if (nf > 0) {
-      if (kd_num_levels((int)nf, 8) > 24) return SM_ERR_BAD_ARGUMENT;
-      SMB_RC(tree.reserve((int)nf, 8, KdCompactTree::kIds));
-      KdWorkspace ws;
-      SMB_RC(ws.carve(kdws, (int)nf, 8));
-      SMB_RC(tree.build((const double*)coord.p, nullptr, cs, (int)nf, 8, ws, s));
-      SMB_RC(knn_mean_distance_query(tree.view(), (const double*)coord.p, cs, (int)nf, K, (const uint32_t*)index.p,
-                                     (float*)dist.p, s));
-    }
-    const int bin_blocks = (int)std::min<int64_t>(ceil_div(n, kSrBinThreads), 4 * kNumSMs);
-    sr_bins_kernel<<<bin_blocks, kSrBinThreads, 0, s>>>((const float*)dist.p, ni, (unsigned long long*)bins.p);
-    sr_finish_kernel<<<1, 32, 0, s>>>((const unsigned long long*)bins.p, cnt, params.std_mul, (double*)stats.p);
-    sr_select_kernel<<<tiles, kCompactThreads, 0, s>>>((const float*)dist.p, ni, (const double*)stats.p,
-                                                       (uint8_t*)flag.p, tc);
-    filter_compact_records(pts, stride, nullptr, ni, (const uint8_t*)flag.p, tc, out, out_index, cnt + 1, s);
-    SMB_CUDA_OK(cudaGetLastError());
-    uint32_t kept = 0;
-    SMB_CUDA_OK(cudaMemcpyAsync(&kept, cnt + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    SMB_CUDA_OK(cudaMemcpyAsync(host_stats, stats.p, 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
-    SMB_CUDA_OK(cudaStreamSynchronize(s));
-    last_n = n;
-    *m = (int64_t)kept;
-    return SM_OK;
+int StatisticRemoval::run(const char* pts, int64_t n, int64_t stride, const uint32_t* index_in, float* out,
+                          uint32_t* out_index, int64_t* m, cudaStream_t s) {
+  const int K = params.point_num_meank;
+  const int ni = (int)n;
+  const int tiles = compact_tiles(n);
+  const int64_t cs = sr_pad64(n);
+  SMB_RC(reserve(n));
+  last_n = 0;
+  uint32_t* cnt = (uint32_t*)count.p;
+  uint32_t* tc = (uint32_t*)tile_cnt.p;
+  SMB_CUDA_OK(cudaMemsetAsync(bins.p, 0, 2 * kSrBins * sizeof(unsigned long long), s));
+  sr_finite_count_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, ni, (uint8_t*)flag.p, tc);
+  compact_scan(tc, tiles, s);
+  sr_pack_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, ni, (const uint8_t*)flag.p, tc, (double*)coord.p, cs,
+                                                   (uint32_t*)index.p, (float*)dist.p, cnt);
+  SMB_CUDA_OK(cudaGetLastError());
+  uint32_t nf = 0;                                   // sizes the tree
+  SMB_CUDA_OK(cudaMemcpyAsync(&nf, cnt, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  if (nf >= 1 && nf <= (uint32_t)K) return SM_ERR_CHECK_FAILED;   // PCL reads past its k-list there
+  if (nf > 0) {
+    if (kd_num_levels((int)nf, 8) > 24) return SM_ERR_BAD_ARGUMENT;
+    SMB_RC(tree.reserve((int)nf, 8, KdCompactTree::kIds));
+    KdWorkspace ws;
+    SMB_RC(ws.carve(kdws, (int)nf, 8));
+    SMB_RC(tree.build((const double*)coord.p, nullptr, cs, (int)nf, 8, ws, s));
+    SMB_RC(knn_mean_distance_query(tree.view(), (const double*)coord.p, cs, (int)nf, K, (const uint32_t*)index.p,
+                                   (float*)dist.p, s));
   }
-};
+  const int bin_blocks = (int)std::min<int64_t>(ceil_div(n, kSrBinThreads), 4 * kNumSMs);
+  sr_bins_kernel<<<bin_blocks, kSrBinThreads, 0, s>>>((const float*)dist.p, ni, (unsigned long long*)bins.p);
+  sr_finish_kernel<<<1, 32, 0, s>>>((const unsigned long long*)bins.p, cnt, params.std_mul, (double*)stats.p);
+  sr_select_kernel<<<tiles, kCompactThreads, 0, s>>>((const float*)dist.p, ni, (const double*)stats.p,
+                                                     (uint8_t*)flag.p, tc);
+  filter_compact_records(pts, stride, index_in, ni, (const uint8_t*)flag.p, tc, out, out_index, cnt + 1, s);
+  SMB_CUDA_OK(cudaGetLastError());
+  uint32_t kept = 0;
+  SMB_CUDA_OK(cudaMemcpyAsync(&kept, cnt + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(host_stats, stats.p, 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  last_n = n;
+  *m = (int64_t)kept;
+  return SM_OK;
+}
 
 }  // namespace smb
 
@@ -209,9 +202,9 @@ namespace {
 int sr_check(sm_statistic_removal* h, const void* points, int64_t n, int64_t stride_bytes, const void* out,
              const int64_t* m_out) {
   if (!h || !records_ok(points, n, stride_bytes, out, m_out)) return SM_ERR_BAD_ARGUMENT;
-  const int K = h->f.params.point_num_meank;
-  if (K < 1 || K > kSrMaxMeanK)
-    return h->fail(SM_ERR_BAD_ARGUMENT, "point_num_meank %d is outside 1..%d", K, kSrMaxMeanK);
+  if (!h->f.k_ok())
+    return h->fail(SM_ERR_BAD_ARGUMENT, "point_num_meank %d is outside 1..%d", h->f.params.point_num_meank,
+                   kSrMaxMeanK);
   return SM_OK;
 }
 }  // namespace
@@ -243,7 +236,8 @@ int sm_statistic_removal_run_device(sm_statistic_removal* h, const float* dev_po
     SMB_RC(h->cuda_fail(h->host_idx.reserve((size_t)n * sizeof(int32_t))));
     idx = (uint32_t*)h->host_idx.p;
   }
-  const int rc = h->f.run((const char*)dev_points, n, stride_bytes, dev_out, idx, m_out, (cudaStream_t)cuda_stream);
+  const int rc = h->f.run((const char*)dev_points, n, stride_bytes, nullptr, dev_out, idx, m_out,
+                          (cudaStream_t)cuda_stream);
   if (rc == SM_ERR_CHECK_FAILED)
     return h->fail(rc, "Check failed: between 1 and point_num_meank finite points (PCL reads past its k-list)");
   if (rc == SM_ERR_BAD_ARGUMENT) return h->fail(rc, "more finite points than the 24-level k-d tree holds");

@@ -8,7 +8,7 @@
 // Here: 63-bit voxel key per point -> stable radix sort (points of a voxel stay in input order)
 // -> segment heads -> points gathered into voxel order -> one warp per voxel adds the four double
 // chains in order (addends staged through shared memory, like ndt_leaf_kernel) -> one output
-// point per voxel.  Every output value is bit-identical to the reference's; the ORDER of the
+// point per voxel; in the filter chain, also the scan index of each voxel's first member.  Every output value is bit-identical to the reference's; the ORDER of the
 // output points is ascending (ix, iy, iz), whereas the reference's is the iteration order of a
 // libstdc++ unordered_map (an accident of its rehash history; nothing downstream depends on it
 // beyond summation order).  Compiled with -fmad=false.
@@ -138,10 +138,66 @@ vf_mean_kernel(const float4* __restrict__ sorted, const uint32_t* __restrict__ v
   if (lane == 4) out[5 * v + 4] = 0.0f;                                      // factor keeps its default
 }
 
+// out_index[v] = the scan index of voxel v's first member in input order (the sort is stable: its first sorted position)
+__global__ void __launch_bounds__(256)
+vf_first_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ voxel_start,
+                const uint32_t* __restrict__ n_voxels_dev, const uint32_t* __restrict__ index_in,
+                uint32_t* __restrict__ out_index) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= (int64_t)*n_voxels_dev) return;
+  const uint32_t i = order[voxel_start[v]];
+  out_index[v] = index_in ? index_in[i] : i;
+}
+
 }  // namespace
 
 // host build of the voxel index of one point (test hook sm_debug_voxel_index op 0)
 bool vf_debug_index_host(const float* p, float voxel, long long* ixyz) { return vf_index(p, voxel, &ixyz[0], &ixyz[1], &ixyz[2]); }
+
+int VoxelGrid::reserve(int64_t n) {
+  const int64_t st = (n + 63) & ~(int64_t)63;
+  SMB_RC(sort.reserve(RadixPairs::bytes(st, (int)n)));
+  SMB_RC(tile_cnt.reserve(compact_count_bytes(n)));
+  SMB_RC(voxel_start.reserve(((size_t)n + 8) * sizeof(uint32_t)));
+  SMB_RC(sorted.reserve((size_t)n * sizeof(float4)));
+  return meta.reserve(8 * sizeof(long long));
+}
+
+int VoxelGrid::run(const char* pts, int64_t n, int64_t stride, float voxel, const uint32_t* index_in, float* out,
+                   uint32_t* out_index, int64_t* m, cudaStream_t s) {
+  const int ni = (int)n;
+  const int tiles = compact_tiles(n);
+  const int64_t st = (n + 63) & ~(int64_t)63;
+  SMB_RC(reserve(n));
+  RadixPairs rp;
+  rp.carve(sort.p, st);
+  uint32_t* tc = (uint32_t*)tile_cnt.p;
+  uint32_t* vs = (uint32_t*)voxel_start.p;
+  float4* sd = (float4*)sorted.p;
+  long long* mt = (long long*)meta.p;
+  const long long meta_init[8] = {LLONG_MAX, LLONG_MAX, LLONG_MAX, 0, 0, 0, 0, 0};
+  SMB_CUDA_OK(cudaMemcpyAsync(mt, meta_init, sizeof(meta_init), cudaMemcpyHostToDevice, s));
+  vf_min_kernel<<<ceil_div(n, 256), 256, 0, s>>>(pts, stride, ni, voxel, mt);
+  vf_key_kernel<<<ceil_div(n, 256), 256, 0, s>>>(pts, stride, ni, voxel, rp.keys[0], rp.vals[0], mt);
+  SMB_RC(radix_sort_pairs_u64(rp.keys[0], rp.vals[0], rp.keys[1], rp.vals[1], ni, 1, st, rp.scratch, s, 8));
+  // 8 passes: the sorted pairs are back in the first buffers
+  vf_heads_count_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], ni, tc);
+  compact_scan(tc, tiles, s);                                                   // tc[tiles] = number of voxels
+  vf_heads_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], ni, tc, vs, mt);
+  vf_gather_kernel<<<ceil_div(n, 256), 256, 0, s>>>(pts, stride, rp.vals[0], ni, sd);
+  vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sd, vs, tc + tiles, out);
+  if (out_index) vf_first_kernel<<<ceil_div(n, 256), 256, 0, s>>>(rp.vals[0], vs, tc + tiles, index_in, out_index);
+  SMB_CUDA_OK(cudaGetLastError());
+  uint32_t voxels = 0;
+  long long host_meta[8] = {0};
+  SMB_CUDA_OK(cudaMemcpyAsync(&voxels, tc + tiles, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(host_meta, mt, sizeof(host_meta), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  if (host_meta[4]) return SM_ERR_BAD_ARGUMENT;   // the finite points span 2^21 voxels or more along an axis
+  *m = (int64_t)voxels;
+  return SM_OK;
+}
+
 }  // namespace smb
 
 using namespace smb;
@@ -154,50 +210,16 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   SMB_RC(select_device(device));
   *m_out = 0;
   if (n == 0) return SM_OK;
-  const int ni = (int)n;
-  const int tiles = compact_tiles(n);
-  const int64_t st = (n + 63) & ~(int64_t)63;
   const size_t in_bytes = (size_t)n * (size_t)stride_bytes;
-  size_t bytes = in_bytes + 256;
-  bytes += 2 * st * sizeof(uint64_t) + 2 * st * sizeof(uint32_t);            // keys, order (ping-pong)
-  bytes += radix_sort_scratch_bytes(ni, 1) + 256;
-  bytes += compact_count_bytes(n) + ((size_t)n + 8) * sizeof(uint32_t);                 // tile counts, voxel_start
-  bytes += (size_t)n * sizeof(float4) + (size_t)n * 5 * sizeof(float) + 1024;
-  DevBuf buf;
-  SMB_RC(buf.reserve(bytes));
-  char* cur = (char*)buf.p;
-  auto take = [&](size_t b) { char* p = cur; cur += (b + 255) & ~(size_t)255; return p; };
-  char* d_in = take(in_bytes);
-  uint64_t* keys0 = (uint64_t*)take(st * sizeof(uint64_t));
-  uint64_t* keys1 = (uint64_t*)take(st * sizeof(uint64_t));
-  uint32_t* ord0 = (uint32_t*)take(st * sizeof(uint32_t));
-  uint32_t* ord1 = (uint32_t*)take(st * sizeof(uint32_t));
-  uint32_t* scratch = (uint32_t*)take(radix_sort_scratch_bytes(ni, 1));
-  uint32_t* tile_cnt = (uint32_t*)take(compact_count_bytes(n));
-  uint32_t* voxel_start = (uint32_t*)take(((size_t)n + 8) * sizeof(uint32_t));
-  float4* sorted = (float4*)take((size_t)n * sizeof(float4));
-  float* d_out = (float*)take((size_t)n * 5 * sizeof(float));
-  long long* meta = (long long*)take(256);
+  DevBuf d_in, d_out;
+  VoxelGrid vg;
+  SMB_RC(d_in.reserve(in_bytes));
+  SMB_RC(d_out.reserve((size_t)n * 20));
   cudaStream_t s = nullptr;
-  const long long meta_init[8] = {LLONG_MAX, LLONG_MAX, LLONG_MAX, 0, 0, 0, 0, 0};
-  SMB_CUDA_OK(cudaMemcpyAsync(d_in, points, in_bytes, cudaMemcpyHostToDevice, s));
-  SMB_CUDA_OK(cudaMemcpyAsync(meta, meta_init, sizeof(meta_init), cudaMemcpyHostToDevice, s));
-  vf_min_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ni, voxel_size, meta);
-  vf_key_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ni, voxel_size, keys0, ord0, meta);
-  SMB_RC(radix_sort_pairs_u64(keys0, ord0, keys1, ord1, ni, 1, st, scratch, s, 8));   // 8 passes: result back in [0]
-  vf_heads_count_kernel<<<tiles, kCompactThreads, 0, s>>>(keys0, ni, tile_cnt);
-  compact_scan(tile_cnt, tiles, s);                                                   // tile_cnt[tiles] = number of voxels
-  vf_heads_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(keys0, ni, tile_cnt, voxel_start, meta);
-  vf_gather_kernel<<<ceil_div(n, 256), 256, 0, s>>>(d_in, stride_bytes, ord0, ni, sorted);
-  vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sorted, voxel_start, tile_cnt + tiles, d_out);
-  uint32_t m = 0;
-  long long host_meta[8] = {0};
-  SMB_CUDA_OK(cudaGetLastError());
-  SMB_CUDA_OK(cudaMemcpyAsync(&m, tile_cnt + tiles, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaMemcpyAsync(host_meta, meta, sizeof(host_meta), cudaMemcpyDeviceToHost, s));
-  SMB_CUDA_OK(cudaStreamSynchronize(s));
-  if (host_meta[4]) return SM_ERR_BAD_ARGUMENT;   // the finite points span 2^21 voxels or more along an axis
-  if (m > 0) SMB_CUDA_OK(cudaMemcpy(out, d_out, (size_t)m * 5 * sizeof(float), cudaMemcpyDeviceToHost));
-  *m_out = (int64_t)m;
+  SMB_CUDA_OK(cudaMemcpyAsync(d_in.p, points, in_bytes, cudaMemcpyHostToDevice, s));
+  int64_t m = 0;
+  SMB_RC(vg.run((const char*)d_in.p, n, stride_bytes, voxel_size, nullptr, (float*)d_out.p, nullptr, &m, s));
+  if (m > 0) SMB_CUDA_OK(cudaMemcpy(out, d_out.p, (size_t)m * 5 * sizeof(float), cudaMemcpyDeviceToHost));
+  *m_out = m;
   return SM_OK;
 }

@@ -1,8 +1,9 @@
 """pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
 chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
-deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster.  StatisticRemoval,
-PCL's statistical outlier removal, GroundRemoval, the voxel height-range ground filter, and the submap sampler
-RandomSamplerWithPlaneDetect run on their own handles (sm_statistic_removal_*, sm_ground_removal_*,
+deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster; with
+Factory.SetAllFilters(True) also StatisticRemoval, GroundRemoval and VoxelGrid.  StatisticRemoval, PCL's statistical
+outlier removal, GroundRemoval, the voxel height-range ground filter, and the submap sampler
+RandomSamplerWithPlaneDetect also run on their own handles (sm_statistic_removal_*, sm_ground_removal_*,
 sm_plane_sampler_*).  There is no CPU fallback."""
 from __future__ import annotations
 
@@ -107,7 +108,9 @@ class _RecordFilter:
 
 class Factory(_RecordFilter):
     """filter::Factory.  InitFromXmlText / InitFromXmlNode take the <filters> node; SetInputCloud + Filter run the
-    chain on the GPU.  `Filter` returns the inlier InnerCloud; Inliers() / Outliers() are indices into the input."""
+    chain on the GPU.  `Filter` returns the InnerCloud of the last filter's records; Inliers() are their indices into
+    the input in emission order (ascending unless the chain holds GroundRemoval or VoxelGrid, whose records are a
+    voxel's and carry its first member's index) and Outliers() the other input indices, ascending."""
     _abi = "sm_filter_chain"
 
     def __init__(self, device: int = 0):
@@ -117,9 +120,8 @@ class Factory(_RecordFilter):
 
     def InitFromXmlNode(self, filters_node):
         """filter_factory.cc:63-81.  A name the reference does not register is skipped with a message; a <param> with
-        an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57), and so does a filter
-        the reference has but this chain does not build: GroundRemoval (see GroundRemoval), StatisticRemoval (see
-        StatisticRemoval) and VoxelGrid."""
+        an unknown name or without a type of 0 / 1 raises CheckFailure (filter_interface.cc:57), and so does
+        GroundRemoval, StatisticRemoval or VoxelGrid unless SetAllFilters(True) was called before."""
         if isinstance(filters_node, (str, bytes)):
             filters_node = ET.fromstring(filters_node)
         for node in filters_node.findall("filter"):
@@ -143,6 +145,12 @@ class Factory(_RecordFilter):
 
     def SetSampleSeed(self, seed):
         self._lib.sm_filter_chain_set_option(self._h, b"sample_seed", str(int(seed)).encode())
+
+    def SetAllFilters(self, flag):
+        """True: the filters added from now on may also be GroundRemoval, StatisticRemoval and VoxelGrid, whose chain
+        stages are the GPU filters of GroundRemoval, StatisticRemoval and VoxelGridFilter (include/sm_b200.h, the
+        all_filters option); False restores the refusal.  Filters already added stay."""
+        self._lib.sm_filter_chain_set_option(self._h, b"all_filters", b"1" if flag else b"0")
 
     def DepthCluster(self, filter_index, cloud):
         """RangeImage::DepthCluster (filter_range_image.cc:143-173) after SetInputCloud(cloud) + Filter on the chain's
