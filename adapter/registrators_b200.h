@@ -204,6 +204,18 @@ class IcpUsingPointMatcherB200 : public FloatCloudMatcherB200<SM_TYPE_ICP_PM> {
   // own float box mean and smallest-eigenvector normal.  Applies from the next Align; a value outside 0..1
   // CHECK-fails.
   void SetSurfaceNormals(int mode) { CheckRc(sm_set_pm_surface_normals(handle_, mode)); }
+  // The reading filter's random stream (sm_pm_reading_sampler): SM_PM_SAMPLING_HASH, the default, is a counter hash;
+  // SM_PM_SAMPLING_GLIBC_RAND is glibc's rand() after srand(sample_seed), drawn from this matcher's stream position,
+  // which every Align in that mode advances by the reading cloud's size.  To reproduce a process that shares one
+  // rand() stream between matchers, hand each matcher the position the process had reached before its Align.
+  // A mode outside 0..1 or a negative position CHECK-fails.
+  void SetReadingSampler(int mode) { CheckRc(sm_set_pm_reading_sampler(handle_, mode)); }
+  int64_t GetRandPosition() const {
+    int64_t position = 0;
+    CheckRc(sm_get_pm_rand_position(handle_, &position));
+    return position;
+  }
+  void SetRandPosition(int64_t position) { CheckRc(sm_set_pm_rand_position(handle_, position)); }
 };
 
 // MotionCompensation (builder/map_builder.cc:232-257) on the GPU: same signature as the static

@@ -76,7 +76,8 @@ int sm_destroy(sm_handle* h);
  * same module chain (DESIGN.md section 4e): bit-checked against a composition of this repository's oracle
  * pieces, and shown to lie within the literal chain's own call-to-call variation by a restatement of
  * libpointmatcher's filters (tests/pyref.py icp_pm_literal, tests/test_oracle_vs_python_restatement.py).
- * sm_set_pm_surface_normals switches its reference filter to libpointmatcher's own eigenvector normals.
+ * sm_set_pm_surface_normals switches its reference filter to libpointmatcher's own eigenvector normals, and
+ * sm_set_pm_reading_sampler its reading filter to glibc's rand() stream at a given seed and stream position.
  * SM_TYPE_ICP_PM (stand-in for IcpUsingPointMatcher's default libpointmatcher chain,
  * icp_pointmatcher.cc:166-247; float clouds through the _f32 setters) registers no option in the
  * reference either; the engine accepts the IcpFast names (max_iteration defaults to 150, :214)
@@ -170,6 +171,38 @@ enum sm_pm_surface_normals {
   SM_PM_NORMALS_EIGENVECTOR = 1
 };
 int sm_set_pm_surface_normals(sm_handle* h, int32_t mode);
+/* The reading filter of SM_TYPE_ICP_PM, libpointmatcher 1.3.1's RandomSamplingDataPointsFilter (prob =
+ * reading_sample_prob, icp_pointmatcher.cc:173), which keeps column i iff (float)rand() / (float)RAND_MAX < prob,
+ * drawing once per column on every ICP::compute.
+ *   HASH (the default)  a counter hash instead of rand(): point i is kept iff murmur3_fmix32(i * 0x9E3779B9 +
+ *             sample_seed) < prob * 2^32.  The filtered reading cloud is kept across Aligns until the source cloud,
+ *             reading_sample_prob or sample_seed changes.
+ *   GLIBC_RAND  glibc's rand() itself: the TYPE_3 additive-feedback generator after srand((unsigned)sample_seed)
+ *             (the default sample_seed 1 is glibc's default seed), read from the handle's stream position (below).
+ *             Every Align filters the reading cloud anew: point i takes draw position + i, non-finite points
+ *             included, and the position then advances by the number of reading points.  Draw p is reached in
+ *             O(log p) (DESIGN.md section 4e), and the keep test is exact: the draw rounded to float and divided by
+ *             2^31, as x86 evaluates it.  With the eigenvector reference filter (sm_set_pm_surface_normals) type 1
+ *             then runs libpointmatcher's default chain's data filters themselves, given the seed and the position.
+ * Applies from the next Align on (sm_align and sm_align_batch alike).  SM_TYPE_ICP_PM only: every other type returns
+ * SM_ERR_UNSUPPORTED_TYPE and is left unchanged.  A mode outside 0..1 returns SM_ERR_BAD_ARGUMENT and leaves the
+ * setting unchanged.  Not an XML option: sm_print_options does not list it. */
+enum sm_pm_reading_sampler {
+  SM_PM_SAMPLING_HASH = 0,
+  SM_PM_SAMPLING_GLIBC_RAND = 1
+};
+int sm_set_pm_reading_sampler(sm_handle* h, int32_t mode);
+/* The GLIBC_RAND sampler's stream position: the number of rand() draws taken since srand(sample_seed).  It starts at
+ * 0, setting sample_seed resets it to 0 (as srand does), and every type-1 Align in GLIBC_RAND mode advances it by
+ * the number of reading points once the filter has run; HASH mode leaves it alone.  A negative position returns
+ * SM_ERR_BAD_ARGUMENT; an Align that would advance it past 2^63 - 1 returns SM_ERR_BAD_ARGUMENT before any work.
+ * A process running the reference draws every Align's points from ONE global stream, in the order its Aligns run.
+ * To reproduce that, give each handle the position the reference process had reached when that Align started: the
+ * previous Align's position plus its reading size, across handles.  sm_align_batch runs type-1 handles on worker
+ * threads, each from its own position, so set every handle's position before the batch.  SM_TYPE_ICP_PM only:
+ * every other type returns SM_ERR_UNSUPPORTED_TYPE and is left unchanged. */
+int sm_get_pm_rand_position(sm_handle* h, int64_t* position);
+int sm_set_pm_rand_position(sm_handle* h, int64_t position);
 /* Interface::GetType (interface.h:106). */
 int sm_get_type(const sm_handle* h);
 

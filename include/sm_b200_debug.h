@@ -30,6 +30,8 @@
  *     sm_debug_statistic_removal_distance_host   StatisticRemoval's per-point mean distance over a neighbour list
  *     sm_debug_ground_removal_index_host, sm_debug_ground_removal_voxel_host  GroundRemoval's voxel index of a point
  *                              and its decision for one voxel
+ *     sm_debug_pm_rand_window_host, sm_debug_pm_rand_advance_host, sm_debug_pm_rand_draws_host  the rand reading
+ *                              sampler's jump-ahead on glibc's rand() stream and the draws it reaches
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -47,6 +49,7 @@
  *                              squared distances of the approximate search, trim counts and mean
  *     sm_debug_pm_surface_normals  the stand-in's reference filter (NormalsPipeline) in either leaf mode: kept means,
  *                              normals and box indices, after an optional earlier build into the same owner
+ *     sm_debug_pm_rand_sample  the stand-in's reading filter with the rand sampler: keep flags and kept points
  *     sm_debug_approx_voxel_grid  ApproximateVoxelGrid's output cloud, in emission order
  *     sm_debug_gicp_covariances   the GICP covariances of a cloud
  *     sm_debug_gicp_step       correspondences, Mahalanobis matrices and cost sums of one GICP outer iteration
@@ -242,6 +245,23 @@ int sm_debug_float_tree_knn(int device, const float* cloud_3n, int64_t n, const 
 int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const float* target_3n, int64_t nt, float prob,
                        uint32_t seed, const double* T_4x4, float knn_epsilon, float ratio, int64_t* kept,
                        double* sampled_3n, double* keys_n, double* out_3);
+
+/* The generator of the rand reading sampler (sm_set_pm_reading_sampler GLIBC_RAND; csrc/icp_pm.cu, the same
+ * __host__ __device__ jump-ahead the device runs) compiled for the host, no GPU needed.  A window is 31 consecutive
+ * words of glibc's TYPE_3 additive recurrence; the window at position p is the one whose next draw is draw p.
+ *   sm_debug_pm_rand_window_host   the window at `position` after srand(seed)
+ *   sm_debug_pm_rand_advance_host  the window `steps` draws after window_31
+ *   sm_debug_pm_rand_draws_host    draws position .. position + count - 1 (rand() values), from the window at
+ *                                  `position` and then the recurrence one step at a time. */
+int sm_debug_pm_rand_window_host(uint32_t seed, int64_t position, uint32_t* window_31);
+int sm_debug_pm_rand_advance_host(const uint32_t* window_31, uint64_t steps, uint32_t* out_31);
+int sm_debug_pm_rand_draws_host(uint32_t seed, int64_t position, int64_t count, int32_t* out);
+
+/* PmStage::sample with the rand sampler as pm_align runs it: the n packed float reading points (n <= 2^24), draw i
+ * taken from position + i of srand(seed)'s stream, kept iff (float)rand() / (float)RAND_MAX < prob -> *kept,
+ * sampled_3n (3 * kept doubles in input order; capacity 3 * n) and keep_n (the device's flag of each point, 0 / 1). */
+int sm_debug_pm_rand_sample(int device, const float* reading_3n, int64_t n, float prob, uint32_t seed,
+                            int64_t position, int64_t* kept, double* sampled_3n, uint8_t* keep_n);
 
 /* The IcpUsingPointMatcher stand-in's reference filter as pm_align runs it: the packed float cloud widened into a
  * NormalsPipeline and run with `mode` (sm_pm_surface_normals).  With n_first > 0 the first cloud is run first, with

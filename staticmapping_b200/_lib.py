@@ -46,6 +46,9 @@ SIGNATURES = {
     "sm_set_ndt_search_method": (C.c_int, [_VP, C.c_int32]),
     "sm_set_icp_error_minimizer": (C.c_int, [_VP, C.c_int32]),
     "sm_set_pm_surface_normals": (C.c_int, [_VP, C.c_int32]),
+    "sm_set_pm_reading_sampler": (C.c_int, [_VP, C.c_int32]),
+    "sm_get_pm_rand_position": (C.c_int, [_VP, _VP]),
+    "sm_set_pm_rand_position": (C.c_int, [_VP, C.c_int64]),
     "sm_get_type": (C.c_int, [_VP]),
     "sm_set_input_source": (C.c_int, [_VP, _VP, C.c_int64]),
     "sm_set_input_target": (C.c_int, [_VP, _VP, _VP, C.c_int64]),
@@ -143,6 +146,10 @@ SIGNATURES = {
     "sm_debug_float_tree_knn": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, _VP, _VP]),
     "sm_debug_pm_stages": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_float, C.c_uint32, _VP, C.c_float,
                                      C.c_float, _VP, _VP, _VP, _VP]),
+    "sm_debug_pm_rand_window_host": (C.c_int, [C.c_uint32, C.c_int64, _VP]),
+    "sm_debug_pm_rand_advance_host": (C.c_int, [_VP, C.c_uint64, _VP]),
+    "sm_debug_pm_rand_draws_host": (C.c_int, [C.c_uint32, C.c_int64, C.c_int64, _VP]),
+    "sm_debug_pm_rand_sample": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_float, C.c_uint32, C.c_int64, _VP, _VP, _VP]),
     "sm_debug_pm_surface_normals": (C.c_int, [C.c_int, C.c_int32, _VP, C.c_int64, _VP, C.c_int64, _VP, _VP, _VP, _VP]),
     "sm_debug_icp_iteration": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.c_int64, _VP, C.c_float, C.c_float,
                                          C.c_int32, C.c_int32, C.c_int32] + [_VP] * 16),

@@ -363,13 +363,28 @@ struct NormalsPipeline {
 };
 
 // ---- icp_pm.cu -------------------------------------------------------------------------
+// glibc's rand() stream (TYPE_3, degree 31) as 31 consecutive words of its additive recurrence: the window at
+// position p (p draws taken since srand) is the one whose next draw is draw p.
+constexpr int kPmRandDeg = 31;
+struct PmRandWindow { uint32_t w[kPmRandDeg]; };
+// the window at `position` after srand(seed), in O(log position) (icp_pm.cu)
+PmRandWindow pm_rand_window(uint32_t seed, uint64_t position);
+// host builds of the generator (test hooks sm_debug_pm_rand_*_host): the window m draws further on, and count draws
+void pm_rand_debug_advance_host(PmRandWindow& at, uint64_t m);
+void pm_rand_debug_draws_host(PmRandWindow at, int64_t count, int32_t* out);
+
 // The reading filter and the score pass of the IcpUsingPointMatcher stand-in (icp_pointmatcher.cc:131-148, :173),
 // with their buffers, sized by reserve() for a reading cloud of n_source points.
 struct PmStage {
   DevBuf cnt, sampled, score;   // tile counts; the kept reading points; pose, output and sort of the score pass
+  DevBuf rand_flags;            // the rand sampler's keep flags, one bit per point
   int reserve(int n_source);
-  // hash-subsample of the packed float cloud src into points(); waits for and returns the number kept
-  int sample(const float* src, int n, float prob, uint32_t seed, cudaStream_t s, uint32_t* kept);
+  // subsample of the packed float cloud src into points(); waits for and returns the number kept.  With rand null,
+  // point i is kept by the counter hash of (i, seed); with rand, by (float)rand() / (float)RAND_MAX < prob where
+  // point i takes the i-th draw from the window *rand (libpointmatcher's RandomSamplingDataPointsFilter).
+  int sample(const float* src, int n, float prob, uint32_t seed, cudaStream_t s, uint32_t* kept,
+             const PmRandWindow* rand = nullptr);
+  const uint32_t* rand_bits() const { return (const uint32_t*)rand_flags.p; }   // after a rand sample: n flag bits
   const double* points() const { return (const double*)sampled.p; }   // AoS 3xM doubles
   // the unfiltered reading moved by T (16 doubles, pinned host memory) against the target's float tree, trimmed at
   // `ratio`; waits for out3_host = mean kept distance, kept, valid

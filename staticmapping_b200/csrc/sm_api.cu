@@ -155,6 +155,8 @@ struct PmMatcher {
   F32Clouds in;
   bool src_dirty = false, tgt_dirty = false, score_tree_dirty = true;
   int surface_normals = SM_PM_NORMALS_LEAST_SQUARES;   // sm_set_pm_surface_normals
+  int reading_sampler = SM_PM_SAMPLING_HASH;           // sm_set_pm_reading_sampler
+  int64_t rand_position = 0;                           // rand() draws since srand(sample_seed)
   NormalsPipeline normals;
   PmStage stage;
   FloatTree score_tree;
@@ -478,8 +480,10 @@ int icp_align(sm_handle* h, IcpFastMatcher& f, const double* guess, double* resu
 
 // ---- IcpUsingPointMatcher stand-in (type 1) ------------------------------------------------
 // registrators/icp_pointmatcher.cc:125-247 drives libpointmatcher 1.3.1 (external, float) with
-//   reading filter    RandomSampling prob 0.9                      -> PmStage::sample (a counter
-//                     hash instead of std::rand, so the kept set is reproducible)
+//   reading filter    RandomSampling prob 0.9                      -> PmStage::sample: by default a
+//                     counter hash instead of std::rand, so the kept set is reproducible; with
+//                     sm_set_pm_reading_sampler(GLIBC_RAND) glibc's rand() stream itself, drawn from
+//                     the handle's stream position (icp_pm.cu pm_rand_flags_kernel)
 //   reference filter  SamplingSurfaceNormal knn 7, one point per box -> NormalsPipeline: by default
 //                     CalculateNormals, the reference author's own restatement of that filter
 //                     (cloud_types.cc:73-144); with sm_set_pm_surface_normals(EIGENVECTOR) the filter's
@@ -491,7 +495,7 @@ int icp_align(sm_handle* h, IcpFastMatcher& f, const double* guess, double* resu
 //   score (:131-148)  unfiltered reading moved by the result vs unfiltered reference, same matcher,
 //                     trim 0.7, exp(-mean kept distance); Align() false below 0.6 (:145)
 // It is a deterministic equivalent, not a bit-level restatement: libpointmatcher's float ICP
-// arithmetic and its rand() stream cannot be pinned from this tree.
+// arithmetic is not reproduced, and its rand() stream only in GLIBC_RAND mode, given seed and position.
 int pm_align(sm_handle* h, PmMatcher& pm, const double* guess, double* result) {
   if (pm.in.n_src <= 0 || pm.in.n_tgt <= 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
   cudaStream_t s = h->stream;
@@ -508,13 +512,20 @@ int pm_align(sm_handle* h, PmMatcher& pm, const double* guess, double* result) {
   }
   PmStage& st = pm.stage;
   H_RC(st.reserve((int)pm.in.n_src));
-  if (pm.src_dirty) {
+  // the rand sampler draws anew on every Align, as the filter does inside ICP::compute
+  const bool rand = pm.reading_sampler == SM_PM_SAMPLING_GLIBC_RAND;
+  if (rand && pm.rand_position > INT64_MAX - pm.in.n_src)
+    return fail(h, SM_ERR_BAD_ARGUMENT, "Align: the rand() stream position would pass 2^63 - 1");
+  if (pm.src_dirty || rand) {
     uint32_t kept = 0;
+    PmRandWindow at;
+    if (rand) at = pm_rand_window((uint32_t)pm.icp.opt.sample_seed, (uint64_t)pm.rand_position);
     H_RC(st.sample((const float*)pm.in.src.p, (int)pm.in.n_src, pm.icp.opt.reading_sample_prob,
-                   (uint32_t)pm.icp.opt.sample_seed, s, &kept));
+                   (uint32_t)pm.icp.opt.sample_seed, s, &kept, rand ? &at : nullptr));
+    if (rand) pm.rand_position += pm.in.n_src;   // one draw per reading point
     if (kept == 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: the reading filter kept no point");
     H_RC(icp_set_source(h, pm.icp, st.points(), (int64_t)kept, true));
-    pm.src_dirty = false;
+    pm.src_dirty = rand;   // the next Align filters anew, whichever sampler it runs
   }
   const int rc = icp_align(h, pm.icp, guess, result);
   h->info.aux[2] = (double)pm.icp.n_source;   // reading points after the filter
@@ -852,6 +863,7 @@ int sm_set_option(sm_handle* h, const char* name, const char* text) {
     // type 1 keeps the filtered reading cloud until the source changes; a new filter option must filter it anew
     PmMatcher* pm = h->as<PmMatcher>();
     if (pm && (strcmp(name, "reading_sample_prob") == 0 || strcmp(name, "sample_seed") == 0)) pm->src_dirty = true;
+    if (pm && strcmp(name, "sample_seed") == 0) pm->rand_position = 0;   // srand restarts the rand() stream
     return SM_OK;
   }
   return fail(h, SM_ERR_UNKNOWN_OPTION, std::string("Init an unknown option of this matcher! ") + name);
@@ -881,6 +893,35 @@ int sm_set_pm_surface_normals(sm_handle* h, int32_t mode) {
     return fail(h, SM_ERR_BAD_ARGUMENT, "SetSurfaceNormals: mode must be 0..1");
   if (mode != pm->surface_normals) pm->tgt_dirty = true;   // the filtered reference cloud is built anew
   pm->surface_normals = mode;
+  return SM_OK;
+}
+
+int sm_set_pm_reading_sampler(sm_handle* h, int32_t mode) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  PmMatcher* pm = h->as<PmMatcher>();
+  if (!pm) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetReadingSampler: IcpUsingPointMatcher (type 1) only");
+  if (mode < SM_PM_SAMPLING_HASH || mode > SM_PM_SAMPLING_GLIBC_RAND)
+    return fail(h, SM_ERR_BAD_ARGUMENT, "SetReadingSampler: mode must be 0..1");
+  if (mode != pm->reading_sampler) pm->src_dirty = true;   // the filtered reading cloud is built anew
+  pm->reading_sampler = mode;
+  return SM_OK;
+}
+
+int sm_get_pm_rand_position(sm_handle* h, int64_t* position) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  PmMatcher* pm = h->as<PmMatcher>();
+  if (!pm) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "GetRandPosition: IcpUsingPointMatcher (type 1) only");
+  if (!position) return fail(h, SM_ERR_BAD_ARGUMENT, "GetRandPosition: null output");
+  *position = pm->rand_position;
+  return SM_OK;
+}
+
+int sm_set_pm_rand_position(sm_handle* h, int64_t position) {
+  if (!h) return SM_ERR_BAD_ARGUMENT;
+  PmMatcher* pm = h->as<PmMatcher>();
+  if (!pm) return fail(h, SM_ERR_UNSUPPORTED_TYPE, "SetRandPosition: IcpUsingPointMatcher (type 1) only");
+  if (position < 0) return fail(h, SM_ERR_BAD_ARGUMENT, "SetRandPosition: the position must be >= 0");
+  pm->rand_position = position;
   return SM_OK;
 }
 

@@ -505,6 +505,48 @@ int sm_debug_pm_stages(int device, const float* reading_3n, int64_t n, const flo
   return SM_OK;
 }
 
+// test hooks: the rand reading sampler's generator (icp_pm.cu) compiled for the host, and its device stage
+int sm_debug_pm_rand_window_host(uint32_t seed, int64_t position, uint32_t* window_31) {
+  if (position < 0 || !window_31) return SM_ERR_BAD_ARGUMENT;
+  const PmRandWindow at = pm_rand_window(seed, (uint64_t)position);
+  memcpy(window_31, at.w, sizeof(at.w));
+  return SM_OK;
+}
+
+int sm_debug_pm_rand_advance_host(const uint32_t* window_31, uint64_t steps, uint32_t* out_31) {
+  if (!window_31 || !out_31) return SM_ERR_BAD_ARGUMENT;
+  PmRandWindow at;
+  memcpy(at.w, window_31, sizeof(at.w));
+  pm_rand_debug_advance_host(at, steps);
+  memcpy(out_31, at.w, sizeof(at.w));
+  return SM_OK;
+}
+
+int sm_debug_pm_rand_draws_host(uint32_t seed, int64_t position, int64_t count, int32_t* out) {
+  if (position < 0 || count < 0 || (count > 0 && !out)) return SM_ERR_BAD_ARGUMENT;
+  pm_rand_debug_draws_host(pm_rand_window(seed, (uint64_t)position), count, out);
+  return SM_OK;
+}
+
+int sm_debug_pm_rand_sample(int device, const float* reading_3n, int64_t n, float prob, uint32_t seed,
+                            int64_t position, int64_t* kept, double* sampled_3n, uint8_t* keep_n) {
+  if (!debug_cloud_ok(reading_3n, n) || position < 0 || !kept || !sampled_3n || !keep_n) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  DevBuf src;
+  PmStage st;
+  SMB_RC(debug_upload_f32(reading_3n, n, src));
+  SMB_RC(st.reserve((int)n));
+  const PmRandWindow at = pm_rand_window(seed, (uint64_t)position);
+  uint32_t m = 0;
+  SMB_RC(st.sample((const float*)src.p, (int)n, prob, seed, nullptr, &m, &at));
+  SMB_CUDA_OK(cudaMemcpy(sampled_3n, st.points(), (size_t)m * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  std::vector<uint32_t> bits((size_t)(n + 31) / 32);
+  SMB_CUDA_OK(cudaMemcpy(bits.data(), st.rand_bits(), bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  for (int64_t i = 0; i < n; ++i) keep_n[i] = (uint8_t)((bits[(size_t)(i >> 5)] >> (i & 31)) & 1u);
+  *kept = (int64_t)m;
+  return SM_OK;
+}
+
 int sm_debug_pm_surface_normals(int device, int32_t mode, const float* first_3n, int64_t n_first, const float* cloud_3n,
                                 int64_t n, double* points_3m, double* normals_3m, int64_t* index_m, int64_t* m) {
   if ((mode != kNormalsLeastSquares && mode != kNormalsEigenvector) || !debug_cloud_ok(cloud_3n, n) || n_first < 0 ||

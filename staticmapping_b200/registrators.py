@@ -66,6 +66,15 @@ class SurfaceNormals(enum.IntEnum):
     EIGENVECTOR = 1
 
 
+class ReadingSampler(enum.IntEnum):
+    """The reading filter of IcpUsingPointMatcher (libpointmatcher's RandomSamplingDataPointsFilter, prob 0.9), for
+    IcpUsingPointMatcher.SetReadingSampler.  HASH (the default) keeps point i by a counter hash of (i, sample_seed);
+    GLIBC_RAND by (float)rand() / (float)RAND_MAX < prob with glibc's rand() stream after srand(sample_seed), from
+    the matcher's stream position (GetRandPosition / SetRandPosition).  See sm_set_pm_reading_sampler."""
+    HASH = 0
+    GLIBC_RAND = 1
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
@@ -366,6 +375,23 @@ class IcpUsingPointMatcher(Ndt):
         """A SurfaceNormals mode for the reference filter; applies from the next Align on, which filters the
         reference cloud anew when the mode changed.  See sm_set_pm_surface_normals in include/sm_b200.h."""
         self._check(self._lib.sm_set_pm_surface_normals(self._h, int(mode)), "SetSurfaceNormals")
+
+    def SetReadingSampler(self, mode):
+        """A ReadingSampler mode for the reading filter; applies from the next Align on.  In GLIBC_RAND mode every
+        Align filters the reading cloud anew and advances the stream position by its size.  See
+        sm_set_pm_reading_sampler in include/sm_b200.h."""
+        self._check(self._lib.sm_set_pm_reading_sampler(self._h, int(mode)), "SetReadingSampler")
+
+    def GetRandPosition(self):
+        """The number of rand() draws taken since srand(sample_seed) (sm_get_pm_rand_position)."""
+        pos = C.c_int64()
+        self._check(self._lib.sm_get_pm_rand_position(self._h, C.byref(pos)), "GetRandPosition")
+        return pos.value
+
+    def SetRandPosition(self, position):
+        """Where the next GLIBC_RAND Align starts drawing: the draws taken since srand(sample_seed), >= 0
+        (sm_set_pm_rand_position).  Setting sample_seed resets it to 0."""
+        self._check(self._lib.sm_set_pm_rand_position(self._h, int(position)), "SetRandPosition")
 
     def Align(self, guess):
         if self._source is None or self._target is None:
