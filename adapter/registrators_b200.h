@@ -310,7 +310,8 @@ inline void FilterRecordsB200(Handle* h, Run run, LastError last_error, const ch
 // body of Factory::InitFromXmlNode becomes one Add per <filter> and one SetParam per <param>, and the body of
 // Factory::Filter (the call in DataCollector::CloudPreProcessing, builder/data/data_collector.cc:137-141)
 //   this->FilterPrepare(cloud); chain_.Filter(*this->inner_cloud_, cloud.get(), &this->inliers_);
-// RandomSampler is a deterministic stand-in for the reference's mt19937 draw (include/sm_b200.h).
+// RandomSampler is a deterministic stand-in for the reference's mt19937 draw unless SetRandomSampler selects that draw
+// at a given seed (include/sm_b200.h).
 class FilterChainB200 {
  public:
   explicit FilterChainB200(int device = 0) { CHECK_EQ(sm_filter_chain_create(device, &chain_), 0); }
@@ -334,6 +335,12 @@ class FilterChainB200 {
   // true: Add also accepts GroundRemoval, StatisticRemoval and VoxelGrid (the chain option all_filters); false
   // restores their refusal.  Filters already added stay.
   void SetAllFilters(bool on) { CHECK_EQ(sm_filter_chain_set_option(chain_, "all_filters", on ? "1" : "0"), 0); }
+  // The generator of RandomSampler `filter`: SM_FILTER_SAMPLER_MT19937 draws from std::mt19937(seed) on every Filter,
+  // as RandomSampler::Filter does when rand_dev() returns `seed`; SM_FILTER_SAMPLER_HASH (the default) is the stand-in.
+  // A filter that is not a RandomSampler or an unknown mode CHECK-fails.
+  void SetRandomSampler(int filter, int mode, uint32_t seed) {
+    CHECK_EQ(sm_filter_chain_set_random_sampler(chain_, filter, mode, seed), 0) << sm_filter_chain_last_error(chain_);
+  }
 
   // inliers: the indices in `input` of the output records, in emission order (include/sm_b200.h)
   void Filter(const data::InnerCloudType& input, data::InnerCloudType* const output,

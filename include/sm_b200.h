@@ -422,10 +422,18 @@ double sm_m2dp_match(const float* P, const float* Q, int64_t n);
  *   BoundingBoxRemoval  filter_bounding_box.cc:49-83 min_x .. max_z (-/+FLT_MAX): REMOVES the points inside the closed
  *                                                    box; the default box removes every finite point.
  *   RandomSampler       filter_random_sample.cc:35-77 sampling_rate (1); a rate > 0.999 passes everything.  The
- *                       reference draws from std::mt19937 seeded by std::random_device: its result is not a function of
- *                       its inputs.  DETERMINISTIC STAND-IN: point i is kept iff
+ *                       reference builds std::mt19937 eng(rand_dev()) on every Filter call and keeps point j of its
+ *                       own input iff uniform_real_distribution<double>(0, 1)(eng) <= sampling_rate: its result is not
+ *                       a function of its inputs, only of them and the seed rand_dev() returned.  Two modes, set per
+ *                       filter by sm_filter_chain_set_random_sampler:
+ *                       HASH (the default), a deterministic stand-in: point i is kept iff
  *                       murmur3_fmix32(i * 0x9E3779B9 + sample_seed) <= sampling_rate * 2^32, i = the point's index in
  *                       the scan handed to the chain (not in the filter's own input), sample_seed a chain option.
+ *                       MT19937, the reference's draw at a given seed: every run builds std::mt19937(seed) anew and
+ *                       point j of the filter's own input (the previous filter's output, in its emission order) takes
+ *                       draw j, two 32-bit engine words w0, w1 -> (double(w0) + double(w1) * 2^32) * 2^-64 as
+ *                       libstdc++'s generate_canonical<double, 53> forms it; the float rate is promoted to double.
+ *                       Such a filter is a stage of its own, and a run with the same seed gives the same points.
  *   RangeImage          filter_range_image.cc:66-141 (Filter only) top_angle (30), btm_angle (-15), offset_x/y/z (0),
  *                       vertical_line_num (40), horizontal_line_num (1800): the first point in input order per pixel.
  *   GroundRemoval2      filter_ground_removal2.cc:127-414  r_max (100), r_min (1), bin_num (200), segment_num (180),
@@ -449,10 +457,10 @@ double sm_m2dp_match(const float* P, const float* Q, int64_t n);
  *                       points: SM_ERR_CHECK_FAILED.
  *   VoxelGrid           voxel_size (0.1): sm_voxel_grid_filter on the stage's input, the same voxel means bit for bit
  *                       (factor 0) in ascending (ix, iy, iz), non-finite points dropped; each record's index is the
- *                       scan index of its voxel's first member in the stage's input order, which a later RandomSampler
- *                       keys on.  voxel_size <= 1e-6 (ConfigsValid, where the reference would run with an undefined
- *                       lround): SM_ERR_BAD_ARGUMENT before any work; finite points spanning 2^21 voxels or more
- *                       along an axis: SM_ERR_BAD_ARGUMENT. */
+ *                       scan index of its voxel's first member in the stage's input order, which a later HASH
+ *                       RandomSampler keys on.  voxel_size <= 1e-6 (ConfigsValid, where the reference would run with
+ *                       an undefined lround): SM_ERR_BAD_ARGUMENT before any work; finite points spanning 2^21 voxels
+ *                       or more along an axis: SM_ERR_BAD_ARGUMENT. */
 typedef struct sm_filter_chain sm_filter_chain;
 /* filter::Factory::Factory (filter_factory.h).  Needs no device; the first run binds CUDA ordinal `device`. */
 int sm_filter_chain_create(int device, sm_filter_chain** out);
@@ -477,6 +485,17 @@ int sm_filter_chain_validate(sm_filter_chain* chain, int filter);
  * all_filters (unsigned, 0): non-zero makes sm_filter_chain_add accept GroundRemoval, StatisticRemoval and VoxelGrid,
  * 0 restores their refusal.  all_filters affects sm_filter_chain_add only: filters already added stay. */
 int sm_filter_chain_set_option(sm_filter_chain* chain, const char* name, const char* text);
+/* The generator of the chain's RandomSampler `filter` (see above), no reference counterpart: the reference registers
+ * only sampling_rate, so this is not a <param>, and it builds one engine per filter, so it is not a chain option.
+ * HASH ignores `seed` (the chain's sample_seed applies); MT19937 draws from std::mt19937(seed), where `seed` is the
+ * value the reference's rand_dev() returned for that filter.  SM_ERR_BAD_ARGUMENT, with the chain unchanged, for a
+ * `filter` out of range or not a RandomSampler, or an unknown mode.  Applies from the next run on; the _device form
+ * runs the generator on its stream. */
+enum sm_filter_sampler {
+  SM_FILTER_SAMPLER_HASH = 0,
+  SM_FILTER_SAMPLER_MT19937 = 1
+};
+int sm_filter_chain_set_random_sampler(sm_filter_chain* chain, int filter, int32_t mode, uint32_t seed);
 /* Factory::SetInputCloud + Factory::Filter (filter_factory.cc:83-106).  `points`: n records `stride_bytes` (>= 20)
  * apart; `out`: capacity n packed 5-float records; *m_out = the number of inliers; inlier_index (optional, capacity
  * n): their indices in `points`, in emission order (ascending without GroundRemoval and VoxelGrid).  An empty chain

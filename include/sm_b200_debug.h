@@ -32,6 +32,7 @@
  *                              and its decision for one voxel
  *     sm_debug_pm_rand_window_host, sm_debug_pm_rand_advance_host, sm_debug_pm_rand_draws_host  the rand reading
  *                              sampler's jump-ahead on glibc's rand() stream and the draws it reaches
+ *     sm_debug_mt19937_words_host  the raw std::mt19937 words the chain's MT19937 RandomSampler draws from
  *   on the device
  *     sm_debug_solve6          the 6x6 solver exactly as icp_finish_kernel calls it
  *     sm_debug_knn1_batched    sm_knn1 with the scheduling the ICP iteration uses when many alignments are in flight
@@ -58,6 +59,7 @@
  *     sm_debug_kd_tree         every array a k-d tree owner (KdCompactTree, NormalsPipeline, FloatTree) fills, after
  *                              an optional earlier build into the same owner
  *     sm_debug_filter_ground_removal2  every intermediate of FilterChain's GroundRemoval2 stage
+ *     sm_debug_filter_mt19937_flags  the keep bytes of FilterChain's MT19937 RandomSampler stage
  *     sm_debug_depth_cluster   DepthCluster's range image, edge mask, labels and BFS level / position per pixel
  *     sm_debug_statistic_removal_distances  the per-point distances of a StatisticRemoval handle's last run
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
@@ -387,6 +389,13 @@ int sm_debug_filter_distance_host(const float* lines_4l, int32_t n_lines, float 
  *                      max_lines must be bin_num / 2 + 1
  *   keep[n]            1 for the points that are not ground
  * Returns SM_OK, or SM_ERR_CHECK_FAILED with the arrays filled when a line does not run outward. */
+/* Raw words 0 .. count - 1 of std::mt19937(seed) (operator() results), from the seeding and recurrence the chain's
+ * MT19937 RandomSampler runs, compiled for the host; no GPU needed. */
+int sm_debug_mt19937_words_host(uint32_t seed, int64_t count, uint32_t* out);
+/* The MT19937 RandomSampler stage's flag kernel alone over n <= 2^30 points at `rate` and `seed`: keep_n[j] = 1 iff
+ * draw j (engine words 2j, 2j + 1) is <= rate, all 1 without a draw at a rate > 0.999; *kept = the sum of the tile
+ * counts the stage leaves for its compaction. */
+int sm_debug_filter_mt19937_flags(int device, int64_t n, float rate, uint32_t seed, uint8_t* keep_n, int64_t* kept);
 int sm_debug_filter_ground_removal2(int device, const struct sm_filter_chain* chain, int32_t filter, const float* points,
                                     int64_t n, int64_t stride_bytes, int32_t max_lines, uint32_t* cell, uint8_t* member,
                                     uint32_t* cell_members, float* cell_min_2c, float* lines_4, int32_t* n_lines,

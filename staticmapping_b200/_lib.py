@@ -86,6 +86,7 @@ SIGNATURES = {
     "sm_filter_chain_set_param": (C.c_int, [_VP, C.c_int, C.c_char_p, C.c_int, C.c_char_p]),
     "sm_filter_chain_validate": (C.c_int, [_VP, C.c_int]),
     "sm_filter_chain_set_option": (C.c_int, [_VP, C.c_char_p, C.c_char_p]),
+    "sm_filter_chain_set_random_sampler": (C.c_int, [_VP, C.c_int, C.c_int32, C.c_uint32]),
     "sm_filter_chain_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
     "sm_filter_chain_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
     "sm_filter_chain_depth_cluster": (C.c_int, [_VP, C.c_int, _VP, C.c_int64, C.c_int64, _VP, _VP, _VP,
@@ -168,6 +169,8 @@ SIGNATURES = {
     "sm_debug_filter_host": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, C.c_int64, _VP, _VP]),
     "sm_debug_filter_fit_host": (C.c_int, [_VP, _VP, C.c_int32, _VP]),
     "sm_debug_filter_distance_host": (C.c_int, [_VP, C.c_int32, C.c_float, C.c_float, _VP]),
+    "sm_debug_mt19937_words_host": (C.c_int, [C.c_uint32, C.c_int64, _VP]),
+    "sm_debug_filter_mt19937_flags": (C.c_int, [C.c_int, C.c_int64, C.c_float, C.c_uint32, _VP, C.POINTER(C.c_int64)]),
     "sm_debug_filter_ground_removal2": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, _VP,
                                                   _VP, _VP, _VP, _VP, _VP]),
     "sm_debug_depth_edge_host": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, C.c_int64, _VP, _VP, _VP]),

@@ -4,7 +4,9 @@
 //
 // Every filter emits its inliers in ascending input index, whole records (x, y, z, intensity, factor) copied.
 //   Range / AxisRange / BoundingBoxRemoval / RandomSampler are per-point predicates: consecutive ones run as ONE
-//     flag kernel, then an ordered compaction (compact.cuh).  RandomSampler is a deterministic stand-in, see filter_keep.
+//     flag kernel, then an ordered compaction (compact.cuh).  RandomSampler is a deterministic stand-in, see filter_keep,
+//     unless it is set to draw from std::mt19937 (mt19937_sampler_kernel): then it is a stage of its own, since its
+//     draw index is the point's position in its own input.
 //   RangeImage (filter_range_image.cc:82-141): the first point in input order to reach an empty pixel is the inlier.
 //     atomicMin of the point index on a pixel-owner image gives exactly that, whatever the thread order.
 //   GroundRemoval2 (filter_ground_removal2.cc:127-414): polar cell per point -> stable radix sort by cell (members of
@@ -443,7 +445,103 @@ gr2_ground_kernel(const FilterParams f, const Gr2Consts c, int n, const uint32_t
 
 int sort_passes(int n_cells) { return n_cells <= (1 << 16) ? 2 : 4; }   // even: the sorted pairs end in the first buffers
 
+// ---- RandomSampler drawing from std::mt19937 ----------------------------------------------------------------------
+// filter_random_sample.cc:49-72 builds std::mt19937 eng(seed) and keeps point j of its input iff distr(eng) <= rate,
+// distr = std::uniform_real_distribution<double>(0, 1).  The engine is [rand.eng.mers]'s MT19937: x[0] = seed,
+// x[i] = 1812433253 (x[i-1] ^ (x[i-1] >> 30)) + i, then x[k+624] = x[k+397] ^ A(upper(x[k]) | lower(x[k+1])), and
+// raw word n is x[n+624] tempered.  Word n depends on words n-227, n-624 and n-623 only, so 227 consecutive words
+// are computed at once.  libstdc++'s generate_canonical<double, 53> takes two words per draw:
+// u_j = (double(w[2j]) + double(w[2j+1]) * 2^32) * 2^-64, the sum rounded to nearest even, the rest exact.
+constexpr int kMtN = 624, kMtM = 397, kMtStep = kMtN - kMtM;   // words per step: 227
+constexpr int kMtRing = 1024, kMtMask = kMtRing - 1;           // >= 624 + 227 words of state in shared memory
+constexpr int kMtEmit = 256;                                   // threads kMtEmit.. write the keep bytes
+constexpr int kMtThreads = kMtEmit + 128;                      // a step completes at most 114 draws
+
+__host__ __device__ inline void mt19937_seed(uint32_t seed, uint32_t* x) {
+  x[0] = seed;
+  for (uint32_t i = 1; i < (uint32_t)kMtN; ++i) x[i] = 1812433253u * (x[i - 1] ^ (x[i - 1] >> 30)) + i;
+}
+
+// x[k+624] from x[k], x[k+1] and x[k+397]
+__host__ __device__ __forceinline__ uint32_t mt19937_next(uint32_t xk, uint32_t xk1, uint32_t xkm) {
+  const uint32_t y = (xk & 0x80000000u) | (xk1 & 0x7fffffffu);
+  return xkm ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
+}
+
+__host__ __device__ __forceinline__ uint32_t mt19937_temper(uint32_t y) {
+  y ^= y >> 11;
+  y ^= (y << 7) & 0x9d2c5680u;
+  y ^= (y << 15) & 0xefc60000u;
+  return y ^ (y >> 18);
+}
+
+// One CTA: threads 0..226 compute step s's 227 state words and their tempered words into two rings while threads
+// kMtEmit.. test the draws whose two words were complete after step s - 1, so each step costs one barrier.  The
+// emitters read slots of x[J - 228] and later and the step writes the slots of x[J - 1024 .. J - 798] (J = the
+// step's first word): they never meet.  flag[j] = point j's keep byte; tile_cnt (zeroed, compact_count_bytes(n))
+// gets each compaction tile's count.
+// A u that rounds to 1.0 is clamped by libstdc++; that cannot move a decision at the rates drawn here (<= 0.999).
+__global__ void __launch_bounds__(kMtThreads)
+mt19937_sampler_kernel(int n, double rate, uint32_t seed, uint8_t* __restrict__ flag, uint32_t* __restrict__ tile_cnt) {
+  __shared__ uint32_t x[kMtRing], w[kMtRing];   // state words; w[slot of x[n + 624]] = raw word n
+  const int t = threadIdx.x;
+  if (t == 0) mt19937_seed(seed, x);
+  __syncthreads();
+  uint32_t done = 0, ready = 0;   // points tested; points whose two words exist (word indices stay below 2^32)
+  for (uint32_t J = kMtN; done < (uint32_t)n; J += kMtStep) {
+    if (t < kMtStep) {
+      if (ready < (uint32_t)n) {
+        const uint32_t k = J + t - kMtN;
+        const uint32_t v = mt19937_next(x[k & kMtMask], x[(k + 1) & kMtMask], x[(k + kMtM) & kMtMask]);
+        x[(J + t) & kMtMask] = v;
+        w[(J + t) & kMtMask] = mt19937_temper(v);
+      }
+    } else if (t >= kMtEmit) {
+      const uint32_t j = done + t - kMtEmit;
+      bool keep = false;
+      if (j < ready) {
+        const uint32_t w0 = w[(2 * j + kMtN) & kMtMask], w1 = w[(2 * j + 1 + kMtN) & kMtMask];
+        const double u = __dmul_rn(__dadd_rn((double)w0, __dmul_rn((double)w1, 4294967296.0)), 0x1p-64);
+        keep = u <= rate;
+        flag[j] = keep ? 1 : 0;
+      }
+      // a warp's 32 draws lie in at most two compaction tiles: lane 0 counts the first, lane 31 the second
+      const uint32_t first = (done + ((t - kMtEmit) & ~31u)) / kCompactTile;
+      const uint32_t lo = __ballot_sync(0xffffffffu, keep && j / kCompactTile == first);
+      const uint32_t hi = __ballot_sync(0xffffffffu, keep) ^ lo;
+      if ((t & 31) == 0 && lo) atomicAdd(&tile_cnt[first], (uint32_t)__popc(lo));
+      if ((t & 31) == 31 && hi) atomicAdd(&tile_cnt[first + 1], (uint32_t)__popc(hi));
+    }
+    __syncthreads();
+    done = ready;
+    ready = min((uint32_t)n, (J + kMtStep - kMtN) >> 1);
+  }
+}
+
 }  // namespace
+
+void mt19937_debug_words_host(uint32_t seed, int64_t count, uint32_t* out) {
+  std::vector<uint32_t> x((size_t)kMtN + (size_t)count);
+  mt19937_seed(seed, x.data());
+  for (int64_t i = 0; i < count; ++i) {
+    x[i + kMtN] = mt19937_next(x[i], x[i + 1], x[i + kMtM]);
+    out[i] = mt19937_temper(x[i + kMtN]);
+  }
+}
+
+int mt19937_sampler_flags(const FilterParams& f, int n, uint8_t* flag, uint32_t* tile_cnt, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int tiles = compact_tiles(n);
+  if ((double)f.sampling_rate > 0.999) {    // filter_random_sample.cc:44-47: every point copied, nothing drawn
+    PredicateRun none = {};                 // an empty predicate run keeps every point
+    filter_predicate_kernel<<<tiles, kCompactThreads, 0, s>>>(nullptr, 0, nullptr, n, none, flag, tile_cnt);
+  } else {
+    SMB_CUDA_OK(cudaMemsetAsync(tile_cnt, 0, compact_count_bytes(n), s));
+    mt19937_sampler_kernel<<<1, kMtThreads, 0, s>>>(n, (double)f.sampling_rate, f.sampler_seed, flag, tile_cnt);
+  }
+  SMB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
 
 // ---- parameters -------------------------------------------------------------------------------------------------
 FilterParams filter_defaults(int kind) {
@@ -464,6 +562,7 @@ FilterParams filter_defaults(int kind) {
     f.min_point_num_in_voxel = 10; f.leaf_size = 0.8f; f.height_threshold = 0.15f;
   }
   if (kind == kFilterVoxelGrid) f.voxel_size = 0.1f;                                   // in Range's storage
+  if (kind == kFilterRandomSampler) { f.sampler_mode = SM_FILTER_SAMPLER_HASH; f.sampler_seed = 0; }   // likewise
   return f;
 }
 
@@ -584,10 +683,15 @@ bool depth_cluster_grid_ok(const FilterParams& f) {
 }
 
 // ---- FilterChain ------------------------------------------------------------------------------------------------
+// a filter that is not one of a fused predicate run: an mt19937 RandomSampler draws by its position in its own input
+static bool own_stage(const FilterParams& f) {
+  return f.kind > kFilterRandomSampler || (f.kind == kFilterRandomSampler && f.sampler_mode == SM_FILTER_SAMPLER_MT19937);
+}
+
 int FilterChain::stage_end(int first) const {
-  if (filters[first].kind > kFilterRandomSampler) return first + 1;
+  if (own_stage(filters[first])) return first + 1;
   int e = first;
-  while (e < (int)filters.size() && e - first < kMaxRun && filters[e].kind <= kFilterRandomSampler) ++e;
+  while (e < (int)filters.size() && e - first < kMaxRun && !own_stage(filters[e])) ++e;
   return e;
 }
 
@@ -628,6 +732,15 @@ int FilterChain::predicate_stage(int first, int cnt, const char* in, const uint3
   const int tiles = compact_tiles(n);
   filter_predicate_kernel<<<tiles, kCompactThreads, 0, s>>>(in, stride, index_in, n, run, (uint8_t*)flag.p,
                                                             (uint32_t*)block_cnt.p);
+  filter_compact_records(in, stride, index_in, n, (const uint8_t*)flag.p, (uint32_t*)block_cnt.p, out, index_out,
+                         (uint32_t*)count.p, s);
+  SMB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int FilterChain::mt19937_sampler_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n,
+                                       int64_t stride, float* out, uint32_t* index_out, cudaStream_t s) {
+  SMB_RC(mt19937_sampler_flags(f, n, (uint8_t*)flag.p, (uint32_t*)block_cnt.p, s));
   filter_compact_records(in, stride, index_in, n, (const uint8_t*)flag.p, (uint32_t*)block_cnt.p, out, index_out,
                          (uint32_t*)count.p, s);
   SMB_CUDA_OK(cudaGetLastError());
@@ -766,7 +879,9 @@ int FilterChain::run(const char* in, int64_t n, int64_t stride, float* out, int3
       continue;
     }
     int gr2_status = 0;
-    if (kind <= kFilterRandomSampler) {
+    if (kind == kFilterRandomSampler && filters[first].sampler_mode == SM_FILTER_SAMPLER_MT19937) {
+      SMB_RC(mt19937_sampler_stage(filters[first], cur, cur_idx, (int)cur_n, cur_stride, dst, dst_idx, s));
+    } else if (kind <= kFilterRandomSampler) {
       SMB_RC(predicate_stage(first, end - first, cur, cur_idx, (int)cur_n, cur_stride, dst, dst_idx, s));
     } else if (kind == kFilterRangeImage) {
       SMB_RC(range_image_stage(filters[first], cur, cur_idx, (int)cur_n, cur_stride, dst, dst_idx, s));
@@ -834,6 +949,17 @@ int sm_filter_chain_set_param(sm_filter_chain* c, int filter, const char* name, 
 int sm_filter_chain_validate(sm_filter_chain* c, int filter) {
   if (!c || filter < 0 || filter >= (int)c->chain.filters.size()) return SM_ERR_BAD_ARGUMENT;
   return filter_configs_valid(c->chain.filters[filter]) ? 1 : 0;
+}
+
+int sm_filter_chain_set_random_sampler(sm_filter_chain* c, int filter, int32_t mode, uint32_t seed) {
+  if (!c || filter < 0 || filter >= (int)c->chain.filters.size()) return SM_ERR_BAD_ARGUMENT;
+  FilterParams& f = c->chain.filters[filter];
+  if (f.kind != kFilterRandomSampler) return c->fail(SM_ERR_BAD_ARGUMENT, "filter %d is not a RandomSampler", filter);
+  if (mode != SM_FILTER_SAMPLER_HASH && mode != SM_FILTER_SAMPLER_MT19937)
+    return c->fail(SM_ERR_BAD_ARGUMENT, "RandomSampler mode must be 0..1");
+  f.sampler_mode = mode;
+  f.sampler_seed = seed;
+  return SM_OK;
 }
 
 int sm_filter_chain_set_option(sm_filter_chain* c, const char* name, const char* text) {

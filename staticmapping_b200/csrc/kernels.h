@@ -435,15 +435,16 @@ enum FilterKind : int {
 // constructors' defaults (filter_range.cc:31-38, filter_axis_range.h:56-57, filter_bounding_box.h,
 // filter_random_sample.cc:29, filter_range_image.cc:29-37, filter_ground_removal2.cc:74-89,
 // filter_statistic_removal.h, filter_ground_removal.cc:29-39, filter_voxel_grid.h:55).  Passed to the kernels by
-// value.  StatisticRemoval's two members and VoxelGrid's one share Range's storage and GroundRemoval's three
-// AxisRange's: a FilterParams holds the parameters of one kind, and its size and layout are what the chain's kernels
-// take.
+// value.  StatisticRemoval's two members, VoxelGrid's one and RandomSampler's generator share Range's storage and
+// GroundRemoval's three AxisRange's: a FilterParams holds the parameters of one kind, and its size and layout are what
+// the chain's kernels take.
 struct FilterParams {
   int kind;
   union {
     struct { float min_range, max_range; };                         // Range
     struct { int32_t point_num_meank; float std_mul; };             // StatisticRemoval
     struct { float voxel_size; };                                   // VoxelGrid
+    struct { int32_t sampler_mode; uint32_t sampler_seed; };        // RandomSampler (sm_filter_chain_set_random_sampler)
   };
   union {
     struct { float min, max; int axis_index; };                     // AxisRange
@@ -478,6 +479,12 @@ bool filter_debug_pixel_host(const FilterParams& f, const float* rec, int* row, 
 void filter_debug_cell_host(const FilterParams& f, const float* rec, float* range, int* s, int* b);
 void filter_debug_fit_host(const float* d, const float* z, int n, float* m, float* b);
 float filter_debug_distance_host(const Gr2Line* lines, int n_lines, float d, float z, int* bad);
+// raw words 0 .. count - 1 of std::mt19937(seed), by the recurrence mt19937_sampler_kernel runs (test hook)
+void mt19937_debug_words_host(uint32_t seed, int64_t count, uint32_t* out);
+// A RandomSampler in SM_FILTER_SAMPLER_MT19937 mode over n points: flag[j] = 1 iff draw j of std::mt19937(sampler_seed)
+// through uniform_real_distribution<double>(0, 1) is <= sampling_rate, every flag 1 without a draw at a rate
+// > 0.999; the tile counts (compact_count_bytes(n)) are left for filter_compact_records.
+int mt19937_sampler_flags(const FilterParams& f, int n, uint8_t* flag, uint32_t* tile_cnt, cudaStream_t s);
 // the RangeImage stage's pixel of every point (0xffffffff: outlier) and the first point per pixel (0xffffffff: empty)
 int range_image_owner(const FilterParams& f, const char* pts, int n, int64_t stride, uint32_t* pixel, uint32_t* owner,
                       cudaStream_t s);
@@ -673,6 +680,8 @@ struct FilterChain {
   // each stage reads n records (index_in: their scan indices, null = identity) and compacts the inliers
   int predicate_stage(int first, int count, const char* in, const uint32_t* index_in, int n, int64_t stride,
                       float* out, uint32_t* index_out, cudaStream_t s);
+  int mt19937_sampler_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,
+                            float* out, uint32_t* index_out, cudaStream_t s);
   int range_image_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,
                         float* out, uint32_t* index_out, cudaStream_t s);
   int ground_removal2_stage(const FilterParams& f, const char* in, const uint32_t* index_in, int n, int64_t stride,

@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "compact.cuh"
 #include "icp_dev.cuh"
 #include "kernels.h"
 #include "linalg_dev.cuh"
@@ -975,6 +976,32 @@ int sm_debug_filter_distance_host(const float* lines_4l, int32_t n_lines, float 
   int bad = 0;
   *distance = filter_debug_distance_host((const Gr2Line*)lines_4l, n_lines, d, z, &bad);
   return bad ? SM_ERR_CHECK_FAILED : SM_OK;
+}
+
+int sm_debug_mt19937_words_host(uint32_t seed, int64_t count, uint32_t* out) {
+  if (count < 0 || (count > 0 && !out)) return SM_ERR_BAD_ARGUMENT;
+  mt19937_debug_words_host(seed, count, out);
+  return SM_OK;
+}
+
+int sm_debug_filter_mt19937_flags(int device, int64_t n, float rate, uint32_t seed, uint8_t* keep_n, int64_t* kept) {
+  if (n < 0 || n > (1 << 30) || (n > 0 && !keep_n) || !kept) return SM_ERR_BAD_ARGUMENT;
+  *kept = 0;
+  if (n == 0) return SM_OK;
+  SMB_RC(select_device(device));
+  FilterParams f = filter_defaults(kFilterRandomSampler);
+  f.sampling_rate = rate;
+  f.sampler_mode = SM_FILTER_SAMPLER_MT19937;
+  f.sampler_seed = seed;
+  DevBuf flag, tile_cnt;
+  SMB_RC(flag.reserve((size_t)n));
+  SMB_RC(tile_cnt.reserve(compact_count_bytes(n)));
+  SMB_RC(mt19937_sampler_flags(f, (int)n, (uint8_t*)flag.p, (uint32_t*)tile_cnt.p, nullptr));
+  std::vector<uint32_t> cnt(compact_count_bytes(n) / sizeof(uint32_t));
+  SMB_CUDA_OK(cudaMemcpy(keep_n, flag.p, (size_t)n, cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(cnt.data(), tile_cnt.p, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  for (uint32_t c : cnt) *kept += c;      // the tile counts the compaction reads, the last slot 0
+  return SM_OK;
 }
 
 int sm_debug_filter_ground_removal2(int device, const sm_filter_chain* chain, int32_t filter, const float* points,

@@ -1,6 +1,7 @@
 """pre_processers::filter::Factory (pre_processors/filter_factory.h, filter_factory.cc:54-106) over the GPU filter
 chain of libsm_b200.so (sm_filter_chain_*, include/sm_b200.h): Range, AxisRange, BoundingBoxRemoval, RandomSampler (a
-deterministic stand-in, see the header), RangeImage and GroundRemoval2, and RangeImage::DepthCluster; with
+deterministic stand-in by default, or std::mt19937 at a given seed, see the header), RangeImage and GroundRemoval2, and
+RangeImage::DepthCluster; with
 Factory.SetAllFilters(True) also StatisticRemoval, GroundRemoval and VoxelGrid.  StatisticRemoval, PCL's statistical
 outlier removal, GroundRemoval, the voxel height-range ground filter, and the submap sampler
 RandomSamplerWithPlaneDetect also run on their own handles (sm_statistic_removal_*, sm_ground_removal_*,
@@ -145,6 +146,14 @@ class Factory(_RecordFilter):
 
     def SetSampleSeed(self, seed):
         self._lib.sm_filter_chain_set_option(self._h, b"sample_seed", str(int(seed)).encode())
+
+    def SetRandomSampler(self, filter_index, mode, seed=0):
+        """The generator of the chain's RandomSampler `filter_index`, a RandomSamplerMode.  MT19937 draws from
+        std::mt19937(seed) anew on every Filter, as the reference does when its random_device returns `seed` (an
+        unsigned 32-bit value); HASH ignores `seed`.  A filter that is not a RandomSampler or an unknown mode raises
+        ValueError and leaves the chain unchanged.  See sm_filter_chain_set_random_sampler."""
+        self._check(self._lib.sm_filter_chain_set_random_sampler(self._h, int(filter_index), int(mode),
+                                                                 int(seed) & 0xFFFFFFFF), "set_random_sampler")
 
     def SetAllFilters(self, flag):
         """True: the filters added from now on may also be GroundRemoval, StatisticRemoval and VoxelGrid, whose chain

@@ -75,6 +75,15 @@ class ReadingSampler(enum.IntEnum):
     GLIBC_RAND = 1
 
 
+class RandomSamplerMode(enum.IntEnum):
+    """The generator of a filter chain's RandomSampler, for Factory.SetRandomSampler.  HASH (the default) keeps scan
+    point i by a counter hash of (i, the chain's sample_seed); MT19937 keeps point j of the filter's own input iff draw j
+    of std::mt19937(seed) through uniform_real_distribution<double>(0, 1) is <= sampling_rate, as the reference does
+    when its random_device returns `seed`.  See sm_filter_chain_set_random_sampler."""
+    HASH = 0
+    MT19937 = 1
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
