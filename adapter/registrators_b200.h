@@ -521,13 +521,19 @@ inline bool M2dpB200(const data::InnerCloudType& source, double r, double max_di
 }
 
 // EigenPointCloud::CalculateNormals on the GPU (cloud_types.cc:347-368); call sites
-// map_builder.cc:286,389 and submap.cc:161.
-inline void CalculateNormalsB200(data::EigenPointCloud* cloud, int device = 0) {
+// map_builder.cc:286,389 and submap.cc:161.  `order` (sm_normals_order): SM_NORMALS_ORDER_INDEX, the default, is
+// sm_calculate_normals; SM_NORMALS_ORDER_NTH_ELEMENT reproduces the reference's own std::nth_element order bit for
+// bit, and CHECK-fails on a non-finite coordinate.
+inline void CalculateNormalsB200(data::EigenPointCloud* cloud, int device = 0,
+                                 int order = SM_NORMALS_ORDER_INDEX) {
   CHECK(cloud);
   const int64_t n = cloud->points.cols();
   Eigen::MatrixXd pts(3, n), nrm(3, n);
   int64_t m = 0;
-  const int rc = sm_calculate_normals(device, cloud->points.data(), n, pts.data(), nrm.data(), &m);
+  const int rc = order == SM_NORMALS_ORDER_INDEX
+                     ? sm_calculate_normals(device, cloud->points.data(), n, pts.data(), nrm.data(), &m)
+                     : sm_calculate_normals_ordered(device, cloud->points.data(), n, order, pts.data(), nrm.data(),
+                                                    &m);
   CHECK_EQ(rc, 0) << "sm_calculate_normals failed";
   cloud->points = pts.leftCols(m);
   cloud->normals = nrm.leftCols(m);

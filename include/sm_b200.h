@@ -353,12 +353,33 @@ int sm_knn_device(int device, const double* target_3xn, int64_t n_target, const 
  * IcpFast::SetInputTarget (map_builder.cc:286,389; submap.cc:161).
  * DEVIATION from the reference (cloud_types.cc:79-100): there a leaf is represented by
  * indices[first] and summed in the member order std::nth_element happens to leave, both of which
- * depend on the standard library's partition internals; here the representative is the member
- * with the smallest original index and members are summed in ascending index.  The SET of surviving
- * leaves is identical (the split is order independent for distinct coordinates); the column order
- * of the output and the last bits of a mean / normal may differ from a run of the real reference. */
+ * depend on the standard library's partition internals; here (SM_NORMALS_ORDER_INDEX) the split
+ * breaks coordinate ties by index, the representative is the member with the smallest original
+ * index and members are summed in ascending index.  With distinct coordinates the SET of leaves is
+ * the reference's; with tied coordinates (float lidar clouds have many) the leaves themselves can
+ * differ, and so can the column order and the last bits of a mean / normal.
+ * sm_calculate_normals_ordered with SM_NORMALS_ORDER_NTH_ELEMENT gives the reference's own order. */
 int sm_calculate_normals(int device, const double* points_3xn, int64_t n, double* out_points,
                          double* out_normals, int64_t* m_out);
+
+/* The order CalculateNormals splits, sums and represents its leaves in.
+ *   SM_NORMALS_ORDER_INDEX        sm_calculate_normals' order: ties broken by index, members summed
+ *                                 in ascending index, representative = smallest index
+ *   SM_NORMALS_ORDER_NTH_ELEMENT  the reference's: every node split by libstdc++'s std::nth_element
+ *                                 with '<' on the cut-axis coordinate over the one index array the
+ *                                 recursion permutes; members summed in the order it leaves,
+ *                                 representative = first member; columns in ascending
+ *                                 representative index.  Bit-identical to that recursion run on the
+ *                                 CPU, so a build that switches to the GPU gets its own targets back.
+ *                                 A non-finite coordinate is refused with SM_ERR_BAD_ARGUMENT (the
+ *                                 library's unguarded scans are undefined on NaN); nothing is written. */
+enum sm_normals_order {
+  SM_NORMALS_ORDER_INDEX = 0,
+  SM_NORMALS_ORDER_NTH_ELEMENT = 1,
+};
+/* sm_calculate_normals in the given order (sm_normals_order); an unknown order is SM_ERR_BAD_ARGUMENT. */
+int sm_calculate_normals_ordered(int device, const double* points_3xn, int64_t n, int32_t order,
+                                 double* out_points, double* out_normals, int64_t* m_out);
 
 /* MotionCompensation (builder/map_builder.cc:232-257; called either side of Align at :320-352
  * when motion_compensation_options.enable is set): every point is moved by

@@ -62,6 +62,8 @@
  *     sm_debug_filter_mt19937_flags  the keep bytes of FilterChain's MT19937 RandomSampler stage
  *     sm_debug_depth_cluster   DepthCluster's range image, edge mask, labels and BFS level / position per pixel
  *     sm_debug_statistic_removal_distances  the per-point distances of a StatisticRemoval handle's last run
+ *     sm_debug_nth_element     one CTA's std::nth_element on one key array (csrc/nth_element.cu block_introselect)
+ *     sm_debug_normals_nth_perm  the index array CalculateNormals' recursion leaves in SM_NORMALS_ORDER_NTH_ELEMENT
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
  *   each stage of M2DP and of IcpFast's iteration meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
@@ -452,6 +454,15 @@ int sm_debug_plane_sampler_trace(struct sm_plane_sampler* sampler, int32_t on);
  * with / without plane points, 3 skipped before RANSAC, 4 / 5 RANSAC with / without.  *n = the voxels (0 when Detect
  * did not run); SM_ERR_BAD_ARGUMENT when capacity < *n. */
 int sm_debug_plane_sampler_voxels(struct sm_plane_sampler* sampler, void* out, int64_t capacity, int64_t* n);
+
+/* std::nth_element(idx, idx + nth, idx + n) over iota comparing keys[a] < keys[b], run by the CTA routine the
+ * normals recursion uses for one node (csrc/nth_element.cu block_introselect, including its serial tail and the
+ * heap-select fallback) -> perm_n.  n in 1..2^24, 0 <= nth <= n; keys may hold anything '<' orders. */
+int sm_debug_nth_element(int device, const double* keys_n, int64_t n, int64_t nth, int32_t* perm_n);
+
+/* CalculateNormals' index array after the whole median-split recursion in SM_NORMALS_ORDER_NTH_ELEMENT, as
+ * NormalsPipeline::run_nth_element leaves it -> perm_n.  SM_ERR_BAD_ARGUMENT for a non-finite coordinate. */
+int sm_debug_normals_nth_perm(int device, const double* points_3n, int64_t n, int32_t* perm_n);
 
 #ifdef __cplusplus
 }

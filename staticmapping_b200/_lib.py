@@ -73,6 +73,7 @@ SIGNATURES = {
     "sm_knn_device": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, C.c_int64, C.c_int32, C.c_double, C.c_double,
                                 C.c_uint32, C.c_int, _VP, _VP, _VP]),
     "sm_calculate_normals": (C.c_int, [C.c_int, _VP, C.c_int64, _VP, _VP, C.POINTER(C.c_int64)]),
+    "sm_calculate_normals_ordered": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int32, _VP, _VP, C.POINTER(C.c_int64)]),
     "sm_motion_compensation": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _DP, _VP]),
     "sm_motion_compensation_device": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _DP, _VP, _VP]),
     "sm_voxel_grid_filter": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_float, _VP, C.POINTER(C.c_int64)]),
@@ -171,6 +172,8 @@ SIGNATURES = {
     "sm_debug_filter_distance_host": (C.c_int, [_VP, C.c_int32, C.c_float, C.c_float, _VP]),
     "sm_debug_mt19937_words_host": (C.c_int, [C.c_uint32, C.c_int64, _VP]),
     "sm_debug_filter_mt19937_flags": (C.c_int, [C.c_int, C.c_int64, C.c_float, C.c_uint32, _VP, C.POINTER(C.c_int64)]),
+    "sm_debug_nth_element": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _VP]),
+    "sm_debug_normals_nth_perm": (C.c_int, [C.c_int, _VP, C.c_int64, _VP]),
     "sm_debug_filter_ground_removal2": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, _VP,
                                                   _VP, _VP, _VP, _VP, _VP]),
     "sm_debug_depth_edge_host": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, C.c_int64, _VP, _VP, _VP]),

@@ -352,15 +352,33 @@ enum NormalsMode : int { kNormalsLeastSquares = 0, kNormalsEigenvector = 1 };
 // with its workspace, the per-leaf scratch, and the AoS 3xM outputs with their count M.
 struct NormalsPipeline {
   DevBuf coord, nodes, order, kdws, tmp_pts, tmp_nrm, keep, bsum, out_pts, out_nrm, count;
+  DevBuf perm, nth_key, lpos, rpos, nth_bounds;   // std::nth_element's order only, sized by run_nth_element
   int64_t stride = 0;
   int reserve(int n);
   double* input() const { return (double*)coord.p; }   // SoA [3][stride], filled by the caller
   // runs the pipeline with the given leaf routine on the first n points of input() and waits for M; keep then holds
   // 1 at the smallest member index of every kept box (the outputs' source positions, in order)
   int run(int n, NormalsMode mode, cudaStream_t stream, uint32_t* m);
+  // CalculateNormals in the order std::nth_element leaves (SM_NORMALS_ORDER_NTH_ELEMENT): the least-squares leaf over
+  // the members in that order, keep set at each leaf's first member; perm then holds the recursion's index array.
+  // SM_ERR_BAD_ARGUMENT, with nothing written, if a coordinate is not finite.
+  int run_nth_element(int n, cudaStream_t stream, uint32_t* m);
+  int fit_leaves(int n, NormalsMode mode, const uint32_t* leaf_order, cudaStream_t stream, uint32_t* m);
   const double* points() const { return (const double*)out_pts.p; }
   const double* normals() const { return (const double*)out_nrm.p; }
 };
+
+// ---- nth_element.cu --------------------------------------------------------------------
+// BuildNormals' index array over the first n points of coord (SoA [3][cstride]) as std::nth_element leaves it;
+// perm, key, lpos, rpos: n entries each; bounds: nth_element_bounds_bytes(n) of scratch
+int nth_element_recursion(const double* coord, int64_t cstride, int n, uint32_t* perm, double* key, uint32_t* lpos,
+                          uint32_t* rpos, double* bounds, cudaStream_t stream);
+size_t nth_element_bounds_bytes(int n);
+// *bad = some coordinate of the first n points is not finite; flag_dev: one device word of scratch.  Waits.
+int any_nonfinite(const double* coord, int64_t cstride, int n, uint32_t* flag_dev, cudaStream_t stream, bool* bad);
+// test hook: one CTA's std::nth_element(nth) over n device keys -> perm; key, lpos, rpos: n entries of scratch
+int nth_element_single(const double* keys, int n, int nth, uint32_t* perm, double* key, uint32_t* lpos,
+                       uint32_t* rpos, cudaStream_t stream);
 
 // ---- icp_pm.cu -------------------------------------------------------------------------
 // glibc's rand() stream (TYPE_3, degree 31) as 31 consecutive words of its additive recurrence: the window at

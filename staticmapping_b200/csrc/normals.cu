@@ -212,8 +212,8 @@ __global__ void normals_leaf_kernel(const double* __restrict__ coord, int64_t cs
     for (int r = 0; r < 3; ++r) d[i][r] = coord[r * cstride + id];
   }
   if (!leaf_plane_fit(d, count, mean, unit)) return;
-  const uint32_t k = leaf_order[first];             // smallest original index of the leaf
-  keep[k] = 1u;
+  const uint32_t k = leaf_order[first];             // the first member: the smallest original index of the leaf
+  keep[k] = 1u;                                     // in the k-d build's order, the reference's in nth_element's
   for (int r = 0; r < 3; ++r) {
     out_pts[3 * (int64_t)k + r] = mean[r];
     out_nrm[3 * (int64_t)k + r] = unit[r];
@@ -311,21 +311,41 @@ int NormalsPipeline::reserve(int n) {
 }
 
 int NormalsPipeline::run(int n, NormalsMode mode, cudaStream_t stream, uint32_t* m) {
-  const int levels = kd_num_levels(n, 7);
-  uint32_t* tile_cnt = (uint32_t*)bsum.p;
   KdWorkspace ws;
   SMB_RC(ws.carve(kdws, n, 7));
   SMB_RC(kd_build(input(), stride, n, 7, ws, (KdNode*)nodes.p, (uint32_t*)order.p, stream));
+  return fit_leaves(n, mode, (const uint32_t*)order.p, stream, m);
+}
+
+int NormalsPipeline::run_nth_element(int n, cudaStream_t stream, uint32_t* m) {
+  SMB_RC(perm.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(nth_key.reserve((size_t)n * sizeof(double)));
+  SMB_RC(lpos.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(rpos.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(nth_bounds.reserve(nth_element_bounds_bytes(n)));
+  bool bad = false;
+  SMB_RC(any_nonfinite(input(), stride, n, (uint32_t*)count.p, stream, &bad));
+  if (bad) return SM_ERR_BAD_ARGUMENT;            // the reference's unguarded scans have no sentinel past a NaN
+  SMB_RC(nth_element_recursion(input(), stride, n, (uint32_t*)perm.p, (double*)nth_key.p, (uint32_t*)lpos.p,
+                               (uint32_t*)rpos.p, (double*)nth_bounds.p, stream));
+  return fit_leaves(n, kNormalsLeastSquares, (const uint32_t*)perm.p, stream, m);
+}
+
+// the leaf routine over every leaf of `leaf_order` (representative = its first member), then the order-preserving
+// compaction of the kept representatives
+int NormalsPipeline::fit_leaves(int n, NormalsMode mode, const uint32_t* leaf_order, cudaStream_t stream, uint32_t* m) {
+  const int levels = kd_num_levels(n, 7);
+  uint32_t* tile_cnt = (uint32_t*)bsum.p;
   SMB_CUDA_OK(cudaMemsetAsync(keep.p, 0, (size_t)n * sizeof(uint32_t), stream));
   const int total = (1 << (levels + 1)) - 1;
   if (mode == kNormalsEigenvector)
-    pm_normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(input(), stride, (const uint32_t*)order.p, n,
-                                                                    levels, (double*)tmp_pts.p, (double*)tmp_nrm.p,
+    pm_normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(input(), stride, leaf_order, n, levels,
+                                                                    (double*)tmp_pts.p, (double*)tmp_nrm.p,
                                                                     (uint32_t*)keep.p);
   else
-    normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(input(), stride, (const KdNode*)nodes.p,
-                                                                 (const uint32_t*)order.p, n, levels, (double*)tmp_pts.p,
-                                                                 (double*)tmp_nrm.p, (uint32_t*)keep.p);
+    normals_leaf_kernel<<<ceil_div(total, 128), 128, 0, stream>>>(input(), stride, (const KdNode*)nodes.p, leaf_order,
+                                                                 n, levels, (double*)tmp_pts.p, (double*)tmp_nrm.p,
+                                                                 (uint32_t*)keep.p);
   const int tiles = compact_tiles(n);
   compact_count_kernel<<<tiles, kCompactThreads, 0, stream>>>((const uint32_t*)keep.p, n, tile_cnt);
   compact_scan(tile_cnt, tiles, stream);

@@ -1107,7 +1107,13 @@ int sm_debug_icp_stamps(const sm_handle* h, long long* out12) {
 
 int sm_calculate_normals(int device, const double* points, int64_t n, double* out_points,
                          double* out_normals, int64_t* m_out) {
-  if (!points || !out_points || !out_normals || !m_out || n <= 0 || n > (1 << 30))
+  return sm_calculate_normals_ordered(device, points, n, SM_NORMALS_ORDER_INDEX, out_points, out_normals, m_out);
+}
+
+int sm_calculate_normals_ordered(int device, const double* points, int64_t n, int32_t order, double* out_points,
+                                 double* out_normals, int64_t* m_out) {
+  if (!points || !out_points || !out_normals || !m_out || n <= 0 || n > (1 << 30) ||
+      (order != SM_NORMALS_ORDER_INDEX && order != SM_NORMALS_ORDER_NTH_ELEMENT))
     return SM_ERR_BAD_ARGUMENT;
   SMB_RC(select_device(device));
   cudaStream_t s = nullptr;
@@ -1116,7 +1122,8 @@ int sm_calculate_normals(int device, const double* points, int64_t n, double* ou
   SMB_RC(np.reserve((int)n));
   SMB_RC(upload_soa(points, n, false, stage, np.input(), np.stride, s));
   uint32_t m = 0;
-  SMB_RC(np.run((int)n, kNormalsLeastSquares, s, &m));
+  if (order == SM_NORMALS_ORDER_NTH_ELEMENT) SMB_RC(np.run_nth_element((int)n, s, &m));
+  else SMB_RC(np.run((int)n, kNormalsLeastSquares, s, &m));
   if (m > 0) {
     SMB_CUDA_OK(cudaMemcpyAsync(out_points, np.points(), (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));
     SMB_CUDA_OK(cudaMemcpyAsync(out_normals, np.normals(), (size_t)3 * m * sizeof(double), cudaMemcpyDeviceToHost, s));

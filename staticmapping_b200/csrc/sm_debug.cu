@@ -1083,4 +1083,38 @@ int sm_debug_depth_cluster(int device, const sm_filter_chain* chain, int32_t fil
   return SM_OK;
 }
 
+// test hook: one CTA's std::nth_element on one key array (nth_element.cu block_introselect)
+int sm_debug_nth_element(int device, const double* keys_n, int64_t n, int64_t nth, int32_t* perm_n) {
+  if (!keys_n || !perm_n || n <= 0 || n > (1 << 24) || nth < 0 || nth > n) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  DevBuf keys, perm, key, lpos, rpos;
+  SMB_RC(keys.reserve((size_t)n * sizeof(double)));
+  SMB_RC(key.reserve((size_t)n * sizeof(double)));
+  SMB_RC(perm.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(lpos.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_RC(rpos.reserve((size_t)n * sizeof(uint32_t)));
+  SMB_CUDA_OK(cudaMemcpy(keys.p, keys_n, (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
+  SMB_RC(nth_element_single((const double*)keys.p, (int)n, (int)nth, (uint32_t*)perm.p, (double*)key.p,
+                            (uint32_t*)lpos.p, (uint32_t*)rpos.p, nullptr));
+  SMB_CUDA_OK(cudaMemcpy(perm_n, perm.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
+// test hook: the recursion's index array of sm_calculate_normals_ordered(SM_NORMALS_ORDER_NTH_ELEMENT)
+int sm_debug_normals_nth_perm(int device, const double* points_3n, int64_t n, int32_t* perm_n) {
+  if (!points_3n || !perm_n || n <= 0 || n > (1 << 30)) return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  NormalsPipeline np;
+  SMB_RC(np.reserve((int)n));
+  std::vector<double> soa((size_t)n);
+  for (int d = 0; d < 3; ++d) {
+    for (int64_t i = 0; i < n; ++i) soa[(size_t)i] = points_3n[3 * i + d];
+    SMB_CUDA_OK(cudaMemcpy(np.input() + d * np.stride, soa.data(), (size_t)n * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  uint32_t m = 0;
+  SMB_RC(np.run_nth_element((int)n, nullptr, &m));
+  SMB_CUDA_OK(cudaMemcpy(perm_n, np.perm.p, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return SM_OK;
+}
+
 }  // extern "C"

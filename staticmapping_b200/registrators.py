@@ -84,6 +84,15 @@ class RandomSamplerMode(enum.IntEnum):
     MT19937 = 1
 
 
+class NormalsOrder(enum.IntEnum):
+    """The order CalculateNormals splits, sums and represents its leaves in.  INDEX (the default) breaks coordinate
+    ties by index, sums each leaf in ascending index and keeps its smallest index; NTH_ELEMENT is the reference's own:
+    libstdc++'s std::nth_element on the cut-axis coordinate, each leaf summed in the order it leaves and represented by
+    its first member, bit-identical to that recursion on the CPU.  See sm_calculate_normals_ordered."""
+    INDEX = 0
+    NTH_ELEMENT = 1
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
@@ -547,18 +556,26 @@ def knn(target, query, k, epsilon=0.0, max_radius=float("inf"), allow_self_match
     return ids, d2
 
 
-def CalculateNormals(points, device=0) -> EigenCloud:
+def CalculateNormals(points, device=0, order=NormalsOrder.INDEX) -> EigenCloud:
     """EigenPointCloud::CalculateNormals on the GPU (cloud_types.cc:347-368): returns the
-    decimated cloud (one mean point + unit normal per valid <=7-point leaf)."""
+    decimated cloud (one mean point + unit normal per valid <=7-point leaf), in the NormalsOrder `order`.
+    NTH_ELEMENT raises ValueError for a non-finite coordinate."""
     lib = _lib.lib()
     p = np.ascontiguousarray(np.asarray(points, dtype=np.float64))
     out_p = np.empty_like(p)
     out_n = np.empty_like(p)
     m = C.c_int64(0)
-    rc = lib.sm_calculate_normals(device, p.ctypes.data, p.shape[0], out_p.ctypes.data,
-                                  out_n.ctypes.data, C.byref(m))
+    order = NormalsOrder(order)
+    if order == NormalsOrder.INDEX:
+        rc = lib.sm_calculate_normals(device, p.ctypes.data, p.shape[0], out_p.ctypes.data,
+                                      out_n.ctypes.data, C.byref(m))
+    else:
+        rc = lib.sm_calculate_normals_ordered(device, p.ctypes.data, p.shape[0], int(order), out_p.ctypes.data,
+                                              out_n.ctypes.data, C.byref(m))
     if rc == -20:
         raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
+    if rc == -1 and order == NormalsOrder.NTH_ELEMENT:
+        raise ValueError("CalculateNormals(order=NTH_ELEMENT): the cloud has a non-finite coordinate")
     if rc != 0:
         raise RuntimeError(f"sm_calculate_normals failed with {rc}")
     return EigenCloud(out_p[:m.value].copy(), out_n[:m.value].copy())
