@@ -264,15 +264,21 @@ inline void AlignBatch(const std::vector<MatcherB200*>& matchers, const std::vec
 // pre_processers::filter::VoxelGrid::Filter (pre_processors/filter_voxel_grid.cc:37-78) on the GPU:
 // the body of that member becomes
 //   this->FilterPrepare(cloud); registrator::VoxelGridFilterB200(*this->inner_cloud_, voxel_size_, cloud.get());
-// Output points come in ascending voxel order instead of unordered_map iteration order.
+// `order` (sm_voxel_order): SM_VOXEL_ORDER_ASCENDING, the default, emits the voxels in ascending (ix, iy, iz);
+// SM_VOXEL_ORDER_UNORDERED_MAP in the reference's own std::unordered_map iteration order, which a submap target fed
+// to CalculateNormalsB200(..., SM_NORMALS_ORDER_NTH_ELEMENT) needs to be the reference's.
 inline void VoxelGridFilterB200(const data::InnerCloudType& input, float voxel_size,
-                                data::InnerCloudType* const output, int device = 0) {
+                                data::InnerCloudType* const output, int device = 0,
+                                int order = SM_VOXEL_ORDER_ASCENDING) {
   CHECK(output);
+  CHECK(order == SM_VOXEL_ORDER_ASCENDING || order == SM_VOXEL_ORDER_UNORDERED_MAP) << "unknown voxel order " << order;
   output->points.resize(input.points.size());
   int64_t m = 0;
   if (!input.points.empty()) {
-    const int rc = sm_voxel_grid_filter(device, &input.points[0].x, static_cast<int64_t>(input.points.size()),
-                                        sizeof(data::InnerPointType), voxel_size, &output->points[0].x, &m);
+    const int rc = sm_voxel_grid_filter_ordered(device, &input.points[0].x,
+                                                static_cast<int64_t>(input.points.size()),
+                                                sizeof(data::InnerPointType), voxel_size, order,
+                                                &output->points[0].x, &m);
     // non-finite points are dropped by the engine (the reference keeps running on such input too).
     // SM_ERR_BAD_ARGUMENT is left for a cloud spanning >= 2^21 voxels along an axis or an invalid voxel
     // size (the reference refuses that one in ConfigsValid()): report and pass the cloud through
@@ -340,6 +346,12 @@ class FilterChainB200 {
   // A filter that is not a RandomSampler or an unknown mode CHECK-fails.
   void SetRandomSampler(int filter, int mode, uint32_t seed) {
     CHECK_EQ(sm_filter_chain_set_random_sampler(chain_, filter, mode, seed), 0) << sm_filter_chain_last_error(chain_);
+  }
+  // The emission order of VoxelGrid `filter` (sm_voxel_order): SM_VOXEL_ORDER_UNORDERED_MAP is the reference's
+  // std::unordered_map order, SM_VOXEL_ORDER_ASCENDING (the default) ascending voxel index.  A filter that is not a
+  // VoxelGrid or an unknown order CHECK-fails.
+  void SetVoxelOrder(int filter, int order) {
+    CHECK_EQ(sm_filter_chain_set_voxel_order(chain_, filter, order), 0) << sm_filter_chain_last_error(chain_);
   }
 
   // inliers: the indices in `input` of the output records, in emission order (include/sm_b200.h)

@@ -405,13 +405,33 @@ int sm_motion_compensation_device(int device, const float* dev_points, int64_t n
  * order (:58-70), factor = 0.  `points`: data::InnerPointType records (x, y, z, intensity, ...)
  * `stride_bytes` (>= 16) apart; `out`: capacity n records of 5 packed floats; *m_out = number of
  * voxels.  Every value is bit-identical to the reference's; the ORDER of the output points is
- * ascending (ix, iy, iz), where the reference emits them in std::unordered_map iteration order.
+ * ascending (ix, iy, iz), where the reference emits them in std::unordered_map iteration order
+ * (sm_voxel_grid_filter_ordered with SM_VOXEL_ORDER_UNORDERED_MAP gives that order).
  * Points with a NaN / inf coordinate are dropped (std::lround of such a value is unspecified in the
  * reference; one bad lidar return must not stop the mapper).  SM_ERR_BAD_ARGUMENT: voxel_size <= 1e-6
  * (ConfigsValid, :35), or finite points that span 2^21 voxels or more along one axis (209 km at the
  * reference's 0.1 m voxels). */
 int sm_voxel_grid_filter(int device, const float* points, int64_t n, int64_t stride_bytes,
                          float voxel_size, float* out, int64_t* m_out);
+
+/* The order VoxelGrid emits its voxels in.
+ *   SM_VOXEL_ORDER_ASCENDING      sm_voxel_grid_filter's: ascending (ix, iy, iz)
+ *   SM_VOXEL_ORDER_UNORDERED_MAP  the reference's: the iteration order of its std::unordered_map<Eigen::Vector3i, ...>
+ *                                 (hash common/eigen_hash.h:31-43, boost's hash_combine over the int keys) as the
+ *                                 libstdc++ this library is built with leaves it after inserting the voxels in the
+ *                                 order of their first member, its rehash schedule included.  Non-finite points are
+ *                                 dropped before insertion, so the order is the container's when fed the finite
+ *                                 points in input order (the reference's lround of such a point is unspecified).
+ *                                 Fed to CalculateNormals in SM_NORMALS_ORDER_NTH_ELEMENT, this gives the
+ *                                 reference's submap targets (Submap::InsertFrame, builder/submap.cc:144-161). */
+enum sm_voxel_order {
+  SM_VOXEL_ORDER_ASCENDING = 0,
+  SM_VOXEL_ORDER_UNORDERED_MAP = 1
+};
+/* sm_voxel_grid_filter in the given order (sm_voxel_order): the same records, permuted.  An unknown order is
+ * SM_ERR_BAD_ARGUMENT, with nothing written. */
+int sm_voxel_grid_filter_ordered(int device, const float* points, int64_t n, int64_t stride_bytes,
+                                 float voxel_size, int32_t order, float* out, int64_t* m_out);
 
 /* descriptor::M2dp (descriptor/m2dp.cc:37-172; parameters of the constructor, m2dp.h:50-51: r = 0.1,
  * max_distance = 100, t = 16, p = 4, q = 16), the loop-closure descriptor of a submap:
@@ -465,9 +485,10 @@ double sm_m2dp_match(const float* P, const float* Q, int64_t n);
  * border or a GroundRemoval2 segment border can land in the neighbouring pixel / segment.  A float -> int conversion
  * outside int's range (undefined in C++) gives INT_MIN, as the reference's x86 build does.
  * With the chain option all_filters, the reference's other three filters are built too, as the GPU filters of their
- * own entry points.  None of them gives the reference Factory's result, which is why the option is off by default:
+ * own entry points.  None of them gives the reference Factory's result by default, which is why the option is off:
  * the reference's StatisticRemoval::Filter is an empty body (filter_statistic_removal.cc:44-59), its VoxelGrid emits
- * in std::unordered_map order, and its GroundRemoval breaks the ascending order above.  With the option on, each
+ * in std::unordered_map order unless sm_filter_chain_set_voxel_order selects that order, and its GroundRemoval breaks
+ * the ascending order above.  With the option on, each
  * stage reads the previous stage's records in their order, and a run's inlier_index holds the scan index of every
  * emitted record in emission order; the six kinds above emit in ascending order, so their chains are unchanged.
  *   GroundRemoval       min_point_num_in_voxel (10), leaf_size (0.8), height_threshold (0.15): sm_ground_removal_*
@@ -477,9 +498,10 @@ double sm_m2dp_match(const float* P, const float* Q, int64_t n);
  *                       input order.  point_num_meank outside 1..63: SM_ERR_BAD_ARGUMENT before any work; 1..K finite
  *                       points: SM_ERR_CHECK_FAILED.
  *   VoxelGrid           voxel_size (0.1): sm_voxel_grid_filter on the stage's input, the same voxel means bit for bit
- *                       (factor 0) in ascending (ix, iy, iz), non-finite points dropped; each record's index is the
- *                       scan index of its voxel's first member in the stage's input order, which a later HASH
- *                       RandomSampler keys on.  voxel_size <= 1e-6 (ConfigsValid, where the reference would run with
+ *                       (factor 0) in ascending (ix, iy, iz), or in the order sm_filter_chain_set_voxel_order sets,
+ *                       non-finite points dropped; each record's index is the scan index of its voxel's first member
+ *                       in the stage's input order, which a later HASH RandomSampler keys on (an MT19937 one draws in
+ *                       emission order).  voxel_size <= 1e-6 (ConfigsValid, where the reference would run with
  *                       an undefined lround): SM_ERR_BAD_ARGUMENT before any work; finite points spanning 2^21 voxels
  *                       or more along an axis: SM_ERR_BAD_ARGUMENT. */
 typedef struct sm_filter_chain sm_filter_chain;
@@ -517,6 +539,12 @@ enum sm_filter_sampler {
   SM_FILTER_SAMPLER_MT19937 = 1
 };
 int sm_filter_chain_set_random_sampler(sm_filter_chain* chain, int filter, int32_t mode, uint32_t seed);
+/* The emission order of the chain's VoxelGrid `filter` (sm_voxel_order, default SM_VOXEL_ORDER_ASCENDING), no
+ * reference counterpart: the reference registers only voxel_size, so this is not a <param>.  Only the order of the
+ * stage's records changes; each keeps the scan index of its voxel's first member.  SM_ERR_BAD_ARGUMENT, with the
+ * chain unchanged, for a `filter` out of range or not a VoxelGrid, or an unknown order.  Applies from the next run on,
+ * in both run forms. */
+int sm_filter_chain_set_voxel_order(sm_filter_chain* chain, int filter, int32_t order);
 /* Factory::SetInputCloud + Factory::Filter (filter_factory.cc:83-106).  `points`: n records `stride_bytes` (>= 20)
  * apart; `out`: capacity n packed 5-float records; *m_out = the number of inliers; inlier_index (optional, capacity
  * n): their indices in `points`, in emission order (ascending without GroundRemoval and VoxelGrid).  An empty chain

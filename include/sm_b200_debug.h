@@ -64,6 +64,8 @@
  *     sm_debug_statistic_removal_distances  the per-point distances of a StatisticRemoval handle's last run
  *     sm_debug_nth_element     one CTA's std::nth_element on one key array (csrc/nth_element.cu block_introselect)
  *     sm_debug_normals_nth_perm  the index array CalculateNormals' recursion leaves in SM_NORMALS_ORDER_NTH_ELEMENT
+ *     sm_debug_voxel_unordered_epochs  VoxelGrid's per-voxel hash and insertion rank and its list positions after
+ *                              every rehash epoch in SM_VOXEL_ORDER_UNORDERED_MAP
  *   so each device stage of Ndt / NdtWithGicp meets the oracle bit for bit, not only through the final pose, and
  *   each stage of M2DP and of IcpFast's iteration meets a float64 model fed with the device's previous stage */
 #ifndef SM_B200_DEBUG_H_
@@ -463,6 +465,22 @@ int sm_debug_nth_element(int device, const double* keys_n, int64_t n, int64_t nt
 /* CalculateNormals' index array after the whole median-split recursion in SM_NORMALS_ORDER_NTH_ELEMENT, as
  * NormalsPipeline::run_nth_element leaves it -> perm_n.  SM_ERR_BAD_ARGUMENT for a non-finite coordinate. */
 int sm_debug_normals_nth_perm(int device, const double* points_3n, int64_t n, int32_t* perm_n);
+
+/* std::unordered_map's bucket_count() after each of m distinct inserts into a default-constructed map, from the
+ * rehash policy of the libstdc++ this library is built with (csrc/voxel_filter.cu unordered_map_epochs) -> out_m. */
+int sm_debug_voxel_bucket_counts_host(int64_t m, uint64_t* out_m);
+
+/* The reference's voxel hash (common/eigen_hash.h:31-43) of n int keys (rows x, y, z) -> out_n. */
+int sm_debug_voxel_hash_host(const int32_t* keys_3n, int64_t n, uint64_t* out_n);
+
+/* sm_voxel_grid_filter_ordered(SM_VOXEL_ORDER_UNORDERED_MAP) through VoxelGrid's own launches, with its intermediates:
+ * per voxel in ascending (ix, iy, iz) order its hash (hash_m) and insertion rank (rank_m, the order of first members;
+ * capacity n each); per rehash epoch e (*n_epochs of them) the list position of the voxel of every rank t after the
+ * epoch, pos[e * m + t], -1 for a rank not yet inserted.  *m_out = m.  SM_ERR_BAD_ARGUMENT, with *m_out and
+ * *n_epochs set, when capacity < m * *n_epochs entries of pos. */
+int sm_debug_voxel_unordered_epochs(int device, const float* points, int64_t n, int64_t stride_bytes,
+                                    float voxel_size, uint64_t* hash_m, int32_t* rank_m, int32_t* pos,
+                                    int64_t capacity, int64_t* m_out, int32_t* n_epochs);
 
 #ifdef __cplusplus
 }

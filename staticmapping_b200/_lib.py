@@ -77,6 +77,8 @@ SIGNATURES = {
     "sm_motion_compensation": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _DP, _VP]),
     "sm_motion_compensation_device": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _DP, _VP, _VP]),
     "sm_voxel_grid_filter": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_float, _VP, C.POINTER(C.c_int64)]),
+    "sm_voxel_grid_filter_ordered": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_float, C.c_int32, _VP,
+                                               C.POINTER(C.c_int64)]),
     "sm_m2dp_descriptor_length": (C.c_int64, [C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32]),
     "sm_m2dp": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_int32, C.c_int32, C.c_int32,
                           _VP, C.c_int64, _VP]),
@@ -88,6 +90,7 @@ SIGNATURES = {
     "sm_filter_chain_validate": (C.c_int, [_VP, C.c_int]),
     "sm_filter_chain_set_option": (C.c_int, [_VP, C.c_char_p, C.c_char_p]),
     "sm_filter_chain_set_random_sampler": (C.c_int, [_VP, C.c_int, C.c_int32, C.c_uint32]),
+    "sm_filter_chain_set_voxel_order": (C.c_int, [_VP, C.c_int, C.c_int32]),
     "sm_filter_chain_run": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP]),
     "sm_filter_chain_run_device": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP, C.POINTER(C.c_int64), _VP, _VP]),
     "sm_filter_chain_depth_cluster": (C.c_int, [_VP, C.c_int, _VP, C.c_int64, C.c_int64, _VP, _VP, _VP,
@@ -174,6 +177,10 @@ SIGNATURES = {
     "sm_debug_filter_mt19937_flags": (C.c_int, [C.c_int, C.c_int64, C.c_float, C.c_uint32, _VP, C.POINTER(C.c_int64)]),
     "sm_debug_nth_element": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, _VP]),
     "sm_debug_normals_nth_perm": (C.c_int, [C.c_int, _VP, C.c_int64, _VP]),
+    "sm_debug_voxel_bucket_counts_host": (C.c_int, [C.c_int64, _VP]),
+    "sm_debug_voxel_hash_host": (C.c_int, [_VP, C.c_int64, _VP]),
+    "sm_debug_voxel_unordered_epochs": (C.c_int, [C.c_int, _VP, C.c_int64, C.c_int64, C.c_float, _VP, _VP, _VP,
+                                                  C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "sm_debug_filter_ground_removal2": (C.c_int, [C.c_int, _VP, C.c_int32, _VP, C.c_int64, C.c_int64, C.c_int32, _VP, _VP,
                                                   _VP, _VP, _VP, _VP, _VP]),
     "sm_debug_depth_edge_host": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, C.c_int64, _VP, _VP, _VP]),

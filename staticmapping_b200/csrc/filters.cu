@@ -561,7 +561,7 @@ FilterParams filter_defaults(int kind) {
   if (kind == kFilterGroundRemoval) {                                                  // in AxisRange's storage
     f.min_point_num_in_voxel = 10; f.leaf_size = 0.8f; f.height_threshold = 0.15f;
   }
-  if (kind == kFilterVoxelGrid) f.voxel_size = 0.1f;                                   // in Range's storage
+  if (kind == kFilterVoxelGrid) { f.voxel_size = 0.1f; f.voxel_order = SM_VOXEL_ORDER_ASCENDING; }   // likewise
   if (kind == kFilterRandomSampler) { f.sampler_mode = SM_FILTER_SAMPLER_HASH; f.sampler_seed = 0; }   // likewise
   return f;
 }
@@ -812,7 +812,7 @@ int FilterChain::record_stage(const FilterParams& f, const char* in, const uint3
       fault = "Check failed: StatisticRemoval between 1 and point_num_meank finite points (PCL reads past its k-list)";
     if (rc == SM_ERR_BAD_ARGUMENT) fault = "StatisticRemoval: more finite points than the 24-level k-d tree holds";
   } else {
-    rc = voxel.run(in, n, stride, f.voxel_size, index_in, out, index_out, m, s);
+    rc = voxel.run(in, n, stride, f.voxel_size, f.voxel_order, index_in, out, index_out, m, s);
     if (rc == SM_ERR_BAD_ARGUMENT) fault = "VoxelGrid: the finite points span 2^21 voxels or more along an axis";
   }
   return rc;
@@ -959,6 +959,16 @@ int sm_filter_chain_set_random_sampler(sm_filter_chain* c, int filter, int32_t m
     return c->fail(SM_ERR_BAD_ARGUMENT, "RandomSampler mode must be 0..1");
   f.sampler_mode = mode;
   f.sampler_seed = seed;
+  return SM_OK;
+}
+
+int sm_filter_chain_set_voxel_order(sm_filter_chain* c, int filter, int32_t order) {
+  if (!c || filter < 0 || filter >= (int)c->chain.filters.size()) return SM_ERR_BAD_ARGUMENT;
+  FilterParams& f = c->chain.filters[filter];
+  if (f.kind != kFilterVoxelGrid) return c->fail(SM_ERR_BAD_ARGUMENT, "filter %d is not a VoxelGrid", filter);
+  if (order != SM_VOXEL_ORDER_ASCENDING && order != SM_VOXEL_ORDER_UNORDERED_MAP)
+    return c->fail(SM_ERR_BAD_ARGUMENT, "VoxelGrid order must be 0..1");
+  f.voxel_order = order;
   return SM_OK;
 }
 

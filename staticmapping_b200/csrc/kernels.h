@@ -461,7 +461,7 @@ struct FilterParams {
   union {
     struct { float min_range, max_range; };                         // Range
     struct { int32_t point_num_meank; float std_mul; };             // StatisticRemoval
-    struct { float voxel_size; };                                   // VoxelGrid
+    struct { float voxel_size; int32_t voxel_order; };              // VoxelGrid (sm_filter_chain_set_voxel_order)
     struct { int32_t sampler_mode; uint32_t sampler_seed; };        // RandomSampler (sm_filter_chain_set_random_sampler)
   };
   union {
@@ -605,17 +605,38 @@ struct StatisticRemoval {
 // ---- voxel_filter.cu ---------------------------------------------------------------------------
 // The device buffers of one VoxelGrid::Filter (filter_voxel_grid.cc:37-78), shared by sm_voxel_grid_filter and the
 // chain's stage.  reserve() sizes them for n records; they only grow.  run(): n >= 1 records of `stride` (>= 16)
-// bytes in device memory, x, y, z, intensity first -> one record per voxel in out (capacity n records), in ascending
-// (ix, iy, iz), the voxel's mean with factor 0, *m; returns after the stream has finished.  out_index (optional,
-// capacity n): the scan index (index_in, null = identity) of each voxel's first member in input order.  Points with
-// a NaN / inf quotient are dropped.  voxel > 1e-6 (the caller checks).  SM_ERR_BAD_ARGUMENT: the finite points span
-// 2^21 voxels or more along an axis; out and out_index have been written then.
+// bytes in device memory, x, y, z, intensity first -> one record per voxel in out (capacity n records), in the
+// sm_voxel_order `order` (the caller checks it), the voxel's mean with factor 0, *m; returns after the stream has
+// finished.  out_index (optional, capacity n): the scan index (index_in, null = identity) of each voxel's first member
+// in input order.  Points with a NaN / inf quotient are dropped.  voxel > 1e-6 (the caller checks).
+// SM_ERR_BAD_ARGUMENT: the finite points span 2^21 voxels or more along an axis; out and out_index may have been
+// written then.
+// SM_VOXEL_ORDER_UNORDERED_MAP keeps, per voxel in insertion rank t (the order of first members): its hash, its
+// ascending index, its first member and its list position; epoch_trace (test hook), when set, receives the positions
+// of the voxels present after every rehash epoch.
 struct VoxelGrid {
   DevBuf sort, tile_cnt, voxel_start, sorted, meta;
+  DevBuf mark, rank_cnt, by_rank, table, staged;   // SM_VOXEL_ORDER_UNORDERED_MAP only
+  std::vector<std::vector<uint32_t>>* epoch_trace = nullptr;
   int reserve(int64_t n);
-  int run(const char* pts, int64_t n, int64_t stride, float voxel, const uint32_t* index_in, float* out,
-          uint32_t* out_index, int64_t* m, cudaStream_t s);
+  int run(const char* pts, int64_t n, int64_t stride, float voxel, int32_t order, const uint32_t* index_in,
+          float* out, uint32_t* out_index, int64_t* m, cudaStream_t s);
+  int64_t rank_stride = 0;                         // by_rank holds five arrays of this many entries
+  uint64_t* hash() const { return (uint64_t*)by_rank.p; }
+  uint32_t* asc() const { return (uint32_t*)(hash() + rank_stride); }
+  uint32_t* first() const { return asc() + rank_stride; }
+  uint32_t* pos() const { return asc() + 2 * rank_stride; }
+  uint32_t* bucket() const { return asc() + 3 * rank_stride; }
+
+ private:
+  int unordered_emit(const char* pts, int n, int64_t stride, float voxel, const uint32_t* index_in, float* out,
+                     uint32_t* out_index, int64_t* m, cudaStream_t s);
 };
+// std::unordered_map's rehash epochs for m distinct inserts, from the libstdc++ this library is built with: pairs
+// (c_e, B_e), the insert of key c_e rehashes to B_e buckets; the first pair is (0, B_0).  Cached up to the largest m.
+std::vector<std::pair<int64_t, uint64_t>> unordered_map_epochs(int64_t m);
+// common/eigen_hash.h:31-43 on an int key (test hook sm_debug_voxel_hash_host)
+uint64_t vf_debug_hash_host(const int32_t* k3);
 
 // ---- plane_sampler.cu --------------------------------------------------------------------------
 // what Detect did with a voxel (plane_detector.h:103-152): skipped (fewer than min points), the z-range rule (iz <= 0)

@@ -1117,4 +1117,52 @@ int sm_debug_normals_nth_perm(int device, const double* points_3n, int64_t n, in
   return SM_OK;
 }
 
+int sm_debug_voxel_bucket_counts_host(int64_t m, uint64_t* out_m) {
+  if (m < 0 || m > (1 << 30) || (m > 0 && !out_m)) return SM_ERR_BAD_ARGUMENT;
+  const std::vector<std::pair<int64_t, uint64_t>> epochs = unordered_map_epochs(m);
+  for (size_t e = 0; e < epochs.size(); ++e) {
+    const int64_t end = e + 1 < epochs.size() ? epochs[e + 1].first : m;
+    for (int64_t k = epochs[e].first; k < end; ++k) out_m[k] = epochs[e].second;
+  }
+  return SM_OK;
+}
+
+int sm_debug_voxel_hash_host(const int32_t* keys_3n, int64_t n, uint64_t* out_n) {
+  if (n < 0 || (n > 0 && (!keys_3n || !out_n))) return SM_ERR_BAD_ARGUMENT;
+  for (int64_t i = 0; i < n; ++i) out_n[i] = vf_debug_hash_host(keys_3n + 3 * i);
+  return SM_OK;
+}
+
+// test hook: VoxelGrid::run in SM_VOXEL_ORDER_UNORDERED_MAP with its per-epoch positions
+int sm_debug_voxel_unordered_epochs(int device, const float* points, int64_t n, int64_t stride_bytes,
+                                    float voxel_size, uint64_t* hash_m, int32_t* rank_m, int32_t* pos,
+                                    int64_t capacity, int64_t* m_out, int32_t* n_epochs) {
+  if (!points || !hash_m || !rank_m || !m_out || !n_epochs || n <= 0 || n > (1 << 30) || stride_bytes < 16 ||
+      stride_bytes % 4 || !(voxel_size > 1.e-6f) || capacity < 0 || (capacity > 0 && !pos))
+    return SM_ERR_BAD_ARGUMENT;
+  SMB_RC(select_device(device));
+  DevBuf d_in, d_out;
+  SMB_RC(d_in.reserve((size_t)n * (size_t)stride_bytes));
+  SMB_RC(d_out.reserve((size_t)n * 20));
+  SMB_CUDA_OK(cudaMemcpy(d_in.p, points, (size_t)n * (size_t)stride_bytes, cudaMemcpyHostToDevice));
+  VoxelGrid vg;
+  std::vector<std::vector<uint32_t>> trace;
+  vg.epoch_trace = &trace;
+  int64_t m = 0;
+  SMB_RC(vg.run((const char*)d_in.p, n, stride_bytes, voxel_size, SM_VOXEL_ORDER_UNORDERED_MAP, nullptr,
+                (float*)d_out.p, nullptr, &m, nullptr));
+  *m_out = m;
+  *n_epochs = (int32_t)trace.size();
+  if (m == 0) return SM_OK;
+  std::vector<uint64_t> hash((size_t)m);
+  std::vector<uint32_t> asc((size_t)m);
+  SMB_CUDA_OK(cudaMemcpy(hash.data(), vg.hash(), (size_t)m * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  SMB_CUDA_OK(cudaMemcpy(asc.data(), vg.asc(), (size_t)m * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  for (int64_t t = 0; t < m; ++t) { hash_m[asc[t]] = hash[t]; rank_m[asc[t]] = (int32_t)t; }
+  if (capacity < m * (int64_t)trace.size()) return SM_ERR_BAD_ARGUMENT;
+  for (size_t e = 0; e < trace.size(); ++e)
+    for (int64_t t = 0; t < m; ++t) pos[e * m + t] = t < (int64_t)trace[e].size() ? (int32_t)trace[e][t] : -1;
+  return SM_OK;
+}
+
 }  // extern "C"

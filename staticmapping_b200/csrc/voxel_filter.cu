@@ -9,11 +9,30 @@
 // -> segment heads -> points gathered into voxel order -> one warp per voxel adds the four double
 // chains in order (addends staged through shared memory, like ndt_leaf_kernel) -> one output
 // point per voxel; in the filter chain, also the scan index of each voxel's first member.  Every output value is bit-identical to the reference's; the ORDER of the
-// output points is ascending (ix, iy, iz), whereas the reference's is the iteration order of a
-// libstdc++ unordered_map (an accident of its rehash history; nothing downstream depends on it
-// beyond summation order).  Compiled with -fmad=false.
+// output points is ascending (ix, iy, iz) by default (SM_VOXEL_ORDER_ASCENDING), whereas the reference's is
+// the iteration order of a libstdc++ unordered_map.  That order matters downstream: CalculateNormals in
+// std::nth_element's order permutes the one index array it is given, so its leaves, their summation order
+// and representatives, and its column order all follow the voxel order.  SM_VOXEL_ORDER_UNORDERED_MAP
+// reproduces the container's order (DESIGN §4f):
+//   libstdc++ keeps all nodes in one singly linked list in which every bucket is one contiguous run.  An insert
+//   into a non-empty bucket goes to the head of its run, one into an empty bucket to the front of the list; a
+//   rehash to B buckets walks the old list front to back and moves each node to the front of the new list if its
+//   new bucket is still empty, else to the head of that bucket's run.  Between two rehashes (an epoch e, from
+//   c_e distinct keys on, B_e buckets, n_e keys at its end) the list is therefore sorted by (run key, within-run
+//   key).  With t the insertion rank, r the position before the epoch's rehash and v = r for a voxel present
+//   before it (t < c_e), v = t for one of the epoch's own: run key = n_e - 1 - (min v over the bucket), within-run
+//   key = n_e - 1 - v.  Every old r is below every new t, so both keys put new runs before old ones and, inside a
+//   run, new voxels (latest first) before old ones (last position first).
+//   Each epoch is one bucket-min pass (atomicMin over B_e entries) and one radix sort of the n_e voxels
+//   present on a key of 2 * ceil(log2 n_e) bits: about 2 m sorted keys over about log2 m epochs.
+// Compiled with -fmad=false.
 #include <limits.h>
 #include <math.h>
+
+#include <mutex>
+#include <unordered_map>
+#include <utility>
+#include <vector>
 
 #include "../../include/sm_b200.h"
 #include "common.cuh"
@@ -149,7 +168,124 @@ vf_first_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__
   out_index[v] = index_in ? index_in[i] : i;
 }
 
+// common/eigen_hash.h:31-43 with Scalar = int: boost's hash_combine on a 64-bit size_t over std::hash<int>, which
+// sign-extends
+__host__ __device__ __forceinline__ uint64_t vf_hash(const int32_t* k) {
+  uint64_t seed = 0;
+  for (int i = 0; i < 3; ++i) seed ^= (uint64_t)(int64_t)k[i] + 0x9e3779b9ull + (seed << 6) + (seed >> 2);
+  return seed;
+}
+
+// mark[first member of voxel v] = v (ascending voxel index); mark is ~0u elsewhere
+__global__ void __launch_bounds__(256)
+vf_mark_kernel(const uint32_t* __restrict__ order, const uint32_t* __restrict__ voxel_start,
+               const uint32_t* __restrict__ n_voxels_dev, uint32_t* __restrict__ mark) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= (int64_t)*n_voxels_dev) return;
+  mark[order[voxel_start[v]]] = (uint32_t)v;
+}
+
+__global__ void __launch_bounds__(kCompactThreads)
+vf_rank_count_kernel(const uint32_t* __restrict__ mark, int n, uint32_t* __restrict__ tile_cnt) {
+  uint32_t c = 0;
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  for (int r = 0; r < kCompactItems; ++r) if (base + r < n) c += mark[base + r] != ~0u;
+  tile_count_store(c, tile_cnt);
+}
+
+// the first members in input order: voxel of insertion rank t -> its ascending index, first member and hash.  The key
+// is int(lround(.)) as the reference forms it: a long past int's range wraps, as on GCC (no two voxels within the
+// key's 2^21 span can meet so).
+__global__ void __launch_bounds__(kCompactThreads)
+vf_rank_scatter_kernel(const char* __restrict__ pts, int64_t stride, float voxel, const uint32_t* __restrict__ mark,
+                       int n, const uint32_t* __restrict__ tile_off, uint64_t* __restrict__ hash,
+                       uint32_t* __restrict__ asc, uint32_t* __restrict__ first) {
+  const int base = blockIdx.x * kCompactTile + threadIdx.x * kCompactItems;
+  uint32_t c = 0;
+  for (int r = 0; r < kCompactItems; ++r) if (base + r < n) c += mark[base + r] != ~0u;
+  uint32_t t = tile_exclusive(c, tile_off);
+  for (int r = 0; r < kCompactItems; ++r) {
+    const int i = base + r;
+    if (i >= n || mark[i] == ~0u) continue;
+    long long ix, iy, iz;
+    vf_index(reinterpret_cast<const float*>(pts + (int64_t)i * stride), voxel, &ix, &iy, &iz);   // finite: a member
+    const int32_t k[3] = {(int32_t)ix, (int32_t)iy, (int32_t)iz};
+    hash[t] = vf_hash(k);
+    asc[t] = mark[i];
+    first[t] = (uint32_t)i;
+    ++t;
+  }
+}
+
+// epoch [c, ne) with `buckets` buckets: table[b] = min v over the voxels present in bucket b (v = pos for t < c,
+// t for the epoch's own inserts)
+__global__ void __launch_bounds__(256)
+vf_bucket_min_kernel(const uint64_t* __restrict__ hash, const uint32_t* __restrict__ pos, int ne, int c,
+                     uint64_t buckets, uint32_t* __restrict__ bucket, uint32_t* __restrict__ table) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= ne) return;
+  const uint32_t b = (uint32_t)(hash[t] % buckets);   // _Mod_range_hashing
+  bucket[t] = b;
+  atomicMin(&table[b], t < c ? pos[t] : (uint32_t)t);
+}
+
+// the list position of every voxel after the epoch's rehash and inserts, as one sort key: run key, within-run key
+__global__ void __launch_bounds__(256)
+vf_epoch_key_kernel(const uint32_t* __restrict__ pos, const uint32_t* __restrict__ bucket,
+                    const uint32_t* __restrict__ table, int ne, int c, int bits, uint64_t* __restrict__ keys,
+                    uint32_t* __restrict__ vals) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= ne) return;
+  const uint32_t top = (uint32_t)(ne - 1), v = t < c ? pos[t] : (uint32_t)t;
+  keys[t] = ((uint64_t)(top - table[bucket[t]]) << bits) | (uint64_t)(top - v);
+  vals[t] = (uint32_t)t;
+}
+
+__global__ void __launch_bounds__(256)
+vf_epoch_pos_kernel(const uint32_t* __restrict__ sorted_vals, int ne, uint32_t* __restrict__ pos) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < ne) pos[sorted_vals[p]] = (uint32_t)p;
+}
+
+// voxel of rank t -> its list position: its mean record and the scan index of its first member
+__global__ void __launch_bounds__(256)
+vf_emit_kernel(const float* __restrict__ staged, const uint32_t* __restrict__ asc, const uint32_t* __restrict__ first,
+               const uint32_t* __restrict__ pos, int m, const uint32_t* __restrict__ index_in, float* __restrict__ out,
+               uint32_t* __restrict__ out_index) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  const int64_t p = pos[t], a = asc[t];
+#pragma unroll
+  for (int k = 0; k < 5; ++k) out[5 * p + k] = staged[5 * a + k];
+  if (out_index) out_index[p] = index_in ? index_in[first[t]] : first[t];
+}
+
+// The schedule of a default-constructed std::unordered_map, from the policy object the container itself consults
+// before every insert (_Hashtable::_M_insert_unique_node): _M_need_rehash(bucket count, element count, 1).
+struct RehashSchedule {
+  std::mutex mu;
+  std::__detail::_Prime_rehash_policy policy;
+  uint64_t buckets = 1;                                // the single bucket of an empty map
+  int64_t done = 0;                                    // element counts 0 .. done - 1 have been asked about
+  std::vector<std::pair<int64_t, uint64_t>> epochs;
+};
+
 }  // namespace
+
+std::vector<std::pair<int64_t, uint64_t>> unordered_map_epochs(int64_t m) {
+  static RehashSchedule sch;
+  std::lock_guard<std::mutex> lock(sch.mu);
+  for (; sch.done < m; ++sch.done) {
+    const std::pair<bool, size_t> r = sch.policy._M_need_rehash(sch.buckets, (size_t)sch.done, 1);
+    if (r.first) sch.buckets = r.second;
+    if (r.first || sch.done == 0) sch.epochs.emplace_back(sch.done, sch.buckets);
+  }
+  std::vector<std::pair<int64_t, uint64_t>> out;
+  for (const auto& e : sch.epochs) if (e.first < m) out.push_back(e);
+  return out;
+}
+
+uint64_t vf_debug_hash_host(const int32_t* k3) { return vf_hash(k3); }
 
 // host build of the voxel index of one point (test hook sm_debug_voxel_index op 0)
 bool vf_debug_index_host(const float* p, float voxel, long long* ixyz) { return vf_index(p, voxel, &ixyz[0], &ixyz[1], &ixyz[2]); }
@@ -163,8 +299,67 @@ int VoxelGrid::reserve(int64_t n) {
   return meta.reserve(8 * sizeof(long long));
 }
 
-int VoxelGrid::run(const char* pts, int64_t n, int64_t stride, float voxel, const uint32_t* index_in, float* out,
-                   uint32_t* out_index, int64_t* m, cudaStream_t s) {
+// SM_VOXEL_ORDER_UNORDERED_MAP, after vf_mean_kernel has written the ascending records into `staged`: the insertion
+// ranks, then one pass per rehash epoch, then every record to its list position
+int VoxelGrid::unordered_emit(const char* pts, int n, int64_t stride, float voxel, const uint32_t* index_in,
+                              float* out, uint32_t* out_index, int64_t* m, cudaStream_t s) {
+  const int tiles = compact_tiles(n);
+  const int64_t st = (n + 63) & ~(int64_t)63;
+  RadixPairs rp;
+  rp.carve(sort.p, st);
+  uint32_t* tc = (uint32_t*)tile_cnt.p;
+  uint32_t* mk = (uint32_t*)mark.p;
+  uint32_t* rc = (uint32_t*)rank_cnt.p;
+  rank_stride = n;
+  SMB_CUDA_OK(cudaMemsetAsync(mk, 0xff, (size_t)n * sizeof(uint32_t), s));
+  vf_mark_kernel<<<ceil_div(n, 256), 256, 0, s>>>(rp.vals[0], (const uint32_t*)voxel_start.p, tc + tiles, mk);
+  vf_rank_count_kernel<<<tiles, kCompactThreads, 0, s>>>(mk, n, rc);
+  compact_scan(rc, tiles, s);
+  vf_rank_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, voxel, mk, n, rc, hash(), asc(), first());
+  SMB_CUDA_OK(cudaGetLastError());
+  uint32_t voxels = 0;
+  long long host_meta[8] = {0};
+  SMB_CUDA_OK(cudaMemcpyAsync(&voxels, tc + tiles, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaMemcpyAsync(host_meta, meta.p, sizeof(host_meta), cudaMemcpyDeviceToHost, s));
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  if (host_meta[4]) return SM_ERR_BAD_ARGUMENT;
+  const int mv = (int)voxels;
+  *m = mv;
+  if (mv == 0) return SM_OK;
+  const std::vector<std::pair<int64_t, uint64_t>> epochs = unordered_map_epochs(mv);
+  SMB_RC(table.reserve((size_t)epochs.back().second * sizeof(uint32_t)));
+  uint32_t* tb = (uint32_t*)table.p;
+  uint32_t* ps = pos();
+  uint32_t* bk = bucket();
+  if (epoch_trace) epoch_trace->clear();
+  for (size_t e = 0; e < epochs.size(); ++e) {
+    const int c = (int)epochs[e].first;
+    const int ne = e + 1 < epochs.size() ? (int)epochs[e + 1].first : mv;
+    const uint64_t buckets = epochs[e].second;
+    const int bits = ne > 1 ? 64 - __builtin_clzll((unsigned long long)(ne - 1)) : 1;
+    const int passes = (2 * bits + 7) / 8;
+    SMB_CUDA_OK(cudaMemsetAsync(tb, 0xff, (size_t)buckets * sizeof(uint32_t), s));
+    vf_bucket_min_kernel<<<ceil_div(ne, 256), 256, 0, s>>>(hash(), ps, ne, c, buckets, bk, tb);
+    vf_epoch_key_kernel<<<ceil_div(ne, 256), 256, 0, s>>>(ps, bk, tb, ne, c, bits, rp.keys[0], rp.vals[0]);
+    SMB_RC(radix_sort_pairs_u64(rp.keys[0], rp.vals[0], rp.keys[1], rp.vals[1], ne, 1, st, rp.scratch, s, passes));
+    vf_epoch_pos_kernel<<<ceil_div(ne, 256), 256, 0, s>>>(rp.vals[passes & 1], ne, ps);
+    SMB_CUDA_OK(cudaGetLastError());
+    if (epoch_trace) {
+      epoch_trace->emplace_back((size_t)ne);
+      SMB_CUDA_OK(cudaMemcpyAsync(epoch_trace->back().data(), ps, (size_t)ne * sizeof(uint32_t),
+                                  cudaMemcpyDeviceToHost, s));
+      SMB_CUDA_OK(cudaStreamSynchronize(s));
+    }
+  }
+  vf_emit_kernel<<<ceil_div(mv, 256), 256, 0, s>>>((const float*)staged.p, asc(), first(), ps, mv, index_in, out,
+                                                   out_index);
+  SMB_CUDA_OK(cudaGetLastError());
+  SMB_CUDA_OK(cudaStreamSynchronize(s));
+  return SM_OK;
+}
+
+int VoxelGrid::run(const char* pts, int64_t n, int64_t stride, float voxel, int32_t order, const uint32_t* index_in,
+                   float* out, uint32_t* out_index, int64_t* m, cudaStream_t s) {
   const int ni = (int)n;
   const int tiles = compact_tiles(n);
   const int64_t st = (n + 63) & ~(int64_t)63;
@@ -185,6 +380,14 @@ int VoxelGrid::run(const char* pts, int64_t n, int64_t stride, float voxel, cons
   compact_scan(tc, tiles, s);                                                   // tc[tiles] = number of voxels
   vf_heads_scatter_kernel<<<tiles, kCompactThreads, 0, s>>>(rp.keys[0], ni, tc, vs, mt);
   vf_gather_kernel<<<ceil_div(n, 256), 256, 0, s>>>(pts, stride, rp.vals[0], ni, sd);
+  if (order == SM_VOXEL_ORDER_UNORDERED_MAP) {
+    SMB_RC(mark.reserve((size_t)n * sizeof(uint32_t)));
+    SMB_RC(rank_cnt.reserve(compact_count_bytes(n)));
+    SMB_RC(by_rank.reserve((size_t)n * (sizeof(uint64_t) + 4 * sizeof(uint32_t))));
+    SMB_RC(staged.reserve((size_t)n * 5 * sizeof(float)));
+    vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sd, vs, tc + tiles, (float*)staged.p);
+    return unordered_emit(pts, ni, stride, voxel, index_in, out, out_index, m, s);
+  }
   vf_mean_kernel<<<ceil_div((int64_t)n * 32, 256), 256, 0, s>>>(sd, vs, tc + tiles, out);
   if (out_index) vf_first_kernel<<<ceil_div(n, 256), 256, 0, s>>>(rp.vals[0], vs, tc + tiles, index_in, out_index);
   SMB_CUDA_OK(cudaGetLastError());
@@ -204,8 +407,15 @@ using namespace smb;
 
 extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, int64_t stride_bytes,
                                     float voxel_size, float* out, int64_t* m_out) {
+  return sm_voxel_grid_filter_ordered(device, points, n, stride_bytes, voxel_size, SM_VOXEL_ORDER_ASCENDING, out,
+                                      m_out);
+}
+
+extern "C" int sm_voxel_grid_filter_ordered(int device, const float* points, int64_t n, int64_t stride_bytes,
+                                            float voxel_size, int32_t order, float* out, int64_t* m_out) {
   if (!points || !out || !m_out || n < 0 || n > (1 << 30) || stride_bytes < 16 || stride_bytes % 4 ||
-      !(voxel_size > 1.e-6f))       // ConfigsValid(), filter_voxel_grid.cc:35
+      !(voxel_size > 1.e-6f) ||     // ConfigsValid(), filter_voxel_grid.cc:35
+      (order != SM_VOXEL_ORDER_ASCENDING && order != SM_VOXEL_ORDER_UNORDERED_MAP))
     return SM_ERR_BAD_ARGUMENT;
   SMB_RC(select_device(device));
   *m_out = 0;
@@ -218,7 +428,7 @@ extern "C" int sm_voxel_grid_filter(int device, const float* points, int64_t n, 
   cudaStream_t s = nullptr;
   SMB_CUDA_OK(cudaMemcpyAsync(d_in.p, points, in_bytes, cudaMemcpyHostToDevice, s));
   int64_t m = 0;
-  SMB_RC(vg.run((const char*)d_in.p, n, stride_bytes, voxel_size, nullptr, (float*)d_out.p, nullptr, &m, s));
+  SMB_RC(vg.run((const char*)d_in.p, n, stride_bytes, voxel_size, order, nullptr, (float*)d_out.p, nullptr, &m, s));
   if (m > 0) SMB_CUDA_OK(cudaMemcpy(out, d_out.p, (size_t)m * 5 * sizeof(float), cudaMemcpyDeviceToHost));
   *m_out = m;
   return SM_OK;

@@ -155,6 +155,14 @@ class Factory(_RecordFilter):
         self._check(self._lib.sm_filter_chain_set_random_sampler(self._h, int(filter_index), int(mode),
                                                                  int(seed) & 0xFFFFFFFF), "set_random_sampler")
 
+    def SetVoxelOrder(self, filter_index, order):
+        """The emission order of the chain's VoxelGrid `filter_index`, a VoxelOrder (ASCENDING by default;
+        UNORDERED_MAP is the reference's std::unordered_map order).  Each record keeps the scan index of its voxel's
+        first member.  A filter that is not a VoxelGrid or an unknown order raises ValueError and leaves the chain
+        unchanged.  See sm_filter_chain_set_voxel_order."""
+        self._check(self._lib.sm_filter_chain_set_voxel_order(self._h, int(filter_index), int(order)),
+                    "set_voxel_order")
+
     def SetAllFilters(self, flag):
         """True: the filters added from now on may also be GroundRemoval, StatisticRemoval and VoxelGrid, whose chain
         stages are the GPU filters of GroundRemoval, StatisticRemoval and VoxelGridFilter (include/sm_b200.h, the

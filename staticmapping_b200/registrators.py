@@ -93,6 +93,14 @@ class NormalsOrder(enum.IntEnum):
     NTH_ELEMENT = 1
 
 
+class VoxelOrder(enum.IntEnum):
+    """The order VoxelGrid emits its voxels in.  ASCENDING (the default) is ascending (ix, iy, iz); UNORDERED_MAP is
+    the reference's own, the iteration order of its std::unordered_map as libstdc++ leaves it after inserting the
+    voxels in the order of their first member.  See sm_voxel_grid_filter_ordered."""
+    ASCENDING = 0
+    UNORDERED_MAP = 1
+
+
 @dataclass
 class EigenCloud:
     """data::EigenPointCloud (cloud_types.h:121-147): (N,3) float64 points, optional normals.
@@ -650,18 +658,24 @@ def AverageTransforms(transforms):
     return out
 
 
-def VoxelGridFilter(cloud, voxel_size, device=0):
+def VoxelGridFilter(cloud, voxel_size, device=0, order=VoxelOrder.ASCENDING):
     """pre_processers::filter::VoxelGrid::Filter (pre_processors/filter_voxel_grid.cc:37-78) on
-    the GPU.  `cloud`: (N,5) float32 InnerPointType rows; returns the (M,5) voxel means in
-    ascending (ix, iy, iz) order (the reference's order is std::unordered_map iteration order)."""
+    the GPU.  `cloud`: (N,5) float32 InnerPointType rows; returns the (M,5) voxel means in the
+    VoxelOrder `order`: ascending (ix, iy, iz) by default, UNORDERED_MAP for the reference's
+    std::unordered_map iteration order."""
     lib = _lib.lib()
     pts = np.ascontiguousarray(np.asarray(cloud, dtype=np.float32))
     if pts.ndim != 2 or pts.shape[1] != 5:
         raise ValueError("cloud must be (N,5): x, y, z, intensity, factor")
     out = np.empty_like(pts)
     m = C.c_int64(0)
-    rc = lib.sm_voxel_grid_filter(device, pts.ctypes.data, pts.shape[0], 20, float(voxel_size), out.ctypes.data,
-                                  C.byref(m))
+    order = VoxelOrder(order)
+    if order == VoxelOrder.ASCENDING:
+        rc = lib.sm_voxel_grid_filter(device, pts.ctypes.data, pts.shape[0], 20, float(voxel_size), out.ctypes.data,
+                                      C.byref(m))
+    else:
+        rc = lib.sm_voxel_grid_filter_ordered(device, pts.ctypes.data, pts.shape[0], 20, float(voxel_size),
+                                              int(order), out.ctypes.data, C.byref(m))
     if rc == -20:
         raise RuntimeError("staticmapping_b200: no CUDA device (no CPU fallback)")
     if rc == -1:
