@@ -21,6 +21,13 @@
 
 #include "registrators/interface.h"
 #include "sm_b200.h"
+// MultiviewRegistratorLumPclB200 needs the multi-view base class, which not every tree has
+#if defined(__has_include)
+#if __has_include("registrators/multiview_registrator_interface.h")
+#include "registrators/multiview_registrator_interface.h"
+#define SM_B200_HAS_MULTIVIEW 1
+#endif
+#endif
 
 namespace static_map {
 namespace registrator {
@@ -585,6 +592,53 @@ class KnnB200 {
   int bucket_size_;
   int device_;
 };
+
+// registrator::MultiviewRegistratorLumPcl (registrators/multiview_registrator_lum_pcl.h:35-88) on the GPU, for a tree
+// that has registrators/multiview_registrator_interface.h.  Same base class and AlignAll; PCL's LUM with the
+// reference's fixed settings.  Each frame is copied to the device handle at the first AlignAll after AddNewCloud, so
+// a cloud changed after that is not seen again.  PointT holds float x, y, z at offset 0 (every PCL point type).
+#ifdef SM_B200_HAS_MULTIVIEW
+template <typename PointT>
+class MultiviewRegistratorLumPclB200 : public MultiviewInterface<PointT> {
+ public:
+  using PointCloudPtr = typename MultiviewInterface<PointT>::PointCloudPtr;
+
+  explicit MultiviewRegistratorLumPclB200(int device = 0) : MultiviewInterface<PointT>() {
+    this->type_ = kLumPCL;
+    CHECK_EQ(sm_lum_create(device, &lum_), 0);
+  }
+  ~MultiviewRegistratorLumPclB200() { sm_lum_destroy(lum_); }
+  MultiviewRegistratorLumPclB200(const MultiviewRegistratorLumPclB200&) = delete;
+  MultiviewRegistratorLumPclB200& operator=(const MultiviewRegistratorLumPclB200&) = delete;
+
+  void AlignAll(const PointCloudPtr& output) override {
+    auto& frames = MultiviewInterface<PointT>::inner_frames_;
+    for (size_t f = static_cast<size_t>(sm_lum_size(lum_)); f < frames.size(); ++f) {
+      const auto& cloud = frames[f].cloud->points;
+      CHECK_EQ(sm_lum_add_cloud(lum_, cloud.empty() ? nullptr : reinterpret_cast<const float*>(cloud.data()),
+                                static_cast<int64_t>(cloud.size()), sizeof(PointT), frames[f].pose.data()),
+               0)
+          << sm_lum_last_error(lum_);
+      sizes_.push_back(static_cast<int64_t>(cloud.size()));
+    }
+    const size_t n = frames.size(), v0 = vertex_frame_.size();
+    int64_t need = 0;
+    for (size_t v = 0; v < n; ++v) need += sizes_[v < v0 ? vertex_frame_[v] : v - v0];
+    std::vector<PointT> out(static_cast<size_t>(need));
+    int64_t m = 0;
+    CHECK_EQ(sm_lum_align_all(lum_, output && need ? reinterpret_cast<float*>(out.data()) : nullptr, need, &m), 0)
+        << sm_lum_last_error(lum_);
+    for (int r = 0; r < 5 && n; ++r)
+      for (size_t f = 0; f < n; ++f) vertex_frame_.push_back(static_cast<int>(f));
+    if (output) output->points.assign(out.begin(), out.end());
+  }
+
+ private:
+  sm_lum* lum_ = nullptr;
+  std::vector<int64_t> sizes_;      // points per frame
+  std::vector<int> vertex_frame_;   // the frame whose cloud vertex v holds
+};
+#endif
 
 }  // namespace registrator
 }  // namespace static_map

@@ -729,6 +729,34 @@ int sm_plane_sampler_indices(const sm_plane_sampler* sampler, int32_t* inliers_o
 int sm_plane_sampler_plane_indices(const sm_plane_sampler* sampler, int32_t* plane_or_null, int64_t* n_plane);
 const char* sm_plane_sampler_last_error(const sm_plane_sampler* sampler);
 
+/* ---- registrator::MultiviewRegistratorLumPcl (registrators/multiview_registrator_lum_pcl.h) ----------------------
+ * PCL's Lu-Milios globally consistent alignment (pcl::registration::LUM, PCL 1.8.1) over the frames given to
+ * sm_lum_add_cloud, with the reference's fixed settings: 5 rounds of AlignAll, 5 LUM iterations, convergence threshold
+ * 0.001, correspondences within 0.25 m.  Each AlignAll adds every frame again as a new graph vertex in each of its 5
+ * rounds, so after k calls on N frames the graph has 5kN vertices; vertex v is the v-th cloud ever added and keeps
+ * the pose LUM reached.  Records are stride_bytes apart with float x, y, z at offset 0; the rest of each record is
+ * copied to the output, so any PCL point type works.  All clouds of a handle share one stride.
+ *   sm_lum_add_cloud   MultiviewInterface::AddNewCloud: a copy of n records (n may be 0) and the frame's pose, a
+ *                      column-major Matrix4f.  SM_ERR_BAD_ARGUMENT: a null pose, a stride below 12 or not a multiple
+ *                      of 4 or unlike the first cloud's, more than 64 frames, more than 2^20 points in a frame.
+ *   sm_lum_size        the number of frames.
+ *   sm_lum_align_all   AlignAll(output): the output is getTransformedCloud(v) for v < N concatenated; *m_out = its
+ *                      record count.  A null out runs the alignment and writes nothing.  SM_ERR_BAD_ARGUMENT, before
+ *                      any work: more than 2^28 correspondence queries (the points of frame j summed over all pairs
+ *                      j < i; the search holds 16 bytes per query), capacity (records) below *m_out; after the search and before the graph changes: a
+ *                      vertex whose cloud has fewer points than the frame whose correspondence indices it is given
+ *                      (PCL reads past the cloud there).
+ *   sm_lum_poses       the graph's vertex poses, 6 floats (x, y, z, roll, pitch, yaw) per vertex; a null array
+ *                      returns the vertex count. */
+typedef struct sm_lum sm_lum;
+int sm_lum_create(int device, sm_lum** out);
+int sm_lum_destroy(sm_lum* h);
+int sm_lum_add_cloud(sm_lum* h, const float* points, int64_t n, int64_t stride_bytes, const float* pose_4x4);
+int64_t sm_lum_size(const sm_lum* h);
+int sm_lum_align_all(sm_lum* h, float* out, int64_t capacity, int64_t* m_out);
+int sm_lum_poses(const sm_lum* h, float* out_or_null, int64_t capacity, int64_t* n_vertices);
+const char* sm_lum_last_error(const sm_lum* h);
+
 int sm_device_count(void);
 const char* sm_version(void);
 

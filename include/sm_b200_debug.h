@@ -482,6 +482,20 @@ int sm_debug_voxel_unordered_epochs(int device, const float* points, int64_t n, 
                                     float voxel_size, uint64_t* hash_m, int32_t* rank_m, int32_t* pos,
                                     int64_t capacity, int64_t* m_out, int32_t* n_epochs);
 
+/* MultiviewRegistratorLumPcl (sm_lum_*) stage hooks.
+ * sm_debug_lum_correspondences: the correspondences of frames (j, i), j < i, from the handle's last AlignAll, as
+ * (query index in frame j, match index in frame i) pairs ascending in query; a null array returns the count.
+ * sm_debug_lum_trace: clears the trace and records (enable != 0) or stops recording every LUM iteration of the
+ * AlignAll calls that follow.  sm_debug_lum_trace_get: iteration < 0 returns the number of recorded iterations in
+ * *n_edges; else that iteration's vertex count, edge count, per edge 67 floats (source vertex, target vertex, finite
+ * pairs, the 15 exact sums, D[6], s^2, cinv[36] row-major, cinvd[6]), X (6(n - 1) doubles), the poses after the update
+ * (6n floats) and the sum of the pose changes' norms.  Null arrays are skipped. */
+int sm_debug_lum_correspondences(const struct sm_lum* h, int32_t j, int32_t i, int32_t* pairs_or_null,
+                                 int64_t capacity, int64_t* n);
+int sm_debug_lum_trace(struct sm_lum* h, int32_t enable);
+int sm_debug_lum_trace_get(const struct sm_lum* h, int64_t iteration, int32_t* n_vertices, int32_t* n_edges,
+                           float* edges_or_null, double* x_or_null, float* poses_or_null, double* sum);
+
 #ifdef __cplusplus
 }
 #endif

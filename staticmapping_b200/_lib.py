@@ -195,6 +195,16 @@ SIGNATURES = {
     "sm_debug_plane_sampler_keep_host": (C.c_int, [C.c_float, C.c_int64, C.c_int64, _VP]),
     "sm_debug_plane_sampler_trace": (C.c_int, [_VP, C.c_int32]),
     "sm_debug_plane_sampler_voxels": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "sm_lum_create": (C.c_int, [C.c_int, C.POINTER(_VP)]),
+    "sm_lum_destroy": (C.c_int, [_VP]),
+    "sm_lum_add_cloud": (C.c_int, [_VP, _VP, C.c_int64, C.c_int64, _VP]),
+    "sm_lum_size": (C.c_int64, [_VP]),
+    "sm_lum_align_all": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "sm_lum_poses": (C.c_int, [_VP, _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "sm_lum_last_error": (C.c_char_p, [_VP]),
+    "sm_debug_lum_correspondences": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, C.c_int64, C.POINTER(C.c_int64)]),
+    "sm_debug_lum_trace": (C.c_int, [_VP, C.c_int32]),
+    "sm_debug_lum_trace_get": (C.c_int, [_VP, C.c_int64, _IP, _IP, _VP, _VP, _VP, _DP]),
     "sm_device_count": (C.c_int, []),
     "sm_version": (C.c_char_p, []),
 }

@@ -8,6 +8,9 @@
 #ifndef SM_B200_REDUCE_CUH_
 #define SM_B200_REDUCE_CUH_
 
+#include <math.h>
+#include <string.h>
+
 #include <cstdint>
 
 namespace smb {
@@ -117,6 +120,121 @@ __device__ __forceinline__ uint32_t block_scan_excl(uint32_t v, uint32_t* warp_t
     if (total) *total = __shfl_sync(0xffffffffu, xi, 31);
     return __shfl_sync(0xffffffffu, xi - x, w) + incl - v;
   }
+}
+
+// ---- exact float sums --------------------------------------------------------------------------------------------
+// A float is m * 2^(b - 150) with an integer mantissa m < 2^24 and a biased exponent b = 1..254 (subnormals: b = 0,
+// taken as b = 1 without the hidden bit), so a sum of floats is sum_b (sum of the m of bin b) * 2^(b - 150).  Each
+// bin's sum is an integer of magnitude below 2^24 * 2^31 < 2^63 for up to 2^31 terms: int64 bins added in any order
+// give the same bins, and a finish turns them into the value nearest the exact sum (ties to even), whatever the launch
+// shape.  StatisticRemoval sums non-negative terms (exact_finish, to double); LUM sums signed ones (exact_finish_float,
+// to float).
+constexpr int kExactBins = 255;       // biased float exponents 1..254; bin 0 counts +inf terms
+constexpr int kExactLimbs = 10;
+
+// bin and mantissa of a non-negative float or +inf (bin 0, mantissa 1: counted apart)
+__host__ __device__ __forceinline__ void exact_bin(float v, int* bin, uint32_t* mant) {
+  uint32_t u;
+#ifdef __CUDA_ARCH__
+  u = __float_as_uint(v);
+#else
+  memcpy(&u, &v, 4);
+#endif
+  const uint32_t e = (u >> 23) & 0xffu, f = u & 0x7fffffu;
+  if (e == 0xffu) { *bin = 0; *mant = 1u; return; }
+  *bin = e == 0u ? 1 : (int)e;
+  *mant = e == 0u ? f : (f | 0x800000u);
+}
+
+// limb = the integer N = sum_b sign * bins[b] * 2^(b - 1) (b = 1..254) over the bins of that sign (sign * bins[b] > 0),
+// in units of 2^-149: N < 2^308, ten 32-bit limbs, carried once.
+__host__ __device__ inline void exact_limbs(const int64_t* bins, int sign, uint64_t* limb) {
+  for (int j = 0; j < kExactLimbs; ++j) limb[j] = 0u;
+  for (int b = 1; b < kExactBins; ++b) {
+    const int64_t sv = sign > 0 ? bins[b] : -bins[b];
+    if (sv <= 0) continue;
+    const uint64_t v = (uint64_t)sv;
+    const int shift = b - 1, w = shift >> 5, s = shift & 31;
+    // v < 2^63 shifted by s < 32 spans three limbs; each limb gets < 2^32 per bin, 254 bins: no overflow of 64 bits
+    const uint64_t lo = (v << s) & 0xffffffffu;
+    const uint64_t mid = s ? ((v >> (32 - s)) & 0xffffffffu) : ((v >> 32) & 0xffffffffu);
+    const uint64_t hi = s ? (v >> (64 - s)) : 0u;
+    limb[w] += lo;
+    if (w + 1 < kExactLimbs) limb[w + 1] += mid;
+    if (w + 2 < kExactLimbs) limb[w + 2] += hi;
+  }
+  for (int j = 0; j + 1 < kExactLimbs; ++j) { limb[j + 1] += limb[j] >> 32; limb[j] &= 0xffffffffu; }
+}
+
+// N * 2^-149 (N in carried limbs) rounded to `bits` significant bits, ties to even, as a double (exact for bits <= 53)
+__host__ __device__ inline double exact_round(const uint64_t* limb, int bits) {
+  int top = kExactLimbs - 1;
+  while (top >= 0 && limb[top] == 0u) --top;
+  if (top < 0) return 0.0;
+  int msb = 31;
+  while (!((limb[top] >> msb) & 1u)) --msb;
+  const int nbits = top * 32 + msb + 1;              // N has nbits bits
+  if (nbits <= bits) {                                // exact
+    uint64_t m = 0u;
+    for (int j = top; j >= 0; --j) m = (m << 32) | limb[j];
+    return ldexp((double)m, -149);
+  }
+  // the top `bits` bits, the next (round) bit and whether any bit below it is set (sticky)
+  auto bit = [&](int p) -> uint64_t { return (limb[p >> 5] >> (p & 31)) & 1u; };
+  const int low = nbits - bits;                       // position of the least significant kept bit
+  uint64_t m = 0u;
+  for (int p = nbits - 1; p >= low; --p) m = (m << 1) | bit(p);
+  const uint64_t round = bit(low - 1);
+  bool sticky = false;
+  for (int p = low - 2; p >= 0 && !sticky; --p) sticky = bit(p) != 0u;
+  if (round && (sticky || (m & 1u))) ++m;            // m may become 2^bits: still exact in a double
+  return ldexp((double)m, low - 149);
+}
+
+// The double nearest sum_b bins[b] * 2^(b - 150) (b = 1..254, bins >= 0), +inf if bins[0] (the +inf terms) is not
+// zero.  limb: kExactLimbs words of scratch (shared memory on the device, where a dynamically indexed array would be
+// local)
+__host__ __device__ inline double exact_finish(const int64_t* bins, uint64_t* limb) {
+  if (bins[0] != 0) return __builtin_huge_val();
+  exact_limbs(bins, 1, limb);
+  return exact_round(limb, 53);
+}
+
+// Signed float terms: bins[1..254] hold signed mantissa sums (exact_bin of |v|, added with v's sign); bins[0], bins[255]
+// and bins[256] count the +inf, -inf and NaN terms.  kExactSignedBins int64 per sum.
+constexpr int kExactSignedBins = kExactBins + 2;
+
+__host__ __device__ __forceinline__ void exact_bin_signed(float v, int* bin, int64_t* mant) {
+  if (v != v) { *bin = kExactBins + 1; *mant = 1; return; }
+  uint32_t m;
+  exact_bin(fabsf(v), bin, &m);
+  if (*bin == 0) { *bin = v > 0.f ? 0 : kExactBins; *mant = 1; return; }
+  *mant = v < 0.f ? -(int64_t)m : (int64_t)m;
+}
+
+// The float nearest the exact sum (ties to even): NaN for a NaN term or for +inf and -inf terms together, else +-inf
+// for an infinite term, else the finite sum (+inf / -inf when it rounds past FLT_MAX; +0 when it is zero).
+// pos, neg: kExactLimbs words of scratch each.
+__host__ __device__ inline float exact_finish_float(const int64_t* bins, uint64_t* pos, uint64_t* neg) {
+  const bool pinf = bins[0] != 0, ninf = bins[kExactBins] != 0;
+  if (bins[kExactBins + 1] != 0 || (pinf && ninf)) return __builtin_nanf("");
+  if (pinf) return __builtin_huge_valf();
+  if (ninf) return -__builtin_huge_valf();
+  exact_limbs(bins, 1, pos);
+  exact_limbs(bins, -1, neg);
+  int cmp = 0;
+  for (int j = kExactLimbs - 1; j >= 0 && cmp == 0; --j) cmp = pos[j] > neg[j] ? 1 : (pos[j] < neg[j] ? -1 : 0);
+  if (cmp == 0) return 0.f;
+  uint64_t* a = cmp > 0 ? pos : neg;                 // a -= b, |a| > |b|
+  const uint64_t* b = cmp > 0 ? neg : pos;
+  uint64_t borrow = 0u;
+  for (int j = 0; j < kExactLimbs; ++j) {
+    const uint64_t sub = b[j] + borrow;
+    borrow = a[j] < sub ? 1u : 0u;
+    a[j] = (a[j] + (borrow << 32)) - sub;
+  }
+  const float r = (float)exact_round(a, 24);          // 24 bits and at least 2^-149: exactly a float (or past FLT_MAX)
+  return cmp > 0 ? r : -r;
 }
 
 }  // namespace smb

@@ -74,22 +74,22 @@ sr_pack_kernel(const char* __restrict__ pts, int64_t stride, int n, const uint8_
   if (blockIdx.x == 0 && threadIdx.x == 0) *nf = tile_off[gridDim.x];
 }
 
-// bins[0 .. kSrBins): the distances, bins[kSrBins ..): their float squares (zeroed before)
+// bins[0 .. kExactBins): the distances, bins[kExactBins ..): their float squares (zeroed before)
 __global__ void __launch_bounds__(kSrBinThreads)
 sr_bins_kernel(const float* __restrict__ dist, int n, unsigned long long* __restrict__ bins) {
-  __shared__ unsigned long long s[2 * kSrBins];
-  for (int b = threadIdx.x; b < 2 * kSrBins; b += blockDim.x) s[b] = 0ull;
+  __shared__ unsigned long long s[2 * kExactBins];
+  for (int b = threadIdx.x; b < 2 * kExactBins; b += blockDim.x) s[b] = 0ull;
   __syncthreads();
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const float v = dist[i];
     int b; uint32_t m;
-    sr_exact_bin(v, &b, &m);
+    exact_bin(v, &b, &m);
     if (m) atomicAdd(&s[b], (unsigned long long)m);
-    sr_exact_bin(__fmul_rn(v, v), &b, &m);
-    if (m) atomicAdd(&s[kSrBins + b], (unsigned long long)m);
+    exact_bin(__fmul_rn(v, v), &b, &m);
+    if (m) atomicAdd(&s[kExactBins + b], (unsigned long long)m);
   }
   __syncthreads();
-  for (int b = threadIdx.x; b < 2 * kSrBins; b += blockDim.x)
+  for (int b = threadIdx.x; b < 2 * kExactBins; b += blockDim.x)
     if (s[b]) atomicAdd(&bins[b], s[b]);
 }
 
@@ -97,10 +97,10 @@ sr_bins_kernel(const float* __restrict__ dist, int n, unsigned long long* __rest
 __global__ void __launch_bounds__(32)
 sr_finish_kernel(const unsigned long long* __restrict__ bins, const uint32_t* __restrict__ nf, float std_mul,
                  double* __restrict__ stats) {
-  __shared__ uint64_t limb[kSrLimbs];
+  __shared__ uint64_t limb[kExactLimbs];
   if (threadIdx.x != 0) return;
-  const double sum = sr_exact_finish(reinterpret_cast<const int64_t*>(bins), limb);
-  const double sq_sum = sr_exact_finish(reinterpret_cast<const int64_t*>(bins) + kSrBins, limb);
+  const double sum = exact_finish(reinterpret_cast<const int64_t*>(bins), limb);
+  const double sq_sum = exact_finish(reinterpret_cast<const int64_t*>(bins) + kExactBins, limb);
   const double valid = (double)*nf;
   const double mean = __ddiv_rn(sum, valid);
   const double variance = __ddiv_rn(__dsub_rn(sq_sum, __ddiv_rn(__dmul_rn(sum, sum), valid)), __dsub_rn(valid, 1.0));
@@ -137,7 +137,7 @@ int StatisticRemoval::reserve(int64_t n) {
   SMB_RC(coord.reserve((size_t)3 * sr_pad64(n) * sizeof(double)));
   SMB_RC(index.reserve((size_t)n * sizeof(uint32_t)));
   SMB_RC(dist.reserve((size_t)n * sizeof(float)));
-  SMB_RC(bins.reserve(2 * kSrBins * sizeof(unsigned long long)));
+  SMB_RC(bins.reserve(2 * kExactBins * sizeof(unsigned long long)));
   SMB_RC(stats.reserve(4 * sizeof(double)));
   return count.reserve(2 * sizeof(uint32_t));
 }
@@ -152,7 +152,7 @@ int StatisticRemoval::run(const char* pts, int64_t n, int64_t stride, const uint
   last_n = 0;
   uint32_t* cnt = (uint32_t*)count.p;
   uint32_t* tc = (uint32_t*)tile_cnt.p;
-  SMB_CUDA_OK(cudaMemsetAsync(bins.p, 0, 2 * kSrBins * sizeof(unsigned long long), s));
+  SMB_CUDA_OK(cudaMemsetAsync(bins.p, 0, 2 * kExactBins * sizeof(unsigned long long), s));
   sr_finite_count_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, ni, (uint8_t*)flag.p, tc);
   compact_scan(tc, tiles, s);
   sr_pack_kernel<<<tiles, kCompactThreads, 0, s>>>(pts, stride, ni, (const uint8_t*)flag.p, tc, (double*)coord.p, cs,
@@ -262,15 +262,15 @@ const char* sm_statistic_removal_last_error(const sm_statistic_removal* h) { ret
 // ---- test hooks (include/sm_b200_debug.h) -------------------------------------------------------------------------
 int sm_debug_statistic_removal_exact_sum_host(const float* terms, int64_t n, double* sum) {
   if ((n > 0 && !terms) || n < 0 || n > (1 << 30) || !sum) return SM_ERR_BAD_ARGUMENT;
-  int64_t bins[kSrBins] = {0};
+  int64_t bins[kExactBins] = {0};
   for (int64_t i = 0; i < n; ++i) {
     if (!(terms[i] >= 0.f)) return SM_ERR_BAD_ARGUMENT;     // the sum is defined for non-negative terms and +inf
     int b; uint32_t m;
-    sr_exact_bin(terms[i], &b, &m);
+    exact_bin(terms[i], &b, &m);
     bins[b] += m;
   }
-  uint64_t limb[kSrLimbs];
-  *sum = sr_exact_finish(bins, limb);
+  uint64_t limb[kExactLimbs];
+  *sum = exact_finish(bins, limb);
   return SM_OK;
 }
 

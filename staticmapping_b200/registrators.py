@@ -723,3 +723,65 @@ def matchTwoM2dpDescriptors(P, Q):
     if P.shape != Q.shape:
         return -1.0
     return float(_lib.lib().sm_m2dp_match(P.ctypes.data, Q.ctypes.data, P.shape[0]))
+
+
+class MultiviewRegistratorLumPcl:
+    """registrator::MultiviewRegistratorLumPcl (registrators/multiview_registrator_lum_pcl.h): PCL's LUM multi-view
+    alignment on the GPU.  AddNewCloud(cloud, pose) copies the frame ((n, c) float32 records, c >= 3, x y z first;
+    every frame has the same c) and its 4x4 pose; AlignAll() returns the aligned records of the graph's first Size()
+    vertices, concatenated.  The LUM graph lives on the object: each AlignAll adds every frame again in each of its 5
+    rounds and keeps the poses it reached, so vertex v holds the cloud of the v-th frame ever added."""
+
+    def __init__(self, device: int = 0):
+        self._lib = _lib.lib()
+        self._h = C.c_void_p()
+        rc = self._lib.sm_lum_create(device, C.byref(self._h))
+        if rc == -20:
+            raise RuntimeError("staticmapping_b200: no CUDA device visible and there is no CPU fallback")
+        if rc != 0:
+            raise RuntimeError(f"sm_lum_create failed with {rc}")
+        self._cols = 3
+        self._sizes = []          # points per frame
+        self._vertex_frame = []   # the frame whose cloud vertex v holds
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h is not None and h.value:
+            self._lib.sm_lum_destroy(h)
+            self._h = C.c_void_p()
+
+    def _check(self, rc, what):
+        if rc < 0:
+            msg = self._lib.sm_lum_last_error(self._h)
+            raise CheckFailure(f"{what}: {msg.decode() if msg else rc} (code {rc})")
+        return rc
+
+    def AddNewCloud(self, cloud, pose):
+        pts = cloud.points if isinstance(cloud, InnerCloud) else np.asarray(cloud, dtype=np.float32)
+        pts = np.ascontiguousarray(pts if pts.ndim == 2 else pts.reshape(-1, 3), np.float32)
+        T = np.ascontiguousarray(np.asarray(pose, dtype=np.float32).reshape(4, 4).T)   # Eigen's column-major layout
+        self._check(self._lib.sm_lum_add_cloud(self._h, pts.ctypes.data if pts.size else None, pts.shape[0],
+                                               4 * pts.shape[1], T.ctypes.data), "AddNewCloud")
+        self._cols = pts.shape[1]
+        self._sizes.append(pts.shape[0])
+
+    def Size(self):
+        return int(self._lib.sm_lum_size(self._h))
+
+    def AlignAll(self):
+        N, V0 = len(self._sizes), len(self._vertex_frame)
+        frames = [self._vertex_frame[v] if v < V0 else v - V0 for v in range(N)]
+        out = np.zeros((max(sum(self._sizes[f] for f in frames), 1), self._cols), np.float32)
+        m = C.c_int64(0)
+        self._check(self._lib.sm_lum_align_all(self._h, out.ctypes.data, out.shape[0], C.byref(m)), "AlignAll")
+        if N:
+            self._vertex_frame += list(range(N)) * 5
+        return out[:m.value]
+
+    def Poses(self):
+        """The LUM graph's vertex poses, (n, 6) float32 (x, y, z, roll, pitch, yaw)."""
+        n = C.c_int64(0)
+        self._check(self._lib.sm_lum_poses(self._h, None, 0, C.byref(n)), "Poses")
+        out = np.zeros((n.value, 6), np.float32)
+        self._check(self._lib.sm_lum_poses(self._h, out.ctypes.data, n.value, C.byref(n)), "Poses")
+        return out
