@@ -257,7 +257,12 @@ int sm_align_wait(sm_handle* h, double* result_4x4);
  * it is given its next pair).  Host clouds are uploaded asynchronously on the instance's stream —
  * unlike sm_set_input_*, the arrays of a pair must stay valid until sm_align_pairs returns (pinned
  * host memory makes the copies overlap the other pipelines' kernels).  scores_n (optional) receives
- * GetFitnessScore per pair. */
+ * GetFitnessScore per pair.  rc_n[k] = what sm_set_input_target, sm_set_input_source and sm_align
+ * would have returned for pair k; returns SM_OK or the most negative rc.
+ * A failed pair (rc_n[k] < 0) gets scores_n[k] = 0.0 wherever it failed, and its results_16n slot
+ * is left as the caller passed it.  Nothing of a pair outlives the call: a pair the counts, pointers
+ * or the instance's options refuse is refused before any of it is enqueued, and when a pair fails
+ * after its uploads were enqueued, its instance's stream is synchronized before the next pair. */
 typedef struct sm_pair {
   const double* source_3xn;          /* SetInputSource */
   int64_t n_source;

@@ -307,9 +307,41 @@ int load_cloud(sm_handle* h, const double* pts, int64_t n, bool on_device, DevBu
   return 0;
 }
 
-int icp_set_source(sm_handle* h, IcpFastMatcher& f, const double* pts, int64_t n, bool on_device, bool async = false) {
+// What can refuse a cloud or an alignment, checked before anything is enqueued: each returns 0 or the rc.
+int icp_check_source(sm_handle* h, const double* pts, int64_t n) {
   if (!pts || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInputSource: empty cloud");
   if (n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInputSource: too many points");
+  return 0;
+}
+
+int icp_check_target(sm_handle* h, const double* pts, const double* nrm, int64_t n) {
+  if (!pts || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: empty cloud");
+  if (!nrm) return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: IcpFast target needs normals");
+  if (n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInputTarget: too many points");
+  return 0;
+}
+
+// an alignment of ns -> nt points under the handle's options (icp_begin)
+int icp_check_align(sm_handle* h, const IcpFastMatcher& f, int64_t ns, int64_t nt) {
+  if (ns <= 0 || nt <= 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
+  const float q = f.opt.dist_outlier_ratio;   // CHECK(quantile >= 0 && quantile <= 1), icp_fast.cc:68
+  if (!(q >= 0.0f && q <= 1.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: dist_outlier_ratio outside [0, 1] (icp_fast.cc:68)");
+  if (!(f.opt.knn_epsilon >= 0.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: knn_epsilon must be >= 0");
+  if (kd_num_levels((int)nt, 8) > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "target too large (tree deeper than 24 levels)");
+  return 0;
+}
+
+// a pair of sm_align_pairs, in the order sm_set_input_target, sm_set_input_source and sm_align check it: the rc is
+// the one those calls would return
+int icp_check_pair(sm_handle* h, const IcpFastMatcher& f, const sm_pair& pr) {
+  int rc = icp_check_target(h, pr.target_3xn, pr.target_normals_3xn, pr.n_target);
+  if (rc == 0) rc = icp_check_source(h, pr.source_3xn, pr.n_source);
+  if (rc == 0) rc = icp_check_align(h, f, pr.n_source, pr.n_target);
+  return rc;
+}
+
+int icp_set_source(sm_handle* h, IcpFastMatcher& f, const double* pts, int64_t n, bool on_device, bool async = false) {
+  if (int rc = icp_check_source(h, pts, n)) return rc;
   H_CUDA(cudaEventRecord(h->ev_up[0], h->stream));
   f.sstride = pad64(n);
   H_RC(load_cloud(h, pts, n, on_device, f.src_raw, f.sstride, async ? f.stage_src : f.stage, async));
@@ -321,9 +353,7 @@ int icp_set_source(sm_handle* h, IcpFastMatcher& f, const double* pts, int64_t n
 
 int icp_set_target(sm_handle* h, IcpFastMatcher& f, const double* pts, const double* nrm, int64_t n, bool on_device,
                    bool async = false) {
-  if (!pts || n <= 0) return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: empty cloud");
-  if (!nrm) return fail(h, SM_ERR_MISSING_INPUT, "SetInputTarget: IcpFast target needs normals");
-  if (n > (1 << 30)) return fail(h, SM_ERR_BAD_ARGUMENT, "SetInputTarget: too many points");
+  if (int rc = icp_check_target(h, pts, nrm, n)) return rc;
   H_CUDA(cudaEventRecord(h->ev_up[2], h->stream));
   f.tstride = pad64(n);
   H_RC(load_cloud(h, pts, n, on_device, f.tgt_raw, f.tstride, async ? f.stage_tgt : f.stage, async));
@@ -373,12 +403,7 @@ int icp_enqueue_chunk(sm_handle* h, IcpFastMatcher& f) {
 int icp_begin(sm_handle* h, IcpFastMatcher& f, const double* guess) {
   auto& r = f.run;
   r.active = false;
-  if (f.n_source <= 0 || f.n_target <= 0) return fail(h, SM_ERR_MISSING_INPUT, "Align: source/target not set");
-  {   // CHECK(quantile >= 0 && quantile <= 1), icp_fast.cc:68
-    const float q = f.opt.dist_outlier_ratio;
-    if (!(q >= 0.0f && q <= 1.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: dist_outlier_ratio outside [0, 1] (icp_fast.cc:68)");
-    if (!(f.opt.knn_epsilon >= 0.0f)) return fail(h, SM_ERR_BAD_ARGUMENT, "Align: knn_epsilon must be >= 0");
-  }
+  if (int rc = icp_check_align(h, f, f.n_source, f.n_target)) return rc;
   NvtxRange nvtx_align("IcpFast::Align");
   const int ns = (int)f.n_source, nt = (int)f.n_target;
   const int levels = kd_num_levels(nt, 8);
@@ -402,7 +427,6 @@ int icp_begin(sm_handle* h, IcpFastMatcher& f, const double* guess) {
   p.inner_compensation = f.inner_compensation ? 1 : 0;
   p.error_minimizer = (int16_t)f.error_minimizer;
   r.deskewed = f.inner_compensation ? (double*)f.bufs.deskewed.p : nullptr;
-  if (levels > 24) return fail(h, SM_ERR_BAD_ARGUMENT, "target too large (tree deeper than 24 levels)");
 
   memcpy(h->host_guess, guess, 16 * sizeof(double));   // pinned: the caller's array may go away
   H_CUDA(cudaMemcpyAsync(f.bufs.guess.p, h->host_guess, 16 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
@@ -1060,7 +1084,8 @@ int sm_align_pairs(sm_handle* const* handles, int32_t n_handles, const sm_pair* 
     sm_handle* h = handles[hi];
     cudaSetDevice(h->device);
     rc_n[k] = icp_end(h, *h->as<IcpFastMatcher>(), results_16n + 16 * (size_t)k);
-    if (scores_n) scores_n[k] = h->final_score;
+    if (rc_n[k] < 0) cudaStreamSynchronize(h->stream);   // a chunk enqueued before the failure runs out here
+    if (scores_n) scores_n[k] = rc_n[k] < 0 ? 0.0 : h->final_score;   // final_score is another pair's
     in_flight[(size_t)hi] = -1;
   };
   for (int k = 0; k < n_pairs; ++k) {
@@ -1072,11 +1097,17 @@ int sm_align_pairs(sm_handle* const* handles, int32_t n_handles, const sm_pair* 
     rc_n[k] = 0;
     if (scores_n) scores_n[k] = 0.0;
     if (cudaSetDevice(h->device) != cudaSuccess) { rc_n[k] = fail(h, SM_ERR_CUDA, "cudaSetDevice failed"); continue; }
+    int rc = icp_check_pair(h, f, pr);                    // a refused pair enqueues nothing
+    if (rc < 0) { rc_n[k] = rc; continue; }
     const bool dev = pr.on_device != 0;
-    int rc = icp_set_target(h, f, pr.target_3xn, pr.target_normals_3xn, pr.n_target, dev, !dev);
+    rc = icp_set_target(h, f, pr.target_3xn, pr.target_normals_3xn, pr.n_target, dev, !dev);
     if (rc >= 0) rc = icp_set_source(h, f, pr.source_3xn, pr.n_source, dev, !dev);
     if (rc >= 0) rc = icp_begin(h, f, pr.guess_4x4 ? pr.guess_4x4 : kIdentity);
-    if (rc < 0) { rc_n[k] = rc; continue; }
+    if (rc < 0) {                                         // the uploads may still read the caller's arrays
+      cudaStreamSynchronize(h->stream);
+      rc_n[k] = rc;
+      continue;
+    }
     in_flight[(size_t)hi] = k;
   }
   for (int hi = 0; hi < n_handles; ++hi) collect(hi);
